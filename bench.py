@@ -1,17 +1,17 @@
 #!/usr/bin/env python
-"""Benchmark of the DCA training hot path on B200 (contract: see the task statement / DESIGN.md).
+"""Benchmark of the DCA training hot path on H100 (see DESIGN.md).
 
   python bench.py --gpus N --steps K --warmup W            # our CUDA path
   python bench.py --impl reference --gpus N ...            # CPU arm: torch-CPU restatement of the
                                                            # reference step (TensorFlow is not installable)
+  python bench.py ... --dump-outputs DIR                   # also write the last timed step's results as .npy
 
 A "step" is one training batch of the hot path: forward (Dense stack, BatchNorm, three-head
 output activations), ZINB loss + gradient, backward, gradient all-reduce (N > 1), clip + RMSprop.
 Metric: cells/sec = steps * batch * n_gpus / device time (CUDA events, max over ranks).
-Workload (``--workload auto``): at N = 1 the largest single-GPU configuration of BASELINE.json,
-configs[2] -- synthetic 68k cells x 20k genes (PBMC shape), zinb-conddisp, hidden 64,32,64;
-under torchrun (N > 1) every rank holds one shard of configs[4] (1M x 20k over 8 GPUs = 125k x 20k
-per GPU).  Every step trains 4096 cells per GPU in both cases (weak scaling), so the per-GPU work of
+Workload (``--workload auto``): at N = 1 synthetic 68k cells x 20k genes (PBMC shape), zinb-conddisp,
+hidden 64,32,64 (X bf16 + Y fp32 = 8.2 GB of HBM); under torchrun (N > 1) every rank holds one shard of
+1M x 20k over 8 GPUs = 125k x 20k per GPU (15 GB).  Every step trains 4096 cells per GPU in both cases (weak scaling), so the per-GPU work of
 a step is identical at every N.  Both arms (ours / --impl reference) print the SAME metric string.
 """
 from __future__ import annotations
@@ -31,9 +31,9 @@ sys.path.insert(0, ROOT)
 
 WORKLOADS = {
     # name: (cells per GPU, genes, ae_type, description)
-    "c2": (10000, 2000, "zinb-conddisp", "synthetic 10k cells x 2k genes ZINB-conddisp, hidden=64,32,64 (BASELINE configs[1])"),
-    "c3": (68000, 20000, "zinb-conddisp", "synthetic 68k cells x 20k genes ZINB-conddisp (BASELINE configs[2], PBMC shape)"),
-    "c5shard": (125000, 20000, "zinb-conddisp", "synthetic 125k cells x 20k genes per GPU (BASELINE configs[4] shard, 1M/8)"),
+    "c2": (10000, 2000, "zinb-conddisp", "synthetic 10k cells x 2k genes ZINB-conddisp, hidden=64,32,64"),
+    "c3": (68000, 20000, "zinb-conddisp", "synthetic 68k cells x 20k genes ZINB-conddisp (PBMC shape)"),
+    "c5shard": (125000, 20000, "zinb-conddisp", "synthetic 125k cells x 20k genes per GPU (1M / 8 shard)"),
 }
 HIDDEN = (64, 32, 64)
 # ONE metric string for both arms (the driver divides the two values only when metric / unit / direction agree)
@@ -63,6 +63,9 @@ def parse():
     ap.add_argument("--e2e-format", default="auto", choices=["auto", "sparse", "dense", "u16", "4", "8", "16"],
                     help="host format of the streamed count matrix: packed bits per entry (io.pack_counts) or plain uint16")
     ap.add_argument("--cpu-seconds", type=float, default=15.0, help="budget of the CPU baseline sample")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last of them computed (loss, gradients, updated parameters, "
+                         "BatchNorm moving statistics) as DIR/<name>.npy; the inputs depend only on the arguments")
     return ap.parse_args()
 
 
@@ -107,7 +110,7 @@ def synth_on_device(n_cells, n_genes, device, seed, x_dtype=torch.float32, chunk
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -152,7 +155,7 @@ def measured_peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -259,6 +262,29 @@ def loss_kernel_standalone(eng, X, Y, sf, rows, genes, batch, peak):
             "note": "stand-alone launch incl. its partial-fold kernel, fp32 gradients, L2 flushed before every launch"}
 
 
+DUMP_BUDGET_BYTES = 60_000_000   # all .npy payloads of one dump together stay under 64 MB
+
+
+def dump_outputs(out_dir, eng):
+    """The results a caller of the timed path holds after its last step: the batch loss, the gradient buffer of that
+    step, the parameters after its update and the BatchNorm moving statistics.  The arrays share DUMP_BUDGET_BYTES,
+    smallest first; an array that does not fit its share is replaced by a fixed, seeded sample of its elements (the
+    same indices for the same array length and share)."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = eng.n_params
+    arrays = {"loss": np.array([eng.read_loss()], dtype=np.float64),
+              "bn_state": eng.bn_state.float().cpu().numpy(),
+              "grads": eng.grads[:n].float().cpu().numpy(),
+              "params": eng.params[:n].float().cpu().numpy()}
+    left = DUMP_BUDGET_BYTES
+    for i, (name, v) in enumerate(arrays.items()):
+        cap = left // (v.itemsize * (len(arrays) - i))            # equal share of what the earlier arrays left
+        if v.size > cap:
+            v = v[np.sort(np.random.default_rng(0).choice(v.size, cap, replace=False))]
+        left -= v.nbytes
+        np.save(os.path.join(out_dir, name + ".npy"), v)
+
+
 # ------------------------------------------------------------------------------------------------
 def main():
     a = parse()
@@ -271,13 +297,13 @@ def main():
     tc_shape = (a.gemm_path != "generic") and genes % 8 == 0 and HIDDEN[0] == 64 and HIDDEN[-1] == 64
     if a.x_dtype == "auto":
         a.x_dtype = "bfloat16" if tc_shape else "float32"
-    # what the arithmetic really is: bf16 operands / fp32 accumulation in the gene-wide GEMMs (tcgen05), fp32 everywhere else
+    # what the arithmetic really is: bf16 operands / fp32 accumulation in the gene-wide GEMMs (tensor cores), fp32 everywhere else
     dtype_label = "bf16-gemm/f32-acc/f32-loss" if tc_shape else "f32"
     config = {"workload": desc, "ae_type": ae_type, "hidden": list(HIDDEN), "cells_per_gpu": cells, "genes": genes,
               "batch_per_gpu": batch, "global_batch": batch * max(world, 1), "x_dtype": a.x_dtype,
               "optimizer": "RMSprop(lr=1e-3, clipvalue=5)", "batchnorm": "per-rank batch statistics",
               "parallelism": "dp%d" % max(world, 1),
-              "l2": "dataset (X+Y %.0f MB/GPU) and per-step head tensors exceed the 126 MB L2; no explicit flush"
+              "l2": "dataset (X+Y %.0f MB/GPU) and per-step head tensors exceed the 50 MB L2; no explicit flush"
                     % (cells * genes * (4 + (2 if a.x_dtype == 'bfloat16' else 4)) / 1e6)}
 
     if a.impl == "reference":
@@ -358,6 +384,8 @@ def main():
     barrier()
     ms = e0.elapsed_time(e1)
     launches = launch_count() - l0
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, eng)
     clocks = sampler.stop() if rank == 0 else None
     final_loss = eng.read_loss()
     if world > 1:
@@ -380,19 +408,8 @@ def main():
     loss_bytes = batch * genes * (4 + 4 * nh + einfo["grad_bytes"] * nh)
     ach = loss_bytes / (loss_ms / max(loss_n, 1) * 1e-3) / 1e9 if loss_ms > 0 else None
     step_ms_prof = sum(v[0] for v in prof.values()) / max(a.steps, 1)
-    traffic, traffic_src = None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "roofline_traffic.json")) as f:
-            tj = json.load(f).get(a.workload)
-        if tj and batch == 4096:
-            traffic = tj["dram_read_bytes"] + tj["dram_write_bytes"]
-            traffic_src = "static: one ncu --set full capture of this kernel at this batch shape, " + tj["source"] + \
-                          " (not re-measured inside this run: ncu cannot run inside the timed process)"
-    except Exception:
-        pass
     roofline = {"kernel": "zinb_loss_bwd_ring_kernel (phase loss_fwd_bwd: K3, the last block folds the partials)", "bound": "hbm", "achieved": ach,
-                "peak": peak, "unit": "GB/s", "frac": (ach / peak) if ach else None, "traffic": traffic,
-                "traffic_source": traffic_src,
+                "peak": peak, "unit": "GB/s", "frac": (ach / peak) if ach else None,
                 "peak_source": peak_src, "algorithmic_bytes_per_launch": loss_bytes,
                 "bytes_per_element": 4 + 4 * nh + einfo["grad_bytes"] * nh, "engine": einfo,
                 "share_of_step": (loss_ms / max(loss_n, 1)) / step_ms_prof if step_ms_prof > 0 else None}
@@ -405,7 +422,6 @@ def main():
         roofline["algorithmic_bytes_per_launch"] = batch * genes * 4
         roofline["achieved"] = (batch * genes * 4) / (loss_ms / max(loss_n, 1) * 1e-3) / 1e9 if loss_n else None
         roofline["frac"] = roofline["achieved"] / peak if roofline["achieved"] else None
-        roofline["traffic"] = None
     roofline["loss_kernel_fp32_io"] = (loss_kernel_standalone(eng, X, Y, sf, stream_idx[:batch], genes, batch, peak)
                                        if "standalone" not in _skip else None)
 

@@ -55,7 +55,7 @@ _DEFAULTS = dict(transpose=False, testsplit=False, saveweights=False, sizefactor
 
 
 def build_parser():
-    parser = argparse.ArgumentParser(prog='dca', description='Autoencoder (B200-native DCA hot path)')
+    parser = argparse.ArgumentParser(prog='dca', description='Autoencoder (H100-native DCA hot path)')
     for flags, kw in _OPTIONS:
         parser.add_argument(*flags, **kw)
     parser.set_defaults(**_DEFAULTS)

@@ -1,4 +1,4 @@
-"""``dca()`` with the signature of dca/api.py:19-45, re-pointed at the B200 engine."""
+"""``dca()`` with the signature of dca/api.py:19-45, re-pointed at the H100 engine."""
 from __future__ import annotations
 
 import os

@@ -109,7 +109,7 @@ int Engine::bn_allreduce(double* a, double* b, int n, cudaStream_t s) {
 }
 
 // phase 1 -> [comm stream: all-reduce of the head gradients] || phase 2 -> all-reduce(rest) -> join.
-// tcgen05 path with several heads: phase 1 itself launches the head backward per head and enqueues each head's all-reduce as
+// tensor-core path with several heads: phase 1 itself launches the head backward per head and enqueues each head's all-reduce as
 // soon as that head's gradients are final (engine.cu), so only the loss slot / theta tail is left for the comm stream here.
 int Engine::train_step_dp_body(const void* X, int64_t ldx, const float* Y, int64_t ldy, const float* sf, const int32_t* rows,
                                int Bn, cudaStream_t s) {

@@ -1,4 +1,4 @@
-// Internal declarations shared by the translation units of libdca_b200.so (sm_100a only).
+// Internal declarations shared by the translation units of libdca_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -107,14 +107,15 @@ int expand_sparse(const void* bitmap, const int64_t* nib_indptr, const void* nib
 int gather_rows_bf16(const void* X, int x_bf16, int64_t ldx, const int32_t* rows, int M, int n, __nv_bfloat16* out,
                      cudaStream_t s);
 
-// ---------------------------------------------------------------- tcgen05 kernels (dense_tc.cu, gene_gemm_tc.cu)
+// ---------------------------------------------------------------- tensor-core kernels (dense_tc.cu, gene_gemm_tc.cu)
 namespace tc {
 int heads_fwd_tc(const __nv_bfloat16* Hb, int B, const __nv_bfloat16* const W[3], const float* const bias[3], int G,
                  int n_heads, const int kind[3], const float* row_scale, float* const out[3], int64_t ld_out, int sm_count,
                  cudaStream_t s);
 int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, int B, int G, int n_heads,
                  const __nv_bfloat16* H, const __nv_bfloat16* const W[3], float* out_b, float* const dW[3], int64_t dW_ld,
-                 int dW_transposed, float* const db[3], int sm_count, cudaStream_t s);
+                 int dW_transposed, float* const db[3], void* ws, size_t ws_bytes, int sm_count, cudaStream_t s);
+size_t gene_gemm_workspace_bytes(int B);
 int flash_zinb_tc(const __nv_bfloat16* H3, int B, int G, const __nv_bfloat16* const W[3], const float* const bias[3],
                   const float* Y, int64_t ldy, const int32_t* rows, const float* sf, float ridge, float inv_n,
                   float* dH3, float* const dW[3], float* const db[3], void* ws, size_t ws_bytes, double* loss_sum,

@@ -2,7 +2,7 @@
 // hidden_size=(), ragged gene counts ...).  64x64x16 register-tiled CUDA-core GEMM with optional
 // transposes, row gather on A, split-K (atomic accumulate) and the fused output activations of
 // dca/network.py:38-39,369-381.  The gene-wide layers of the flagship shape (hidden 64) run on
-// the tcgen05 kernels in dense_tc.cu instead; this file is the shape-general path.
+// the tensor-core kernels in dense_tc.cu instead; this file is the shape-general path.
 #include "dca_internal.cuh"
 
 namespace dca {

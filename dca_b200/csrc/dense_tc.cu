@@ -1,12 +1,10 @@
-// tcgen05 / TMEM / TMA Dense kernels for the gene-wide layers of the flagship shape (hidden 64).
+// wgmma / TMA Dense kernels for the gene-wide layers of the flagship shape (hidden 64).
 //
 //   heads_fwd_tc (K2): Z = H3[B x 64] . Wh[64 x nh*G] + b, MeanAct / DispAct / sigmoid fused into the
 //       epilogue (dca/network.py:369-381, :38-39; dca/layers.py:85 for predict).  bf16 operands staged
-//       by TMA (SWIZZLE_128B), fp32 accumulators in TMEM (2 x 256 columns, double buffered), epilogue
-//       TMEM -> registers -> swizzled smem -> TMA store.  Persistent, warp specialised: warp 0 = TMA
-//       producer, warp 1 = MMA issuer (one elected thread), warp 2 = TMEM allocator, warps 4..11 =
-//       epilogue.  HBM-bound: 128 flop per 4-byte output element (SURVEY.md 7.3-1).
-//   tc_probe: single-tile kernel used by the tests to pin the UMMA descriptor conventions
+//       by TMA (SWIZZLE_128B), fp32 accumulators in registers (two warpgroups x m64n128), epilogue
+//       registers -> global.  HBM-bound: 128 flop per 4-byte output element (SURVEY.md 7.3-1).
+//   tc_probe: single-tile kernel used by the tests to pin the wgmma descriptor conventions
 //       (K-major / MN-major operands) against a plain matmul.
 #include <mutex>
 #include "engine.h"
@@ -59,235 +57,151 @@ struct ProbeParams {
   int a_mn, b_mn, M, N, K;
   int a_boxes, a_box_bytes, a_box_c0, a_box_c1;      // per box: coordinate increments (cols, rows)
   int b_boxes, b_box_bytes, b_box_c0, b_box_c1;
-  uint32_t a_lbo, a_sbo, a_kstep, a_kblock_steps, a_kblock_bytes;
-  uint32_t b_lbo, b_sbo, b_kstep, b_kblock_steps, b_kblock_bytes;
-  uint32_t tmem_cols;
+  uint32_t a_lbo, a_sbo, a_kstep, a_kblock_steps, a_kblock_bytes, a_mn64_bytes;
+  uint32_t b_lbo, b_sbo, b_kstep, b_kblock_steps, b_kblock_bytes, b_mn64_bytes;   // mn64: bytes per 64 M / N elements
 };
+
+template <int NC, int TA, int TB>
+__device__ __forceinline__ void probe_mma(float (&acc)[NC / 2], uint64_t da, uint64_t db) {
+  if constexpr (NC == 128) wgmma_m64n128k16<TA, TB>(acc, da, db, 1u);
+  else wgmma_m64n64k16<TA, TB>(acc, da, db, 1u);
+}
+
+// one warpgroup: D[rows m0.., cols n0..n0+NC) of the 128 x N product, K / 16 wgmma steps
+template <int NC>
+__device__ __forceinline__ void probe_chunk(const ProbeParams& p, uint32_t sa, uint32_t sb, int m0, int n0, float* D) {
+  float acc[NC / 2];
+#pragma unroll
+  for (int i = 0; i < NC / 2; ++i) acc[i] = 0.f;
+  const uint32_t a0 = sa + (uint32_t)(m0 / 64) * p.a_mn64_bytes, b0 = sb + (uint32_t)(n0 / 64) * p.b_mn64_bytes;
+  wgmma_fence();
+  for (int j = 0; j < p.K / 16; ++j) {
+    const uint32_t aoff = (j / p.a_kblock_steps) * p.a_kblock_bytes + (j % p.a_kblock_steps) * p.a_kstep;
+    const uint32_t boff = (j / p.b_kblock_steps) * p.b_kblock_bytes + (j % p.b_kblock_steps) * p.b_kstep;
+    const uint64_t da = make_smem_desc(a0 + aoff, p.a_lbo, p.a_sbo), db = make_smem_desc(b0 + boff, p.b_lbo, p.b_sbo);
+    // transpose flags are immediates: one instantiation per operand-major combination
+    if (p.a_mn) { if (p.b_mn) probe_mma<NC, 1, 1>(acc, da, db); else probe_mma<NC, 1, 0>(acc, da, db); }
+    else        { if (p.b_mn) probe_mma<NC, 0, 1>(acc, da, db); else probe_mma<NC, 0, 0>(acc, da, db); }
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  acc_fence(acc);
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < NC / 2; ++i) {
+    const int row = m0 + 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), col = n0 + 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+    D[(size_t)row * p.N + col] = acc[i];
+  }
+}
 
 __global__ void __launch_bounds__(128, 1)
 tc_probe_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                 const ProbeParams p, float* __restrict__ D) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // 1024-byte alignment by OFFSET (not by an integer round trip): the pointer keeps the shared address space, so the
-  // staging stores / bias loads compile to STS / LDS instead of generic ST / LD
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ uint64_t bar_load, bar_mma;
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t bar_load;
   uint8_t* sa = smem;
   uint8_t* sb = smem + (size_t)p.a_boxes * p.a_box_bytes;
-  const int warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) { mbar_init(&bar_load, 1); mbar_init(&bar_mma, 1); fence_barrier_init(); }
-  if (warp == 0) tmem_alloc(&tmem_base_s, p.tmem_cols);
-  tcgen05_fence_before();
+  if (threadIdx.x == 0) { mbar_init(&bar_load, 1); fence_barrier_init(); }
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = tmem_base_s;
   if (threadIdx.x == 0) {
     mbar_expect_tx(&bar_load, (uint32_t)(p.a_boxes * p.a_box_bytes + p.b_boxes * p.b_box_bytes));
     for (int i = 0; i < p.a_boxes; ++i) tma_load_2d(sa + (size_t)i * p.a_box_bytes, &map_a, i * p.a_box_c0, i * p.a_box_c1, &bar_load);
     for (int i = 0; i < p.b_boxes; ++i) tma_load_2d(sb + (size_t)i * p.b_box_bytes, &map_b, i * p.b_box_c0, i * p.b_box_c1, &bar_load);
-    mbar_wait(&bar_load, 0);
-    tcgen05_fence_after();
-    const uint32_t idesc = make_idesc_bf16(p.M, p.N, p.a_mn, p.b_mn);
-    const int steps = p.K / 16;
-    for (int j = 0; j < steps; ++j) {
-      const uint32_t aoff = (j / p.a_kblock_steps) * p.a_kblock_bytes + (j % p.a_kblock_steps) * p.a_kstep;
-      const uint32_t boff = (j / p.b_kblock_steps) * p.b_kblock_bytes + (j % p.b_kblock_steps) * p.b_kstep;
-      const uint64_t da = make_smem_desc(smem_u32(sa) + aoff, p.a_lbo, p.a_sbo);
-      const uint64_t db = make_smem_desc(smem_u32(sb) + boff, p.b_lbo, p.b_sbo);
-      umma_bf16(tmem, da, db, idesc, j > 0 ? 1u : 0u);
+  }
+  mbar_wait(&bar_load, 0);
+  // N chunks of 128 where possible: an MN-major B operand then spans two 64-wide blocks (exercises its LBO)
+  for (int m0 = 0; m0 < p.M; m0 += 64)
+    for (int n0 = 0; n0 < p.N;) {
+      if (p.N - n0 >= 128) { probe_chunk<128>(p, smem_u32(sa), smem_u32(sb), m0, n0, D); n0 += 128; }
+      else { probe_chunk<64>(p, smem_u32(sa), smem_u32(sb), m0, n0, D); n0 += 64; }
     }
-    umma_commit(&bar_mma);
-  }
-  __syncwarp();
-  mbar_wait(&bar_mma, 0);
-  tcgen05_fence_after();
-  for (int c0 = 0; c0 < p.N; c0 += 32) {
-    uint32_t v[32];
-    tmem_ld_32x32(tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-    tmem_ld_wait();
-    const int row = warp * 32 + (threadIdx.x & 31);
-    if (row < p.M)
-      for (int j = 0; j < 32; ++j)
-        if (c0 + j < p.N) D[(size_t)row * p.N + c0 + j] = __uint_as_float(v[j]);
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, p.tmem_cols);
 }
 
 // ------------------------------------------------------------------------------------ K2: heads forward
 namespace k2 {
-constexpr int BM = 128, BN = 256, BK = 64;
-constexpr int kStages = 2, kAccStages = 2;
-constexpr int kEpiWarps = 16, kEpiWarp0 = 4;                     // 4 TMEM lane quarters x 4 column groups of 64
-constexpr int kThreads = (kEpiWarp0 + kEpiWarps) * 32;            // 640
-constexpr uint32_t kABytes = BM * BK * 2, kBBytes = BN * BK * 2;  // 16 KB, 32 KB
-constexpr uint32_t kStageBytes = kABytes + kBBytes;
-constexpr uint32_t kChunkBytes = 32 * 32 * 4;                     // one warp's 32x32 fp32 staging tile
-constexpr uint32_t kOutBytes = kEpiWarps * kChunkBytes;           // one staging tile per warp
-constexpr uint32_t kSmemBytes = kStages * kStageBytes + kOutBytes + kEpiWarps * 64 * 4 + 1024;
+constexpr int BM = 128, BN = 128, BK = 64;
+constexpr int kThreads = 256;                                     // two warpgroups, 64 cells each
+constexpr uint32_t kABytes = BM * BK * 2, kBBytes = BN * BK * 2;  // 16 KB, 16 KB
+constexpr uint32_t kSmemBytes = kABytes + kBBytes + 1024;
 
 struct Params {
   int B, G, n_heads;
   int kind[3];                 // EPI_MEAN_ACT / EPI_DISP_ACT / EPI_SIGMOID per packed head slot
-  int m_tiles, n_tiles_per_head, total_tiles;
+  int m_tiles, n_tiles_per_head;
   const float* bias[3];        // per head slot: float[G]
   const float* row_scale;      // [B] or nullptr
+  float* out[3]; int64_t ld_out;
 };
 
-
-__global__ void __launch_bounds__(kThreads, 1)
+// One 128 x 128 output tile per CTA (grid = m tiles fastest, so that consecutive CTAs share the weight tile in L2).
+// K = 64: the whole operand pair arrives with one TMA transaction; two CTAs per SM overlap one tile's loads with the
+// other's MMA and stores.  The kernel is bound by the fp32 output stores (128 flop per 4-byte element): every warp
+// store instruction covers 8 rows x 32 contiguous bytes, i.e. whole sectors.
+__global__ void __launch_bounds__(kThreads, 2)
 heads_fwd_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_w0,
-                 const __grid_constant__ CUtensorMap map_w1, const __grid_constant__ CUtensorMap map_w2,
-                 const __grid_constant__ CUtensorMap map_o0, const __grid_constant__ CUtensorMap map_o1,
-                 const __grid_constant__ CUtensorMap map_o2, const Params p) {
+                 const __grid_constant__ CUtensorMap map_w1, const __grid_constant__ CUtensorMap map_w2, const Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // 1024-byte alignment by OFFSET (not by an integer round trip): the pointer keeps the shared address space, so the
-  // staging stores / bias loads compile to STS / LDS instead of generic ST / LD
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* s_ab = smem;                                           // stages of [A | B]
-  uint8_t* s_out = smem + kStages * kStageBytes;                  // epilogue staging
-  float* s_bias = reinterpret_cast<float*>(s_out + kOutBytes);    // [kEpiWarps][64]: every epilogue warp keeps ITS 64 biases (no block barrier)
-  __shared__ uint64_t full_bar[kStages], empty_bar[kStages], tfull_bar[kAccStages], tempty_bar[kAccStages];
-  __shared__ uint32_t tmem_base_s;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __shared__ uint64_t full_bar;
+  const int mt = blockIdx.x % p.m_tiles, r = blockIdx.x / p.m_tiles;
+  const int nt = r % p.n_tiles_per_head, hs = r / p.n_tiles_per_head;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < kAccStages; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], kEpiWarps); }
+    mbar_init(&full_bar, 1);
     fence_barrier_init();
-    tma_prefetch_desc(&map_h); tma_prefetch_desc(&map_w0);
-    tma_prefetch_desc(&map_o0); tma_prefetch_desc(&map_o1); tma_prefetch_desc(&map_o2);
+    const CUtensorMap* mw = hs == 0 ? &map_w0 : (hs == 1 ? &map_w1 : &map_w2);
+    mbar_expect_tx(&full_bar, kABytes + kBBytes);
+    tma_load_2d(smem, &map_h, 0, mt * BM, &full_bar);
+    // B = the head kernel in its Keras layout [64 k][G genes] (bf16 shadow): two 64-gene boxes, MN-major
+    tma_load_2d(smem + kABytes, mw, nt * BN, 0, &full_bar);
+    tma_load_2d(smem + kABytes + kBBytes / 2, mw, nt * BN + 64, 0, &full_bar);
   }
-  if (warp == 2) tmem_alloc(&tmem_base_s, kAccStages * BN);      // 512 columns
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = tmem_base_s;
-
-  // tile -> (head slot, n tile, m tile): m fastest so that consecutive CTAs share the weight tile in L2
-  auto decode = [&](int t, int& hs, int& nt, int& mt) { mt = t % p.m_tiles; const int r = t / p.m_tiles; nt = r % p.n_tiles_per_head; hs = r / p.n_tiles_per_head; };
-
-  // Producer and MMA roles: the WHOLE warp walks the tile loop and one elected lane issues (gene_gemm_tc.cu: with the loop
-  // inside `if (lane == 0)` every TMA / MMA descriptor goes through a uniform-register waterfall loop)
-  if (warp == 0) {
-    const bool leader = elect_one();
-    int it = 0;
-    for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++it) {
-      int hs, nt, mt; decode(t, hs, nt, mt);
-      const int st = it % kStages; const uint32_t ph = (it / kStages) & 1;
-      mbar_wait(&empty_bar[st], ph ^ 1);
-      uint8_t* a = s_ab + (size_t)st * kStageBytes;
-      if (leader) {
-        mbar_expect_tx(&full_bar[st], kStageBytes);
-        tma_load_2d(a, &map_h, 0, mt * BM, &full_bar[st]);
-        // B = the head kernel in its Keras layout [64 k][G genes] (bf16 shadow): four 64-gene boxes, MN-major
-        const CUtensorMap* mw = hs == 0 ? &map_w0 : (hs == 1 ? &map_w1 : &map_w2);
+  const int wg = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+  // bias / row scale of this thread's fragment, fetched while the operands are in flight
+  const int col0 = nt * BN + 2 * (l & 3);
+  const int row0 = mt * BM + wg * 64 + 16 * w + (l >> 2);
+  const float* bias = p.bias[hs];
+  const int kind = p.kind[hs];
+  float2 bz[16];
 #pragma unroll
-        for (int j = 0; j < BN / 64; ++j) tma_load_2d(a + kABytes + j * (kBBytes / 4), mw, nt * BN + j * 64, 0, &full_bar[st]);
-      }
-    }
-  } else if (warp == 1) {
-    const bool leader = elect_one();
-    constexpr uint32_t idesc = make_idesc_bf16(BM, BN, 0, 1);     // A = H K-major, B = W MN-major (genes contiguous)
-    int it = 0;
-    for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++it) {
-      const int st = it % kStages; const uint32_t ph = (it / kStages) & 1;
-      const int as = it % kAccStages; const uint32_t aph = (it / kAccStages) & 1;
-      mbar_wait(&tempty_bar[as], aph ^ 1);
-      mbar_wait(&full_bar[st], ph);
-      tcgen05_fence_after();
-      const uint32_t a0 = smem_u32(s_ab + (size_t)st * kStageBytes), b0 = a0 + kABytes;
-      if (leader) {
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          umma_bf16(tmem + as * BN, make_smem_desc(a0 + k * 32, 0, 1024), make_smem_desc(b0 + k * 2048, kBBytes / 4, 1024), idesc, k > 0);
-        umma_commit(&empty_bar[st]);
-        umma_commit(&tfull_bar[as]);
-      }
-    }
-  } else if (warp >= kEpiWarp0) {
-    const bool st_leader = elect_one();            // issues this warp's TMA stores and owns their bulk groups
-    const int ew = warp - kEpiWarp0;               // 0..15
-    const int quarter = warp & 3;                  // TMEM lane quarter this warp may read
-    const int cgrp = ew >> 2;                      // 64-column group of the tile
-    uint8_t* ob = s_out + (size_t)ew * kChunkBytes;
-    int it = 0;
-    // bias / row scale of a tile are fetched one tile AHEAD into registers (the loads sat on the critical path of every tile:
-    // long_scoreboard was the top stall, profiles/r2_ncu_k2_final_raw.csv)
-    float nb0 = 0.f, nb1 = 0.f, nrs = 1.0f;
-    auto fetch = [&](int t) {
-      int hs, nt, mt; decode(t, hs, nt, mt);
-      const int g0 = nt * BN + cgrp * 64 + lane;
-      nb0 = (g0 < p.G) ? p.bias[hs][g0] : 0.f;
-      nb1 = (g0 + 32 < p.G) ? p.bias[hs][g0 + 32] : 0.f;
-      const int row = mt * BM + quarter * 32 + lane;
-      nrs = (p.row_scale && row < p.B) ? p.row_scale[row] : 1.0f;
-    };
-    if ((int)blockIdx.x < p.total_tiles) fetch(blockIdx.x);
-    for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++it) {
-      int hs, nt, mt; decode(t, hs, nt, mt);
-      const int as = it % kAccStages; const uint32_t aph = (it / kAccStages) & 1;
-      // bias of this warp's 64 columns -> its private smem slot (a block-wide barrier here cost 3 of every 12 stall cycles,
-      // profiles/r2_ncu_k2_c3_raw.csv: the 16 warps drift by up to two tiles)
-      const float rs = nrs;
-      {
-        float* mine = s_bias + ew * 64;
-        __syncwarp();                                          // the previous tile's reads of the slot are done
-        mine[lane] = nb0;
-        mine[lane + 32] = nb1;
-        __syncwarp();
-      }
-      if (t + (int)gridDim.x < p.total_tiles) fetch(t + gridDim.x);
-      mbar_wait(&tfull_bar[as], aph);
-      tcgen05_fence_after();
-      const int row = mt * BM + quarter * 32 + lane;
-      (void)row;
-      const int kind = p.kind[hs];
-      const CUtensorMap* mo = hs == 0 ? &map_o0 : (hs == 1 ? &map_o1 : &map_o2);
-      const uint32_t tbase = tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(as * BN + cgrp * 64);
-      const bool have[2] = {nt * BN + cgrp * 64 < p.G, nt * BN + cgrp * 64 + 32 < p.G};
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        if (have[c]) { tmem_ld_32x32(tbase + c * 32, v); tmem_ld_wait(); }
-        if (c == 1) {                                       // accumulator fully read: release it to the MMA warp
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty_bar[as]);
-        }
-        if (!have[c]) continue;
-        const int col0 = cgrp * 64 + c * 32;
-        if (st_leader) bulk_wait_read<0>();                 // previous store has finished reading the staging tile
-        __syncwarp();
-        const float* bz = s_bias + ew * 64 + c * 32;
-        auto emit = [&](auto act) {
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            float o[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) o[j] = act(__uint_as_float(v[q * 4 + j]) + bz[q * 4 + j]);
-            // 128-byte rows, 16-byte chunks XOR-swizzled with the row index (matches SWIZZLE_128B)
-            *reinterpret_cast<float4*>(ob + lane * 128 + ((q ^ (lane & 7)) << 4)) = make_float4(o[0], o[1], o[2], o[3]);
-          }
-        };
-        if (kind == EPI_MEAN_ACT) emit([rs](float z) { return act_mean(z) * rs; });
-        else if (kind == EPI_DISP_ACT) emit([](float z) { return act_disp(z); });
-        else emit([](float z) { return act_sigmoid(z); });
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (st_leader) {
-          tma_store_2d(mo, nt * BN + col0, mt * BM + quarter * 32, ob);
-          bulk_commit();
-        }
-      }
-    }
-    if (st_leader) bulk_wait<0>();
+  for (int c = 0; c < 16; ++c) bz[c] = (col0 + 8 * c < p.G) ? *reinterpret_cast<const float2*>(bias + col0 + 8 * c) : make_float2(0.f, 0.f);
+  float rs[2] = {1.f, 1.f};
+  if (kind == EPI_MEAN_ACT && p.row_scale) {
+    if (row0 < p.B) rs[0] = p.row_scale[row0];
+    if (row0 + 8 < p.B) rs[1] = p.row_scale[row0 + 8];
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem, kAccStages * BN);
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  mbar_wait(&full_bar, 0);
+  const uint32_t a0 = smem_u32(smem) + wg * 64 * 128, b0 = smem_u32(smem) + kABytes;
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < BK / 16; ++k)
+    wgmma_m64n128k16<0, 1>(acc, make_smem_desc(a0 + k * 32, 0, 1024), make_smem_desc(b0 + k * 2048, kBBytes / 2, 1024), k > 0);
+  wgmma_commit();
+  wgmma_wait<0>();
+  acc_fence(acc);
+  float* out = p.out[hs];
+  auto emit = [&](auto act) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 8 * h;
+      if (row >= p.B) continue;
+      float* orow = out + (int64_t)row * p.ld_out;
+#pragma unroll
+      for (int c = 0; c < 16; ++c) {
+        const int col = col0 + 8 * c;
+        if (col < p.G)      // G % 8 == 0: the pair is all in or all out
+          *reinterpret_cast<float2*>(orow + col) =
+              make_float2(act(acc[4 * c + 2 * h] + bz[c].x, rs[h]), act(acc[4 * c + 2 * h + 1] + bz[c].y, rs[h]));
+      }
+    }
+  };
+  if (kind == EPI_MEAN_ACT) emit([](float z, float s) { return act_mean(z) * s; });
+  else if (kind == EPI_DISP_ACT) emit([](float z, float) { return act_disp(z); });
+  else emit([](float z, float) { return act_sigmoid(z); });
 }
 }  // namespace k2
 
@@ -297,25 +211,23 @@ int heads_fwd_tc(const __nv_bfloat16* Hb, int B, const __nv_bfloat16* const W[3]
                  cudaStream_t s) {
   using namespace k2;
   if (ld_out % 4 != 0 || G % 8 != 0) { set_error("heads_fwd_tc: G must be a multiple of 8 and ld_out of 4 (TMA strides)"); return DCA_ERR_BAD_ARG; }
-  CUtensorMap mh, mw[3], mo[3];
+  CUtensorMap mh, mw[3];
   DCA_TRY(make_tensor_map_2d(&mh, Hb, 2, 1, (uint64_t)B, 64, 64, BM, BK, 1));
-  for (int i = 0; i < 3; ++i) {
-    const int k = i < n_heads ? i : 0;
-    DCA_TRY(make_tensor_map_2d(&mw[i], W[k], 2, 1, 64, (uint64_t)G, (uint64_t)G, 64, 64, 1));
-    DCA_TRY(make_tensor_map_2d(&mo[i], out[k], 4, 0, (uint64_t)B, (uint64_t)G, (uint64_t)ld_out, 32, 32, 1));
-  }
+  for (int i = 0; i < 3; ++i)
+    DCA_TRY(make_tensor_map_2d(&mw[i], W[i < n_heads ? i : 0], 2, 1, 64, (uint64_t)G, (uint64_t)G, 64, 64, 1));
   Params p;
   p.B = B; p.G = G; p.n_heads = n_heads;
-  for (int i = 0; i < 3; ++i) { p.kind[i] = kind[i]; p.bias[i] = bias[i < n_heads ? i : 0]; }
-  p.m_tiles = cdiv(B, BM); p.n_tiles_per_head = cdiv(G, BN); p.total_tiles = p.m_tiles * p.n_tiles_per_head * n_heads;
-  p.row_scale = row_scale;
+  for (int i = 0; i < 3; ++i) { const int k = i < n_heads ? i : 0; p.kind[i] = kind[i]; p.bias[i] = bias[k]; p.out[i] = out[k]; }
+  p.m_tiles = cdiv(B, BM); p.n_tiles_per_head = cdiv(G, BN);
+  p.row_scale = row_scale; p.ld_out = ld_out;
+  (void)sm_count;
   static bool attr_set = false;
   if (!attr_set) {
     DCA_CUDA_OK(cudaFuncSetAttribute(heads_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     attr_set = true;
   }
-  const int grid = p.total_tiles < sm_count ? p.total_tiles : sm_count;
-  heads_fwd_kernel<<<grid, kThreads, kSmemBytes, s>>>(mh, mw[0], mw[1], mw[2], mo[0], mo[1], mo[2], p);
+  const int grid = p.m_tiles * p.n_tiles_per_head * n_heads;
+  heads_fwd_kernel<<<grid, kThreads, kSmemBytes, s>>>(mh, mw[0], mw[1], mw[2], p);
   DCA_LAUNCH_CHECK();
   return DCA_OK;
 }
@@ -347,36 +259,34 @@ extern "C" int dca_tc_probe(const void* A, int32_t a_rows, int32_t a_cols, const
                             int32_t a_mn_major, int32_t b_mn_major, int32_t M, int32_t N, int32_t K,
                             int32_t a_lbo, int32_t a_sbo, int32_t b_lbo, int32_t b_sbo, float* D, void* stream) {
   using namespace tc;
-  if (M != 128 || N % 16 != 0 || N < 16 || N > 256 || K % 64 != 0 || K <= 0 || K > 256) {
-    set_error("dca_tc_probe: need M=128, N%%16==0 (16..256), K%%64==0 (<=256)"); return DCA_ERR_BAD_ARG;
+  if (M != 128 || N % 64 != 0 || N < 64 || N > 256 || K % 64 != 0 || K <= 0 || K > 256) {
+    set_error("dca_tc_probe: need M=128, N%%64==0 (64..256), K%%64==0 (<=256)"); return DCA_ERR_BAD_ARG;
   }
   ProbeParams p{};
   p.a_mn = a_mn_major; p.b_mn = b_mn_major; p.M = M; p.N = N; p.K = K;
   CUtensorMap ma, mb;
   auto setup = [&](int mn, int mn_extent, int rows, int cols, const void* base, CUtensorMap* map, int& boxes, int& box_bytes,
                    int& c0, int& c1, uint32_t& lbo, uint32_t& sbo, uint32_t& kstep, uint32_t& kb_steps, uint32_t& kb_bytes,
-                   int lbo_o, int sbo_o) -> int {
+                   uint32_t& mn64_bytes, int lbo_o, int sbo_o) -> int {
     if (!mn) {   // K-major: storage [mn_extent rows][K cols]; one box per 64-wide K block
       if (rows != mn_extent || cols != K) { set_error("dca_tc_probe: K-major operand must be [MN x K]"); return DCA_ERR_BAD_ARG; }
       DCA_TRY(make_tensor_map_2d(map, base, 2, 1, rows, cols, cols, mn_extent, 64, 1));
       boxes = K / 64; box_bytes = mn_extent * 128; c0 = 64; c1 = 0;
-      lbo = 0; sbo = 1024; kstep = 32; kb_steps = 4; kb_bytes = box_bytes;
+      lbo = 0; sbo = 1024; kstep = 32; kb_steps = 4; kb_bytes = box_bytes; mn64_bytes = 64 * 128;
     } else {     // MN-major: storage [K rows][mn_extent cols]; one box per 64-wide MN block
       if (rows != K || cols != mn_extent || mn_extent % 64) { set_error("dca_tc_probe: MN-major operand must be [K x MN], MN%%64==0"); return DCA_ERR_BAD_ARG; }
       DCA_TRY(make_tensor_map_2d(map, base, 2, 1, rows, cols, cols, K, 64, 1));
       boxes = mn_extent / 64; box_bytes = K * 128; c0 = 64; c1 = 0;
-      lbo = box_bytes; sbo = 1024; kstep = 2048; kb_steps = 1u << 30; kb_bytes = 0;
+      lbo = box_bytes; sbo = 1024; kstep = 2048; kb_steps = 1u << 30; kb_bytes = 0; mn64_bytes = box_bytes;
     }
     if (lbo_o >= 0) lbo = lbo_o;
     if (sbo_o >= 0) sbo = sbo_o;
     return DCA_OK;
   };
   DCA_TRY(setup(a_mn_major, M, a_rows, a_cols, A, &ma, p.a_boxes, p.a_box_bytes, p.a_box_c0, p.a_box_c1, p.a_lbo, p.a_sbo,
-                p.a_kstep, p.a_kblock_steps, p.a_kblock_bytes, a_lbo, a_sbo));
+                p.a_kstep, p.a_kblock_steps, p.a_kblock_bytes, p.a_mn64_bytes, a_lbo, a_sbo));
   DCA_TRY(setup(b_mn_major, N, b_rows, b_cols, Bm, &mb, p.b_boxes, p.b_box_bytes, p.b_box_c0, p.b_box_c1, p.b_lbo, p.b_sbo,
-                p.b_kstep, p.b_kblock_steps, p.b_kblock_bytes, b_lbo, b_sbo));
-  uint32_t tc_cols = 32; while ((int)tc_cols < N) tc_cols *= 2;
-  p.tmem_cols = tc_cols;
+                p.b_kstep, p.b_kblock_steps, p.b_kblock_bytes, p.b_mn64_bytes, b_lbo, b_sbo));
   const size_t smem = (size_t)p.a_boxes * p.a_box_bytes + (size_t)p.b_boxes * p.b_box_bytes + 1024;
   DCA_CUDA_OK(cudaFuncSetAttribute(tc_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   tc_probe_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(ma, mb, p, D);
@@ -390,7 +300,7 @@ extern "C" int dca_tc_heads_fwd(const void* Hb, int32_t batch, const void* Wk, c
   if (!Hb || !Wk || !bias || batch <= 0 || genes <= 0 || n_heads < 1 || n_heads > 3 || !out0) {
     set_error("dca_tc_heads_fwd: bad argument"); return DCA_ERR_BAD_ARG;
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   int k[3] = {kind[0], n_heads > 1 ? kind[1] : 0, n_heads > 2 ? kind[2] : 0};

@@ -171,7 +171,8 @@ int Engine::plan(const dca_config& c) {
   mid_ok = !x_kind && plain_hidden() && mid_supported(c.hidden, L);     // the one-launch hidden stack is relu-only, no dropout
   o_bar = take(256);
   o_midpart = take(sizeof(double) * mid_partial_doubles());
-  // tcgen05 path (flagship shape): gene-wide layers with a 64-wide partner dimension
+  o_midgpart = take(sizeof(float) * mid_grad_partial_floats(L));
+  // tensor-core path (flagship shape): gene-wide layers with a 64-wide partner dimension
   n_slots = 0;
   slot_head[0] = 0; slot_kind[0] = EPI_MEAN_ACT; n_slots = 1;
   if (cond) { slot_head[n_slots] = 1; slot_kind[n_slots] = EPI_DISP_ACT; ++n_slots; }
@@ -179,7 +180,7 @@ int Engine::plan(const dca_config& c) {
   const bool want_tc = c.gemm_path != DCA_GEMM_GENERIC && !x_kind;     // the extra AE types run the shape-general fp32 path
   tc_heads = want_tc && L >= 1 && K_head == 64 && (G % 8 == 0);
   tc_enc = want_tc && L >= 1 && c.hidden[0] == 64 && (c.n_in % 8 == 0);
-  // the tcgen05 kernels read the kernels in place from the flat bf16 parameter copy: TMA needs 16-byte aligned bases
+  // the tensor-core kernels read the kernels in place from the flat bf16 parameter copy: TMA needs 16-byte aligned bases
   if (tc_heads) for (int k = 0; k < 3; ++k) if (head_W[k] >= 0 && (head_W[k] % 8) != 0) tc_heads = false;
   {
     const char* ev = getenv("DCA_FUSED_HEADS");
@@ -188,6 +189,7 @@ int Engine::plan(const dca_config& c) {
   }
   if (tc_enc && (lay[0].W % 8) != 0) tc_enc = false;
   if (tc_heads || tc_enc) o_pbf = take(2 * (size_t)P);       // bf16 copy of the parameters, same flat layout
+  if (tc_heads || tc_enc) { ggws_bytes = tc::gene_gemm_workspace_bytes((int)B); o_ggws = take(ggws_bytes); }
   if (tc_heads) {
     o_h3b = take(2 * B * 64);
     for (int k = 0; k < n_slots; ++k) o_dzb[k] = take(2 * B * (size_t)G);
@@ -247,11 +249,11 @@ void Engine::bind(void* base_) {
 
 // ------------------------------------------------------------------------------------ forward
 int Engine::gemm_auto(GemmArgs g, cudaStream_t s) {
-  // split-K so that skinny outputs still fill the 148 SMs
-  const long long tiles = (long long)cdiv(g.M, 64) * cdiv(g.N, 64);
+  // split-K so that skinny outputs still fill the SMs: at least two tiles per SM
+  const long long tiles = (long long)cdiv(g.M, 64) * cdiv(g.N, 64), target = 2ll * sm_count;
   int splits = 1;
-  if (g.epilogue == EPI_ACCUM && tiles < 296 && g.K >= 256) {
-    splits = (int)((296 + tiles - 1) / tiles);
+  if (g.epilogue == EPI_ACCUM && tiles < target && g.K >= 256) {
+    splits = (int)((target + tiles - 1) / tiles);
     const int maxs = g.K / 128;
     if (splits > maxs) splits = maxs;
     if (splits < 1) splits = 1;
@@ -262,7 +264,7 @@ int Engine::gemm_auto(GemmArgs g, cudaStream_t s) {
 
 int Engine::forward(const void* X, int64_t ldx, const int32_t* rows, int Bn, bool training, cudaStream_t s) {
   const void* hin = X; int64_t ldin = ldx; int in_bf16 = x_override_bf16 ? 1 : (cfg.x_dtype == DCA_BF16); const int32_t* gather = rows;
-  // tcgen05 encoder: needs a contiguous bf16 batch (gathered / converted once, reused by the backward pass)
+  // tensor-core encoder: needs a contiguous bf16 batch (gathered / converted once, reused by the backward pass)
   cur_xb = nullptr;
   if (tc_enc) {
     const bool direct = in_bf16 && !rows && (ldx % 8 == 0) && ((reinterpret_cast<uintptr_t>(X) & 15) == 0);
@@ -281,7 +283,7 @@ int Engine::forward(const void* X, int64_t ldx, const int32_t* rows, int Bn, boo
     if (i == 0 && cur_xb) {
       const __nv_bfloat16* Z[3] = {cur_xb, cur_xb, cur_xb};
       const __nv_bfloat16* W1[3] = {bf(o_pbf) + lay[0].W, bf(o_pbf) + lay[0].W, bf(o_pbf) + lay[0].W};
-      DCA_TRY(tc::gene_gemm_tc(1, Z, cur_ldxb, Bn, cfg.n_in, 1, nullptr, W1, a, nullptr, 0, 0, nullptr, sm_count, s));
+      DCA_TRY(tc::gene_gemm_tc(1, Z, cur_ldxb, Bn, cfg.n_in, 1, nullptr, W1, a, nullptr, 0, 0, nullptr, base + o_ggws, ggws_bytes, sm_count, s));
     } else {
     GemmArgs g{};
     g.A = hin; g.lda = ldin; g.a_bf16 = in_bf16; g.transA = 0; g.a_rows = gather;
@@ -332,7 +334,7 @@ void Engine::mid_params(mid::Params& p, int Bn, bool training) {
   }
   p.a0 = f(lay[0].o_a); p.a_center = f(lay[L / 2].o_a);
   p.h_last_bf16 = tc_heads ? bf(o_h3b) : nullptr;
-  p.partial = d(o_midpart); p.bar = reinterpret_cast<unsigned*>(base + o_bar);
+  p.partial = d(o_midpart); p.gpart = f(o_midgpart); p.bar = reinterpret_cast<unsigned*>(base + o_bar);
   p.eps = cfg.bn_eps; p.momentum = cfg.bn_momentum;
 }
 
@@ -500,7 +502,7 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
   la.m = Mb; la.d = cond ? Db : f(o_theta); la.pi = has_pi ? Pb : nullptr; la.ld = G;
   la.B = Bn; la.G = G; la.ae_type = cfg.ae_type; la.ridge = cfg.ridge; la.inv_n = inv_n;
   la.dzm = Mb; la.dzd = cond ? Db : nullptr; la.dzp = has_pi ? Pb : nullptr; la.grad_bf16 = 0;
-  if (tc_heads) {          // bf16 gradients for the tcgen05 head-backward kernel, packed-slot order
+  if (tc_heads) {          // bf16 gradients for the tensor-core head-backward kernel, packed-slot order
     void* slot_buf[3] = {nullptr, nullptr, nullptr};
     for (int k = 0; k < n_slots; ++k) slot_buf[slot_head[k]] = bf(o_dzb[k]);
     la.dzm = slot_buf[0]; la.dzd = cond ? slot_buf[1] : nullptr; la.dzp = has_pi ? slot_buf[2] : nullptr; la.grad_bf16 = 1;
@@ -533,14 +535,14 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
       for (int k = 0; k < n_slots; ++k) {
         const __nv_bfloat16* Z1[3] = {Z[k], Z[k], Z[k]}; const __nv_bfloat16* W1[3] = {Wk[k], Wk[k], Wk[k]};
         float* dW1[3] = {dWp[k], dWp[k], dWp[k]}; float* db1[3] = {dbp[k], dbp[k], dbp[k]};
-        DCA_TRY(tc::gene_gemm_tc(3, Z1, G, Bn, G, 1, bf(o_h3b), W1, dh, dW1, G, 1, db1, sm_count, s));
+        DCA_TRY(tc::gene_gemm_tc(3, Z1, G, Bn, G, 1, bf(o_h3b), W1, dh, dW1, G, 1, db1, base + o_ggws, ggws_bytes, sm_count, s));
         const int h = slot_head[k];
         DCA_CUDA_OK(cudaEventRecord(ev_fork, s));
         DCA_CUDA_OK(cudaStreamWaitEvent(comm_stream, ev_fork, 0));
         DCA_TRY(allreduce_range(head_W[h], head_b[h] + G, comm_stream));
       }
     } else
-    DCA_TRY(tc::gene_gemm_tc(3, Z, G, Bn, G, n_slots, bf(o_h3b), Wk, dh, dWp, G, 1, dbp, sm_count, s));
+    DCA_TRY(tc::gene_gemm_tc(3, Z, G, Bn, G, n_slots, bf(o_h3b), Wk, dh, dWp, G, 1, dbp, base + o_ggws, ggws_bytes, sm_count, s));
   } else
   for (int k = 0; k < 3; ++k) {
     if (head_W[k] < 0 || !dz[k]) continue;
@@ -574,7 +576,7 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
     if (cur_xb) {
       const __nv_bfloat16* Z[3] = {cur_xb, cur_xb, cur_xb};
       float* dWp[3] = {gp(l.W), gp(l.W), gp(l.W)};
-      DCA_TRY(tc::gene_gemm_tc(2, Z, cur_ldxb, Bn, cfg.n_in, 1, bf(o_da1b), nullptr, nullptr, dWp, l.out, 0, nullptr, sm_count - dp_reserve_sms, s));
+      DCA_TRY(tc::gene_gemm_tc(2, Z, cur_ldxb, Bn, cfg.n_in, 1, bf(o_da1b), nullptr, nullptr, dWp, l.out, 0, nullptr, nullptr, 0, sm_count - dp_reserve_sms, s));
     } else {
       GemmArgs g{};
       g.A = X; g.lda = ldx; g.a_bf16 = x_override_bf16 ? 1 : (cfg.x_dtype == DCA_BF16); g.transA = 1; g.a_rows = xrows;
@@ -599,7 +601,7 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
       DCA_TRY(cast_to_bf16(dh, bf(o_da1b), (int64_t)Bn * l.out, s));
       const __nv_bfloat16* Z[3] = {cur_xb, cur_xb, cur_xb};
       float* dWp[3] = {gp(l.W), gp(l.W), gp(l.W)};
-      DCA_TRY(tc::gene_gemm_tc(2, Z, cur_ldxb, Bn, cfg.n_in, 1, bf(o_da1b), nullptr, nullptr, dWp, l.out, 0, nullptr, sm_count, s));
+      DCA_TRY(tc::gene_gemm_tc(2, Z, cur_ldxb, Bn, cfg.n_in, 1, bf(o_da1b), nullptr, nullptr, dWp, l.out, 0, nullptr, nullptr, 0, sm_count, s));
       DCA_TRY(col_sums(dh, nullptr, l.out, Bn, l.out, d(o_dsum), nullptr, d(o_scratch), s));
       DCA_TRY(col_sum_to_float(d(o_dsum), l.out, gp(l.b), s));
       continue;
@@ -709,7 +711,7 @@ int Engine::predict(const void* X, int64_t ldx, const float* sf, const int32_t* 
 
 bool Engine::tc_supported() const { return tc_heads && tc_enc; }
 const char* Engine::tc_reason() const {
-  return "tcgen05 path needs hidden_size[0] == hidden_size[-1] == 64, n_in % 8 == 0 and n_out % 8 == 0";
+  return "tensor-core path needs hidden_size[0] == hidden_size[-1] == 64, n_in % 8 == 0 and n_out % 8 == 0";
 }
 int Engine::setup_tc() {
   if (const char* e = getenv("DCA_GRAPH")) graphs_enabled = !(e[0] == '0');
@@ -720,11 +722,11 @@ int Engine::setup_tc() {
   if (tc_heads || tc_enc) {
     int major = 0;
     DCA_CUDA_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-    if (major != 10) { set_error("libdca_b200 is built for sm_100a only (device compute capability %d.x)", major); return DCA_ERR_UNSUPPORTED; }
+    if (major != 9) { set_error("libdca_b200 is built for sm_90a only (device compute capability %d.x)", major); return DCA_ERR_UNSUPPORTED; }
   }
   return DCA_OK;
 }
-// Re-derive the bf16 copy of the parameters (the tcgen05 kernels read every kernel in its Keras layout, so the
+// Re-derive the bf16 copy of the parameters (the tensor-core kernels read every kernel in its Keras layout, so the
 // "shadow" is a plain element-wise cast; after an optimizer step the RMSprop kernel writes it directly).
 int Engine::refresh_shadows(cudaStream_t s) {
   if (!tc_heads && !tc_enc) return DCA_OK;
@@ -1123,9 +1125,9 @@ extern "C" int dca_stream_begin_packed(dca_handle* h, const void* packed_host, i
     int least = 0, greatest = 0;
     DCA_CUDA_OK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
     DCA_CUDA_OK(cudaStreamCreateWithFlags(&hs.copy, cudaStreamNonBlocking));
-    // expansion stream: HIGHEST priority.  Its blocks only find room between the (persistent, one CTA per SM) kernels of
-    // the step; at the lowest priority the expansion of batch i+1 mostly ran AFTER step i and 0.25 ms of it were exposed
-    // (profiles/r2_diag_e2e_timeline.log); DCA_EXPAND_PRIO=low restores the old behaviour
+    // expansion stream: HIGHEST priority.  Its blocks only find room between the kernels of the step; at the lowest
+    // priority the expansion of batch i+1 can run after step i instead of under it.  DCA_EXPAND_PRIO=low selects the
+    // lowest priority
     const char* pe = getenv("DCA_EXPAND_PRIO");
     DCA_CUDA_OK(cudaStreamCreateWithPriority(&hs.expand, cudaStreamNonBlocking, (pe && pe[0] == 'l') ? least : greatest));
     for (int k = 0; k < 2; ++k) {
@@ -1199,7 +1201,7 @@ extern "C" int dca_stream_step(dca_handle* h, int64_t i, int64_t next, void* str
   static const int diag = [] { const char* v = getenv("DCA_STREAM_DIAG"); return v ? atoi(v) : 0; }();
   int st = DCA_OK;
   if (diag != 1) {                                  // (1 = diagnosis: copies + expansion only)
-    e.x_override_bf16 = e.tc_enc ? 1 : 0;           // the tcgen05 encoder reads the expanded bf16 batch in place
+    e.x_override_bf16 = e.tc_enc ? 1 : 0;           // the tensor-core encoder reads the expanded bf16 batch in place
     st = e.train_step(e.base + e.o_sx[xb], e.cfg.n_in, e.f(e.o_sy[xb]), e.cfg.n_out, e.f(e.o_ssf[xb]), nullptr, nb, s, 0);
     e.x_override_bf16 = 0;
   }

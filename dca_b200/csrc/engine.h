@@ -81,7 +81,7 @@ struct Engine {
   void mark(int phase, cudaStream_t s);
   int prof_collect();
   // fused hidden stack (mid_stack.cu)
-  bool mid_ok = false; size_t o_bar = 0, o_midpart = 0;
+  bool mid_ok = false; size_t o_bar = 0, o_midpart = 0, o_midgpart = 0;
   bool use_mid(int Bn) const { return mid_ok && !bn_synced() && Bn <= mid::kMaxRows * mid::kMaxCtas; }
   void mid_params(mid::Params& p, int Bn, bool training);
   // activations other than relu, PReLU slopes, dropout (activations.cu): per-layer hidden path only
@@ -91,13 +91,13 @@ struct Engine {
   int act_fwd(Layer& l, int Bn, bool training, __nv_bfloat16* hb, cudaStream_t s);
   int act_bwd(Layer& l, float* dh, int Bn, cudaStream_t s);
   int drop_input(const void* X, int in_bf16, int64_t ldx, const int32_t* rows, int Bn, cudaStream_t s);
-  // tcgen05 path: flags + operand-layout shadows / bf16 activations in the arena
+  // tensor-core path: flags + operand-layout shadows / bf16 activations in the arena
   bool tc_heads = false, tc_enc = false;
   bool fused_heads = false;       // flash_zinb.cu replaces K2 + K3 + K4 of the training step (zinb-conddisp only)
-  int sm_count = 148, n_slots = 1;
+  int sm_count = 132, n_slots = 1;
   int slot_head[3] = {0, -1, -1};          // packed head slot -> head index (0 mean, 1 dispersion, 2 pi)
   int slot_kind[3] = {0, 0, 0};
-  size_t o_pbf = 0, o_h3b = 0, o_da1b = 0, o_xb = 0, o_dzb[3] = {0, 0, 0};
+  size_t o_pbf = 0, o_h3b = 0, o_da1b = 0, o_xb = 0, o_dzb[3] = {0, 0, 0}, o_ggws = 0, ggws_bytes = 0;
   const __nv_bfloat16* cur_xb = nullptr; int64_t cur_ldxb = 0;   // bf16 batch input of the current step
   __nv_bfloat16* bf(size_t byte_off) const { return reinterpret_cast<__nv_bfloat16*>(base + byte_off); }
 
@@ -169,7 +169,7 @@ struct Engine {
               float* pi_out, int64_t ld_out, float* latent_out, cudaStream_t s);
   int init_params(uint64_t seed, cudaStream_t s);
 
-  // tcgen05 path hooks (dense_tc.cu)
+  // tensor-core path hooks (dense_tc.cu)
   bool tc_supported() const;
   const char* tc_reason() const;
   int setup_tc();

@@ -3,17 +3,13 @@
 // their autodiff).  The B x 3G head activations and their gradients never reach HBM:
 //
 //   per tile (128 cells x 64 genes, all three heads):
-//     MMA1   Z[128 x 192] = H3[128 x 64] . [Wm | Wd | Wp][64 x 3*64]          -> TMEM (fp32)
-//     epilogue (16 warps)  z + bias -> MeanAct / DispAct / sigmoid -> ZINB NLL and d/dz (zinb_math.cuh, same
-//                          arithmetic and warp compaction as the stand-alone loss kernel) -> dZ bf16 written into
-//                          shared memory in the SWIZZLE_128B operand layout
+//     MMA1   Z_h[128 x 64] = H3[128 x 64] . W_h[64 x 64]                     -> registers (fp32, wgmma)
+//     elements  z + bias -> MeanAct / DispAct / sigmoid -> ZINB NLL and d/dz (zinb_math.cuh, the arithmetic of the
+//               stand-alone loss kernel) -> dZ bf16 written into shared memory in the SWIZZLE_128B operand layout
 //     MMA2   dH3[128 x 64]  = sum_h dZ_h[128 x 64] . W_h^T                    (dZ as K-major A)
-//     MMA3   dW_h[64g x 64] += dZ_h^T . H3, db_h += dZ_h^T . 1                (the same bytes as MN-major A; two
-//                          heads stacked per M = 128 accumulator)
+//     MMA3   dW_h[64g x 64] += dZ_h^T . H3, db_h += dZ_h^T . 1                (the same bytes as MN-major A)
 //   HBM traffic: the count tile (4 B / element) in, 1/64 of it out.  dH3 leaves per tile by TMA reduce-add,
-//   dW / db stay in TMEM over all cell blocks of a gene tile and are added to the gradient buffer once.
-//
-// Warp roles (768 threads): 0 TMA producer, 1 MMA issuer, 2 TMEM allocator, 4-19 loss epilogue, 20-23 flush.
+//   dW / db stay in shared memory over all cell blocks of a gene tile and are added to the gradient buffer once.
 #include "engine.h"
 #include "tc_common.cuh"
 #include "head_act.cuh"
@@ -23,21 +19,16 @@ namespace dca {
 namespace tc {
 namespace fz {
 
-constexpr int kEpiWarp0 = 4, kEpiWarps = 16, kFlushWarp0 = 20, kFlushWarps = 4;
-constexpr int kThreads = (kFlushWarp0 + kFlushWarps) * 32;     // 768
+constexpr int kThreads = 256;                                  // two warpgroups, 64 cells of the tile each
 constexpr uint32_t kHBytes = 128 * 64 * 2;                     // [128 cells x 64 feats] bf16
 constexpr uint32_t kWBox = 64 * 64 * 2, kWBytes = 3 * kWBox;   // per head [64 feats x 64 genes] bf16
-constexpr uint32_t kZBox = 128 * 64 * 2, kZBytes = 3 * kZBox;  // per head [128 cells x 64 genes] bf16
-constexpr uint32_t kOutBytes = 2 * 128 * 32 * 4;               // dH3 staging: two [128 x 32] fp32 tiles
-constexpr uint32_t kQueueBytes = 128 * 16;                     // per epilogue warp: 128 items of 16 B
-constexpr uint32_t kOffH = 0, kOffW = kOffH + 2 * kHBytes, kOffZ = kOffW + kWBytes, kOffO = kOffZ + 2 * kZBytes,
-                   kOffOnes = kOffO + kOutBytes, kOffQ = kOffOnes + 2048, kSmemUsed = kOffQ + kEpiWarps * kQueueBytes;
+constexpr uint32_t kZBox = 128 * 64 * 2, kZBytes = 3 * kZBox;  // per head dZ [128 cells x 64 genes] bf16
+constexpr uint32_t kOutBytes = 128 * 64 * 4;                   // dH3 staging [128 x 64] fp32
+constexpr uint32_t kDwFloats = 3 * 64 * 64;                    // dW accumulators [head][feat][gene] fp32
+constexpr uint32_t kOffH = 0, kOffW = kOffH + 2 * kHBytes, kOffZ = kOffW + kWBytes, kOffO = kOffZ + kZBytes,
+                   kOffDw = kOffO + kOutBytes, kOffDb = kOffDw + kDwFloats * 4, kOffOnes = kOffDb + 3 * 64 * 4,
+                   kSmemUsed = kOffOnes + 2048;
 constexpr uint32_t kSmemBytes = kSmemUsed + 1024;
-constexpr uint32_t kTmemCols = 512;
-// TMEM (512 columns): two pre-activation accumulators of 192 columns (double-buffered over tiles) and the two dW
-// accumulators.  Once the epilogue has consumed accumulator b, the head-backward products of the same tile reuse
-// its columns: dH3 at +0..63, the per-tile column sums (bias gradient) at +64..95.
-constexpr uint32_t kTmD1 = 0, kTmD1Stride = 192, kTmDhOff = 0, kTmCsOff = 64, kTmDw = 384;
 
 struct Params {
   int B, G, n_cb, n_gt, total_tiles;
@@ -50,15 +41,10 @@ struct Params {
   int batch;
 };
 
-__device__ __forceinline__ void bulk_prefetch_l2(const void* gptr, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(gptr)), "r"(bytes) : "memory");
-}
-
-// NB branch of one queued element; deliberately not inlined (one copy of the lgamma / digamma code keeps the
-// epilogue loop inside the instruction cache)
-__device__ __noinline__ float4 nb_item(float4 it, const float* lf) {
-  const zmath::Raw1 e = zmath::zinb_nb_raw<zmath::FastOps>(it.x, it.y, it.z, it.w, lf);     // raw derivatives, see zinb_math.cuh
-  return make_float4(e.gmu, e.dth, e.dpi, e.loss);
+// NB branch of one element; deliberately not inlined (one copy of the lgamma / digamma code keeps the element loop
+// inside the instruction cache)
+__device__ __noinline__ zmath::Raw1 nb_item(float y, float mu, float th, float pi, const float* lf) {
+  return zmath::zinb_nb_raw<zmath::FastOps>(y, mu, th, pi, lf);       // raw derivatives, see zinb_math.cuh
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
@@ -66,387 +52,251 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// One CTA walks a contiguous range of tiles; tile t -> gene tile t / n_cb, cell block t % n_cb (cells fastest, so the
+// weight tile and the dW accumulators stay put over a run of cell blocks = one "segment").  Per tile:
+//   MMA1 (wgmma, registers)  z_h[64 cells x 64 genes] = H3 . W_h for the three heads, per warpgroup
+//   element loop             activations, ZINB NLL and d/dz of the thread's 2 x 16 element pairs (the f32x2
+//                            formulation of the stand-alone loss kernel) -> dZ_h bf16 into shared memory in the
+//                            SWIZZLE_128B operand layout
+//   MMA2                     dH3 = sum_h dZ_h . W_h^T (dZ as K-major A) -> staging tile -> TMA reduce-add
+//   MMA3                     dW_h^T += dZ_h^T . H3, db_h += dZ_h^T . 1 (the same bytes as MN-major A; the two
+//                            warpgroups split the cells) -> shared-memory fp32 accumulators, added to the gradient
+//                            buffer once per segment
 __global__ void __launch_bounds__(kThreads, 1)
 flash_zinb_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_w0,
                   const __grid_constant__ CUtensorMap map_w1, const __grid_constant__ CUtensorMap map_w2,
                   const __grid_constant__ CUtensorMap map_o, const Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // 1024-byte alignment by OFFSET (not by an integer round trip) so that the compiler keeps the shared address space
-  // and emits LDS / STS instead of generic loads and stores
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* s_h = smem + kOffH; uint8_t* s_w = smem + kOffW; uint8_t* s_z = smem + kOffZ; uint8_t* s_o = smem + kOffO;
-  uint8_t* s_ones = smem + kOffOnes; uint8_t* s_q = smem + kOffQ;
-  __shared__ uint64_t h_full[2], h_empty[2], w_full, w_empty, d1_full[2], d1_empty[2], dz_full[2], dz_empty[2], dh_full[2],
-      dh_empty[2], dw_full, dw_empty;
-  __shared__ uint32_t tmem_base_s;
+  uint8_t* s_h = smem + kOffH; uint8_t* s_w = smem + kOffW; uint8_t* s_z = smem + kOffZ;
+  float* s_o = reinterpret_cast<float*>(smem + kOffO);
+  float* s_dw = reinterpret_cast<float*>(smem + kOffDw);
+  float* s_db = reinterpret_cast<float*>(smem + kOffDb);
+  uint8_t* s_ones = smem + kOffOnes;
+  __shared__ uint64_t h_full[2], w_full;
   __shared__ float lf[zmath::kLogFactN];
-  __shared__ double red[kEpiWarps];
+  __shared__ double red[kThreads / 32];
   __shared__ int s_last;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&h_full[i], 1); mbar_init(&h_empty[i], 1);
-      mbar_init(&dz_full[i], kEpiWarps); mbar_init(&dz_empty[i], 1);
-      mbar_init(&dh_full[i], 1); mbar_init(&dh_empty[i], kFlushWarps);
-      mbar_init(&d1_full[i], 1); mbar_init(&d1_empty[i], kEpiWarps);
-    }
-    mbar_init(&w_full, 1); mbar_init(&w_empty, 1);
-    mbar_init(&dw_full, 1); mbar_init(&dw_empty, kFlushWarps);
-    fence_barrier_init();
-    tma_prefetch_desc(&map_h); tma_prefetch_desc(&map_w0); tma_prefetch_desc(&map_w1); tma_prefetch_desc(&map_w2);
-    tma_prefetch_desc(&map_o);
-  }
-  if (warp == 2) tmem_alloc(&tmem_base_s, kTmemCols);
-  if (threadIdx.x < zmath::kLogFactN) lf[threadIdx.x] = p.lf_global[threadIdx.x];
-  for (int i = threadIdx.x; i < 2048 / 4; i += kThreads) reinterpret_cast<uint32_t*>(s_ones)[i] = 0x3F803F80u;   // bf16 ones
-  fence_proxy_async_smem();
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = tmem_base_s;
-
-  // this CTA's contiguous range of tiles; tile t -> gene tile t / n_cb, cell block t % n_cb (cells fastest, so the
-  // weight tile and the dW accumulators stay put over a run of cell blocks = one "segment")
   const int t0 = (int)((long long)p.total_tiles * blockIdx.x / gridDim.x);
   const int t1 = (int)((long long)p.total_tiles * (blockIdx.x + 1) / gridDim.x);
+  auto issue_h = [&](int t, int buf) {
+    mbar_expect_tx(&h_full[buf], kHBytes);
+    tma_load_2d(s_h + buf * kHBytes, &map_h, 0, (t % p.n_cb) * 128, &h_full[buf]);
+  };
+  auto issue_w = [&](int t) {
+    const int gt = t / p.n_cb;
+    mbar_expect_tx(&w_full, kWBytes);
+    tma_load_2d(s_w, &map_w0, gt * 64, 0, &w_full);
+    tma_load_2d(s_w + kWBox, &map_w1, gt * 64, 0, &w_full);
+    tma_load_2d(s_w + 2 * kWBox, &map_w2, gt * 64, 0, &w_full);
+  };
+  if (threadIdx.x == 0) {
+    mbar_init(&h_full[0], 1); mbar_init(&h_full[1], 1); mbar_init(&w_full, 1);
+    fence_barrier_init();
+    if (t0 < t1) { issue_w(t0); issue_h(t0, 0); }
+  }
+  if (threadIdx.x < zmath::kLogFactN) lf[threadIdx.x] = p.lf_global[threadIdx.x];
+  for (int i = threadIdx.x; i < 2048 / 4; i += kThreads) reinterpret_cast<uint32_t*>(s_ones)[i] = 0x3F803F80u;   // bf16 ones
+  for (int i = threadIdx.x; i < (int)kDwFloats; i += kThreads) s_dw[i] = 0.f;
+  for (int i = threadIdx.x; i < 3 * 64; i += kThreads) s_db[i] = 0.f;
+  fence_proxy_async_smem();
+  __syncthreads();
 
-  if (warp == 0) {
-    // ===================================================== TMA producer
-    if (lane == 0) {
-      uint32_t hi = 0, seg = 0;
-      for (int t = t0; t < t1; ++t) {
-        const int gt = t / p.n_cb, cb = t % p.n_cb;
-        if (t == t0 || cb == 0) {
-          mbar_wait(&w_empty, (seg & 1) ^ 1); ++seg;
-          mbar_expect_tx(&w_full, kWBytes);
-          tma_load_2d(s_w, &map_w0, gt * 64, 0, &w_full);
-          tma_load_2d(s_w + kWBox, &map_w1, gt * 64, 0, &w_full);
-          tma_load_2d(s_w + 2 * kWBox, &map_w2, gt * 64, 0, &w_full);
+  using Ops = zmath::FastOps;
+  using namespace zmath;
+  const int wg = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+  const int frow = 16 * w + (l >> 2), fcol = 2 * (l & 3);            // fragment origin (see tc_common.cuh)
+  const uint32_t wb = smem_u32(s_w), zb = smem_u32(s_z), ob = smem_u32(s_ones);
+  float lsum = 0.f, lsum_lg = 0.f;        // NLL of the NB elements (+ ridge) | sum of lg2(D) over the zero counts
+  uint32_t seg = 0;
+  for (int t = t0, ti = 0; t < t1; ++t, ++ti) {
+    const int gt = t / p.n_cb, cb = t % p.n_cb;
+    const bool new_seg = (t == t0 || cb == 0);
+    if (threadIdx.x == 0) {
+      if (new_seg && t != t0) issue_w(t);                              // the previous segment's MMAs are complete
+      if (t + 1 < t1) issue_h(t + 1, (ti + 1) & 1);                     // its buffer was released at the end of tile ti-1
+    }
+    if (new_seg) { mbar_wait(&w_full, seg & 1); ++seg; }
+    const int hbuf = ti & 1;
+    mbar_wait(&h_full[hbuf], (ti >> 1) & 1);
+    const uint32_t hb = smem_u32(s_h + hbuf * kHBytes);
+
+    // ---- MMA1: pre-activations of the three heads, rows 64*wg.. of the tile
+    float zm[32], zd[32], zp[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) { zm[i] = 0.f; zd[i] = 0.f; zp[i] = 0.f; }
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint64_t da = make_smem_desc(hb + wg * 64 * 128 + k * 32, 0, 1024);
+      wgmma_m64n64k16<0, 1>(zm, da, make_smem_desc(wb + k * 2048, 0, 1024), k > 0);
+      wgmma_m64n64k16<0, 1>(zd, da, make_smem_desc(wb + kWBox + k * 2048, 0, 1024), k > 0);
+      wgmma_m64n64k16<0, 1>(zp, da, make_smem_desc(wb + 2 * kWBox + k * 2048, 0, 1024), k > 0);
+    }
+    wgmma_commit();
+
+    // ---- per-row operands while the MMAs run
+    int yr[2]; float sfv[2]; bool vrow[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int grow = cb * 128 + wg * 64 + frow + 8 * h;
+      vrow[h] = grow < p.B; yr[h] = 0; sfv[h] = 1.0f;
+      if (vrow[h]) { yr[h] = p.rows ? p.rows[grow] : grow; sfv[h] = p.sf ? p.sf[yr[h]] : 1.0f; }
+    }
+    wgmma_wait<0>();
+    acc_fence(zm); acc_fence(zd); acc_fence(zp);
+
+    // ---- element loop: pair c of row half h = columns 8*c + fcol, +1 of row frow + 8*h
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      const int col = 8 * c + fcol, g = gt * 64 + col;
+      const bool cols_in = g < p.G;                                      // G % 8 == 0: the pair is all in or all out
+      float2 bm = make_float2(0.f, 0.f), bd = bm, bp = bm;
+      if (cols_in) {
+        bm = *reinterpret_cast<const float2*>(p.bias[0] + g);
+        bd = *reinterpret_cast<const float2*>(p.bias[1] + g);
+        bp = *reinterpret_cast<const float2*>(p.bias[2] + g);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int i = 4 * c + 2 * h;
+        const bool active = vrow[h] && cols_in;
+        float2 y = make_float2(0.f, 0.f);
+        if (active) y = *reinterpret_cast<const float2*>(p.Y + (int64_t)yr[h] * p.ldy + g);
+        const float2 m = make_float2(act_mean(zm[i] + bm.x), act_mean(zm[i + 1] + bm.y));
+        const float2 d = make_float2(act_disp(zd[i] + bd.x), act_disp(zd[i + 1] + bd.y));
+        const float2 pi = make_float2(act_sigmoid(zp[i] + bp.x), act_sigmoid(zp[i + 1] + bp.y));
+        const float2 mu = mul2(m, splat(sfv[h]));                                          // dca/layers.py:85
+        Raw2 z = zinb_zero_pair<Ops>(mu, d, pi);
+        const Fin2 f = finish_factors_pair<Ops, true>(m, d, pi, p.inv_n);
+        const bool nz0 = active && !(y.x < 1e-8f), nz1 = active && !(y.y < 1e-8f);       // loss.py:138
+        if (nz0) { const Raw1 e = nb_item(y.x, mu.x, d.x, pi.x, lf); lsum += e.loss; z.gmu.x = e.gmu; z.dth.x = e.dth; z.dpi.x = e.dpi; }
+        if (nz1) { const Raw1 e = nb_item(y.y, mu.y, d.y, pi.y, lf); lsum += e.loss; z.gmu.y = e.gmu; z.dth.y = e.dth; z.dpi.y = e.dpi; }
+        lsum_lg += ((active && !nz0) ? z.lgD.x : 0.f) + ((active && !nz1) ? z.lgD.y : 0.f);
+        if (p.ridge != 0.f) {                                                              // loss.py:139-140
+          if (active) lsum += p.ridge * (pi.x * pi.x + pi.y * pi.y);
+          z.dpi = fma2(splat(2.0f * p.ridge), pi, z.dpi);
         }
-        const uint32_t hs = hi & 1, hp = (hi >> 1) & 1; ++hi;
-        mbar_wait(&h_empty[hs], hp ^ 1);
-        mbar_expect_tx(&h_full[hs], kHBytes);
-        tma_load_2d(s_h + hs * kHBytes, &map_h, 0, cb * 128, &h_full[hs]);
+        const float2 msk = splat(active ? 1.0f : 0.0f);        // rows / genes outside the matrix contribute exact zeros
+        const float2 gm = mul2(mul2(z.gmu, f.fm), msk), gd = mul2(mul2(z.dth, f.fd), msk), gp = mul2(mul2(z.dpi, f.fp), msk);
+        // SWIZZLE_128B operand layout: 16-byte chunk (8 genes) c ^ (row % 8) of the row's 128 bytes
+        const int row = wg * 64 + frow + 8 * h;
+        uint8_t* dst = s_z + row * 128 + ((c ^ (row & 7)) << 4) + fcol * 2;
+        *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(gm.x, gm.y);
+        *reinterpret_cast<uint32_t*>(dst + kZBox) = pack_bf16x2(gd.x, gd.y);
+        *reinterpret_cast<uint32_t*>(dst + 2 * kZBox) = pack_bf16x2(gp.x, gp.y);
       }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc_1 = make_idesc_bf16(128, 192, 0, 1);   // H K-major x [Wm|Wd|Wp] MN-major (genes contiguous)
-      constexpr uint32_t idesc_b = make_idesc_bf16(128, 64, 0, 0);    // dZ K-major x W K-major ([64 feats x genes])
-      constexpr uint32_t idesc_a = make_idesc_bf16(128, 64, 1, 1);    // dZ MN-major (2 heads stacked) x H MN-major
-      constexpr uint32_t idesc_c = make_idesc_bf16(128, 16, 1, 0);    // dZ MN-major x ones -> column sums
-      const uint32_t wb = smem_u32(s_w), ob = smem_u32(s_ones);
-      uint32_t hi = 0, ti = 0, seg = 0;
-      struct Pend { int valid; uint32_t hs, b, ph; int first, last; } pend = {0, 0, 0, 0, 0, 0};
-      auto mma23 = [&](const Pend& u) {
-        mbar_wait(&dz_full[u.b], u.ph);                                // the epilogue has written dZ of this tile
-        if (u.first) mbar_wait(&dw_empty, ((seg - 1) & 1) ^ 1);       // previous segment's dW has been flushed
-        tcgen05_fence_after();
-        const uint32_t zb = smem_u32(s_z + u.b * kZBytes), hb = smem_u32(s_h + u.hs * kHBytes);
-        const uint32_t tm = tmem + kTmD1 + u.b * kTmD1Stride;          // consumed pre-activation accumulator: reuse
+    fence_proxy_async_smem();
+    if (threadIdx.x == 0) bulk_wait_read<0>();                           // the previous dH3 reduce has read the staging tile
+    __syncthreads();
+
+    // ---- MMA2: dH3 rows 64*wg.. = sum_h dZ_h . W_h^T
+    {
+      float dh[32];
 #pragma unroll
-        for (int h = 0; h < 3; ++h)
+      for (int i = 0; i < 32; ++i) dh[i] = 0.f;
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16(tm + kTmDhOff, make_smem_desc(zb + h * kZBox + k * 32, 0, 1024),
-                      make_smem_desc(wb + h * kWBox + k * 32, 0, 1024), idesc_b, (h > 0 || k > 0) ? 1u : 0u);
-#pragma unroll
-        for (int a = 0; a < 2; ++a) {                                  // accumulator 0: heads (0,1); 1: heads (1,2)
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const uint64_t da = make_smem_desc(zb + a * kZBox + k * 2048, kZBox, 1024);
-            umma_bf16(tm + kTmCsOff + a * 16, da, make_smem_desc(ob + (k & 3) * 32, 0, 1024), idesc_c, k > 0 ? 1u : 0u);
-            umma_bf16(tmem + kTmDw + a * 64, da, make_smem_desc(hb + k * 2048, 0, 1024), idesc_a, (u.first && k == 0) ? 0u : 1u);
-          }
-        }
-        umma_commit(&dh_full[u.b]);
-        umma_commit(&dz_empty[u.b]);
-        umma_commit(&h_empty[u.hs]);
-        if (u.last) { umma_commit(&dw_full); umma_commit(&w_empty); }
-      };
-      for (int t = t0; t < t1; ++t, ++ti) {
-        const int cb = t % p.n_cb;
-        const bool new_seg = (t == t0 || cb == 0);
-        if (new_seg) {
-          if (pend.valid) { mma23(pend); pend.valid = 0; }             // drain before the weight tile changes
-          mbar_wait(&w_full, seg & 1); ++seg;
-        }
-        const uint32_t hs = hi & 1, hp = (hi >> 1) & 1; ++hi;
-        const uint32_t bb = ti & 1, ph = (ti >> 1) & 1;
-        mbar_wait(&h_full[hs], hp);
-        mbar_wait(&d1_empty[bb], ph ^ 1);                              // epilogue of tile ti-2 has read the accumulator
-        mbar_wait(&dh_empty[bb], ph ^ 1);                              // flush of tile ti-2 has read dH3 / column sums
-        tcgen05_fence_after();
-        const uint32_t hb = smem_u32(s_h + hs * kHBytes);
+      for (int h = 0; h < 3; ++h)
 #pragma unroll
         for (int k = 0; k < 4; ++k)
-          umma_bf16(tmem + kTmD1 + bb * kTmD1Stride, make_smem_desc(hb + k * 32, 0, 1024), make_smem_desc(wb + k * 2048, kWBox, 1024), idesc_1, k > 0);
-        umma_commit(&d1_full[bb]);
-        if (pend.valid) mma23(pend);
-        pend.valid = 1; pend.hs = hs; pend.b = bb; pend.ph = ph; pend.first = new_seg;
-        pend.last = (t + 1 == t1) || ((t + 1) % p.n_cb == 0);
+          wgmma_m64n64k16<0, 0>(dh, make_smem_desc(zb + h * kZBox + wg * 64 * 128 + k * 32, 0, 1024),
+                                make_smem_desc(wb + h * kWBox + k * 32, 0, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(dh);
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int row = wg * 64 + frow + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + fcol;
+        *reinterpret_cast<float2*>(s_o + row * 64 + col) = make_float2(dh[i], dh[i + 1]);
       }
-      if (pend.valid) mma23(pend);
     }
-  } else if (warp == 3) {
-    // ===================================================== L2 prefetch of the count rows, two tiles ahead of the epilogue
-    // (the epilogue threads read their own row segments straight from global memory; this turns their DRAM
-    // latency into L2 latency without spending shared memory on a staging tile)
-    auto prefetch_tile = [&](int tt) {
-      const int gt = tt / p.n_cb, cb = tt % p.n_cb;
-      const int g0 = gt * 64;
-      const uint32_t bytes = (uint32_t)min(64, p.G - g0) * 4u;
-      for (int r = lane; r < 128; r += 32) {
-        const int grow = cb * 128 + r;
-        if (grow < p.B) {
-          const int yr = p.rows ? p.rows[grow] : grow;
-          bulk_prefetch_l2(p.Y + (int64_t)yr * p.ldy + g0, bytes);
-        }
-      }
-    };
-    prefetch_tile(t0);
-    if (t0 + 1 < t1) prefetch_tile(t0 + 1);
-    uint32_t ti = 0;
-    for (int t = t0; t < t1; ++t, ++ti) {
-      if (t + 2 < t1) prefetch_tile(t + 2);
-      mbar_wait_backoff(&dz_full[ti & 1], (ti >> 1) & 1, 500);   // pace: the epilogue has finished tile t
-    }
-  } else if (warp >= kEpiWarp0 && warp < kEpiWarp0 + kEpiWarps) {
-    // ===================================================== loss epilogue
-    using Ops = zmath::FastOps;
-    constexpr unsigned kFull = 0xffffffffu;
-    const int ew = warp - kEpiWarp0, quarter = warp & 3, cg = ew >> 2;
-    float4* q = reinterpret_cast<float4*>(s_q + ew * kQueueBytes);
-    const unsigned lt = (1u << lane) - 1u;
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(quarter * 32) << 16;
-    float lsum = 0.f, lsum_lg = 0.f;            // NLL of the NB items I evaluated (+ ridge) | sum of lg2(D) over my zero counts
-    uint32_t ti = 0;
-    for (int t = t0; t < t1; ++t, ++ti) {
-      const int gt = t / p.n_cb, cb = t % p.n_cb;
-      const int grow = cb * 128 + row;
-      const bool valid_row = grow < p.B;
-      int yr = 0; float sfv = 1.0f;
-      if (valid_row) { yr = p.rows ? p.rows[grow] : grow; sfv = p.sf ? p.sf[yr] : 1.0f; }
-      const float* yrow = p.Y + (int64_t)yr * p.ldy;
-      const uint32_t zbuf = ti & 1, zph = (ti >> 1) & 1;
-      uint8_t* zrow = s_z + zbuf * kZBytes + row * 128;
-      mbar_wait_backoff(&d1_full[zbuf], zph, 64);
-      tcgen05_fence_after();
+    // ---- MMA3: dW_h^T [64 genes x 64 feats] and column sums, cells 64*wg.. of the tile
 #pragma unroll 1
-      for (int half = 0; half < 2; ++half) {
-        // ---- operands of 8 genes x 3 heads: counts and biases from global/L2, pre-activations from TMEM
-        const int gh = gt * 64 + cg * 16 + half * 8;
-        const bool cols_in = gh < p.G;                          // G % 8 == 0: the 8 genes are all in or all out
-        const bool active = valid_row && cols_in;
-        float y[8], bm[8], bd[8], bp[8];
+    for (int h = 0; h < 3; ++h) {
+      float dw[32], cs[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { y[j] = 0.f; bm[j] = bd[j] = bp[j] = 0.f; }
-        if (active) {
-          const float4 a = *reinterpret_cast<const float4*>(yrow + gh), b = *reinterpret_cast<const float4*>(yrow + gh + 4);
-          y[0] = a.x; y[1] = a.y; y[2] = a.z; y[3] = a.w; y[4] = b.x; y[5] = b.y; y[6] = b.z; y[7] = b.w;
-        }
-        if (cols_in) {
+      for (int i = 0; i < 32; ++i) dw[i] = 0.f;
 #pragma unroll
-          for (int v = 0; v < 2; ++v) {
-            const float4 a = *reinterpret_cast<const float4*>(p.bias[0] + gh + 4 * v);
-            const float4 b = *reinterpret_cast<const float4*>(p.bias[1] + gh + 4 * v);
-            const float4 c = *reinterpret_cast<const float4*>(p.bias[2] + gh + 4 * v);
-            bm[4 * v] = a.x; bm[4 * v + 1] = a.y; bm[4 * v + 2] = a.z; bm[4 * v + 3] = a.w;
-            bd[4 * v] = b.x; bd[4 * v + 1] = b.y; bd[4 * v + 2] = b.z; bd[4 * v + 3] = b.w;
-            bp[4 * v] = c.x; bp[4 * v + 1] = c.y; bp[4 * v + 2] = c.z; bp[4 * v + 3] = c.w;
-          }
-        }
-        uint32_t zm[8], zd[8], zp[8];
-        const uint32_t tcol = tmem + kTmD1 + zbuf * kTmD1Stride + lane_off + (uint32_t)(cg * 16 + half * 8);
-        tmem_ld_32x8(tcol, zm); tmem_ld_32x8(tcol + 64, zd); tmem_ld_32x8(tcol + 128, zp);
-        tmem_ld_wait();
-        if (half == 1) {                                      // accumulator fully read: release it to the MMA warp
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&d1_empty[zbuf]);
-        }
-        float mm[8], dd[8], pp[8];
+      for (int i = 0; i < 8; ++i) cs[i] = 0.f;
+      wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {                           // 24 independent activation chains
-          mm[j] = act_mean(__uint_as_float(zm[j]) + bm[j]);
-          dd[j] = act_disp(__uint_as_float(zd[j]) + bd[j]);
-          pp[j] = act_sigmoid(__uint_as_float(zp[j]) + bp[j]);
-        }
-        if (half == 0) mbar_wait_backoff(&dz_empty[zbuf], zph ^ 1, 64);   // the MMAs that read this dZ buffer two tiles ago are done
-        // SWIZZLE_128B: 16-byte chunk (8 genes) ^ (row % 8); each pass over 4 genes fills one 8-byte half of it
-        uint8_t* zdst = zrow + (uint32_t)(((cg * 2 + half) ^ (row & 7)) << 4);
-#pragma unroll 1
-        for (int sub = 0; sub < 2; ++sub) {
-          float ys[4], ms[4], ds[4], ps[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            ys[j] = sub ? y[4 + j] : y[j]; ms[j] = sub ? mm[4 + j] : mm[j]; ds[j] = sub ? dd[4 + j] : dd[j]; ps[j] = sub ? pp[4 + j] : pp[j];
-          }
-          // ---- queue the non-zero counts of this warp's 32 rows x 4 genes (ballot compaction: ordered by j, lane)
-          using namespace zmath;
-          const float2 mA = make_float2(ms[0], ms[1]), mB = make_float2(ms[2], ms[3]);
-          const float2 dA = make_float2(ds[0], ds[1]), dB = make_float2(ds[2], ds[3]);
-          const float2 pA = make_float2(ps[0], ps[1]), pB = make_float2(ps[2], ps[3]);
-          const float2 muA = mul2(mA, splat(sfv)), muB = mul2(mB, splat(sfv));               // dca/layers.py:85
-          const float mu[4] = {muA.x, muA.y, muB.x, muB.y};
-          bool isnz[4];
-          int pos[4], base = 0;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            isnz[j] = active && !(ys[j] < 1e-8f);                       // loss.py:138
-            const unsigned bal = __ballot_sync(kFull, isnz[j]);
-            pos[j] = base + __popc(bal & lt); base += __popc(bal);
-          }
-          const int total = base;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (isnz[j]) q[pos[j]] = make_float4(ys[j], mu[j], ds[j], ps[j]);
-          __syncwarp();
-          // ---- zero branch of all four elements as two f32x2 chains (zinb_math.cuh), finishing factors shared with the
-          // queued NB items, which come back as raw derivatives
-          Raw2 zA = zinb_zero_pair<Ops>(muA, dA, pA), zB = zinb_zero_pair<Ops>(muB, dB, pB);
-          const Fin2 fA = finish_factors_pair<Ops, true>(mA, dA, pA, p.inv_n), fB = finish_factors_pair<Ops, true>(mB, dB, pB, p.inv_n);
-          lsum_lg += ((active && !isnz[0]) ? zA.lgD.x : 0.f) + ((active && !isnz[1]) ? zA.lgD.y : 0.f)
-                   + ((active && !isnz[2]) ? zB.lgD.x : 0.f) + ((active && !isnz[3]) ? zB.lgD.y : 0.f);
-          for (int k = lane; k < total; k += 32) { const float4 e = nb_item(q[k], lf); lsum += e.w; q[k] = e; }
-          __syncwarp();
-          if (isnz[0]) { const float4 e = q[pos[0]]; zA.gmu.x = e.x; zA.dth.x = e.y; zA.dpi.x = e.z; }
-          if (isnz[1]) { const float4 e = q[pos[1]]; zA.gmu.y = e.x; zA.dth.y = e.y; zA.dpi.y = e.z; }
-          if (isnz[2]) { const float4 e = q[pos[2]]; zB.gmu.x = e.x; zB.dth.x = e.y; zB.dpi.x = e.z; }
-          if (isnz[3]) { const float4 e = q[pos[3]]; zB.gmu.y = e.x; zB.dth.y = e.y; zB.dpi.y = e.z; }
-          __syncwarp();
-          if (p.ridge != 0.f) {                                         // loss.py:139-140 (uniform; ridge defaults to 0)
-            if (active) lsum += p.ridge * (pA.x * pA.x + pA.y * pA.y + pB.x * pB.x + pB.y * pB.y);
-            zA.dpi = fma2(splat(2.0f * p.ridge), pA, zA.dpi); zB.dpi = fma2(splat(2.0f * p.ridge), pB, zB.dpi);
-          }
-          const float2 msk = splat(active ? 1.0f : 0.0f);              // rows / genes outside the matrix contribute exact zeros
-          const float2 gmA = mul2(mul2(zA.gmu, fA.fm), msk), gmB = mul2(mul2(zB.gmu, fB.fm), msk);
-          const float2 gdA = mul2(mul2(zA.dth, fA.fd), msk), gdB = mul2(mul2(zB.dth, fB.fd), msk);
-          const float2 gpA = mul2(mul2(zA.dpi, fA.fp), msk), gpB = mul2(mul2(zB.dpi, fB.fp), msk);
-          uint8_t* zd8 = zdst + sub * 8;
-          *reinterpret_cast<uint2*>(zd8) = make_uint2(pack_bf16x2(gmA.x, gmA.y), pack_bf16x2(gmB.x, gmB.y));
-          *reinterpret_cast<uint2*>(zd8 + kZBox) = make_uint2(pack_bf16x2(gdA.x, gdA.y), pack_bf16x2(gdB.x, gdB.y));
-          *reinterpret_cast<uint2*>(zd8 + 2 * kZBox) = make_uint2(pack_bf16x2(gpA.x, gpA.y), pack_bf16x2(gpB.x, gpB.y));
-        }
+      for (int k = 0; k < 4; ++k) {
+        const int kk = wg * 4 + k;
+        const uint64_t da = make_smem_desc(zb + h * kZBox + kk * 2048, 0, 1024);
+        wgmma_m64n64k16<1, 1>(dw, da, make_smem_desc(hb + kk * 2048, 0, 1024), 1u);
+        wgmma_m64n16k16<1, 0>(cs, da, make_smem_desc(ob + k * 32, 0, 1024), 1u);
       }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&dz_full[zbuf]);
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(dw); acc_fence(cs);
+      float* acc = s_dw + h * 4096;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int gl = frow + 8 * ((i >> 1) & 1), f = 8 * (i >> 2) + fcol + (i & 1);
+        atomicAdd(acc + f * 64 + gl, dw[i]);
+      }
+      if ((l & 3) == 0) { atomicAdd(s_db + h * 64 + frow, cs[0]); atomicAdd(s_db + h * 64 + frow + 8, cs[2]); }
     }
-    // ---- loss: CTA partial, the last CTA folds all partials in a fixed order and finalises (as in zinb_loss.cu)
-    double dsum = (double)lsum - (double)zmath::kLn2 * (double)lsum_lg;        // -log D = -ln2 * lg2 D
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) dsum += __shfl_xor_sync(kFull, dsum, o);
-    if (lane == 0) red[ew] = dsum;
-    named_barrier_sync(2, kEpiWarps * 32);
-    if (ew == 0 && lane == 0) {
-      double tsum = 0.0;
-#pragma unroll
-      for (int w = 0; w < kEpiWarps; ++w) tsum += red[w];
-      p.loss_partial[blockIdx.x] = tsum;
-      __threadfence();
-      const unsigned done = atomicAdd(p.counter, 1u);
-      s_last = (done == gridDim.x - 1);
-      if (s_last) *p.counter = 0;                                       // self-resetting
+    fence_proxy_async_smem();
+    __syncthreads();                                   // dZ, H and W buffers free; staging tile and accumulators complete
+    if (threadIdx.x == 0) { tma_reduce_add_2d(&map_o, 0, cb * 128, s_o); bulk_commit(); }
+    const bool last = (t + 1 == t1) || ((t + 1) % p.n_cb == 0);
+    if (last) {                                        // end of the segment: dW / db of this gene tile -> gradient buffer
+      for (int idx = threadIdx.x; idx < (int)kDwFloats; idx += kThreads) {
+        const int h = idx >> 12, f = (idx >> 6) & 63, g = gt * 64 + (idx & 63);
+        if (g < p.G) atomicAdd(p.dW[h] + (int64_t)f * p.dW_ld + g, s_dw[idx]);
+        s_dw[idx] = 0.f;
+      }
+      for (int idx = threadIdx.x; idx < 3 * 64; idx += kThreads) {
+        const int h = idx >> 6, g = gt * 64 + (idx & 63);
+        if (g < p.G) atomicAdd(p.db[h] + g, s_db[idx]);
+        s_db[idx] = 0.f;
+      }
+      __syncthreads();
     }
-    named_barrier_sync(2, kEpiWarps * 32);
-    if (s_last && ew == 0) {
-      __threadfence();
-      double a = 0.0;
-      for (int i = lane; i < (int)gridDim.x; i += 32) a += __ldcg(p.loss_partial + i);
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(kFull, a, o);
-      if (lane == 0) {
-        *p.loss_sum = a;
-        if (p.loss_slot) {
-          double l = a * (double)p.inv_n;
-          if (l != l) l = INFINITY;                                     // _nan2inf, dca/loss.py:148
-          if (p.penalty) l += *p.penalty;
-          const float lf32 = (float)l;
-          p.loss_slot[0] = lf32;
-          p.loss_slot[1] = (isfinite(lf32)) ? 0.f : 1.f;
-          if (p.epoch_acc) { p.epoch_acc[0] += l * (double)p.batch; p.epoch_acc[1] += (double)p.batch; }
-        }
-      }
-    }
-  } else if (warp >= kFlushWarp0) {
-    // ===================================================== flush: dH3 per tile, dW / db per segment
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(quarter * 32) << 16;
-    uint32_t ti = 0, seg = 0;
-    for (int t = t0; t < t1; ++t, ++ti) {
-      const int gt = t / p.n_cb, cb = t % p.n_cb;
-      const uint32_t bb = ti & 1, ph = (ti >> 1) & 1;
-      const uint32_t tm = tmem + kTmD1 + bb * kTmD1Stride + lane_off;
-      const int g = gt * 64 + (row & 63);
-      mbar_wait_backoff(&dh_full[bb], ph, 256);
-      tcgen05_fence_after();
-      if (warp == kFlushWarp0 && lane == 0) bulk_wait_read<0>();        // previous reduce has read the staging tiles
-      named_barrier_sync(3, kFlushWarps * 32);
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tm + kTmDhOff + c * 32, v);
-        tmem_ld_wait();
-        uint8_t* tile = s_o + c * (kOutBytes / 2);
-#pragma unroll
-        for (int qq = 0; qq < 8; ++qq)
-          *reinterpret_cast<uint4*>(tile + row * 128 + ((qq ^ (row & 7)) << 4)) = make_uint4(v[qq * 4], v[qq * 4 + 1], v[qq * 4 + 2], v[qq * 4 + 3]);
-      }
-      {
-        // bias gradient of this tile: column sums of dZ.  accumulator 0: lanes 0-63 = head 0, 64-127 = head 1;
-        // accumulator 1: lanes 64-127 = head 2 (lanes 0-63 duplicate head 1)
-        uint32_t cs[32];
-        tmem_ld_32x32(tm + kTmCsOff, cs);
-        tmem_ld_wait();
-        if (g < p.G) {
-          atomicAdd(p.db[row >> 6] + g, __uint_as_float(cs[0]));
-          if (row >= 64) atomicAdd(p.db[2] + g, __uint_as_float(cs[16]));
-        }
-      }
-      tcgen05_fence_before();
-      fence_proxy_async_smem();
-      named_barrier_sync(3, kFlushWarps * 32);
-      if (lane == 0) mbar_arrive(&dh_empty[bb]);
-      if (warp == kFlushWarp0 && lane == 0) {
-        tma_reduce_add_2d(&map_o, 0, cb * 128, s_o);
-        tma_reduce_add_2d(&map_o, 32, cb * 128, s_o + kOutBytes / 2);
-        bulk_commit();
-      }
-      const bool last = (t + 1 == t1) || ((t + 1) % p.n_cb == 0);
-      if (last) {
-        mbar_wait_backoff(&dw_full, seg & 1, 64); ++seg;
-        tcgen05_fence_after();
-#pragma unroll
-        for (int a = 0; a < 2; ++a) {
-          const int head = a == 0 ? (row >> 6) : 2;
-          const bool mine = (a == 0 || row >= 64) && g < p.G;
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t v[32];
-            tmem_ld_32x32(tmem + kTmDw + lane_off + a * 64 + c * 32, v);
-            tmem_ld_wait();
-            if (mine) {
-              float* dst = p.dW[head];
-#pragma unroll
-              for (int j = 0; j < 32; ++j) atomicAdd(dst + (int64_t)(c * 32 + j) * p.dW_ld + g, __uint_as_float(v[j]));
-            }
-          }
-        }
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&dw_empty);
-      }
-    }
-    if (warp == kFlushWarp0 && lane == 0) bulk_wait<0>();
   }
-  tcgen05_fence_before();
+  if (threadIdx.x == 0) bulk_wait<0>();
+
+  // ---- loss: CTA partial, the last CTA folds all partials in a fixed order and finalises (as in zinb_loss.cu)
+  constexpr unsigned kFull = 0xffffffffu;
+  double dsum = (double)lsum - (double)zmath::kLn2 * (double)lsum_lg;        // -log D = -ln2 * lg2 D
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) dsum += __shfl_xor_sync(kFull, dsum, o);
+  if (l == 0) red[threadIdx.x >> 5] = dsum;
   __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem, kTmemCols);
+  if (threadIdx.x == 0) {
+    double tsum = 0.0;
+#pragma unroll
+    for (int i = 0; i < kThreads / 32; ++i) tsum += red[i];
+    p.loss_partial[blockIdx.x] = tsum;
+    __threadfence();
+    const unsigned done = atomicAdd(p.counter, 1u);
+    s_last = (done == gridDim.x - 1);
+    if (s_last) *p.counter = 0;                                       // self-resetting
+  }
+  __syncthreads();
+  if (s_last && threadIdx.x < 32) {
+    __threadfence();
+    double a = 0.0;
+    for (int i = l; i < (int)gridDim.x; i += 32) a += __ldcg(p.loss_partial + i);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(kFull, a, o);
+    if (l == 0) {
+      *p.loss_sum = a;
+      if (p.loss_slot) {
+        double lv = a * (double)p.inv_n;
+        if (lv != lv) lv = INFINITY;                                  // _nan2inf, dca/loss.py:148
+        if (p.penalty) lv += *p.penalty;
+        const float lf32 = (float)lv;
+        p.loss_slot[0] = lf32;
+        p.loss_slot[1] = (isfinite(lf32)) ? 0.f : 1.f;
+        if (p.epoch_acc) { p.epoch_acc[0] += lv * (double)p.batch; p.epoch_acc[1] += (double)p.batch; }
+      }
+    }
+  }
 }
 
 }  // namespace fz
@@ -467,7 +317,7 @@ int flash_zinb_tc(const __nv_bfloat16* H3, int B, int G, const __nv_bfloat16* co
   CUtensorMap mh, mw[3], mo;
   DCA_TRY(make_tensor_map_2d(&mh, H3, 2, 1, (uint64_t)B, 64, 64, 128, 64, 1));
   for (int i = 0; i < 3; ++i) DCA_TRY(make_tensor_map_2d(&mw[i], W[i], 2, 1, 64, (uint64_t)G, (uint64_t)G, 64, 64, 1));
-  DCA_TRY(make_tensor_map_2d(&mo, dH3, 4, 0, (uint64_t)B, 64, 64, 128, 32, 1));
+  DCA_TRY(make_tensor_map_2d(&mo, dH3, 4, 0, (uint64_t)B, 64, 64, 128, 64, 0));
   Params p{};
   p.B = B; p.G = G; p.n_cb = cdiv(B, 128); p.n_gt = cdiv(G, 64); p.total_tiles = p.n_cb * p.n_gt;
   p.Y = Y; p.ldy = ldy; p.rows = rows; p.sf = sf;

@@ -1,42 +1,48 @@
-// One tcgen05 kernel for the three gene-wide Dense products whose reduction or output dimension is
-// the gene axis (all with a 64-wide partner dimension):
+// One wgmma kernel for the gene-wide Dense products whose reduction or output dimension is the gene axis (all with a
+// 64-wide partner dimension):
 //
-//   encoder forward  (K1)  A1[B x 64]  += X[B x G] . W1[G x 64]                      DO_B
-//   head backward    (K4)  dWh[64 x G] += H3^T . dZ,  dH3[B x 64] += dZ . Wh^T,  db = colsum(dZ)   DO_A + DO_B + COLSUM
-//   encoder backward (K5)  dW1[G x 64] += X^T . dA1                                   DO_A
+//   encoder forward  (K1)  A1[B x 64]  += X[B x G] . W1[G x 64]                      (b), W MN-major
+//   head backward    (K4)  dH3[B x 64] += sum_h dZ_h . Wh^T                          (b), W K-major
+//                          dWh[64 x G] += H3^T . dZ_h,  db_h += colsum(dZ_h)         (a) + column sums
+//   encoder backward (K5)  dW1[G x 64] += X^T . dA1                                   (a)
 //
-// "Z" is the cells x genes bf16 operand (X or dZ).  A 128-cell x 128-gene tile of Z is brought into
-// shared memory ONCE by TMA (two SWIZZLE_128B boxes of 64 genes) and feeds both products:
-//   (b) as a K-major  A operand (M = 128 cells, K = genes) against W  [64 x genes]  (K-major B), and
-//   (a) as an MN-major A operand (M = 128 genes, K = cells) against H [cells x 64] (MN-major B),
-// i.e. the same bytes with two different UMMA descriptors, so Z is read from HBM once per step for
-// both gradients (SURVEY.md 7.2 K4).  Accumulators live in TMEM: one 128x64 fp32 tile per gene block
-// of the item for (a), a double-buffered 128x64 tile per cell block for (b).  (b) leaves through a
-// swizzled staging tile and a TMA reduce-add (split over gene ranges); (a) is added to the gradient
-// buffer by the epilogue warps at the end of the item; the per-gene column sums (bias gradient) are one
-// more tcgen05 product of the same tile with a constant ones operand (Z^T . 1, N = 16).
+// "Z" is the cells x genes bf16 operand (X or dZ), brought into shared memory by TMA as 128-cell x 128-gene tiles
+// (two SWIZZLE_128B boxes of 64 genes).  (b) reads a tile as a K-major A operand (M = 64 cells per warpgroup,
+// K = genes), (a) as an MN-major A operand (M = 64 genes per warpgroup, K = cells) against H [cells x 64].  A CTA owns
+// one item = (head, range of gene blocks, range of cell blocks) and keeps its fp32 accumulators in registers.
 //
-// Warp roles (256 threads): 0 TMA producer, 1 MMA issuer, 2 TMEM allocator, 4-7 epilogue.
-#include <cstdio>
-#include <vector>
+// Every output element is summed in a fixed order, so a step computes the same bits on every run:
+//   (a) items span ALL cells of their gene blocks: one CTA owns each dW / db element and adds it once (TMA reduce-add
+//       of a staging tile, one atomic per db element);
+//   (b) items span one cell block and a gene range; each writes its partial [128 x 64] into its own slot of a
+//       workspace, and gene_gemm_reduce_kernel adds the slots to the output in slot order.
+//
+// 256 threads = two warpgroups; thread 0 also issues the TMA loads, kStages - 1 tiles ahead.
 #include "engine.h"
 #include "tc_common.cuh"
 
 namespace dca {
 namespace tc {
-int g_gg_prefetch = 0;      // dca_set_tunable("gg_prefetch", 0 | 1)
-int g_gg_profile = 0;       // dca_set_tunable("gg_profile", 1): per-role wait-time counters, printed after every launch (diagnosis; DCA_GRAPH=0)
-int g_gg_flat = 1;          // dca_set_tunable("gg_flat", 0 | 1): flat unit partition of the backward kernels (every SM busy)
+int g_gg_profile = 0;       // dca_set_tunable("gg_profile", 1): phase timeline of the hidden-stack kernels (mid_stack.cu)
 namespace gg {
 
 constexpr int kThreads = 256;
-constexpr int kZStages = 3;
 constexpr uint32_t kZBytes = 128 * 128 * 2;          // 2 boxes x [128 cells x 64 genes] bf16
-constexpr uint32_t kWBytes = 64 * 128 * 2;           // 2 boxes x [64 feats x 64 genes] bf16
+constexpr uint32_t kWBytes = 64 * 128 * 2;           // 2 boxes x [64 feats x 64 genes] | 1 box [128 genes x 64 feats] bf16
 constexpr uint32_t kHBytes = 128 * 64 * 2;           // [128 cells x 64 feats] bf16
-constexpr uint32_t kOutBytes = 2 * 128 * 32 * 4;     // two [128 x 32] fp32 staging tiles
-constexpr int kMaxGb = 4;                            // gene blocks (of 128) per item: 4 x 64 TMEM columns
-constexpr uint32_t kTmemCols = 512;
+constexpr uint32_t kOutBytes = 128 * 64 * 4;         // fp32 staging tile of one flush
+constexpr uint32_t kOnesBytes = 16 * 128;            // [16 x 64] bf16 ones, K-major B operand of the column sums
+constexpr int kMaxGb = 4;                            // (a): gene blocks per item held in registers
+constexpr int kMaxSlots = 16;                        // (b): partial slots (heads x gene ranges)
+
+template <bool DO_A, bool DO_B>
+constexpr int stages() { return DO_A && DO_B ? 2 : 3; }
+template <bool DO_A, bool DO_B>
+constexpr uint32_t stage_bytes() { return kZBytes + (DO_B ? kWBytes : 0) + (DO_A ? kHBytes : 0); }
+template <bool DO_A, bool DO_B, bool COLSUM>
+constexpr uint32_t smem_bytes() {
+  return stages<DO_A, DO_B>() * stage_bytes<DO_A, DO_B>() + (DO_A ? kOutBytes : 0) + (COLSUM ? kOnesBytes : 0) + 1024;
+}
 
 struct Params {
   int B, G, n_heads;
@@ -44,458 +50,292 @@ struct Params {
   int gb_per_item, cb_per_item;
   int gene_ranges, cell_splits;   // per head
   int total_items;
-  unsigned long long* dbg;        // gg_profile: [grid][16] cycle counters (nullptr = off)
-  int flat, total_units;          // flat: units = (head, gene range, cell block) in that order, an equal contiguous run per CTA
-  float* dW[3]; int64_t dW_ld; int dW_transposed;   // (a): transposed -> dW[f*ld + g] (Keras [64 x G]); else dW[g*ld + f]
-  float* db[3];                                     // column sums of Z per head (COLSUM)
-  const __nv_bfloat16* Zp[3]; int64_t ldz; int prefetch;   // raw Z pointers: L2 prefetch of whole row segments ahead of the TMA boxes
+  float* db[3];                   // column sums of Z per head (COLSUM)
+  float* part; int64_t part_stride;   // (b): partial slot (head * gene_ranges + gene range) of part_stride floats
 };
 
-__device__ __forceinline__ void gg_prefetch_l2(const void* gptr, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(gptr)), "r"(bytes) : "memory");
-}
-
-// diagnosis: accumulate the cycles a single-thread role spends inside one wait / section into its counter slot
-#define GG_TIMED(slot, stmt)                                             \
-  do {                                                                   \
-    if (p.dbg) { const long long t0_ = clock64(); stmt; dbg_acc[slot] += (unsigned long long)(clock64() - t0_); } \
-    else { stmt; }                                                       \
-  } while (0)
-
-template <bool DO_A, bool DO_B, bool COLSUM>
+// MAXG: gene blocks per item held in registers (the (a) accumulators); WK: W is K-major (Keras [64 x G] head kernel)
+template <bool DO_A, bool DO_B, bool COLSUM, bool WK, int MAXG>
 __global__ void __launch_bounds__(kThreads, 1)
 gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_constant__ CUtensorMap map_z1,
                  const __grid_constant__ CUtensorMap map_z2, const __grid_constant__ CUtensorMap map_h,
                  const __grid_constant__ CUtensorMap map_w0, const __grid_constant__ CUtensorMap map_w1,
-                 const __grid_constant__ CUtensorMap map_w2, const __grid_constant__ CUtensorMap map_o, const Params p) {
+                 const __grid_constant__ CUtensorMap map_w2, const __grid_constant__ CUtensorMap map_dw0, const __grid_constant__ CUtensorMap map_dw1,
+                 const __grid_constant__ CUtensorMap map_dw2, const int dw_transposed, const Params p) {
+  constexpr int kStages = stages<DO_A, DO_B>();
+  constexpr uint32_t kStage = stage_bytes<DO_A, DO_B>();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // 1024-byte alignment by OFFSET (not by an integer round trip): the pointer keeps the shared address space, so the
-  // staging stores / bias loads compile to STS / LDS instead of generic ST / LD
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  constexpr uint32_t kStage = kZBytes + (DO_B ? kWBytes : 0);
-  uint8_t* s_z = smem;                                          // [kZStages][Z | W]
-  uint8_t* s_h = s_z + kZStages * kStage;                       // [2][H]
-  uint8_t* s_o = s_h + (DO_A ? 2 * kHBytes : 0);                // staging for (b)
-  // COLSUM: a [128 cells x 64] bf16 tile of ones in H's layout -- the second N chunk of the dW product's B operand (N = 64 + 16):
-  // the 16 extra accumulator columns are the column sums of Z (every element equal, so the swizzle pattern does not matter)
-  uint8_t* s_ones = s_o + ((DO_B || (DO_A && !DO_B)) ? kOutBytes : 0);
-  __shared__ uint64_t z_full[kZStages], z_empty[kZStages], h_full[2], h_empty[2], dh_full[2], dh_empty[2], dw_full, dw_empty;
-  __shared__ uint32_t tmem_base_s;
-  __shared__ int s_unit;
+  uint8_t* s_st = smem;                                                  // [kStages][Z | W | H]
+  float* s_o = reinterpret_cast<float*>(s_st + kStages * kStage);         // (a) flush staging
+  uint8_t* s_ones = reinterpret_cast<uint8_t*>(s_o) + (DO_A ? kOutBytes : 0);
+  __shared__ uint64_t full[kStages];
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    s_unit = -1;
-    for (int i = 0; i < kZStages; ++i) { mbar_init(&z_full[i], 1); mbar_init(&z_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&h_full[i], 1); mbar_init(&h_empty[i], 1); mbar_init(&dh_full[i], 1); mbar_init(&dh_empty[i], 4); }
-    mbar_init(&dw_full, 1); mbar_init(&dw_empty, 4);
+    for (int i = 0; i < kStages; ++i) mbar_init(&full[i], 1);
     fence_barrier_init();
-    tma_prefetch_desc(&map_z0); tma_prefetch_desc(&map_h); tma_prefetch_desc(&map_w0); tma_prefetch_desc(&map_o);
   }
-  if (warp == 2) tmem_alloc(&tmem_base_s, kTmemCols);
   if (COLSUM) {   // bf16 1.0 = 0x3F80
-    for (int i = threadIdx.x; i < (int)kHBytes / 4; i += kThreads) reinterpret_cast<uint32_t*>(s_ones)[i] = 0x3F803F80u;
+    for (int i = threadIdx.x; i < (int)kOnesBytes / 4; i += kThreads) reinterpret_cast<uint32_t*>(s_ones)[i] = 0x3F803F80u;
     fence_proxy_async_smem();
   }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = tmem_base_s;
-  constexpr uint32_t kDwCols = COLSUM ? 80 : 64;   // per gene block: 64 dW columns (+ 16 column-sum columns)
-  const uint32_t tm_dw = tmem;                 // kMaxGb x kDwCols columns
-  const uint32_t tm_dh = tmem + kMaxGb * kDwCols;   // 2 x 64 columns
 
-  struct Item { int head, gb0, gb1, cb0, cb1; };
-  auto decode = [&](int it) {
-    Item x;
-    const int cs = it % p.cell_splits; const int r = it / p.cell_splits;
-    const int gr = r % p.gene_ranges; x.head = r / p.gene_ranges;
-    x.gb0 = gr * p.gb_per_item; x.gb1 = min(p.n_gb, x.gb0 + p.gb_per_item);
-    x.cb0 = cs * p.cb_per_item; x.cb1 = min(p.n_cb, x.cb0 + p.cb_per_item);
-    return x;
+  const int wg = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+  const int frow = 16 * w + (l >> 2), fcol = 2 * (l & 3);           // fragment origin (see tc_common.cuh)
+
+  // staging tile -> global (+=) by TMA; the previous reduce must have read the tile before it is rewritten
+  auto stage_begin = [&]() {
+    if (threadIdx.x == 0) bulk_wait_read<0>();
+    __syncthreads();
   };
-  // Item sequence of this CTA.  Strided: items blockIdx.x, +gridDim.x, ...  Flat: the CTA owns units [u0, u1) of the
-  // (head, gene range, cell block) order; an item is the part of ONE gene range inside that run, so that a CTA switches
-  // dW accumulators (and flushes them) at most (run length / n_cb) + 1 times and every SM gets the same number of tiles.
-  struct Cursor { int u, u1; };
-  auto first = [&]() {
-    Cursor c;
-    if (p.flat) { c.u = (int)((long long)blockIdx.x * p.total_units / gridDim.x); c.u1 = (int)((long long)(blockIdx.x + 1) * p.total_units / gridDim.x); }
-    else { c.u = blockIdx.x; c.u1 = p.total_items; }
-    return c;
-  };
-  auto next = [&](Cursor& c, Item& x) {
-    if (c.u >= c.u1) return false;
-    if (!p.flat) { x = decode(c.u); c.u += gridDim.x; return true; }
-    const int r = c.u / p.n_cb, cb0 = c.u % p.n_cb, n = min(p.n_cb - cb0, c.u1 - c.u);
-    const int gr = r % p.gene_ranges; x.head = r / p.gene_ranges;
-    x.gb0 = gr * p.gb_per_item; x.gb1 = min(p.n_gb, x.gb0 + p.gb_per_item);
-    x.cb0 = cb0; x.cb1 = cb0 + n; c.u += n;
-    return true;
+  auto stage_end = [&](const CUtensorMap* m, int c0, int c1) {
+    fence_proxy_async_smem();
+    __syncthreads();
+    if (threadIdx.x == 0) { tma_reduce_add_2d(m, c0, c1, s_o); bulk_commit(); }
   };
 
-  if (warp == 0) {
-    // ===================================================== TMA producer (whole warp walks the loops, one elected lane issues)
-    const bool leader = elect_one();
-    {
-      unsigned long long dbg_acc[4] = {0, 0, 0, 0};          // 0 wait z_empty, 1 wait h_empty, 2 total
-      const long long t_begin = clock64();
-      uint32_t zi = 0, hi = 0;
-      int unit = 0;
-      Cursor cur = first(); Item x;
-      while (next(cur, x)) {
-        const CUtensorMap* mz = x.head == 0 ? &map_z0 : (x.head == 1 ? &map_z1 : &map_z2);
-        for (int cb = x.cb0; cb < x.cb1; ++cb) {
-          if (DO_A) {
-            const uint32_t hs = hi & 1, hp = (hi >> 1) & 1; ++hi;
-            GG_TIMED(1, mbar_wait(&h_empty[hs], hp ^ 1));
-            if (leader) { mbar_expect_tx(&h_full[hs], kHBytes); tma_load_2d(s_h + hs * kHBytes, &map_h, 0, cb * 128, &h_full[hs]); }
-          }
-          for (int gb = x.gb0; gb < x.gb1; ++gb) {
-            if (((gb - x.gb0) & 3) == 0) { if (leader) *reinterpret_cast<volatile int*>(&s_unit) = unit; ++unit; }      // progress mark for the prefetch warp
-            const uint32_t st = zi % kZStages, ph = (zi / kZStages) & 1; ++zi;
-            GG_TIMED(0, mbar_wait(&z_empty[st], ph ^ 1));
-            uint8_t* dst = s_z + st * kStage;
-            if (leader) {
-              mbar_expect_tx(&z_full[st], kStage);
-              tma_load_2d(dst, mz, gb * 128, cb * 128, &z_full[st]);
-              tma_load_2d(dst + kZBytes / 2, mz, gb * 128 + 64, cb * 128, &z_full[st]);
-              if (DO_B) {
-                const CUtensorMap* mw = x.head == 0 ? &map_w0 : (x.head == 1 ? &map_w1 : &map_w2);
-                if (DO_A) {      // head backward: W = Keras [64 x G] (K-major B): two [64 feats x 64 genes] boxes
-                  tma_load_2d(dst + kZBytes, mw, gb * 128, 0, &z_full[st]);
-                  tma_load_2d(dst + kZBytes + kWBytes / 2, mw, gb * 128 + 64, 0, &z_full[st]);
-                } else {         // encoder forward: W = Keras [G x 64] (MN-major B): one [128 genes x 64 feats] box
-                  tma_load_2d(dst + kZBytes, mw, 0, gb * 128, &z_full[st]);
-                }
-              }
-            }
-          }
-        }
-      }
-      if (p.dbg && leader) { dbg_acc[2] = (unsigned long long)(clock64() - t_begin); for (int i = 0; i < 3; ++i) p.dbg[blockIdx.x * 16 + i] = dbg_acc[i]; }
-    }
-  } else if (warp == 3 && p.prefetch) {
-    // ===================================================== L2 prefetch (optional, dca_set_tunable "gg_prefetch")
-    // A SWIZZLE_128B box is 128 rows x 128 bytes, i.e. every box touches 128 DRAM pages for 128 bytes each.  This warp
-    // walks the producer's sequence ONE unit ahead (unit = up to four gene blocks of one cell block = one contiguous
-    // segment of up to 1 KB per row) and prefetches the unit's row segments into L2 with bulk prefetches (lane = row
-    // mod 32), paced by the producer's progress mark in shared memory.
-    int unit = 0;
-    auto prefetch_unit = [&](int head, int cb, int g0, int g1) {              // genes [g0*128, g1*128) of cell block cb
-      const int c0 = g0 * 128, c1 = min(g1 * 128, p.G);
-      if (c1 <= c0) return;
-      const uint32_t bytes = (uint32_t)(c1 - c0) * 2u;
-      const __nv_bfloat16* zp = p.Zp[head];
-      for (int r = lane; r < 128; r += 32) {
-        const int row = cb * 128 + r;
-        if (row < p.B) gg_prefetch_l2(zp + (int64_t)row * p.ldz + c0, bytes);
-      }
-    };
-    Cursor cur = first(); Item x;
-    while (next(cur, x)) {
-      for (int cb = x.cb0; cb < x.cb1; ++cb)
-        for (int g4 = x.gb0; g4 < x.gb1; g4 += 4, ++unit) {
-          if (unit > 0) {                                                      // unit 0 is not worth prefetching (its loads are already in flight)
-            long long spins = 0;
-            while (*reinterpret_cast<volatile int*>(&s_unit) < unit - 1) { __nanosleep(64); if (++spins > (1ll << 26)) break; }
-            prefetch_unit(x.head, cb, g4, min(g4 + 4, x.gb1));
-          }
-        }
-    }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    // The WHOLE warp walks the loops (so that smem addresses, descriptors and barrier phases are warp-uniform values the
-    // compiler keeps in uniform registers); only the tcgen05.mma / commit instructions are issued by one lane.  With the
-    // loops inside `if (lane == 0)` every descriptor went through a R2UR waterfall loop: ~75 cycles per MMA, 1800 per tile
-    // of the head backward (24 MMAs) -- the issuing thread, not HBM, bounded the kernel (gg_profile).
-    const bool leader = elect_one();
-    {
-      constexpr uint32_t idesc_b = make_idesc_bf16(128, 64, 0, DO_A ? 0 : 1);   // Z K-major x W (K-major [64xG] | MN-major [Gx64])
-      constexpr uint32_t idesc_a = make_idesc_bf16(128, kDwCols, 1, 1);     // Z MN-major x [H | ones] MN-major
-      uint32_t zi = 0, hi = 0, di = 0, wi = 0;
-      unsigned long long dbg_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // 0 wait z_full, 1 wait h_full, 2 wait dh_empty, 3 wait dw_empty, 4 total, 5 tiles
-      const long long t_begin = clock64();
-      Cursor cur = first(); Item x;
-      for (; next(cur, x); ++wi) {
-        if (DO_A) { GG_TIMED(3, mbar_wait(&dw_empty, (wi & 1) ^ 1)); tcgen05_fence_after(); }
-        for (int cb = x.cb0; cb < x.cb1; ++cb) {
-          uint32_t hs = 0, ds = 0;
-          if (DO_A) { hs = hi & 1; const uint32_t hp = (hi >> 1) & 1; ++hi; GG_TIMED(1, mbar_wait(&h_full[hs], hp)); }
-          if (DO_B) { ds = di & 1; const uint32_t dp = (di >> 1) & 1; ++di; GG_TIMED(2, mbar_wait(&dh_empty[ds], dp ^ 1)); }
-          for (int gb = x.gb0; gb < x.gb1; ++gb) {
-            const uint32_t st = zi % kZStages, ph = (zi / kZStages) & 1; ++zi;
-            GG_TIMED(0, mbar_wait(&z_full[st], ph));
-            ++dbg_acc[5];
-            tcgen05_fence_after();
-            const uint32_t zb = smem_u32(s_z + st * kStage);
-            if (DO_B) {
-              const uint32_t wb = zb + kZBytes;
-#pragma unroll
-              for (int h = 0; h < 2; ++h)
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                  if (leader) umma_bf16(tm_dh + ds * 64, make_smem_desc(zb + h * (kZBytes / 2) + k * 32, 0, 1024),
-                            DO_A ? make_smem_desc(wb + h * (kWBytes / 2) + k * 32, 0, 1024)
-                                 : make_smem_desc(wb + (h * 4 + k) * 2048, 0, 1024), idesc_b,
-                            (gb > x.gb0 || h > 0 || k > 0) ? 1u : 0u);
-            }
-            if (DO_A) {
-              const uint32_t hb = smem_u32(s_h + hs * kHBytes);
-              // COLSUM: N = 80 -- the B operand's second 64-element chunk (leading-dimension offset) is the ones tile, so the
-              // same MMA that forms dW also leaves db[g] = sum over the tile's cells of Z[cell][g] in 16 more columns
-              const uint32_t ones_off = smem_u32(s_ones) - hb;
-#pragma unroll
-              for (int k = 0; k < 8; ++k)
-                if (leader) umma_bf16(tm_dw + (gb - x.gb0) * kDwCols, make_smem_desc(zb + k * 2048, kZBytes / 2, 1024),
-                          make_smem_desc(hb + k * 2048, COLSUM ? ones_off : 0u, 1024), idesc_a, (cb > x.cb0 || k > 0) ? 1u : 0u);
-            }
-            if (leader) umma_commit(&z_empty[st]);
-          }
-          if (DO_A) if (leader) umma_commit(&h_empty[hs]);
-          if (DO_B) if (leader) umma_commit(&dh_full[ds]);
-        }
-        if (DO_A) if (leader) umma_commit(&dw_full);
-      }
-      if (p.dbg && leader) { dbg_acc[4] = (unsigned long long)(clock64() - t_begin); for (int i = 0; i < 6; ++i) p.dbg[blockIdx.x * 16 + 4 + i] = dbg_acc[i]; }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ===================================================== epilogue
-    const int quarter = warp & 3;
-    // ONE elected lane of warp 4 issues every TMA reduce-add and owns their bulk groups (commit / wait are per thread)
-    bool epi_leader = false;
-    if (warp == 4) epi_leader = elect_one();
-    uint32_t di = 0, wi = 0;
-    unsigned long long dbg_acc[6] = {0, 0, 0, 0, 0, 0};       // 0 wait dh_full, 1 dH flush, 2 wait dw_full, 3 dW flush, 4 total
-    const long long t_begin = clock64();
-    Cursor cur = first(); Item x;
-    for (; next(cur, x); ++wi) {
+  // The grid may be smaller than the item count (SMs left to other work): CTAs stride over the items.  T0 = tiles this
+  // CTA consumed in earlier items, so that stage and mbarrier phase continue across items (every issued tile is consumed
+  // before the next item starts).
+  uint32_t T0 = 0;
+  for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
+    // item -> (head, gene blocks [gb0, gb1), cell blocks [cb0, cb1))
+    const int cs = item % p.cell_splits, r = item / p.cell_splits;
+    const int gr = r % p.gene_ranges, head = r / p.gene_ranges;
+    const int gb0 = gr * p.gb_per_item, ng = min(p.n_gb, gb0 + p.gb_per_item) - gb0;
+    const int cb0 = cs * p.cb_per_item, ncb = min(p.n_cb, cb0 + p.cb_per_item) - cb0;
+    const int n_tiles = ng * ncb;
+    const CUtensorMap* mz = head == 0 ? &map_z0 : (head == 1 ? &map_z1 : &map_z2);
+    const CUtensorMap* mw = head == 0 ? &map_w0 : (head == 1 ? &map_w1 : &map_w2);
+    const CUtensorMap* mdw = head == 0 ? &map_dw0 : (head == 1 ? &map_dw1 : &map_dw2);
+
+    auto issue = [&](int t) {                       // thread 0: TMA loads of the item's tile t into its stage
+      const int st = (T0 + t) % kStages;
+      const int cb = cb0 + t / ng, gb = gb0 + t % ng;
+      uint8_t* dst = s_st + st * kStage;
+      mbar_expect_tx(&full[st], kStage);
+      tma_load_2d(dst, mz, gb * 128, cb * 128, &full[st]);
+      tma_load_2d(dst + kZBytes / 2, mz, gb * 128 + 64, cb * 128, &full[st]);
       if (DO_B) {
-        for (int cb = x.cb0; cb < x.cb1; ++cb) {
-          const uint32_t ds = di & 1, dp = (di >> 1) & 1; ++di;
-          GG_TIMED(0, mbar_wait(&dh_full[ds], dp));
-          const long long t_fl = clock64();
-          tcgen05_fence_after();
-          if (epi_leader) bulk_wait_read<0>();          // previous reduce has read the staging tiles
-          named_barrier_sync(3, 128);
-          const int row = quarter * 32 + lane;
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t v[32];
-            tmem_ld_32x32(tm_dh + ((uint32_t)(quarter * 32) << 16) + ds * 64 + c * 32, v);
-            tmem_ld_wait();
-            uint8_t* tile = s_o + c * (kOutBytes / 2);
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              *reinterpret_cast<uint4*>(tile + row * 128 + ((q ^ (row & 7)) << 4)) = make_uint4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
-          }
-          tcgen05_fence_before();
-          fence_proxy_async_smem();
-          named_barrier_sync(3, 128);
-          if (lane == 0) mbar_arrive(&dh_empty[ds]);
-          if (epi_leader) {
-            tma_reduce_add_2d(&map_o, 0, cb * 128, s_o);
-            tma_reduce_add_2d(&map_o, 32, cb * 128, s_o + kOutBytes / 2);
-            bulk_commit();
-          }
-          dbg_acc[1] += (unsigned long long)(clock64() - t_fl);
+        if (WK) {        // head backward: W = Keras [64 x G] (K-major B): two [64 feats x 64 genes] boxes
+          tma_load_2d(dst + kZBytes, mw, gb * 128, 0, &full[st]);
+          tma_load_2d(dst + kZBytes + kWBytes / 2, mw, gb * 128 + 64, 0, &full[st]);
+        } else {         // encoder forward: W = Keras [G x 64] (MN-major B): one [128 genes x 64 feats] box
+          tma_load_2d(dst + kZBytes, mw, 0, gb * 128, &full[st]);
         }
       }
-      if (DO_A) {
-        GG_TIMED(2, mbar_wait(&dw_full, wi & 1));
-        const long long t_fw = clock64();
-        tcgen05_fence_after();
-        float* dst = p.dW[x.head];
-        if (!DO_B && !p.dW_transposed) {
-          // [128 genes x 64] accumulator == row-major block of dW[G x 64]: swizzled staging + TMA reduce-add
-          for (int gb = x.gb0; gb < x.gb1; ++gb) {
-            if (epi_leader) bulk_wait_read<0>();
-            named_barrier_sync(3, 128);
-            const int row = quarter * 32 + lane;
+      if (DO_A) tma_load_2d(dst + kZBytes + (DO_B ? kWBytes : 0), &map_h, 0, cb * 128, &full[st]);
+    };
+    if (threadIdx.x == 0)
+      for (int t = 0; t < kStages - 1 && t < n_tiles; ++t) issue(t);
+
+    float acc_b[DO_B ? 32 : 1];                                        // (b): cells 64*wg.. of the current cell block
+    float acc_a[DO_A ? MAXG : 1][32];                                  // (a): genes 64*wg.. of each gene block of the item
+    float acc_c[COLSUM ? MAXG : 1][8];                                 // column sums
 #pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              uint32_t v[32];
-              tmem_ld_32x32(tm_dw + ((uint32_t)(quarter * 32) << 16) + (gb - x.gb0) * kDwCols + c * 32, v);
-              tmem_ld_wait();
-              uint8_t* tile = s_o + c * (kOutBytes / 2);
+    for (int j = 0; j < (DO_A ? MAXG : 1); ++j)
 #pragma unroll
-              for (int q = 0; q < 8; ++q)
-                *reinterpret_cast<uint4*>(tile + row * 128 + ((q ^ (row & 7)) << 4)) = make_uint4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
+      for (int i = 0; i < 32; ++i) acc_a[j][i] = 0.f;
+#pragma unroll
+    for (int j = 0; j < (COLSUM ? MAXG : 1); ++j)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc_c[j][i] = 0.f;
+
+    int t = 0;
+    for (int cbi = 0; cbi < ncb; ++cbi) {
+      const int cb = cb0 + cbi;
+#pragma unroll
+      for (int i = 0; i < (DO_B ? 32 : 1); ++i) acc_b[i] = 0.f;
+      // (a) needs a compile-time accumulator index per gene block: unrolled over MAXG; the (b) products walk their
+      // whole gene range with one accumulator
+#pragma unroll
+      for (int jj = 0; jj < (DO_A ? MAXG : 1); ++jj)
+      for (int j = jj; j < (DO_A ? min(jj + 1, ng) : ng); ++j) {
+        if (threadIdx.x == 0 && t + kStages - 1 < n_tiles) issue(t + kStages - 1);   // its stage was released at tile t-1
+        const int st = (T0 + t) % kStages;
+        mbar_wait(&full[st], ((T0 + t) / kStages) & 1);
+        const uint32_t zb = smem_u32(s_st + st * kStage), wb = zb + kZBytes, hb = wb + (DO_B ? kWBytes : 0);
+        wgmma_fence();
+        if constexpr (DO_B) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const uint64_t da = make_smem_desc(zb + h * (kZBytes / 2) + wg * 64 * 128 + k * 32, 0, 1024);
+              if (WK) wgmma_m64n64k16<0, 0>(acc_b, da, make_smem_desc(wb + h * (kWBytes / 2) + k * 32, 0, 1024), 1u);
+              else wgmma_m64n64k16<0, 1>(acc_b, da, make_smem_desc(wb + (h * 4 + k) * 2048, 0, 1024), 1u);
             }
-            fence_proxy_async_smem();
-            named_barrier_sync(3, 128);
-            if (epi_leader) {
-              tma_reduce_add_2d(&map_o, 0, gb * 128, s_o);
-              tma_reduce_add_2d(&map_o, 32, gb * 128, s_o + kOutBytes / 2);
-              bulk_commit();
-            }
-          }
-        } else
-        for (int gb = x.gb0; gb < x.gb1; ++gb) {
-          const int g = gb * 128 + quarter * 32 + lane;
-          if (COLSUM) {
-            uint32_t v[32];
-            tmem_ld_32x32(tm_dw + ((uint32_t)(quarter * 32) << 16) + (gb - x.gb0) * kDwCols + 64, v);
-            tmem_ld_wait();
-            if (g < p.G && p.db[x.head]) atomicAdd(p.db[x.head] + g, __uint_as_float(v[0]));
-          }
+        }
+        if constexpr (DO_A) {
 #pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t v[32];
-            tmem_ld_32x32(tm_dw + ((uint32_t)(quarter * 32) << 16) + (gb - x.gb0) * kDwCols + c * 32, v);
-            tmem_ld_wait();
-            if (g < p.G) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const int f = c * 32 + j;
-                float* a = p.dW_transposed ? dst + (int64_t)f * p.dW_ld + g : dst + (int64_t)g * p.dW_ld + f;
-                atomicAdd(a, __uint_as_float(v[j]));
-              }
-            }
+          for (int k = 0; k < 8; ++k) {
+            const uint64_t da = make_smem_desc(zb + wg * (kZBytes / 2) + k * 2048, 0, 1024);
+            wgmma_m64n64k16<1, 1>(acc_a[jj], da, make_smem_desc(hb + k * 2048, 0, 1024), 1u);
+            if constexpr (COLSUM) wgmma_m64n16k16<1, 0>(acc_c[jj], da, make_smem_desc(smem_u32(s_ones) + (k & 3) * 32, 0, 1024), 1u);
           }
         }
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&dw_empty);
-        dbg_acc[3] += (unsigned long long)(clock64() - t_fw);
+        wgmma_commit();
+        wgmma_wait<0>();
+        if constexpr (DO_B) acc_fence(acc_b);
+        if constexpr (DO_A) {
+#pragma unroll
+          for (int jj2 = 0; jj2 < MAXG; ++jj2) acc_fence(acc_a[jj2]);
+        }
+        if constexpr (COLSUM) {
+#pragma unroll
+          for (int jj2 = 0; jj2 < MAXG; ++jj2) acc_fence(acc_c[jj2]);
+        }
+        __syncthreads();                            // every warpgroup is done with stage st
+        ++t;
+      }
+      if constexpr (DO_B) {  // (b) of this cell block -> this item's partial slot (rows padded to whole cell blocks)
+        float* dst = p.part + (int64_t)(head * p.gene_ranges + gr) * p.part_stride + (int64_t)cb * 128 * 64;
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+          const int row = wg * 64 + frow + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + fcol;
+          *reinterpret_cast<float2*>(dst + row * 64 + col) = make_float2(acc_b[i], acc_b[i + 1]);
+        }
       }
     }
-    if (epi_leader) bulk_wait<0>();
-    if (p.dbg && epi_leader) { dbg_acc[4] = (unsigned long long)(clock64() - t_begin); for (int i = 0; i < 5; ++i) p.dbg[blockIdx.x * 16 + 10 + i] = dbg_acc[i]; }
+    T0 += n_tiles;
+    if constexpr (DO_A) {  // (a) of the item: one [128 genes x 64] block per gene block
+#pragma unroll
+      for (int j = 0; j < MAXG; ++j) {
+        if (j >= ng) break;
+        const int gb = gb0 + j;
+        stage_begin();
+        if (dw_transposed) {      // Keras [64 x G]: staging [64 feats][128 genes]
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const int g = wg * 64 + frow + 8 * ((i >> 1) & 1), f = 8 * (i >> 2) + fcol + (i & 1);
+            s_o[f * 128 + g] = acc_a[j][i];
+          }
+          stage_end(mdw, gb * 128, 0);
+        } else {                  // [G x 64]: staging [128 genes][64 feats]
+#pragma unroll
+          for (int i = 0; i < 32; i += 2) {
+            const int g = wg * 64 + frow + 8 * ((i >> 1) & 1), f = 8 * (i >> 2) + fcol;
+            *reinterpret_cast<float2*>(s_o + g * 64 + f) = make_float2(acc_a[j][i], acc_a[j][i + 1]);
+          }
+          stage_end(mdw, 0, gb * 128);
+        }
+        if constexpr (COLSUM) {
+          float* dbh = head == 0 ? p.db[0] : (head == 1 ? p.db[1] : p.db[2]);   // (no dynamic index into the parameters)
+          if ((l & 3) == 0 && dbh) {               // every column of the column-sum accumulator holds the sum
+            const int g = gb * 128 + wg * 64 + frow;
+            if (g < p.G) atomicAdd(dbh + g, acc_c[j][0]);
+            if (g + 8 < p.G) atomicAdd(dbh + g + 8, acc_c[j][2]);
+          }
+        }
+      }
+    }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem, kTmemCols);
+  if (threadIdx.x == 0) bulk_wait<0>();
 }
 
-template <bool DO_A, bool DO_B, bool COLSUM>
-constexpr uint32_t smem_bytes() {
-  return kZStages * (kZBytes + (DO_B ? kWBytes : 0)) + (DO_A ? 2 * kHBytes : 0) + kOutBytes + (COLSUM ? kHBytes : 0) + 1024;
+// out[i] += sum over s of part[s * stride + i], s in slot order (float4 per thread; n and stride are multiples of 4)
+__global__ void gene_gemm_reduce_kernel(const float* __restrict__ part, int slots, int64_t stride, float* __restrict__ out,
+                                        int64_t n) {
+  const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  if (i >= n) return;
+  float4 acc = *reinterpret_cast<const float4*>(out + i);
+  for (int sl = 0; sl < slots; ++sl) {
+    const float4 v = __ldcs(reinterpret_cast<const float4*>(part + sl * stride + i));
+    acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+  }
+  *reinterpret_cast<float4*>(out + i) = acc;
 }
 
 }  // namespace gg
 
+size_t gene_gemm_workspace_bytes(int B) { return sizeof(float) * (size_t)gg::kMaxSlots * cdiv(B, 128) * 128 * 64; }
+
 // Z: bf16 [B x G] per head (ldz elements); H: bf16 [B x 64]; W[i]: bf16 Keras-layout kernels -- [G x 64] for mode 1 (the
 // encoder kernel), [64 x G] per head for mode 3; out_b: fp32 [B x 64] (+=).
-// mode: 1 = DO_B (K1), 2 = DO_A (K5), 3 = DO_A|DO_B|COLSUM (K4).
+// mode: 1 = encoder forward (K1), 2 = encoder backward (K5), 3 = head backward (K4: dW / db pass, then the dH pass).
+// ws: gene_gemm_workspace_bytes(B) of device memory for the partial slots of modes 1 and 3.
 int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, int B, int G, int n_heads,
                  const __nv_bfloat16* H, const __nv_bfloat16* const W[3], float* out_b, float* const dW[3], int64_t dW_ld,
-                 int dW_transposed, float* const db[3], int sm_count, cudaStream_t s) {
+                 int dW_transposed, float* const db[3], void* ws, size_t ws_bytes, int sm_count, cudaStream_t s) {
   using namespace gg;
   if (ldz % 8 != 0) { set_error("gene_gemm_tc: ldz must be a multiple of 8 (16-byte TMA stride)"); return DCA_ERR_BAD_ARG; }
+  if (mode < 1 || mode > 3) { set_error("gene_gemm_tc: bad mode %d", mode); return DCA_ERR_BAD_ARG; }
   const bool do_a = mode & 2, do_b = mode & 1;
-  CUtensorMap mz[3], mh, mw[3], mo;
+  if (do_b && (!ws || ws_bytes < gene_gemm_workspace_bytes(B))) { set_error("gene_gemm_tc: workspace too small"); return DCA_ERR_BAD_ARG; }
+  CUtensorMap mz[3], mh, mw[3], mdw[3];
   for (int i = 0; i < 3; ++i) DCA_TRY(make_tensor_map_2d(&mz[i], Z[i < n_heads ? i : 0], 2, 1, (uint64_t)B, (uint64_t)G, (uint64_t)ldz, 128, 64, 1));
-  if (do_a) DCA_TRY(make_tensor_map_2d(&mh, H, 2, 1, (uint64_t)B, 64, 64, 128, 64, 1)); else mh = mz[0];
+  mh = mz[0];
+  for (int i = 0; i < 3; ++i) mw[i] = mdw[i] = mz[0];
+  if (do_a) {
+    DCA_TRY(make_tensor_map_2d(&mh, H, 2, 1, (uint64_t)B, 64, 64, 128, 64, 1));
+    for (int i = 0; i < 3; ++i) {
+      float* d = dW[i < n_heads ? i : 0];
+      if (dW_transposed) DCA_TRY(make_tensor_map_2d(&mdw[i], d, 4, 0, 64, (uint64_t)G, (uint64_t)dW_ld, 64, 128, 0));
+      else {
+        if (dW_ld != 64) { set_error("gene_gemm_tc: non-transposed dW needs ld == 64"); return DCA_ERR_BAD_ARG; }
+        DCA_TRY(make_tensor_map_2d(&mdw[i], d, 4, 0, (uint64_t)G, 64, 64, 128, 64, 0));
+      }
+    }
+  }
   if (do_b) {
     for (int i = 0; i < 3; ++i) {
       const __nv_bfloat16* w = W[i < n_heads ? i : 0];
-      if (do_a) DCA_TRY(make_tensor_map_2d(&mw[i], w, 2, 1, 64, (uint64_t)G, (uint64_t)G, 64, 64, 1));
+      if (mode == 3) DCA_TRY(make_tensor_map_2d(&mw[i], w, 2, 1, 64, (uint64_t)G, (uint64_t)G, 64, 64, 1));
       else DCA_TRY(make_tensor_map_2d(&mw[i], w, 2, 1, (uint64_t)G, 64, 64, 128, 64, 1));
     }
-    DCA_TRY(make_tensor_map_2d(&mo, out_b, 4, 0, (uint64_t)B, 64, 64, 128, 32, 1));
-  } else {
-    mw[0] = mw[1] = mw[2] = mz[0]; mo = mz[0];
-    if (do_a && !dW_transposed) {
-      if (dW_ld != 64) { set_error("gene_gemm_tc: non-transposed dW needs ld == 64"); return DCA_ERR_BAD_ARG; }
-      DCA_TRY(make_tensor_map_2d(&mo, dW[0], 4, 0, (uint64_t)G, 64, 64, 128, 32, 1));
-    }
   }
-  Params p{};
-  p.B = B; p.G = G; p.n_heads = n_heads;
-  p.n_cb = cdiv(B, 128); p.n_gb = cdiv(G, 128);
-  // Work decomposition: items = (head, gene range, cell range), processed by a persistent grid.
-  if (do_a && do_b) {
-    // head backward: gene ranges limited by TMEM (kMaxGb accumulators); cells split so that one wave of fat items fills the
-    // SMs.  Search the small space for the shortest makespan in tile units: rounds x (tiles per item + one tile-equivalent
-    // per cell block for the dH reduce-add the item issues + a flush / start-up term per gene block -- the (a) outputs
-    // leave by atomics, every extra cell split repeats the dW flush, every extra gene range the dH traffic).
-    int best_gpi = 1, best_splits = 1; long long best_cost = -1;
-    for (int gpi = 1; gpi <= kMaxGb; ++gpi) {
-      const int ranges = cdiv(p.n_gb, gpi) * n_heads;
-      for (int splits = 1; splits <= (p.n_cb < 8 ? p.n_cb : 8); ++splits) {
-        const int cbpi = cdiv(p.n_cb, splits), cs = cdiv(p.n_cb, cbpi);
-        const long long items = (long long)ranges * cs, rounds = (items + sm_count - 1) / sm_count;
-        const long long cost = rounds * ((long long)gpi * cbpi + cbpi + 2ll * gpi);
-        if (best_cost < 0 || cost < best_cost) { best_cost = cost; best_gpi = gpi; best_splits = splits; }
-      }
-    }
-    p.gb_per_item = best_gpi; p.gene_ranges = cdiv(p.n_gb, best_gpi);
-    p.cb_per_item = cdiv(p.n_cb, best_splits); p.cell_splits = cdiv(p.n_cb, p.cb_per_item);
-  } else if (do_a) {
-    // encoder backward: the same search (per item: tiles + half a tile per cell block for the H tile it loads + the dW flush
-    // by TMA reduce-add per gene block); TMEM holds up to kMaxGb accumulators, so one H tile serves four gene blocks
-    int best_gpi = 1, best_splits = 1; long long best_cost = -1;
-    for (int gpi = 1; gpi <= kMaxGb; ++gpi) {
-      const int ranges = cdiv(p.n_gb, gpi) * n_heads;
-      for (int splits = 1; splits <= (p.n_cb < 8 ? p.n_cb : 8); ++splits) {
-        const int cbpi = cdiv(p.n_cb, splits), cs = cdiv(p.n_cb, cbpi);
-        const long long items = (long long)ranges * cs, rounds = (items + sm_count - 1) / sm_count;
-        const long long cost = rounds * (2ll * gpi * cbpi + cbpi + 4ll * gpi);      // in half tiles
-        if (best_cost < 0 || cost < best_cost) { best_cost = cost; best_gpi = gpi; best_splits = splits; }
-      }
-    }
-    p.gb_per_item = best_gpi; p.gene_ranges = cdiv(p.n_gb, best_gpi);
-    p.cb_per_item = cdiv(p.n_cb, best_splits); p.cell_splits = cdiv(p.n_cb, p.cb_per_item);
-  } else {
-    // encoder forward: one cell block per item, genes split so that there are ~4 items per SM
-    p.cb_per_item = 1; p.cell_splits = p.n_cb;
-    int gsplits = cdiv(4 * sm_count, p.n_cb); if (gsplits < 1) gsplits = 1; if (gsplits > p.n_gb) gsplits = p.n_gb;
-    while (gsplits > 1 && cdiv(p.n_gb, gsplits) < 4) --gsplits;
-    p.gb_per_item = cdiv(p.n_gb, gsplits); p.gene_ranges = cdiv(p.n_gb, p.gb_per_item);
-  }
-  p.total_items = p.gene_ranges * p.cell_splits * n_heads;
-  if (do_a && g_gg_flat) {
-    // Flat partition (backward kernels): units = (head, gene range of gpi blocks, cell block); every CTA takes an equal
-    // contiguous run.  gpi by a small cost model in tile units per CTA: tiles + one per cell block (H tile / dH reduce-add)
-    // + two per gene block for each dW flush (one per gene range the run touches).
-    int best_gpi = 1; long long best_cost = -1;
-    for (int gpi = 1; gpi <= kMaxGb; ++gpi) {
-      const long long units = (long long)cdiv(p.n_gb, gpi) * n_heads * p.n_cb;
-      const long long ctas = units < sm_count ? units : sm_count, per = (units + ctas - 1) / ctas;
-      const long long cost = per * gpi + per + ((per + p.n_cb - 1) / p.n_cb + 1) * 2 * gpi;
-      if (best_cost < 0 || cost < best_cost) { best_cost = cost; best_gpi = gpi; }
-    }
-    p.flat = 1; p.gb_per_item = best_gpi; p.gene_ranges = cdiv(p.n_gb, best_gpi);
-    p.cb_per_item = p.n_cb; p.cell_splits = 1;
-    p.total_units = p.gene_ranges * n_heads * p.n_cb;
-    p.total_items = p.total_units;          // grid size below
-  }
-  for (int i = 0; i < 3; ++i) { p.dW[i] = dW ? dW[i] : nullptr; p.db[i] = db ? db[i] : nullptr; p.Zp[i] = Z[i < n_heads ? i : 0]; }
-  p.ldz = ldz; p.prefetch = p.flat ? 0 : g_gg_prefetch;
-  if (g_gg_profile) {
-    static unsigned long long* dbg_buf = nullptr;
-    if (!dbg_buf) DCA_CUDA_OK(cudaMalloc(&dbg_buf, sizeof(unsigned long long) * 16 * 1024));
-    DCA_CUDA_OK(cudaMemsetAsync(dbg_buf, 0, sizeof(unsigned long long) * 16 * 1024, s));
-    p.dbg = dbg_buf;
-  }
-  p.dW_ld = dW_ld; p.dW_transposed = dW_transposed;
-  const int grid = p.total_items < sm_count ? p.total_items : sm_count;
-#define DCA_GG_LAUNCH(A, Bb, Cc)                                                                                       \
+  Params base{};
+  base.B = B; base.G = G; base.n_heads = n_heads;
+  base.n_cb = cdiv(B, 128); base.n_gb = cdiv(G, 128);
+  for (int i = 0; i < 3; ++i) base.db[i] = db ? db[i] : nullptr;
+  base.part = reinterpret_cast<float*>(ws); base.part_stride = (int64_t)base.n_cb * 128 * 64;
+
+  // at most one CTA per SM (shared memory) and at most sm_count CTAs: a caller that passes fewer SMs than the device has
+  // leaves the others free; the CTAs stride over the items
+#define DCA_GG_LAUNCH(P, A, Bb, Cc, WKk, MG)                                                                           \
   do {                                                                                                                 \
     static bool attr = false;                                                                                          \
-    constexpr uint32_t sm = smem_bytes<A, Bb, Cc>();                                                                   \
-    if (!attr) { DCA_CUDA_OK(cudaFuncSetAttribute(gene_gemm_kernel<A, Bb, Cc>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); attr = true; } \
-    gene_gemm_kernel<A, Bb, Cc><<<grid, kThreads, sm, s>>>(mz[0], mz[1], mz[2], mh, mw[0], mw[1], mw[2], mo, p);                         \
+    constexpr uint32_t sm = smem_bytes<A, Bb, Cc>();                                                                       \
+    if (!attr) { DCA_CUDA_OK(cudaFuncSetAttribute(gene_gemm_kernel<A, Bb, Cc, WKk, MG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); attr = true; } \
+    gene_gemm_kernel<A, Bb, Cc, WKk, MG><<<min(P.total_items, sm_count), kThreads, sm, s>>>(mz[0], mz[1], mz[2], mh, mw[0], mw[1], mw[2],      \
+                                                                          mdw[0], mdw[1], mdw[2], dW_transposed, P);  \
+    DCA_LAUNCH_CHECK();                                                                                                \
   } while (0)
-  if (mode == 1) DCA_GG_LAUNCH(false, true, false);
-  else if (mode == 2) DCA_GG_LAUNCH(true, false, false);
-  else if (mode == 3) DCA_GG_LAUNCH(true, true, true);
-  else { set_error("gene_gemm_tc: bad mode %d", mode); return DCA_ERR_BAD_ARG; }
-#undef DCA_GG_LAUNCH
-  DCA_LAUNCH_CHECK();
-  if (p.dbg) {          // diagnosis only: synchronises the stream
-    std::vector<unsigned long long> h((size_t)grid * 16);
-    DCA_CUDA_OK(cudaStreamSynchronize(s));
-    DCA_CUDA_OK(cudaMemcpy(h.data(), p.dbg, h.size() * 8, cudaMemcpyDeviceToHost));
-    double a[16] = {0}; double mx_total = 0;
-    for (int b = 0; b < grid; ++b) { for (int i = 0; i < 16; ++i) a[i] += (double)h[(size_t)b * 16 + i] / grid; if ((double)h[(size_t)b * 16 + 8] > mx_total) mx_total = (double)h[(size_t)b * 16 + 8]; }
-    fprintf(stderr, "[gg_profile mode %d grid %d flat %d gpi %d] kcycles avg/CTA  producer: wait_z_empty %.0f wait_h_empty %.0f total %.0f | "
-                    "mma: wait_z_full %.0f wait_h_full %.0f wait_dh_empty %.0f wait_dw_empty %.0f total %.0f (max %.0f) tiles %.1f | "
-                    "epilogue: wait_dh_full %.0f dh_flush %.0f wait_dw_full %.0f dw_flush %.0f total %.0f\n",
-            mode, grid, p.flat, p.gb_per_item, a[0] / 1e3, a[1] / 1e3, a[2] / 1e3, a[4] / 1e3, a[5] / 1e3, a[6] / 1e3, a[7] / 1e3, a[8] / 1e3,
-            mx_total / 1e3, a[9], a[10] / 1e3, a[11] / 1e3, a[12] / 1e3, a[13] / 1e3, a[14] / 1e3);
+
+  if (do_a) {
+    // (a): items = (head, gene range) over all cells.  gpi (gene blocks per item, <= kMaxGb for the registers) by the
+    // shortest makespan in tile units: rounds x (tiles per item + a flush term per gene block)
+    Params p = base;
+    int best_gpi = 1; long long best_cost = -1;
+    for (int gpi = 1; gpi <= kMaxGb; ++gpi) {
+      const long long items = (long long)cdiv(p.n_gb, gpi) * n_heads, rounds = (items + sm_count - 1) / sm_count;
+      const long long cost = rounds * ((long long)gpi * p.n_cb + 2ll * gpi);
+      if (best_cost < 0 || cost < best_cost) { best_cost = cost; best_gpi = gpi; }
+    }
+    p.gb_per_item = best_gpi; p.gene_ranges = cdiv(p.n_gb, best_gpi);
+    p.cb_per_item = p.n_cb; p.cell_splits = 1;
+    p.total_items = p.gene_ranges * n_heads;
+    if (mode == 3) DCA_GG_LAUNCH(p, true, false, true, false, kMaxGb);
+    else DCA_GG_LAUNCH(p, true, false, false, false, kMaxGb);
   }
+  if (do_b) {
+    // (b): items = (head, gene range, cell block), ~4 per SM, at most kMaxSlots partial slots
+    Params p = base;
+    p.cb_per_item = 1; p.cell_splits = p.n_cb;
+    int gsplits = cdiv(4 * sm_count, p.n_cb * n_heads); if (gsplits < 1) gsplits = 1;
+    if (gsplits > kMaxSlots / n_heads) gsplits = kMaxSlots / n_heads;
+    if (gsplits > p.n_gb) gsplits = p.n_gb;
+    while (gsplits > 1 && cdiv(p.n_gb, gsplits) < 4) --gsplits;
+    p.gb_per_item = cdiv(p.n_gb, gsplits); p.gene_ranges = cdiv(p.n_gb, p.gb_per_item);
+    p.total_items = p.gene_ranges * p.cell_splits * n_heads;
+    if (mode == 3) DCA_GG_LAUNCH(p, false, true, false, true, 1);
+    else DCA_GG_LAUNCH(p, false, true, false, false, 1);
+    const int64_t n = (int64_t)B * 64;
+    gene_gemm_reduce_kernel<<<(unsigned)cdiv(n / 4, 256), 256, 0, s>>>(p.part, p.gene_ranges * n_heads, p.part_stride, out_b, n);
+    DCA_LAUNCH_CHECK();
+  }
+#undef DCA_GG_LAUNCH
   return DCA_OK;
 }
 
@@ -509,7 +349,7 @@ extern "C" int dca_tc_gene_gemm(int32_t mode, const void* Z0, const void* Z1, co
                                 float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed, float* db0, float* db1,
                                 float* db2, void* stream) {
   if (!Z0 || batch <= 0 || genes <= 0 || n_heads < 1 || n_heads > 3) { set_error("dca_tc_gene_gemm: bad argument"); return DCA_ERR_BAD_ARG; }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const __nv_bfloat16* Z[3] = {(const __nv_bfloat16*)Z0, (const __nv_bfloat16*)Z1, (const __nv_bfloat16*)Z2};
@@ -517,6 +357,12 @@ extern "C" int dca_tc_gene_gemm(int32_t mode, const void* Z0, const void* Z1, co
   float* db[3] = {db0, db1, db2};
   const __nv_bfloat16* Wp[3];
   for (int i = 0; i < 3; ++i) Wp[i] = (const __nv_bfloat16*)W + (mode == 3 ? (size_t)(i < n_heads ? i : 0) * 64 * genes : 0);
-  return tc::gene_gemm_tc(mode, Z, ldz, batch, genes, n_heads, (const __nv_bfloat16*)H, Wp, out_b, dW,
-                          dW_ld, dW_transposed, db, sms, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t ws_bytes = tc::gene_gemm_workspace_bytes(batch);
+  void* ws = nullptr;
+  DCA_CUDA_OK(cudaMallocAsync(&ws, ws_bytes, st));
+  const int rc = tc::gene_gemm_tc(mode, Z, ldz, batch, genes, n_heads, (const __nv_bfloat16*)H, Wp, out_b, dW,
+                                  dW_ld, dW_transposed, db, ws, ws_bytes, sms, st);
+  DCA_CUDA_OK(cudaFreeAsync(ws, st));
+  return rc;
 }

@@ -1,4 +1,4 @@
-// Output activations of the three heads as evaluated in the tcgen05 epilogues (dca/network.py:38-39,369):
+// Output activations of the three heads as evaluated in the tensor-core epilogues (dca/network.py:38-39,369):
 // MeanAct = clip(exp(z), 1e-5, 1e6), DispAct = clip(softplus(z), 1e-4, 1e4), sigmoid.  One definition shared by
 // the head-forward kernel (dense_tc.cu) and the fused head/loss/backward kernel (flash_zinb.cu) so that both
 // produce bit-identical head outputs.

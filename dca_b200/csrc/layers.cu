@@ -219,7 +219,7 @@ __global__ void rmsprop_kernel(float* __restrict__ p, const float* __restrict__ 
     o.z = rmsprop_one(pv.z, gv.z, rv.z, lr, clip, rho, eps, gs); o.w = rmsprop_one(pv.w, gv.w, rv.w, lr, clip, rho, eps, gs);
     *reinterpret_cast<float4*>(r + i) = rv;
     *reinterpret_cast<float4*>(p + i) = o;
-    if (shadow) {                        // bf16 operand copy for the tcgen05 kernels (same layout)
+    if (shadow) {                        // bf16 operand copy for the tensor-core kernels (same layout)
       __nv_bfloat162 a = __floats2bfloat162_rn(o.x, o.y), b = __floats2bfloat162_rn(o.z, o.w);
       uint2 w; w.x = *reinterpret_cast<uint32_t*>(&a); w.y = *reinterpret_cast<uint32_t*>(&b);
       *reinterpret_cast<uint2*>(shadow + i) = w;

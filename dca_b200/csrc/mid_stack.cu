@@ -9,8 +9,9 @@
 //             saves x_hat_i, h_i (training) for the backward pass, the pre-BN 'center' output (latent,
 //             dca/network.py:184-185) and updates the moving statistics (momentum 0.99).
 //   backward: dh_last -> for each layer: relu mask, BN backward (two column sums -> barrier), bias / beta /
-//             kernel gradients of the inner layers (atomicAdd into the flat gradient buffer), dh of the
-//             previous layer; ends with da_0 (fp32 + bf16) for the first layer's weight gradient.
+//             kernel gradients of the inner layers (per-CTA partials, added to the flat gradient buffer in CTA
+//             order after a last barrier), dh of the previous layer; ends with da_0 (fp32 + bf16) for the first
+//             layer's weight gradient.
 #include "dca_internal.cuh"
 #include "mid_stack.h"
 #include <cstdio>
@@ -315,6 +316,7 @@ __global__ void __launch_bounds__(kThreads, 1) mid_backward_kernel(const Params 
   MID_STAMP(1);
   for (int l = p.L - 1; l >= 0; --l) {
     const int w = p.w[l];
+    float* gpart_l = p.gpart + (size_t)l * kGradSlots * kMaxCtas + blockIdx.x;   // this CTA's column of the layer's slots
     // relu mask (+ load x_hat): loads first, then the dependent shared-memory traffic
     {
       constexpr int kRowIters = kMaxRows / 4;
@@ -365,7 +367,7 @@ __global__ void __launch_bounds__(kThreads, 1) mid_backward_kernel(const Params 
       if (c < w) for (int r = q; r < rows; r += 4) s += g[r][c];
       red[q][c] = (double)s;
       __syncthreads();
-      if (threadIdx.x < w) atomicAdd(&p.gb[l][threadIdx.x], (float)(red[0][c] + red[1][c] + red[2][c] + red[3][c]));
+      if (threadIdx.x < w) gpart_l[(size_t)threadIdx.x * kMaxCtas] = (float)(red[0][c] + red[1][c] + red[2][c] + red[3][c]);
       __syncthreads();
     }
     MID_STAMP(6 + (p.L - 1 - l) * 8);
@@ -415,7 +417,7 @@ __global__ void __launch_bounds__(kThreads, 1) mid_backward_kernel(const Params 
         if (k0 == tr * 4) MID_STAMP(25 + (p.L - 1 - l) * 3);
 #pragma unroll
         for (int j = 0; j < 4; ++j)
-          if (k0 + j < win) atomicAdd(&p.gW[l][(size_t)(k0 + j) * w + tc], s[j]);
+          if (k0 + j < win) gpart_l[(size_t)(kMaxW + (k0 + j) * w + tc) * kMaxCtas] = s[j];
         if (k0 == tr * 4) MID_STAMP(26 + (p.L - 1 - l) * 3);
       }
     __syncthreads();
@@ -457,6 +459,19 @@ __global__ void __launch_bounds__(kThreads, 1) mid_backward_kernel(const Params 
     __syncthreads();
     MID_STAMP(8 + (p.L - 1 - l) * 8);
   }
+  // bias / kernel gradients: every CTA has written its partial of every slot; one thread per slot adds the partials in
+  // CTA order, so the sum does not depend on which CTA finished first
+  grid_barrier(p.bar, gridDim.x, gen);
+  for (int e = blockIdx.x * kThreads + threadIdx.x; e < p.L * kGradSlots; e += gridDim.x * kThreads) {
+    const int l = e / kGradSlots, o = e % kGradSlots, w = p.w[l];
+    float* dst;
+    if (o < kMaxW) { if (o >= w) continue; dst = p.gb[l] + o; }
+    else { if (l == 0 || o - kMaxW >= p.w[l - 1] * w) continue; dst = p.gW[l] + (o - kMaxW); }
+    const float* src = p.gpart + (size_t)e * kMaxCtas;
+    float sum = 0.f;
+    for (int c = 0; c < (int)gridDim.x; ++c) sum += __ldcg(src + c);
+    *dst += sum;
+  }
   MID_STAMP(31);
 }
 
@@ -485,6 +500,7 @@ static int mid_fill(mid::Params& p, int B) {
 }
 
 size_t mid_partial_doubles() { return (size_t)2 * mid::kMaxCtas * 2 * mid::kMaxW; }
+size_t mid_grad_partial_floats(int L) { return (size_t)L * mid::kGradSlots * mid::kMaxCtas; }
 
 static int mid_attr() {
   static bool done = false;

@@ -8,6 +8,7 @@ namespace mid {
 constexpr int kMaxW = 64;          // widest hidden layer handled by the fused kernels
 constexpr int kMaxCtas = 128;      // co-resident CTAs (one per SM, cooperative launch)
 constexpr int kMaxRows = 64;       // rows per CTA strip  (=> batch <= 8192; larger batches use the per-layer kernels)
+constexpr int kGradSlots = kMaxW + kMaxW * kMaxW;   // per layer: bias gradient, then the kernel gradient [w_in x w]
 
 struct Params {
   int L, B, training, batchnorm, center, rows_per_cta, n_ctas;
@@ -27,6 +28,7 @@ struct Params {
   float* gW[DCA_MAX_HIDDEN]; float* gb[DCA_MAX_HIDDEN]; float* gbeta[DCA_MAX_HIDDEN];
   float* da0; __nv_bfloat16* da0_bf16;
   double* partial;                    // [n_ctas][2][kMaxW] scratch per barrier round
+  float* gpart;                       // [L][kGradSlots][kMaxCtas]: per-CTA bias / kernel gradients, folded in CTA order
   unsigned* bar;                      // {count, generation}
   float eps, momentum;
   long long* dbg;                     // gg_profile: clock64 stamps of CTA 0 at the phase boundaries (nullptr = off)
@@ -37,6 +39,7 @@ struct Params {
 bool mid_supported(const int* widths, int L);
 bool mid_device_ok();   // cooperative launch available and the largest grid fits the device
 size_t mid_partial_doubles();
+size_t mid_grad_partial_floats(int L);
 int mid_forward(mid::Params& p, cudaStream_t s);
 int mid_backward(mid::Params& p, cudaStream_t s);
 

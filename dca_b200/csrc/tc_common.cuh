@@ -1,11 +1,13 @@
-// sm_100a building blocks written as inline PTX: mbarrier, TMA (cp.async.bulk.tensor), TMEM
-// allocation, tcgen05.mma / commit / ld, UMMA shared-memory + instruction descriptors, and the
+// sm_90a building blocks written as inline PTX: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma.mma_async
+// with both operands in shared memory, fp32 accumulators in registers), the wgmma shared-memory descriptor and the
 // host-side CUtensorMap encoder (resolved through cudaGetDriverEntryPoint, no -lcuda).
 //
-// Descriptor bit layouts follow the PTX ISA "tcgen05 matrix / instruction descriptor" tables
-// (start address >>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout [61,64);
-// idesc: c_format [4,6), a_format [7,10), b_format [10,13), a_major 15, b_major 16, N>>3 [17,23),
-// M>>4 [24,29)).
+// Descriptor bit layout follows the PTX ISA "matrix descriptor" table for wgmma (start address >>4 [0,14),
+// LBO>>4 [16,30), SBO>>4 [32,46), base offset [49,52) = 0 (1024-byte aligned swizzle atoms), layout [62,64):
+// 1 = SWIZZLE_128B).
+//
+// Accumulator fragment of one m64nNk16 instruction (PTX ISA "wgmma register fragments"): thread t of the warpgroup
+// holds d[i] at row 16*(t/32) + (t%32)/4 + 8*((i/2)%2), column 8*(i/4) + 2*(t%4) + i%2.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -26,9 +28,6 @@ __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarr
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -38,7 +37,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
   return ok != 0;
 }
-// Bounded spin: a lost TMA / MMA completion traps (kernel error) instead of hanging the GPU.
+// Bounded spin: a lost TMA completion traps (kernel error) instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t polls = 0;
   long long t0 = 0;
@@ -49,6 +48,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       else if (now - t0 > 4000000000ll) __trap();
     }
   }
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 // Same, with a sleep between polls: a waiting warp stops competing for issue slots with the warps that do
@@ -68,9 +70,8 @@ __device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity
 }
 
 // ------------------------------------------------------------------------------------ fences
+// generic-proxy writes to shared memory (st.shared) -> visible to the async proxy (wgmma operands, TMA stores)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -85,12 +86,7 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
 }
-// shared -> global (bulk async group)
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, int32_t c0, int32_t c1, const void* smem_src) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(smem_u32(smem_src)) : "memory");
-}
-// shared -> global with += (fp32 add performed at L2)
+// shared -> global with += (fp32 add performed at L2); elements outside the tensor are skipped
 __device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, int32_t c0, int32_t c1, const void* smem_src) {
   asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%1, %2}], [%3];"
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(smem_u32(smem_src)) : "memory");
@@ -101,87 +97,75 @@ __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.w
 template <int N>
 __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
-// ------------------------------------------------------------------------------------ TMEM
-// One full warp calls alloc / dealloc.  ncols: power of two in [32, 512].
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// 32 lanes x 32 columns of fp32: thread i of the warp receives columns [col, col+32) of TMEM lane
-// (lane_base + i); lane_base must be 32*(warp_id % 4).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-}
-// same shape, 8 / 16 columns
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------------------------ UMMA
-enum : uint32_t { kLayoutSw128 = 2 };
-
-// Shared-memory matrix descriptor, SWIZZLE_128B.  K-major operand (rows of 128 B = 64 bf16 along K,
-// 8-row swizzle atoms 1024 B apart): lbo = 0, sbo = 1024.  MN-major operand (rows of 128 B = 64
-// bf16 along M/N, one row per k, 8-k groups `sbo` bytes apart, 64-wide MN blocks `lbo` bytes apart).
+// ------------------------------------------------------------------------------------ wgmma
+// Shared-memory matrix descriptor, SWIZZLE_128B.  K-major operand (rows of 128 B = 64 bf16 along K, 8-row swizzle
+// atoms 1024 B apart): lbo unused, sbo = 1024; a k16 step advances the start address by 32 B.  MN-major operand (rows
+// of 128 B = 64 bf16 along M/N, one row per k, 8-k groups `sbo` bytes apart, 64-wide MN blocks `lbo` bytes apart);
+// a k16 step advances the start address by 2048 B.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;                       // descriptor version (Blackwell)
-  d |= (uint64_t)kLayoutSw128 << 61;
+  d |= (uint64_t)1 << 62;                       // SWIZZLE_128B
   return d;
 }
 
-// one lane of the (converged) warp: the predicate the compiler recognises as single-lane, so that operands of the
-// instructions it guards move to uniform registers without a waterfall loop
+// Issued by all 128 threads of a warpgroup.  fence: before the first wgmma that touches accumulator registers the
+// threads wrote; commit / wait: wgmma groups of this thread (wait<0>: every issued wgmma has completed).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64 x N] (+)= A[64 x 16] . B[16 x N], bf16 operands from shared memory, fp32 D in registers (acc = 0: D = A.B).
+// TA / TB: 0 = K-major operand, 1 = MN-major operand.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7},"
+      " %8, %9, p, 1, 1, %11, %12;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31},"
+      " %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63},"
+      " %64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+}
+
+// keep the accumulator registers live and ordered across the asynchronous wgmma (no reads before wgmma_wait)
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// one lane of the (converged) warp
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
   asm volatile("{\n\t.reg .pred px;\n\telect.sync _|px, 0xFFFFFFFF;\n\tselp.u32 %0, 1, 0, px;\n\t}" : "=r"(pred));
   return pred != 0;
-}
-
-// kind::f16 instruction descriptor: bf16 x bf16 -> fp32
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4)                              // c_format = F32
-         | (1u << 7) | (1u << 10)               // a_format = b_format = BF16
-         | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16)
-         | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 // ------------------------------------------------------------------------------------ fast math for epilogues

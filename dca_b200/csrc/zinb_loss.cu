@@ -14,7 +14,7 @@
 #include <cstdlib>
 
 namespace dca {
-namespace tc { extern int g_gg_prefetch; extern int g_gg_flat; extern int g_gg_profile; }
+namespace tc { extern int g_gg_profile; }
 
 namespace {
 
@@ -23,14 +23,14 @@ constexpr int kVec = 4;
 constexpr int kColsPerBlock = kThreads * kVec;   // 1024 genes per block
 constexpr int kMaxBlocks = 65536;                // bound of the per-block loss-partial buffer
 
-// Launch tunables (dca_set_tunable; defaults chosen from the sweep in profiles/r1_loss_sweep.log)
+// Launch tunables (dca_set_tunable; defaults from a launch-parameter sweep, tests/diag_loss_sweep.py)
 struct LossTune { int target_blocks; unsigned producer_sleep_ns, consumer_sleep_ns; int branch_free; int ring; };
-LossTune g_tune = {0 /* auto */, 0u, 0u, 1 /* branch-free zero branch: -7 % at 4096 x 20000, profiles/r1_loss_sweep2.log */,
+LossTune g_tune = {0 /* auto */, 0u, 0u, 1 /* branch-free zero branch (the faster variant in the sweep) */,
                    1 /* per-warp rings + f32x2 arithmetic (zinb_loss_bwd_ring_kernel); 0 = block-wide ring (staged kernel) */};
 
 int sm_count_cached() {
   static int n = 0;
-  if (!n) { int dev = 0; if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148; }
+  if (!n) { int dev = 0; if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132; }
   return n;
 }
 
@@ -40,7 +40,7 @@ inline Plan make_plan(int B, int G, int cols_per_block, int max_rpb = 1 << 30) {
   Plan p;
   p.col_blocks = cdiv(G, cols_per_block);
   // auto: small batches (C2: 4096 x 2000) run as ONE wave of 3 resident blocks per SM (block start-up and the
-  // partial last wave cost 15 % there), large ones as ~5 waves for dynamic balance (profiles/r1_loss_sweep.log)
+  // partial last wave cost 15 % there), large ones as ~5 waves for dynamic balance
   const int target = g_tune.target_blocks > 0 ? g_tune.target_blocks
                      : ((long long)B * G <= (32ll << 20) ? 3 * sm_count_cached() : 16 * sm_count_cached());
   int chunks = target / p.col_blocks;
@@ -501,7 +501,7 @@ zinb_loss_bwd_staged_kernel(const float* __restrict__ Y, int64_t ldy, const int3
 // no single-lane issue path: in the block-wide bulk-copy ring of zinb_loss_bwd_staged_kernel a warp could run at
 // most three rows ahead of the slowest warp of its block (the one that met a large count and took the Stirling
 // path), and a fifth of all issued instructions were mbarrier polls of warps waiting for a slot their neighbour
-// had not released (profiles/r1_ncu_k3_v5_c3: 3-instruction loops executed 9-13x per row).  The gather of the count
+// had not released (3-instruction loops executed 9-13x per row).  The gather of the count
 // rows costs one address computation (rows[] cached in shared memory).  The arithmetic runs on f32x2 pairs
 // (zinb_math.cuh: zinb_zero_pair / finish_factors_pair), the queued non-zero counts return raw derivatives only
 // (zinb_nb_raw) and the activation chain / clip masks / 1/N are applied once per element by its owner.
@@ -936,8 +936,6 @@ extern "C" int dca_set_tunable(const char* name, int64_t value) {
   else if (n == "fused_heads" && (value == 0 || value == 1)) g_fused_heads_default = (int)value;
   else if (n == "loss_branch_free" && (value == 0 || value == 1)) g_tune.branch_free = (int)value;
   else if (n == "loss_ring" && value >= 0 && value <= 2) g_tune.ring = (int)value;
-  else if (n == "gg_prefetch" && (value == 0 || value == 1)) tc::g_gg_prefetch = (int)value;
-  else if (n == "gg_flat" && (value == 0 || value == 1)) tc::g_gg_flat = (int)value;
   else if (n == "gg_profile" && (value == 0 || value == 1)) tc::g_gg_profile = (int)value;
   else { set_error("dca_set_tunable: unknown name or value out of range (%s = %lld)", name, (long long)value); return DCA_ERR_BAD_ARG; }
   return DCA_OK;

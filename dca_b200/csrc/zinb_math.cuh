@@ -287,19 +287,13 @@ DCA_HD Elem zinb_elem_nb_mu(float y, float mu, float th, float pi, float ridge, 
 }
 
 // ------------------------------------------------------------------------------------ packed (f32x2) formulation
-// sm_100 executes fma / mul / add on PAIRS of fp32 values in one instruction (fma.rn.f32x2 -> FFMA2): the element-wise
-// chains below are written over float2 so that two genes of a thread share every FMA-pipe instruction; MUFU, min/max
-// and selects stay scalar.  The host build evaluates the same expressions component-wise (fmaf), so the formulas
-// are unit-tested without a GPU (dca_zinb_elem_host, variant 0x200).
-#if defined(__CUDA_ARCH__)
-DCA_HD float2 fma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
-DCA_HD float2 mul2(float2 a, float2 b) { return __fmul2_rn(a, b); }
-DCA_HD float2 add2(float2 a, float2 b) { return __fadd2_rn(a, b); }
-#else
+// The element-wise chains below are written over float2 (two genes of a thread): the two chains are independent, so
+// they interleave in the FMA pipe; MUFU, min/max and selects stay scalar.  sm_90 has no paired fp32 FMA, so device
+// and host evaluate the same component-wise expressions (fmaf) and the formulas are unit-tested without a GPU
+// (dca_zinb_elem_host, variant 0x200).
 DCA_HD float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 DCA_HD float2 mul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
 DCA_HD float2 add2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
-#endif
 DCA_HD float2 splat(float v) { return make_float2(v, v); }
 DCA_HD float2 neg2(float2 a) { return make_float2(-a.x, -a.y); }
 

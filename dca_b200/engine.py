@@ -37,7 +37,7 @@ class DeviceEngine:
                                       % (ae_type, sorted(_lib.AE_TYPE_IDS)))
         self.lib = _lib.load()
         if not torch.cuda.is_available():
-            raise _lib.DcaError("dca_b200 needs a CUDA device (B200); there is no CPU fallback")
+            raise _lib.DcaError("dca_b200 needs a CUDA device (H100); there is no CPU fallback")
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self.n_in, self.n_out, self.hidden = int(n_in), int(n_out), tuple(int(h) for h in hidden)
         self.ae_type, self.batchnorm, self.max_batch = ae_type, bool(batchnorm), int(max_batch)

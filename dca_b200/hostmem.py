@@ -3,9 +3,8 @@
 The streaming path (dca_stream_*) copies every batch host->device over PCIe.  On a two-socket host a
 pinned buffer whose pages sit on the far socket crosses the socket interconnect on every copy, so pinned
 buffers are allocated while the calling thread is restricted to the CPUs NVML reports as local to the GPU;
-the previous affinity is restored afterwards (pages stay where they were pinned).  Best effort: on the
-shared B200 boxes of this pool the effect was 25-30 GB/s vs 22-23 GB/s for 4-16 MiB copies
-(profiles/r1_diag_e2e_v2.log), inside the 14-55 GB/s run-to-run spread of those hosts.
+the previous affinity is restored afterwards (pages stay where they were pinned).  Best effort: the gain
+is host-dependent and has not been measured on H100 hosts.
 No reference counterpart (the reference never leaves the host).
 """
 from __future__ import annotations

@@ -78,7 +78,7 @@ class Autoencoder:
     # -- dca/network.py:92-156
     def build(self, max_batch: int = 32, seed: Optional[int] = None):
         if self.ae_type is None:
-            raise NotImplementedError("autoencoder type %s is not on the B200-accelerated path"
+            raise NotImplementedError("autoencoder type %s is not on the GPU-accelerated path"
                                       % type(self).__name__)
         if self.init != 'glorot_uniform':
             raise NotImplementedError("only init='glorot_uniform' is on the accelerated path")

@@ -1,4 +1,4 @@
-/* dca_b200.h -- C ABI of libdca_b200.so: the B200-native DCA training hot path.
+/* dca_b200.h -- C ABI of libdca_b200.so: the H100-native DCA training hot path.
  *
  * The reference (theislab/dca @ 6abd124) has no FFI: its boundary is the Python API, and the
  * arithmetic runs inside Keras/TensorFlow.  Each entry point below names the reference call
@@ -78,9 +78,9 @@ typedef enum dca_activation {
 typedef enum dca_dtype { DCA_F32 = 0, DCA_BF16 = 1 } dca_dtype;
 
 typedef enum dca_gemm_path {
-  DCA_GEMM_AUTO = 0,          /* tcgen05 tiles whenever the shape qualifies, else generic */
+  DCA_GEMM_AUTO = 0,          /* tensor-core (wgmma) tiles whenever the shape qualifies, else generic */
   DCA_GEMM_GENERIC = 1,       /* fp32 CUDA-core tiles for every layer (arbitrary shapes)  */
-  DCA_GEMM_TCGEN05 = 2        /* require the tcgen05 path; create fails if shape unsupported */
+  DCA_GEMM_TCGEN05 = 2        /* require the tensor-core path; create fails if shape unsupported */
 } dca_gemm_path;
 
 typedef enum dca_region_id {
@@ -320,7 +320,7 @@ int dca_dense_heads_fwd(const float* H, int64_t ldh, int32_t batch, int32_t K, i
                         const float* row_scale,
                         float* m_out, float* d_out, float* pi_out, int64_t ld_out, void* stream);
 
-/* tcgen05 head layer: Hb = bf16 [batch x 64] (decoder output), Wk = bf16 [n_heads][64][genes] (the Keras
+/* tensor-core head layer: Hb = bf16 [batch x 64] (decoder output), Wk = bf16 [n_heads][64][genes] (the Keras
  * kernels, read in place as MN-major operands), bias = float [n_heads*genes]; kind[i] in {2 MeanAct,
  * 3 DispAct, 4 sigmoid} per head slot.  Same arithmetic as dca_dense_heads_fwd with bf16-rounded operands
  * and fp32 accumulation. */
@@ -328,7 +328,7 @@ int dca_tc_heads_fwd(const void* Hb, int32_t batch, const void* Wk, const float*
                      int32_t n_heads, const int32_t kind[3], const float* row_scale,
                      float* out0, float* out1, float* out2, int64_t ld_out, void* stream);
 
-/* The gene-wide tcgen05 product kernel (one smem tile of Z = X or dZ feeds both products):
+/* The gene-wide tensor-core product kernel (one smem tile of Z = X or dZ feeds both products):
  * mode 1: out_b[B x 64] += Z . W (W = bf16 [genes x 64], Keras layout)             -- encoder forward
  * mode 2: dW += Z^T . H (H = bf16 [B x 64])                                       -- encoder backward
  * mode 3: both (W = bf16 [n_heads][64][genes]), plus db = column sums of Z         -- head backward
@@ -339,7 +339,7 @@ int dca_tc_gene_gemm(int32_t mode, const void* Z0, const void* Z1, const void* Z
                      float* dW0, float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed,
                      float* db0, float* db1, float* db2, void* stream);
 
-/* Single-tile tcgen05 probe used by the tests to pin the UMMA operand conventions: D[128 x N] =
+/* Single-tile wgmma probe used by the tests to pin the operand descriptor conventions: D[128 x N] =
  * A . B with bf16 operands; a K-major operand is stored [MN x K], an MN-major one [K x MN].
  * *_lbo / *_sbo < 0 select the library's defaults for that layout. */
 int dca_tc_probe(const void* A, int32_t a_rows, int32_t a_cols, const void* B, int32_t b_rows, int32_t b_cols,
@@ -354,7 +354,7 @@ int dca_tc_probe(const void* A, int32_t a_rows, int32_t a_cols, const void* B, i
 int dca_profile_enable(dca_handle* h, int32_t on);
 int dca_profile_read(dca_handle* h, double ms[DCA_N_PHASES], int64_t counts[DCA_N_PHASES], int32_t reset);
 
-/* Which code paths an engine selected: info = {tcgen05 heads (K2/K4), tcgen05 encoder (K1/K5),
+/* Which code paths an engine selected: info = {tensor-core heads (K2/K4), tensor-core encoder (K1/K5),
  * fused hidden stack, head slots, SM count, bytes per loss-gradient element (4 fp32 | 2 bf16),
  * instantiated step graphs, graphs enabled}. */
 int dca_engine_info(const dca_handle* h, int32_t info[8]);

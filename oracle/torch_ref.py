@@ -3,7 +3,7 @@
 Purpose (a) an autograd-based cross-check of the closed-form gradients in
 ``oracle/dca_oracle.py`` (autograd plays the role TF autodiff plays in the reference);
 (b) the CPU baseline timed by ``bench.py`` ("torch-CPU restatement of the reference
-path (TensorFlow unavailable in image)", BASELINE.md section 2).
+path (TensorFlow unavailable in image)").
 
 The op sequence mirrors what Keras executes for
   dca/network.py:92-141 (Dense -> BatchNormalization(center, no scale) -> relu),

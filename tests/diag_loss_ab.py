@@ -2,7 +2,7 @@
 cp.async ring with f32x2 arithmetic) on realistic operands: timing (L2 flushed, CUDA events) and a numerical check
 of loss + the three gradient tensors against a float64 torch statement of dca/loss.py:122-148 on sampled rows.
 
-Not a test: run by hand on a GPU box,  python tests/diag_loss_ab.py > gpurun_out/loss_ab.log
+Not a test: run by hand on a GPU box,  python tests/diag_loss_ab.py > loss_ab.log
 """
 import ctypes as C
 import os

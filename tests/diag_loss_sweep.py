@@ -1,6 +1,6 @@
 """Sweep of the loss kernel's launch tunables (dca_set_tunable) on synthetic head outputs.
 
-Not a test: run by hand on a GPU box,  python tests/diag_loss_sweep.py > gpurun_out/loss_sweep.log
+Not a test: run by hand on a GPU box,  python tests/diag_loss_sweep.py > loss_sweep.log
 Prints one line per (shape, gradient dtype, target blocks, producer/consumer sleep): median ms over
 launches with the L2 flushed in between, and the algorithmic GB/s (28 B / element fp32 gradients,
 22 B / element bf16 gradients).

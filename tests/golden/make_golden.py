@@ -1,6 +1,6 @@
 """Build tests/golden/biochemists.npz from the reference's own R-fitted fixtures.
 
-Run IN THE BUILD CONTAINER ONLY (needs /root/reference):  python tests/golden/make_golden.py
+Needs a checkout of theislab/dca:  python tests/golden/make_golden.py /path/to/dca-checkout
 
 Sources (theislab/dca @ 6abd124, read-only data files, provenance data/biochemists.R:16-42):
   data/biochemists.tsv                   915 x 6 table: count response `art` + 5 covariates
@@ -19,13 +19,13 @@ import os, sys
 import numpy as np
 import pandas as pd
 
-REF = "/root/reference/data"
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "..", ".."))
 from oracle import dca_oracle as O  # noqa: E402
 
 
 def main():
+    REF = os.path.join(sys.argv[1], "data")
     tab = pd.read_csv(os.path.join(REF, "biochemists.tsv"), sep="\t")
     y = tab["art"].to_numpy(np.float64)
     cov = tab[["fem", "mar", "kid5", "phd", "ment"]].to_numpy(np.float64)

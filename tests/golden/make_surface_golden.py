@@ -1,6 +1,6 @@
 """Build tests/golden/api_surface.json: the public Python surface of the reference that the host layer must keep.
 
-Run IN THE BUILD CONTAINER ONLY (needs /root/reference):  python tests/golden/make_surface_golden.py
+Needs a checkout of theislab/dca:  python tests/golden/make_surface_golden.py /path/to/dca-checkout
 
 Read with `ast` (TensorFlow / scanpy are not importable here, and nothing of the reference is executed):
   dca/api.py:19-45       dca(...)           parameter names, order and default values
@@ -13,7 +13,9 @@ import ast
 import json
 import os
 
-REF = "/root/reference/dca"
+import sys
+
+REF = os.path.join(sys.argv[1] if len(sys.argv) > 1 else ".", "dca")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
@@ -64,7 +66,7 @@ def _cli_flags(path):
 
 
 def main():
-    out = {"source": "theislab/dca @ /root/reference (read with ast, not executed)",
+    out = {"source": "theislab/dca @ 6abd124 (read with ast, not executed)",
            "api.dca": _function(os.path.join(REF, "api.py"), "dca"),
            "train.train": _function(os.path.join(REF, "train.py"), "train"),
            "network.Autoencoder.__init__": _function(os.path.join(REF, "network.py"), "__init__", cls="Autoencoder"),

@@ -3,7 +3,7 @@ float64 AUTOGRAD statement of the same network (oracle/torch_ref.py) -- autograd
 reference.  Dropout masks are a counter-based stream (dca_dropout_mask_host reproduces the mask of any layer / step), so
 the oracle applies exactly the mask the device applied: the comparison is element-exact, not distributional.
 Reference behaviour: dca/network.py:98-99 (input dropout), :129-138 (activation layer, hidden dropout), :41; the CLI
-flags --activation / --dropoutrate / --inputdropout.  Needs a B200: -m gpu."""
+flags --activation / --dropoutrate / --inputdropout.  Needs an H100: -m gpu."""
 import ctypes as C
 
 import numpy as np

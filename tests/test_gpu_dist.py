@@ -11,7 +11,7 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs (run with gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")
 def test_two_rank_nccl_gradients_equal_global_batch():
     port = 29600 + (os.getpid() % 300)
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",

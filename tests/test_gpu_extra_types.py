@@ -2,7 +2,7 @@
 nb-fork, zinb-fork) through the C ABI against the float64 AUTOGRAD statement of the same networks
 (oracle/torch_ref.py:TorchExtraNet -- autograd plays the role TF autodiff plays in the reference): one training step
 (loss, every gradient tensor), a short trajectory with the RMSprop update and BatchNorm moving statistics, validation
-loss and predict outputs.  Needs a B200: -m gpu."""
+loss and predict outputs.  Needs an H100: -m gpu."""
 import numpy as np
 import pytest
 import torch

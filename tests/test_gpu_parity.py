@@ -1,4 +1,4 @@
-"""Parity of the CUDA path (through the C ABI) with the CPU oracle.  Needs a B200: -m gpu."""
+"""Parity of the CUDA path (through the C ABI) with the CPU oracle.  Needs an H100: -m gpu."""
 import ctypes as C
 import os
 import numpy as np
@@ -336,7 +336,7 @@ def _make_pair_tc(ae_type, batchnorm, B, G, seed=0):
 
 @pytest.mark.parametrize("ae_type,batchnorm", TC_CASES)
 def test_tc_train_step_vs_oracle(ae_type, batchnorm):
-    """Whole step through the tcgen05 kernels vs the SAME-ROUNDING fp64 oracle (GEMM operands of the
+    """Whole step through the tensor-core kernels vs the SAME-ROUNDING fp64 oracle (GEMM operands of the
     gene-wide layers rounded to bf16 exactly where the kernels round them, everything else exact).
     ReLU-mask flips make the exact-oracle comparison discontinuous (a 2^-9 perturbation of W1 moves
     single columns of dW1 by ~10 % at batch 300), so parity of the bf16 path is defined against this."""
@@ -538,3 +538,25 @@ def test_two_phase_step_equals_single_call(gemm_path):
         tol = 1e-5 if gemm_path == "generic" else 1e-3
         assert np.max(np.abs(g1 - g2)) <= tol * np.max(np.abs(g1)) + 1e-12
         e1.apply_update(1e-3, 5.0); e2.apply_update(1e-3, 5.0)
+
+
+def test_tc_step_is_bit_reproducible():
+    """Two engines with the same seed and inputs compute bit-identical gradients and parameters on the tensor-core path
+    (direct call, graph capture and replay on a side stream): every gradient of the step is summed in a fixed order.
+    The shape spreads the gene-wide products over several cell blocks, gene ranges and partial slots."""
+    from dca_b200.engine import DeviceEngine
+    N, G, B = 1100, 2000, 1024
+    Y = synth_counts(N, G, 7); X, sf = O.normalize_inputs(Y)
+    rows = torch.as_tensor(np.random.default_rng(1).permutation(N)[:B].astype(np.int32)).to(DEV)
+    engines = [DeviceEngine(G, G, (64, 32, 64), "zinb-conddisp", max_batch=B, seed=3, gemm_path="tcgen05") for _ in range(2)]
+    Xd, Yd, sfd = _t(X), _t(Y), _t(sf)
+    side = torch.cuda.Stream(DEV)
+    with torch.cuda.stream(side):
+        for step in range(4):
+            for e in engines:
+                e.train_step(Xd, Yd, sfd, rows=rows)
+                e.apply_update(1e-3, 5.0)
+            side.synchronize()
+            assert torch.equal(engines[0].grads, engines[1].grads), step
+            assert torch.equal(engines[0].params, engines[1].params), step
+            assert torch.equal(engines[0].bn_state, engines[1].bn_state), step

@@ -1,6 +1,6 @@
 """Parity at the benchmark's sizes and at the edges of the domain (VERDICT r1 "close the parity gaps").
 
- * the loss kernel at 4096 x 20000 (BASELINE configs[2..4] batch shape) against the float64 oracle on sampled rows,
+ * the loss kernel at 4096 x 20000 (the benchmark's batch shape) against the float64 oracle on sampled rows,
    plus a checksum of checksums over the whole batch;
  * one tcgen05 training step at G = 20000, B = 512 against the same-rounding oracle AND, with a stated bound, against
    the exact (fp32-semantics) oracle -- loss, every gradient tensor norm-wise -- and predict() after K steps;
@@ -8,7 +8,7 @@
    a gradient beyond the clip value;
  * train() epoch semantics against oracle.fit(batch_order=...);
  * the fused head/loss/backward kernel against the oracle (not against the three-kernel path).
-Needs a B200: -m gpu.  Reference behaviour: dca/loss.py:85-148, dca/network.py:38-39, dca/train.py:54-98.
+Needs an H100: -m gpu.  Reference behaviour: dca/loss.py:85-148, dca/network.py:38-39, dca/train.py:54-98.
 """
 import ctypes as C
 import numpy as np

@@ -1,4 +1,4 @@
-"""tcgen05 kernels against same-rounding references (bf16-rounded operands, fp32/fp64 accumulate)."""
+"""wgmma kernels against same-rounding references (bf16-rounded operands, fp32/fp64 accumulate)."""
 import ctypes as C
 import numpy as np
 import pytest
@@ -22,7 +22,7 @@ def _bf(a):
 @pytest.mark.parametrize("a_mn,b_mn", [(0, 0), (1, 0), (0, 1), (1, 1)])
 @pytest.mark.parametrize("N,K", [(64, 64), (256, 64), (64, 128), (128, 256)])
 def test_tc_probe_operand_layouts(a_mn, b_mn, N, K):
-    """D = A.B for every (K-major | MN-major) operand combination the Dense kernels rely on."""
+    """D = A.B for every (K-major | MN-major) operand combination the Dense kernels rely on (wgmma descriptors)."""
     L = _L(); lib = L.load()
     M = 128
     rng = np.random.default_rng(N * 7 + K + a_mn * 2 + b_mn)
