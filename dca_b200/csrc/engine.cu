@@ -1001,7 +1001,7 @@ extern "C" int dca_engine_info(const dca_handle* h, int32_t info[8]) {
   DCA_NEED_HANDLE(h);
   if (!info) { set_error("dca_engine_info: info is NULL"); return DCA_ERR_BAD_ARG; }
   const Engine& e = h->e;
-  info[0] = e.tc_heads; info[1] = e.tc_enc; info[2] = e.mid_ok; info[3] = e.n_slots; info[4] = e.sm_count;
+  info[0] = e.tc_heads; info[1] = e.tc_enc; info[2] = e.use_mid(e.cfg.max_batch); info[3] = e.n_slots; info[4] = e.sm_count;
   info[5] = e.tc_heads ? 2 : 4;
   int ng = 0; for (auto& g : e.graphs) if (g.exec) ++ng;
   info[6] = ng; info[7] = e.graphs_enabled;

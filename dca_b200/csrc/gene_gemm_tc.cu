@@ -344,14 +344,15 @@ int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, int B, 
 
 // ------------------------------------------------------------------------------------ C ABI (tests / profiling)
 using namespace dca;
-extern "C" int dca_tc_gene_gemm(int32_t mode, const void* Z0, const void* Z1, const void* Z2, int64_t ldz, int32_t batch,
-                                int32_t genes, int32_t n_heads, const void* H, const void* W, float* out_b, float* dW0,
-                                float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed, float* db0, float* db1,
-                                float* db2, void* stream) {
+extern "C" int dca_tc_gene_gemm_sms(int32_t mode, const void* Z0, const void* Z1, const void* Z2, int64_t ldz,
+                                    int32_t batch, int32_t genes, int32_t n_heads, const void* H, const void* W, float* out_b,
+                                    float* dW0, float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed, float* db0,
+                                    float* db1, float* db2, void* stream, int32_t sm_count) {
   if (!Z0 || batch <= 0 || genes <= 0 || n_heads < 1 || n_heads > 3) { set_error("dca_tc_gene_gemm: bad argument"); return DCA_ERR_BAD_ARG; }
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (sm_count > 0 && sm_count < sms) sms = sm_count;      // a smaller grid: the CTAs stride over the items
   const __nv_bfloat16* Z[3] = {(const __nv_bfloat16*)Z0, (const __nv_bfloat16*)Z1, (const __nv_bfloat16*)Z2};
   float* dW[3] = {dW0, dW1, dW2};
   float* db[3] = {db0, db1, db2};
@@ -365,4 +366,11 @@ extern "C" int dca_tc_gene_gemm(int32_t mode, const void* Z0, const void* Z1, co
                                   dW_ld, dW_transposed, db, ws, ws_bytes, sms, st);
   DCA_CUDA_OK(cudaFreeAsync(ws, st));
   return rc;
+}
+extern "C" int dca_tc_gene_gemm(int32_t mode, const void* Z0, const void* Z1, const void* Z2, int64_t ldz, int32_t batch,
+                                int32_t genes, int32_t n_heads, const void* H, const void* W, float* out_b, float* dW0,
+                                float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed, float* db0, float* db1,
+                                float* db2, void* stream) {
+  return dca_tc_gene_gemm_sms(mode, Z0, Z1, Z2, ldz, batch, genes, n_heads, H, W, out_b, dW0, dW1, dW2, dW_ld,
+                              dW_transposed, db0, db1, db2, stream, 0);
 }

@@ -224,10 +224,21 @@ class DeviceEngine:
             check(self.lib.dca_train_step_phase(self.handle, _ptr(X), X.stride(0), _ptr(Y), Y.stride(0), _ptr(sf),
                                                 _ptr(rows), b, phase, self._stream()), "dca_train_step_phase")
 
-    def comm_init(self):
+    def comm_init(self, single_rank: bool = False):
         """Create the engine's own NCCL communicator (dca_comm_init) over the ranks of the default torch.distributed
         group: rank 0 draws the unique id, torch.distributed carries its 128 bytes to the others.  Afterwards
-        train_step_allreduce runs the gradient exchange inside the library (one CUDA graph per step)."""
+        train_step_allreduce runs the gradient exchange inside the library (one CUDA graph per step).
+
+        single_rank=True builds a one-rank communicator without torch.distributed: the data-parallel step
+        (dca_train_step_dp, with its DCA_DP_* launch plans) then runs on this GPU alone and its all-reduces leave the
+        gradients as they are -- the way to exercise that step on a single GPU."""
+        if single_rank:
+            buf = (C.c_char * 128)()
+            check(self.lib.dca_comm_unique_id(buf), "dca_comm_unique_id")
+            with torch.cuda.device(self.device):
+                check(self.lib.dca_comm_init(self.handle, buf.raw, 0, 1), "dca_comm_init")
+            self._comm = True
+            return True
         import torch.distributed as dist
         if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size() == 1:
             return False

@@ -333,11 +333,18 @@ int dca_tc_heads_fwd(const void* Hb, int32_t batch, const void* Wk, const float*
  * mode 2: dW += Z^T . H (H = bf16 [B x 64])                                       -- encoder backward
  * mode 3: both (W = bf16 [n_heads][64][genes]), plus db = column sums of Z         -- head backward
  * Z0..Z2: bf16 [B x genes] per head (leading dim ldz); dW per head: float, dW[f*dW_ld + g] when
- * dW_transposed (Keras [64 x genes]) else dW[g*dW_ld + f].  All outputs are accumulated (+=). */
+ * dW_transposed (Keras [64 x genes]) else dW[g*dW_ld + f].  All outputs are accumulated (+=).
+ * The grid is at most the device's SM count. */
 int dca_tc_gene_gemm(int32_t mode, const void* Z0, const void* Z1, const void* Z2, int64_t ldz, int32_t batch,
                      int32_t genes, int32_t n_heads, const void* H, const void* W, float* out_b,
                      float* dW0, float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed,
                      float* db0, float* db1, float* db2, void* stream);
+/* The same with the grid capped at sm_count CTAs (what the engine does when SMs are left to a collective): the CTAs
+ * then stride over the items.  sm_count <= 0 uses the device's SM count. */
+int dca_tc_gene_gemm_sms(int32_t mode, const void* Z0, const void* Z1, const void* Z2, int64_t ldz, int32_t batch,
+                         int32_t genes, int32_t n_heads, const void* H, const void* W, float* out_b,
+                         float* dW0, float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed,
+                         float* db0, float* db1, float* db2, void* stream, int32_t sm_count);
 
 /* Single-tile wgmma probe used by the tests to pin the operand descriptor conventions: D[128 x N] =
  * A . B with bf16 operands; a K-major operand is stored [MN x K], an MN-major one [K x MN].
@@ -355,7 +362,7 @@ int dca_profile_enable(dca_handle* h, int32_t on);
 int dca_profile_read(dca_handle* h, double ms[DCA_N_PHASES], int64_t counts[DCA_N_PHASES], int32_t reset);
 
 /* Which code paths an engine selected: info = {tensor-core heads (K2/K4), tensor-core encoder (K1/K5),
- * fused hidden stack, head slots, SM count, bytes per loss-gradient element (4 fp32 | 2 bf16),
+ * fused hidden stack at a batch of max_batch (larger than 8192 rows: the per-layer kernels), head slots, SM count, bytes per loss-gradient element (4 fp32 | 2 bf16),
  * instantiated step graphs, graphs enabled}. */
 int dca_engine_info(const dca_handle* h, int32_t info[8]);
 

@@ -25,7 +25,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 from scipy import special as _sp
@@ -335,11 +335,18 @@ class OracleNet:
     bn_momentum: float = KERAS_DEFAULTS["bn_momentum"]
     bn_eps: float = KERAS_DEFAULTS["bn_eps"]
     # same-rounding emulation of the tcgen05 path: GEMM operands of the gene-wide layers are rounded
-    # to bf16 (X, first kernel, last hidden activation, head kernels, dZ, dA of the first layer)
-    emulate_bf16: bool = False
+    # to bf16 (X, first kernel, last hidden activation, head kernels, dZ, dA of the first layer).
+    # The engine picks the tensor-core encoder and heads independently, so either side can be emulated
+    # alone: "encoder" (X, first kernel, dA of the first layer), "heads" (last hidden activation, head
+    # kernels, dZ), "both" (= True) or "none" (= False).
+    emulate_bf16: Union[bool, str] = False
 
     def __post_init__(self):
         assert self.ae_type in AE_TYPES
+        side = {True: "both", False: "none"}.get(self.emulate_bf16, self.emulate_bf16)
+        assert side in ("both", "none", "encoder", "heads"), self.emulate_bf16
+        self._rnd_enc = bf16_round if side in ("both", "encoder") else (lambda t: t)
+        self._rnd_heads = bf16_round if side in ("both", "heads") else (lambda t: t)
         self.names = layer_names(len(self.hidden))
         self.heads = head_names(self.ae_type)
         if not self.params:
@@ -361,10 +368,10 @@ class OracleNet:
         h = np.asarray(X, dt)
         c = {"h_in": [h]} if cache is not None else None
         latent = None
-        rnd = bf16_round if self.emulate_bf16 else (lambda t: t)
+        rnd_e, rnd_h = self._rnd_enc, self._rnd_heads
         for i, nm in enumerate(self.names):
             if i == 0:
-                a = rnd(h) @ rnd(self.params[nm + "/kernel"]) + self.params[nm + "/bias"]
+                a = rnd_e(h) @ rnd_e(self.params[nm + "/kernel"]) + self.params[nm + "/bias"]
             else:
                 a = h @ self.params[nm + "/kernel"] + self.params[nm + "/bias"]
             if nm == "center":
@@ -390,7 +397,7 @@ class OracleNet:
         out = {"latent": latent, "decoded": h}
         z = {}
         for nm in self.heads:
-            z[nm] = rnd(h) @ rnd(self.params[nm + "/kernel"]) + self.params[nm + "/bias"]
+            z[nm] = rnd_h(h) @ rnd_h(self.params[nm + "/kernel"]) + self.params[nm + "/bias"]
         out["z"] = z
         out["mean_norm"] = mean_act(z["mean"])
         sfc = np.asarray(sf, dt).reshape(-1, 1)
@@ -439,16 +446,16 @@ class OracleNet:
                                     self.ridge)
         loss = hg["loss"] + self.penalty()
         g: Dict[str, np.ndarray] = {}
-        rnd = bf16_round if self.emulate_bf16 else (lambda t: t)
+        rnd_e, rnd_h = self._rnd_enc, self._rnd_heads
         h_last = cache["h_in"][-1]
         dh = np.zeros_like(h_last)
         for nm, key in (("mean", "dzm"), ("dispersion", "dzd"), ("pi", "dzp")):
             if nm in z:
-                dz = rnd(hg[key])
+                dz = rnd_h(hg[key])
                 W = self.params[nm + "/kernel"]
-                g[nm + "/kernel"] = rnd(h_last).T @ dz + self.l1 * np.sign(W) + 2 * self.l2 * W
+                g[nm + "/kernel"] = rnd_h(h_last).T @ dz + self.l1 * np.sign(W) + 2 * self.l2 * W
                 g[nm + "/bias"] = dz.sum(axis=0)
-                dh = dh + dz @ rnd(W).T
+                dh = dh + dz @ rnd_h(W).T
         if "dtheta_raw" in hg:
             g["dispersion/theta"] = hg["dtheta_raw"]
         for i in reversed(range(len(self.names))):
@@ -464,7 +471,7 @@ class OracleNet:
             W = self.params[nm + "/kernel"]
             l1, l2 = self._reg(i)
             if i == 0:
-                g[nm + "/kernel"] = rnd(cache["h_in"][i]).T @ rnd(da) + l1 * np.sign(W) + 2 * l2 * W
+                g[nm + "/kernel"] = rnd_e(cache["h_in"][i]).T @ rnd_e(da) + l1 * np.sign(W) + 2 * l2 * W
             else:
                 g[nm + "/kernel"] = cache["h_in"][i].T @ da + l1 * np.sign(W) + 2 * l2 * W
             g[nm + "/bias"] = da.sum(axis=0)

@@ -34,7 +34,8 @@ def main():
     # batchnorm off: plain data parallelism; batchnorm on + sync_bn: BatchNorm statistics all-reduced over the ranks
     # (forward and backward), i.e. exactly the single-GPU model at the global batch size (SURVEY.md 8e)
     # tcgen05 self-consistency 2e-3: the encoder backward rounds dA1 to bf16; the two runs sum dH3 in different orders
-    # (fp32 atomics, 1e-7), which flips single bf16 roundings of dA1 (2^-9 of that element) -- measured 2e-5 ... 2e-4
+    # (per-rank partials plus the all-reduce against one engine's slots, 1e-7), which flips single bf16 roundings of dA1
+    # (2^-9 of that element)
     for gemm_path, G, hidden, bn, tol_self, tol_oracle in (("generic", 200, (16, 8, 16), False, 2e-5, 2e-3),
                                                            ("tcgen05", 264, (64, 32, 64), False, 2e-3, 3e-2),
                                                            ("generic", 200, (16, 8, 16), True, 5e-5, 2e-3),

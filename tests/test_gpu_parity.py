@@ -1,6 +1,8 @@
 """Parity of the CUDA path (through the C ABI) with the CPU oracle.  Needs an H100: -m gpu."""
 import ctypes as C
 import os
+import subprocess
+import sys
 import numpy as np
 import pytest
 import torch
@@ -299,9 +301,9 @@ def test_full_size_properties_c2():
     rows = torch.randperm(9000, device=DEV)[:B].to(torch.int32)
     eng.train_step(Xd, Yd, sfd, rows=rows); l1 = eng.read_loss(); g1 = eng.grads.clone()
     eng.train_step(Xd, Yd, sfd, rows=rows); l2 = eng.read_loss(); g2 = eng.grads.clone()
-    assert np.isfinite(l1) and abs(l1 - l2) < 1e-5 * abs(l1)                   # repeatable
+    assert np.isfinite(l1) and l1 == l2                                        # repeatable: every sum has a fixed order
     assert torch.isfinite(g1).all()
-    assert (g1[:-2] - g2[:-2]).abs().max().item() <= 1e-4 * g1[:-2].abs().max().item() + 1e-12
+    assert torch.equal(g1, g2)
     # loss of the batch == mean of the losses of its two halves (checksum of checksums)
     eng.read_epoch_acc(reset=True)
     eng.eval_step(Xd, Yd, sfd, rows=rows); a = eng.read_epoch_acc()
@@ -531,12 +533,13 @@ def test_two_phase_step_equals_single_call(gemm_path):
         e2.train_step(Xd, Yd, sfd, phase=2)
         torch.cuda.synchronize()
         assert torch.equal(head_after_1, e2.grads[e2.head_bucket:])
-        g1, g2 = e1.grads.cpu().numpy(), e2.grads.cpu().numpy()
-        # fp32 path: summation order of the atomics only.  tcgen05 path: that order noise (1e-7) in dH3 can flip single bf16
-        # roundings of dA1 in front of the encoder backward (2^-9 of one element of one row: measured 1.2e-4 of the largest
-        # gradient in 2 of 5 runs, 1e-6 otherwise)
-        tol = 1e-5 if gemm_path == "generic" else 1e-3
-        assert np.max(np.abs(g1 - g2)) <= tol * np.max(np.abs(g1)) + 1e-12
+        if gemm_path == "tcgen05":
+            # the two halves launch the same kernels as the single call, and no sum on this path depends on timing
+            assert torch.equal(e1.grads, e2.grads)
+        else:
+            # the fp32 path's split-K GEMMs add their partial products with atomics: order noise only
+            g1, g2 = e1.grads.cpu().numpy(), e2.grads.cpu().numpy()
+            assert np.max(np.abs(g1 - g2)) <= 1e-5 * np.max(np.abs(g1)) + 1e-12
         e1.apply_update(1e-3, 5.0); e2.apply_update(1e-3, 5.0)
 
 
@@ -560,3 +563,172 @@ def test_tc_step_is_bit_reproducible():
             assert torch.equal(engines[0].grads, engines[1].grads), step
             assert torch.equal(engines[0].params, engines[1].params), step
             assert torch.equal(engines[0].bn_state, engines[1].bn_state), step
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The launch plans the tensor-core step chooses by batch size, model shape and SM budget, each against the oracle.
+def _grad_errors(g, param_info, ref, batchnorm):
+    """max |g - ref| / max |ref| per gradient tensor of the flat buffer g; ref: tensor name -> array, or a second flat
+    buffer.  Hidden biases in front of a BatchNorm are skipped: exactly zero in exact arithmetic, pure noise here."""
+    errs = {}
+    for name, off, r, c in param_info:
+        if batchnorm and name.endswith("/bias") and not name.startswith(("mean", "dispersion", "pi")):
+            continue
+        want = ref[name].reshape(-1) if isinstance(ref, dict) else ref[off: off + r * c]
+        got = g[off: off + r * c]
+        errs[name] = float(np.max(np.abs(got - want)) / (np.max(np.abs(want)) + 1e-30))
+    return errs
+
+
+# the bounds of test_tc_train_step_at_20k_genes_vs_both_oracles: loss 1e-4 relative, head tensors 3e-3 and hidden-stack
+# tensors 3e-2 of their largest element (the hidden ones sit behind the bf16 rounding of dA1 in front of the encoder
+# backward: an fp32 ulp of difference upstream can move one element of dW1 by 2^-9 of its size)
+def _assert_step_bounds(errs, tag):
+    for name, e in errs.items():
+        head = name.startswith(("mean", "dispersion", "pi"))
+        assert e < (3e-3 if head else 3e-2), (tag, name, e)
+
+
+def _fmt_errs(errs):
+    heads = max((e for n, e in errs.items() if n.startswith(("mean", "dispersion", "pi"))), default=0.0)
+    hidden = max((e for n, e in errs.items() if not n.startswith(("mean", "dispersion", "pi"))), default=0.0)
+    return "worst head %.2e, worst hidden %.2e" % (heads, hidden)
+
+
+# (B, G, batchnorm, fused hidden stack): B <= 4096 runs 32-row strips on up to 128 CTAs; 4096 < B <= 8192 128 CTAs of
+# 36-64 rows; B > 8192 the per-layer hidden kernels and the tensor-core encoder backward of that path.
+#   6001: 126 strips of 48 rows with a 1-row last strip, 47 cell blocks of 128 with a 113-row last block
+#   8192: 128 strips of 64 rows
+#   129 x 56: one partial gene tile, one cell past a block
+TC_REGIMES = [(4096, 2000, True, True), (6001, 2000, True, True), (8192, 2000, True, True), (8200, 2000, True, False),
+              (8200, 2000, False, False), (129, 56, True, True)]
+
+
+@pytest.mark.parametrize("B,G,batchnorm,fused", TC_REGIMES)
+def test_tc_train_step_batch_regimes_vs_oracle(B, G, batchnorm, fused):
+    """One tensor-core step (zinb-conddisp, row gather from a larger dataset) in every batch regime of the hidden stack
+    against the same-rounding float64 oracle: loss, every gradient tensor, and the BatchNorm moving statistics after
+    the step.  Without BatchNorm the hidden biases carry a real gradient and are compared too."""
+    N = B + 300
+    X, Y, sf = _problem(N, G, 29)
+    rows = np.random.default_rng(2).permutation(N)[:B].astype(np.int32)
+    net, eng = _make_pair_tc("zinb-conddisp", batchnorm, B, G)
+    info = eng.info()
+    assert info["tc_heads"] and info["tc_encoder"] and info["fused_hidden"] == fused, info
+    w0 = eng.get_weights()
+    eng.train_step(_t(X), _t(Y), _t(sf), rows=torch.as_tensor(rows).to(DEV))
+    loss = eng.read_loss()
+    oloss, og = net.loss_and_grads(X[rows].astype(np.float64), Y[rows].astype(np.float64), sf[rows].astype(np.float64))
+    errs = _grad_errors(eng.grads.cpu().numpy(), eng.param_info, og, batchnorm)
+    # moving statistics: recover the batch statistics from the update m' = mom * m + (1 - mom) * s of both
+    mom = O.KERAS_DEFAULTS["bn_momentum"]
+    w1 = eng.get_weights()
+    bn_err = 0.0
+    for k in (w0 if batchnorm else ()):
+        if "bn_moving" not in k:
+            continue
+        s_got = (w1[k].astype(np.float64) - mom * w0[k]) / (1 - mom)
+        s_ref = (net.params[k] - mom * w0[k]) / (1 - mom)
+        bn_err = max(bn_err, float(np.max(np.abs(s_got - s_ref)) / (np.max(np.abs(s_ref)) + 1e-30)))
+    print("\n[tc step B=%d G=%d bn=%d] loss rel %.2e, %s, batch statistics %.2e"
+          % (B, G, batchnorm, abs(loss - oloss) / abs(oloss), _fmt_errs(errs), bn_err))
+    assert abs(loss - oloss) < 1e-4 * abs(oloss), (loss, oloss)
+    _assert_step_bounds(errs, (B, G, batchnorm))
+    assert bn_err < 1e-3, bn_err
+
+
+# gemm_path="auto" picks the tensor-core heads (last hidden width 64, n_out % 8 == 0) and the tensor-core encoder (first
+# hidden width 64, n_in % 8 == 0) independently: (n_in, n_out), hidden, tc_heads, tc_encoder
+MIXED_AUTO = [((264, 264), (64, 32), False, True), ((264, 264), (32, 64), True, False), ((264, 264), (64,), True, True),
+              ((1000, 1004), (64, 32, 64), False, True), ((1004, 1000), (64, 32, 64), True, False)]
+
+
+@pytest.mark.parametrize("io,hidden,tc_heads,tc_enc", MIXED_AUTO)
+def test_auto_mixed_paths_vs_oracle(io, hidden, tc_heads, tc_enc):
+    """Models whose tensor-core encoder and heads are chosen independently by gemm_path="auto" (one side bf16 wgmma,
+    the other fp32), including a single hidden layer (L = 1, center 0) and n_in != n_out: the engine reports the path
+    it chose, and loss and gradients match the oracle that rounds exactly that side to bf16."""
+    from dca_b200.engine import DeviceEngine
+    n_in, n_out = io
+    B = 300; N = B + 40
+    X, _ = O.normalize_inputs(synth_counts(N, n_in, 33))
+    Y = synth_counts(N, n_out, 34); _, sf = O.normalize_inputs(Y)
+    rows = np.random.default_rng(5).permutation(N)[:B].astype(np.int32)
+    p0 = O.init_params(n_in, n_out, hidden, "zinb-conddisp", True, seed=3, dtype=np.float32)
+    rng = np.random.default_rng(4)
+    for k in p0:
+        if k.endswith(("/bias", "/bn_beta")):
+            p0[k] = rng.normal(0, 0.2, p0[k].shape).astype(np.float32)
+    side = {(True, True): "both", (True, False): "heads", (False, True): "encoder"}[(tc_heads, tc_enc)]
+    net = O.OracleNet(n_in, n_out, hidden, "zinb-conddisp", True, dtype=np.float64, params=p0, emulate_bf16=side)
+    eng = DeviceEngine(n_in, n_out, hidden, "zinb-conddisp", True, max_batch=B, seed=None)
+    eng.set_weights(p0)
+    info = eng.info()
+    assert (info["tc_heads"], info["tc_encoder"]) == (tc_heads, tc_enc), info
+    eng.train_step(_t(X), _t(Y), _t(sf), rows=torch.as_tensor(rows).to(DEV))
+    loss = eng.read_loss()
+    oloss, og = net.loss_and_grads(X[rows].astype(np.float64), Y[rows].astype(np.float64), sf[rows].astype(np.float64))
+    errs = _grad_errors(eng.grads.cpu().numpy(), eng.param_info, og, True)
+    print("\n[auto %s hidden %s: bf16 %s] loss rel %.2e, %s" % (io, hidden, side, abs(loss - oloss) / abs(oloss), _fmt_errs(errs)))
+    assert abs(loss - oloss) < 1e-4 * abs(oloss), (loss, oloss)
+    _assert_step_bounds(errs, (io, hidden))
+
+
+DP_CONFIGS = {"defaults": {}, "reserve_sms_32": {"DCA_DP_RESERVE_SMS": "32"},
+              # 132 - 100 = 32 CTAs cannot hold 4096 rows in 64-row strips: 64 CTAs of 64 rows instead of 128 of 32
+              "reserve_sms_100": {"DCA_DP_RESERVE_SMS": "100"}, "split_heads": {"DCA_DP_SPLIT_HEADS": "1"}}
+
+
+@pytest.fixture(scope="module")
+def dp_plain_and_oracle():
+    """dca_train_step and the same-rounding oracle on the problem of tests/run_dp_one_rank.py (computed once)."""
+    from dca_b200.engine import DeviceEngine
+    from tests.run_dp_one_rank import problem, B, G, HIDDEN
+    X, Y, sf, rows, p0 = problem()
+    eng = DeviceEngine(G, G, HIDDEN, "zinb-conddisp", True, max_batch=B, seed=None)
+    eng.set_weights(p0)
+    eng.train_step(_t(X), _t(Y), _t(sf), rows=torch.as_tensor(rows).to(DEV))
+    torch.cuda.synchronize()
+    plain = {"grads": eng.grads.cpu().numpy(), "bn_state": eng.bn_state.cpu().numpy(), "P": eng.n_params,
+             "head_bucket": eng.head_bucket, "param_info": eng.param_info}
+    eng.close()
+    net = O.OracleNet(G, G, HIDDEN, "zinb-conddisp", True, dtype=np.float64, params=p0, emulate_bf16=True)
+    oloss, og = net.loss_and_grads(X[rows].astype(np.float64), Y[rows].astype(np.float64), sf[rows].astype(np.float64))
+    return plain, oloss, og
+
+
+@pytest.mark.parametrize("config", list(DP_CONFIGS))
+def test_dp_step_one_rank_launch_plans_vs_plain_step_and_oracle(config, dp_plain_and_oracle, tmp_path):
+    """dca_train_step_dp on a one-rank communicator (B = 4096, G = 2000) with the default launch plan, SMs reserved for
+    the collective (32: a narrower hidden-stack backward grid whose strips differ from the forward's; 100: 64-row
+    strips) and one head-backward launch per head.  Each runs in its own process (the switches are read once).
+    Three calls (direct, graph capture, replay) give the same bits; the BatchNorm state and the head gradients (the
+    phase before the reserve applies; per-head launches own the same dW / db elements as one launch) equal the plain
+    step's bits; the default plan equals it everywhere; the rest is within the step bounds of the plain step and of
+    the oracle."""
+    plain, oloss, og = dp_plain_and_oracle
+    env = {k: v for k, v in os.environ.items() if not k.startswith("DCA_DP_")}
+    env.update(DP_CONFIGS[config])
+    out = tmp_path / "dp.npz"
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    r = subprocess.run([sys.executable, os.path.join(root, "tests", "run_dp_one_rank.py"), str(out)], env=env, cwd=root,
+                       capture_output=True, text=True, timeout=900)
+    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
+    d = np.load(out)
+    runs = d["grads"]
+    assert int(d["step_graphs"]) >= 1
+    for it in (1, 2):
+        assert np.array_equal(runs[it], runs[0]), (config, "call %d differs from the direct call" % it)
+    g, P, hb = runs[0], plain["P"], plain["head_bucket"]
+    assert np.array_equal(d["bn_state"], plain["bn_state"]), config
+    assert np.array_equal(g[hb:], plain["grads"][hb:]), config            # head kernels / biases, loss slot, flag
+    if config == "defaults":
+        assert np.array_equal(g, plain["grads"])
+    loss = float(g[P])
+    e_plain = _grad_errors(g, plain["param_info"], plain["grads"], True)
+    e_oracle = _grad_errors(g, plain["param_info"], og, True)
+    print("\n[dp one rank, %s] vs plain step: %s; vs oracle: loss rel %.2e, %s"
+          % (config, _fmt_errs(e_plain), abs(loss - oloss) / abs(oloss), _fmt_errs(e_oracle)))
+    assert abs(loss - oloss) < 1e-4 * abs(oloss), (loss, oloss)
+    _assert_step_bounds(e_plain, (config, "plain"))
+    _assert_step_bounds(e_oracle, (config, "oracle"))

@@ -121,3 +121,35 @@ def test_fit_keras_semantics_history_keys():
     net = O.OracleNet(12, 12, (4, 2, 4), "nb-conddisp", True)
     h = O.fit(net, X, Y, sf, epochs=3, batch_size=8)
     assert set(h) == {"loss", "val_loss", "lr"} and len(h["loss"]) == 3 and len(h["val_loss"]) == 3
+
+
+def test_oracle_bf16_emulation_per_side():
+    """emulate_bf16 rounds the encoder side (X, first kernel, dA of the first layer), the head side (last hidden
+    activation, head kernels, dZ), both (True) or neither (False), independently -- the engine chooses its tensor-core
+    encoder and heads independently."""
+    from tests.util import synth_counts
+    n_in, n_out, hidden, B = 24, 16, (8, 4, 8), 20
+    X, _ = O.normalize_inputs(synth_counts(B, n_in, 1))
+    Y = synth_counts(B, n_out, 2); _, sf = O.normalize_inputs(Y)
+    X, Y, sf = X.astype(np.float64), Y.astype(np.float64), sf.astype(np.float64)
+    p0 = O.init_params(n_in, n_out, hidden, "zinb-conddisp", True, seed=0)
+    nets = {s: O.OracleNet(n_in, n_out, hidden, "zinb-conddisp", True, params=p0, emulate_bf16=s)
+            for s in (True, False, "both", "none", "encoder", "heads")}
+    out = {s: n.forward(X, sf, training=True) for s, n in nets.items()}
+    grads = {s: n.loss_and_grads(X, Y, sf, update_bn=False)[1] for s, n in nets.items()}
+    for a, b in ((True, "both"), (False, "none")):
+        for k in grads[a]:
+            assert np.array_equal(grads[a][k], grads[b][k]), (a, k)
+    # the encoder side alone decides the hidden stack's forward; the head side the heads' rounding
+    assert np.array_equal(out["encoder"]["latent"], out["both"]["latent"])
+    assert np.array_equal(out["heads"]["latent"], out["none"]["latent"])
+    assert not np.array_equal(out["encoder"]["latent"], out["none"]["latent"])
+    h = out["heads"]["decoded"]
+    zm = O.bf16_round(h) @ O.bf16_round(p0["mean/kernel"].astype(np.float64)) + p0["mean/bias"]
+    assert np.array_equal(out["heads"]["z"]["mean"], zm)
+    assert np.array_equal(out["encoder"]["z"]["mean"], out["encoder"]["decoded"] @ p0["mean/kernel"].astype(np.float64) + p0["mean/bias"])
+    # all four variants differ in the first kernel's gradient
+    g0 = [grads[s]["enc0/kernel"] for s in ("both", "none", "encoder", "heads")]
+    assert all(not np.array_equal(g0[i], g0[j]) for i in range(4) for j in range(i + 1, 4))
+    with pytest.raises(AssertionError):
+        O.OracleNet(n_in, n_out, hidden, "zinb-conddisp", True, params=p0, emulate_bf16="decoder")
