@@ -104,6 +104,8 @@ PROTOTYPES = {
     "dca_dense_heads_fwd": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                       _vp, _vp, _vp, _i64, _vp]),
     "dca_tc_heads_fwd": (C.c_int, [_vp, _i32, _vp, _vp, _i32, _i32, C.POINTER(_i32 * 3), _vp, _vp, _vp, _vp, _i64, _vp]),
+    "dca_tc_heads_loss": (C.c_int, [_vp, _i32, _vp, _vp, _i32, _vp, _i64, _vp, _vp, _f, _f, _vp, _vp, _vp, _i64, _vp,
+                                    _vp, _sz, _vp]),
     "dca_tc_gene_gemm": (C.c_int, [_i32, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32,
                                    _vp, _vp, _vp, _vp]),
     "dca_tc_gene_gemm_sms": (C.c_int, [_i32, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64,

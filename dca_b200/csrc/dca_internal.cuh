@@ -141,6 +141,20 @@ extern int g_fused_heads_default;       // dca_set_tunable("fused_heads", 0 | 1)
 const float* loss_log_fact_table();      // device table of log(k!), k < 64 (filled on first use)
 int zinb_loss_fwd_bwd(const LossArgs& a, cudaStream_t s);
 int zinb_loss_fwd(const LossArgs& a, cudaStream_t s);
+
+// heads + loss kernel of the zinb-conddisp tensor-core training step (zinb_loss.cu): the dZ of
+// heads_fwd_tc -> zinb_loss_fwd_bwd (bf16 gradients) bit for bit, without the fp32 head outputs
+struct HeadsLossArgs {
+  const __nv_bfloat16* H3; int B, G;                   // H3: bf16 [B x 64]
+  const __nv_bfloat16* W[3]; const float* bias[3];     // mean, dispersion, pi: bf16 [64 x G] (Keras layout), float[G]
+  const float* Y; int64_t ldy; const int32_t* rows; const float* sf;
+  float ridge, inv_n;
+  __nv_bfloat16* dz[3]; int64_t ldz;                   // dL/dz of the three heads
+  double* loss_sum; void* ws; size_t ws_bytes;         // ws: loss_workspace_bytes
+  int counter_ready = 0;
+  float* fin_loss_slot = nullptr; double* fin_epoch_acc = nullptr; const double* fin_penalty = nullptr; int fin_batch = 0;
+};
+int heads_loss_tc(const HeadsLossArgs& a, cudaStream_t s);
 // writes grads[P] = loss_sum*inv_n + penalty, grads[P+1] = nonfinite flag, epoch acc update
 
 }  // namespace dca

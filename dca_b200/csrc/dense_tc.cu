@@ -175,14 +175,7 @@ heads_fwd_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constan
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
   mbar_wait(&full_bar, 0);
-  const uint32_t a0 = smem_u32(smem) + wg * 64 * 128, b0 = smem_u32(smem) + kABytes;
-  wgmma_fence();
-#pragma unroll
-  for (int k = 0; k < BK / 16; ++k)
-    wgmma_m64n128k16<0, 1>(acc, make_smem_desc(a0 + k * 32, 0, 1024), make_smem_desc(b0 + k * 2048, kBBytes / 2, 1024), k > 0);
-  wgmma_commit();
-  wgmma_wait<0>();
-  acc_fence(acc);
+  head_tile_mma(acc, smem_u32(smem) + wg * 64 * 128, smem_u32(smem) + kABytes);
   float* out = p.out[hs];
   auto emit = [&](auto act) {
 #pragma unroll
@@ -195,13 +188,13 @@ heads_fwd_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constan
         const int col = col0 + 8 * c;
         if (col < p.G)      // G % 8 == 0: the pair is all in or all out
           *reinterpret_cast<float2*>(orow + col) =
-              make_float2(act(acc[4 * c + 2 * h] + bz[c].x, rs[h]), act(acc[4 * c + 2 * h + 1] + bz[c].y, rs[h]));
+              make_float2(act(acc[4 * c + 2 * h], bz[c].x, rs[h]), act(acc[4 * c + 2 * h + 1], bz[c].y, rs[h]));
       }
     }
   };
-  if (kind == EPI_MEAN_ACT) emit([](float z, float s) { return act_mean(z) * s; });
-  else if (kind == EPI_DISP_ACT) emit([](float z, float) { return act_disp(z); });
-  else emit([](float z, float) { return act_sigmoid(z); });
+  if (kind == EPI_MEAN_ACT) emit([](float a, float b, float s) { return head_out<EPI_MEAN_ACT>(a, b, s); });
+  else if (kind == EPI_DISP_ACT) emit([](float a, float b, float s) { return head_out<EPI_DISP_ACT>(a, b, s); });
+  else emit([](float a, float b, float s) { return head_out<EPI_SIGMOID>(a, b, s); });
 }
 }  // namespace k2
 

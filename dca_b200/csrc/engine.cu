@@ -493,10 +493,23 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
                               loss_ws_bytes, d(o_acc) + 4, any_pen ? d(o_acc) + 5 : nullptr, gp(P), d(o_acc), Bn, lf_dev,
                               sm_count, s));
   } else {
-  DCA_TRY(heads_forward(Bn, Mb, cond ? Db : nullptr, has_pi ? Pb : nullptr, G, nullptr, s));
+  // zinb-conddisp on the tensor-core heads: the head activations are computed inside the loss kernel (zinb_loss.cu,
+  // heads_loss_kernel) and never stored; the heads_fwd profile phase stays, empty
+  const bool heads_loss = tc_heads && cond && has_pi && (ldy % 4 == 0) && ((reinterpret_cast<uintptr_t>(Y) & 15) == 0);
+  if (!heads_loss) DCA_TRY(heads_forward(Bn, Mb, cond ? Db : nullptr, has_pi ? Pb : nullptr, G, nullptr, s));
   if (!cond) DCA_TRY(theta_prepare(pp(theta_off), G, f(o_theta), f(o_chain), s));
   mark(2, s);
 
+  if (heads_loss) {
+    HeadsLossArgs ha{};
+    ha.H3 = bf(o_h3b); ha.B = Bn; ha.G = G;
+    for (int k = 0; k < 3; ++k) { ha.W[k] = bf(o_pbf) + head_W[slot_head[k]]; ha.bias[k] = pp(head_b[slot_head[k]]); ha.dz[k] = bf(o_dzb[k]); }
+    ha.Y = Y; ha.ldy = ldy; ha.rows = rows; ha.sf = sf; ha.ridge = cfg.ridge; ha.inv_n = inv_n; ha.ldz = G;
+    ha.loss_sum = d(o_acc) + 4; ha.ws = base + o_lossws; ha.ws_bytes = loss_ws_bytes;
+    ha.counter_ready = 1;
+    ha.fin_loss_slot = gp(P); ha.fin_epoch_acc = d(o_acc); ha.fin_penalty = any_pen ? d(o_acc) + 5 : nullptr; ha.fin_batch = Bn;
+    DCA_TRY(heads_loss_tc(ha, s));
+  } else {
   LossArgs la{};
   la.Y = Y; la.ldy = ldy; la.rows = rows; la.sf = sf;
   la.m = Mb; la.d = cond ? Db : f(o_theta); la.pi = has_pi ? Pb : nullptr; la.ld = G;
@@ -516,6 +529,7 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
     // dtheta currently holds sum over rows of dL/dtheta (not / N)
     DCA_TRY(theta_grad_finish(f(o_dtheta), f(o_chain), G, inv_n, gp(theta_off), s));
   }
+  }  // !heads_loss
 
   // ---- head backward
   mark(3, s);

@@ -3,6 +3,7 @@
 // the head-forward kernel (dense_tc.cu) and the fused head/loss/backward kernel (flash_zinb.cu) so that both
 // produce bit-identical head outputs.
 #pragma once
+#include "dca_internal.cuh"
 #include "tc_common.cuh"
 
 namespace dca {
@@ -18,6 +19,30 @@ __device__ __forceinline__ float act_disp(float z) {
   return fminf(fmaxf(sp, 1e-4f), 1e4f);
 }
 __device__ __forceinline__ float act_sigmoid(float z) { return rcpf(1.0f + ex2f(-z * 1.442695041f)); }
+
+// Pre-activations of one 64-cell x 128-gene head tile, issued by one warpgroup: H (K-major, 64 rows of 128 B, SWIZZLE_128B,
+// 32 B per k16 step) times W (MN-major, the Keras [64 k][genes] layout as two 64-gene boxes 8 KB apart, 2 KB per k16 step),
+// four k16 steps from a zero accumulator.  Shared by the head-forward kernel (dense_tc.cu) and the head+loss kernel
+// (zinb_loss.cu) so that both see the same accumulators bit for bit.
+__device__ __forceinline__ void head_tile_mma(float (&acc)[64], uint32_t h_smem, uint32_t w_smem) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    wgmma_m64n128k16<0, 1>(acc, make_smem_desc(h_smem + k * 32, 0, 1024), make_smem_desc(w_smem + k * 2048, 8192, 1024), k > 0);
+  wgmma_commit();
+  wgmma_wait<0>();
+  acc_fence(acc);
+}
+
+// Epilogue of one head output: activation of (accumulator + bias), MeanAct scaled by the row's scale (1 in training).
+// KIND: EPI_MEAN_ACT / EPI_DISP_ACT / EPI_SIGMOID.
+template <int KIND>
+__device__ __forceinline__ float head_out(float acc, float bias, float row_scale) {
+  const float z = acc + bias;
+  if (KIND == EPI_MEAN_ACT) return act_mean(z) * row_scale;
+  if (KIND == EPI_DISP_ACT) return act_disp(z);
+  return act_sigmoid(z);
+}
 
 }  // namespace tc
 }  // namespace dca

@@ -11,6 +11,7 @@
 #include <string>
 #include "zinb_math.cuh"
 #include "tc_common.cuh"
+#include "head_act.cuh"
 #include <cstdlib>
 
 namespace dca {
@@ -511,6 +512,138 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
+// One row of one warp's 128-gene group: lane owns genes 4 lane .. 4 lane + 3 (vy / vm / vd / vp; const-disp: vd = theta of
+// those genes), lanes past G carry a duplicate of the last valid vector and are !active.  The unit of the plain / general
+// decision below is this warp and row, so every kernel that calls this function rounds every element the same way.
+// q: the warp's queue of 128 items (16 B); refill() runs once the queued operands are in shared memory.  Returns the
+// finished gradients (dzm, dzd, dzp of genes 0,1 | 2,3); accumulates the loss terms and (const-disp) the raw dL/dtheta.
+struct RowGrads { float2 gmA, gmB, gdA, gdB, gpA, gpB; };
+
+template <bool COND_DISP, class Refill>
+__device__ __forceinline__ RowGrads zinb_row_ring(const float4 vy, const float4 vm, const float4 vd, const float4 vp, const float row_sf,
+                                                  const bool active, const float ridge, const float inv_n, float4* q,
+                                                  const float* lf, float& lsum_lg, float& lsum_nb, float& lsum_r,
+                                                  float (&tacc)[kVec], Refill refill) {
+  using Ops = zmath::FastOps;
+  using namespace zmath;
+  constexpr unsigned kFull = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const unsigned lt = (1u << lane) - 1u;
+  const float y[kVec] = {vy.x, vy.y, vy.z, vy.w};
+  const float2 mA = make_float2(vm.x, vm.y), mB = make_float2(vm.z, vm.w);
+  const float2 dA = make_float2(vd.x, vd.y), dB = make_float2(vd.z, vd.w);
+  const float2 pA = make_float2(vp.x, vp.y), pB = make_float2(vp.z, vp.w);
+  const float2 muA = mul2(mA, splat(row_sf)), muB = mul2(mB, splat(row_sf));        // dca/layers.py:85
+  const float mu[kVec] = {muA.x, muA.y, muB.x, muB.y};
+  const float dd[kVec] = {dA.x, dA.y, dB.x, dB.y};
+  const float pp[kVec] = {pA.x, pA.y, pB.x, pB.y};
+  // ---- queue the non-zero counts of this warp's strip (ballot compaction: items ordered by j, then lane)
+  bool isnz[kVec];
+  int pos[kVec], base = 0;
+#pragma unroll
+  for (int j = 0; j < kVec; ++j) {
+    isnz[j] = active && !(y[j] < 1e-8f);                           // loss.py:138
+    const unsigned bal = __ballot_sync(kFull, isnz[j]);
+    pos[j] = base + __popc(bal & lt); base += __popc(bal);
+  }
+  const int total = base;
+#pragma unroll
+  for (int j = 0; j < kVec; ++j)
+    if (isnz[j]) q[pos[j]] = make_float4(y[j], mu[j], dd[j], pp[j]);
+  __syncwarp();
+  refill();
+  // ---- zero branch of my four elements, two f32x2 chains.  One range test per thread and row (min / max over its four
+  // genes, FMNMX3) decides warp-uniformly whether the clip masks / the small-theta series can be skipped.
+  const float m_lo = fminf(fminf(vm.x, vm.y), fminf(vm.z, vm.w)), m_hi = fmaxf(fmaxf(vm.x, vm.y), fmaxf(vm.z, vm.w));
+  const float d_lo = fminf(fminf(dd[0], dd[1]), fminf(dd[2], dd[3])), d_hi = fmaxf(fmaxf(dd[0], dd[1]), fmaxf(dd[2], dd[3]));
+  const bool plain = (m_lo > 1e-5f) && (m_hi < 1e6f) &&
+                     (COND_DISP ? (d_lo > 0.03125f) && (d_hi < 1e4f) : (d_hi <= 1e6f));   // const-disp: theta is not an activation
+  Raw2 zA, zB; Fin2 fA, fB;
+  if (__all_sync(kFull, plain)) {
+    zA = zinb_zero_pair<Ops, true>(muA, dA, pA); zB = zinb_zero_pair<Ops, true>(muB, dB, pB);
+    fA = finish_factors_pair_plain<Ops, COND_DISP>(dA, pA, inv_n); fB = finish_factors_pair_plain<Ops, COND_DISP>(dB, pB, inv_n);
+  } else {
+    zA = zinb_zero_pair<Ops>(muA, dA, pA); zB = zinb_zero_pair<Ops>(muB, dB, pB);
+    fA = finish_factors_pair<Ops, COND_DISP>(mA, dA, pA, inv_n); fB = finish_factors_pair<Ops, COND_DISP>(mB, dB, pB, inv_n);
+  }
+  lsum_lg += ((active && !isnz[0]) ? zA.lgD.x : 0.f) + ((active && !isnz[1]) ? zA.lgD.y : 0.f)
+           + ((active && !isnz[2]) ? zB.lgD.x : 0.f) + ((active && !isnz[3]) ? zB.lgD.y : 0.f);
+  // ---- dense NB pass over the queue (item k by lane k mod 32): raw derivatives back into the queue
+  for (int k = lane; k < total; k += 32) {
+    const float4 it = q[k];
+    const Raw1 e = zinb_nb_raw<Ops>(it.x, it.y, it.z, it.w, lf);
+    lsum_nb += e.loss;
+    q[k] = make_float4(e.gmu, e.dth, e.dpi, 0.f);
+  }
+  __syncwarp();
+  if (isnz[0]) { const float4 e = q[pos[0]]; zA.gmu.x = e.x; zA.dth.x = e.y; zA.dpi.x = e.z; }
+  if (isnz[1]) { const float4 e = q[pos[1]]; zA.gmu.y = e.x; zA.dth.y = e.y; zA.dpi.y = e.z; }
+  if (isnz[2]) { const float4 e = q[pos[2]]; zB.gmu.x = e.x; zB.dth.x = e.y; zB.dpi.x = e.z; }
+  if (isnz[3]) { const float4 e = q[pos[3]]; zB.gmu.y = e.x; zB.dth.y = e.y; zB.dpi.y = e.z; }
+  __syncwarp();
+  if (ridge != 0.f) {                                              // loss.py:139-140 (uniform; ridge defaults to 0)
+    if (active) lsum_r += ridge * (pA.x * pA.x + pA.y * pA.y + pB.x * pB.x + pB.y * pB.y);
+    zA.dpi = fma2(splat(2.0f * ridge), pA, zA.dpi); zB.dpi = fma2(splat(2.0f * ridge), pB, zB.dpi);
+  }
+  if (!COND_DISP && active) { tacc[0] += zA.dth.x; tacc[1] += zA.dth.y; tacc[2] += zB.dth.x; tacc[3] += zB.dth.y; }
+  RowGrads g;
+  g.gmA = mul2(zA.gmu, fA.fm); g.gmB = mul2(zB.gmu, fB.fm);
+  g.gdA = mul2(zA.dth, fA.fd); g.gdB = mul2(zB.dth, fB.fd);
+  g.gpA = mul2(zA.dpi, fA.fp); g.gpB = mul2(zB.dpi, fB.fp);
+  return g;
+}
+
+// Block sum of the per-thread loss terms into loss_partial[block]; the last block to finish folds the per-block partials
+// in a FIXED order (deterministic) and finalises the loss slot.  Called by all NT threads of the block.
+template <int NT>
+__device__ __forceinline__ void block_loss_fold(double dsum, double* red, int* s_last, double* __restrict__ loss_partial,
+                                                const FoldArgs& fa, float inv_n) {
+  constexpr unsigned kFull = 0xffffffffu;
+  constexpr int kWarps = NT / 32;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) dsum += __shfl_xor_sync(kFull, dsum, o);
+  if (lane == 0) red[warp] = dsum;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) t += red[w];
+    loss_partial[blockIdx.y * gridDim.x + blockIdx.x] = t;
+    __threadfence();
+    const unsigned nblk = gridDim.x * gridDim.y;
+    const unsigned done = atomicAdd(fa.counter, 1u);
+    *s_last = (done == nblk - 1);
+    if (*s_last) *fa.counter = 0;                                      // self-resetting
+  }
+  __syncthreads();
+  if (!*s_last) return;
+  __threadfence();
+  const int n = gridDim.x * gridDim.y;
+  double a = 0.0;
+  for (int i = threadIdx.x; i < n; i += NT) a += __ldcg(loss_partial + i);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(kFull, a, o);
+  __syncthreads();
+  if (lane == 0) red[warp] = a;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) t += red[w];
+    *fa.loss_sum = t;
+    if (fa.loss_slot) {
+      double l = t * (double)inv_n;
+      if (l != l) l = INFINITY;                                        // _nan2inf, dca/loss.py:148
+      if (fa.penalty) l += *fa.penalty;
+      const float lf32 = (float)l;
+      fa.loss_slot[0] = lf32;
+      fa.loss_slot[1] = (isfinite(lf32)) ? 0.f : 1.f;
+      if (fa.epoch_acc) { fa.epoch_acc[0] += l * (double)fa.batch; fa.epoch_acc[1] += (double)fa.batch; }
+    }
+  }
+}
+
 // IDXQ (tunable loss_ring = 2): the queue of non-zero counts holds one-byte ELEMENT INDICES instead of 16-byte operand
 // copies -- the evaluating lane reads y / m / d / pi of the element from the staging slot itself and writes the three raw
 // derivatives back in place, the owner re-reads its vector -- which frees 15 KB of shared memory for a fourth ring slot.
@@ -608,20 +741,27 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
       cp_async_wait<RING - 1>();                                       // my copies of row i have landed
       const uint32_t cslot = rslot, wstrip = rslot - (uint32_t)lane * 16u;       // my vector / my warp's strip in this slot
       const float4 vy = lds128(rslot), vm = lds128(rslot + kSegBytes);
-      const float4 vd = COND_DISP ? lds128(rslot + 2 * kSegBytes) : make_float4(0.f, 0.f, 0.f, 0.f);
+      const float4 vd = COND_DISP ? lds128(rslot + 2 * kSegBytes) : make_float4(thg[0], thg[1], thg[2], thg[3]);
       const float4 vp = lds128(rslot + (kArrays - 1) * kSegBytes);
       rslot += kSlotBytes;
       if (rslot == ring_end) rslot = my;
       const float row_sf = s_sf[i];
+      if constexpr (!IDXQ) {
+        // refill: the operands of row i have been consumed (they fed the ballots / the queue): stream row i + kRing
+        const RowGrads g = zinb_row_ring<COND_DISP>(vy, vm, vd, vp, row_sf, active, ridge, inv_n, q, lf, lsum_lg, lsum_nb,
+                                                    lsum_r, tacc, [&] { if (nxt < nrows) issue_next(); cp_async_commit(); });
+        if (active) {
+          st4(om, g.gmA.x, g.gmA.y, g.gmB.x, g.gmB.y);
+          if (COND_DISP) st4(od, g.gdA.x, g.gdA.y, g.gdB.x, g.gdB.y);
+          st4(op, g.gpA.x, g.gpA.y, g.gpB.x, g.gpB.y);
+        }
+      } else {
       const float y[kVec] = {vy.x, vy.y, vy.z, vy.w};
       const float2 mA = make_float2(vm.x, vm.y), mB = make_float2(vm.z, vm.w);
-      const float2 dA = COND_DISP ? make_float2(vd.x, vd.y) : make_float2(thg[0], thg[1]);
-      const float2 dB = COND_DISP ? make_float2(vd.z, vd.w) : make_float2(thg[2], thg[3]);
+      const float2 dA = make_float2(vd.x, vd.y), dB = make_float2(vd.z, vd.w);
       const float2 pA = make_float2(vp.x, vp.y), pB = make_float2(vp.z, vp.w);
       const float2 muA = mul2(mA, splat(row_sf)), muB = mul2(mB, splat(row_sf));        // dca/layers.py:85
-      const float mu[kVec] = {muA.x, muA.y, muB.x, muB.y};
       const float dd[kVec] = {dA.x, dA.y, dB.x, dB.y};
-      const float pp[kVec] = {pA.x, pA.y, pB.x, pB.y};
       // ---- queue the non-zero counts of this warp's strip (ballot compaction: items ordered by j, then lane)
       bool isnz[kVec];
       int pos[kVec], base = 0;
@@ -634,15 +774,9 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
       const int total = base;
 #pragma unroll
       for (int j = 0; j < kVec; ++j)
-        if (isnz[j]) { if (IDXQ) qb[pos[j]] = (unsigned char)(lane * kVec + j); else q[pos[j]] = make_float4(y[j], mu[j], dd[j], pp[j]); }
+        if (isnz[j]) qb[pos[j]] = (unsigned char)(lane * kVec + j);
       __syncwarp();
-      if (!IDXQ) {
-        // the operands of row i have been consumed (they fed the ballots / the queue): refill my slot with row i + kRing
-        if (nxt < nrows) issue_next();
-        cp_async_commit();
-      }
-      // ---- zero branch of my four elements, two f32x2 chains.  One range test per thread and row (min / max over its four
-      // genes, FMNMX3) decides warp-uniformly whether the clip masks / the small-theta series can be skipped.
+      // ---- zero branch of my four elements (as in zinb_row_ring)
       const float m_lo = fminf(fminf(vm.x, vm.y), fminf(vm.z, vm.w)), m_hi = fmaxf(fmaxf(vm.x, vm.y), fmaxf(vm.z, vm.w));
       const float d_lo = fminf(fminf(dd[0], dd[1]), fminf(dd[2], dd[3])), d_hi = fmaxf(fmaxf(dd[0], dd[1]), fmaxf(dd[2], dd[3]));
       const bool plain = (m_lo > 1e-5f) && (m_hi < 1e6f) &&
@@ -657,40 +791,25 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
       }
       lsum_lg += ((active && !isnz[0]) ? zA.lgD.x : 0.f) + ((active && !isnz[1]) ? zA.lgD.y : 0.f)
                + ((active && !isnz[2]) ? zB.lgD.x : 0.f) + ((active && !isnz[3]) ? zB.lgD.y : 0.f);
-      // ---- dense NB pass over the queue (item k by lane k mod 32): raw derivatives back into the queue
-      if (IDXQ) {
-        for (int k = lane; k < total; k += 32) {
-          const int idx = qb[k];
-          const uint32_t e4 = wstrip + (uint32_t)idx * 4u;
-          const float th = COND_DISP ? lds32(e4 + 2 * kSegBytes) : __ldg(d + c0 + warp * (32 * kVec) + idx);
-          const Raw1 e = zinb_nb_raw<Ops>(lds32(e4), lds32(e4 + kSegBytes) * row_sf, th, lds32(e4 + (kArrays - 1) * kSegBytes), lf);
-          lsum_nb += e.loss;
-          sts32(e4, e.gmu); sts32(e4 + kSegBytes, e.dth); sts32(e4 + (kArrays - 1) * kSegBytes, e.dpi);   // in place of y, m, pi
-        }
-        __syncwarp();
-        const float4 r0v = lds128(cslot), r1v = lds128(cslot + kSegBytes), r2v = lds128(cslot + (kArrays - 1) * kSegBytes);
-        zA.gmu.x = isnz[0] ? r0v.x : zA.gmu.x; zA.dth.x = isnz[0] ? r1v.x : zA.dth.x; zA.dpi.x = isnz[0] ? r2v.x : zA.dpi.x;
-        zA.gmu.y = isnz[1] ? r0v.y : zA.gmu.y; zA.dth.y = isnz[1] ? r1v.y : zA.dth.y; zA.dpi.y = isnz[1] ? r2v.y : zA.dpi.y;
-        zB.gmu.x = isnz[2] ? r0v.z : zB.gmu.x; zB.dth.x = isnz[2] ? r1v.z : zB.dth.x; zB.dpi.x = isnz[2] ? r2v.z : zB.dpi.x;
-        zB.gmu.y = isnz[3] ? r0v.w : zB.gmu.y; zB.dth.y = isnz[3] ? r1v.w : zB.dth.y; zB.dpi.y = isnz[3] ? r2v.w : zB.dpi.y;
-        __syncwarp();
-        // the slot has been read back by its owners: refill it with row i + RING
-        if (nxt < nrows) issue_next();
-        cp_async_commit();
-      } else {
+      // ---- dense NB pass over the queue (item k by lane k mod 32): raw derivatives back into the staging slot
       for (int k = lane; k < total; k += 32) {
-        const float4 it = q[k];
-        const Raw1 e = zinb_nb_raw<Ops>(it.x, it.y, it.z, it.w, lf);
+        const int idx = qb[k];
+        const uint32_t e4 = wstrip + (uint32_t)idx * 4u;
+        const float th = COND_DISP ? lds32(e4 + 2 * kSegBytes) : __ldg(d + c0 + warp * (32 * kVec) + idx);
+        const Raw1 e = zinb_nb_raw<Ops>(lds32(e4), lds32(e4 + kSegBytes) * row_sf, th, lds32(e4 + (kArrays - 1) * kSegBytes), lf);
         lsum_nb += e.loss;
-        q[k] = make_float4(e.gmu, e.dth, e.dpi, 0.f);
+        sts32(e4, e.gmu); sts32(e4 + kSegBytes, e.dth); sts32(e4 + (kArrays - 1) * kSegBytes, e.dpi);   // in place of y, m, pi
       }
       __syncwarp();
-      if (isnz[0]) { const float4 e = q[pos[0]]; zA.gmu.x = e.x; zA.dth.x = e.y; zA.dpi.x = e.z; }
-      if (isnz[1]) { const float4 e = q[pos[1]]; zA.gmu.y = e.x; zA.dth.y = e.y; zA.dpi.y = e.z; }
-      if (isnz[2]) { const float4 e = q[pos[2]]; zB.gmu.x = e.x; zB.dth.x = e.y; zB.dpi.x = e.z; }
-      if (isnz[3]) { const float4 e = q[pos[3]]; zB.gmu.y = e.x; zB.dth.y = e.y; zB.dpi.y = e.z; }
+      const float4 r0v = lds128(cslot), r1v = lds128(cslot + kSegBytes), r2v = lds128(cslot + (kArrays - 1) * kSegBytes);
+      zA.gmu.x = isnz[0] ? r0v.x : zA.gmu.x; zA.dth.x = isnz[0] ? r1v.x : zA.dth.x; zA.dpi.x = isnz[0] ? r2v.x : zA.dpi.x;
+      zA.gmu.y = isnz[1] ? r0v.y : zA.gmu.y; zA.dth.y = isnz[1] ? r1v.y : zA.dth.y; zA.dpi.y = isnz[1] ? r2v.y : zA.dpi.y;
+      zB.gmu.x = isnz[2] ? r0v.z : zB.gmu.x; zB.dth.x = isnz[2] ? r1v.z : zB.dth.x; zB.dpi.x = isnz[2] ? r2v.z : zB.dpi.x;
+      zB.gmu.y = isnz[3] ? r0v.w : zB.gmu.y; zB.dth.y = isnz[3] ? r1v.w : zB.dth.y; zB.dpi.y = isnz[3] ? r2v.w : zB.dpi.y;
       __syncwarp();
-      }
+      // the slot has been read back by its owners: refill it with row i + RING
+      if (nxt < nrows) issue_next();
+      cp_async_commit();
       if (ridge != 0.f) {                                              // loss.py:139-140 (uniform; ridge defaults to 0)
         if (active) lsum_r += ridge * (pA.x * pA.x + pA.y * pA.y + pB.x * pB.x + pB.y * pB.y);
         zA.dpi = fma2(splat(2.0f * ridge), pA, zA.dpi); zB.dpi = fma2(splat(2.0f * ridge), pB, zB.dpi);
@@ -706,6 +825,7 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
         }
         st4(op, gpA.x, gpA.y, gpB.x, gpB.y);
       }
+      }
       om += ld; op += ld;
       if (COND_DISP) od += ld;
     }
@@ -715,48 +835,177 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
     }
   }
   // ---- block reduction, then the last block to finish folds the per-block partials in a FIXED order
-  double dsum = (double)lsum_nb + (double)lsum_r - (double)kLn2 * (double)lsum_lg;       // -log D = -ln2 * lg2 D
+  block_loss_fold<kThreads>((double)lsum_nb + (double)lsum_r - (double)kLn2 * (double)lsum_lg,   // -log D = -ln2 * lg2 D
+                            red, &s_last, loss_partial, fa, inv_n);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Heads + loss kernel (zinb-conddisp, tensor-core training step): the head pre-activations are computed where the loss is
+// computed, so the fp32 mean / dispersion / pi never reach HBM.  Per element the kernel moves the count (4 B in) and the
+// three bf16 gradients (6 B out); H3 and the head weights are re-read from L2.
+//
+// One CTA = three warpgroups sharing the bf16 weights of one 128-gene tile (3 x 16 KB, TMA).  A CTA owns a contiguous range
+// of (gene tile, 64-cell block) units, tile-major; its warpgroups take the blocks of a tile in turn.  Per block a warpgroup
+// loads H3 (TMA, 8 KB) and, for each of the two 8-row halves of its warps' accumulator fragments ("pieces"), runs the three
+// m64n128 products of head_tile_mma (the same products and epilogue as heads_fwd_kernel, so the activations are bit-identical
+// to K2's outputs), keeps the fragment rows of the piece and stages their activations in warp-private shared memory
+// (8 rows x 128 genes x 3 heads, fp32).  The warp then walks its 8 rows with zinb_row_ring -- the per-row body of the ring
+// kernel, with the same warp / lane / 128-gene mapping -- and stores bf16 dZ.  Recomputing the products for the second
+// piece costs tensor time the kernel has to spare and halves the staging, which is what fits three warpgroups on an SM.
+namespace hl {
+constexpr int kWG = 3;                                       // warpgroups per CTA
+constexpr int kCtaThreads = 128 * kWG;
+constexpr int kRows = 8;                                     // rows per warp and piece
+constexpr uint32_t kWHeadBytes = 64 * 128 * 2;               // one head's W tile: two 64-gene boxes of [64 k][64 genes] bf16
+constexpr uint32_t kHBytes = 64 * 64 * 2;                    // one 64-cell H3 block
+constexpr uint32_t kRowBytes = 3 * 128 * 4;                  // m | d | pi of one row's 128 genes
+constexpr uint32_t kQPad = 512;                              // the NB queue of row k (2 KB) starts 512 B ahead of row k's
+constexpr uint32_t kWarpBytes = kQPad + kRows * kRowBytes;   // operands and overwrites them once they are in registers
+constexpr uint32_t kOffH = 3 * kWHeadBytes;
+constexpr uint32_t kOffStage = kOffH + kWG * kHBytes;
+constexpr uint32_t kOffBias = kOffStage + kWG * 4 * kWarpBytes;
+constexpr uint32_t kSmemBytes = kOffBias + 3 * 128 * 4 + 1024;   // + alignment of the swizzled TMA destinations
+
+struct Params {
+  const float* bias[3];
+  const float* Y; int64_t ldy; const int32_t* rows; const float* sf;
+  int B, G, nblk; long long units;
+  float ridge, inv_n;
+  __nv_bfloat16* dz[3]; int64_t ldz;
+  double* loss_partial; const float* lf;
+};
+
+// float4 slot of genes 4i..4i+3 in staged row k: XOR-swizzled so that the fragment stores of the 8 rows of a piece spread
+// over all banks (rows are 1536 B apart, a multiple of 128 B)
+__device__ __forceinline__ uint32_t slot16(int i, int k) { return (uint32_t)((i ^ ((2 * k) & 6)) * 16); }
+
+template <int KIND>
+__device__ __forceinline__ void stage_head(const float (&acc)[64], int piece, const float* s_bias, uint8_t* rows_base) {
+  const int lane = threadIdx.x & 31, k = lane >> 2;
+  uint8_t* dst = rows_base + k * kRowBytes + (KIND == EPI_MEAN_ACT ? 0 : (KIND == EPI_DISP_ACT ? 512 : 1024)) + (lane & 1) * 8;
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) dsum += __shfl_xor_sync(kFull, dsum, o);
-  if (lane == 0) red[warp] = dsum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-#pragma unroll
-    for (int w = 0; w < kWarps; ++w) t += red[w];
-    loss_partial[blockIdx.y * gridDim.x + blockIdx.x] = t;
-    __threadfence();
-    const unsigned nblk = gridDim.x * gridDim.y;
-    const unsigned done = atomicAdd(fa.counter, 1u);
-    s_last = (done == nblk - 1);
-    if (s_last) *fa.counter = 0;                                       // self-resetting
+  for (int c = 0; c < 16; ++c) {
+    const int g = 8 * c + 2 * (lane & 3);
+    const float2 b = *reinterpret_cast<const float2*>(s_bias + g);
+    *reinterpret_cast<float2*>(dst + slot16(g >> 2, k)) =
+        make_float2(tc::head_out<KIND>(piece ? acc[4 * c + 2] : acc[4 * c], b.x, 1.0f),
+                    tc::head_out<KIND>(piece ? acc[4 * c + 3] : acc[4 * c + 1], b.y, 1.0f));
+  }
+}
+}  // namespace hl
+
+__global__ void __launch_bounds__(hl::kCtaThreads, 1)
+heads_loss_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_w0,
+                  const __grid_constant__ CUtensorMap map_w1, const __grid_constant__ CUtensorMap map_w2, const hl::Params p,
+                  const FoldArgs fa) {
+  using namespace hl;
+  using namespace tc;
+  extern __shared__ __align__(1024) uint8_t smem_hl_raw[];
+  uint8_t* smem = smem_hl_raw + ((1024u - (smem_u32(smem_hl_raw) & 1023u)) & 1023u);
+  __shared__ uint64_t w_bar, h_bar[kWG];
+  __shared__ float lf[zmath::kLogFactN];
+  __shared__ double red[kCtaThreads / 32];
+  __shared__ int s_last;
+  const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+  float* s_bias = reinterpret_cast<float*>(smem + kOffBias);
+  uint8_t* h_buf = smem + kOffH + wg * kHBytes;
+  uint8_t* wbase = smem + kOffStage + (wg * 4 + warp) * kWarpBytes;       // this warp's queue pad + 8 staged rows
+  uint8_t* rows_base = wbase + kQPad;
+  if (tid < zmath::kLogFactN) lf[tid] = p.lf[tid];
+  if (tid == 0) {
+    mbar_init(&w_bar, 1);
+    for (int g = 0; g < kWG; ++g) mbar_init(&h_bar[g], 1);
+    fence_barrier_init();
   }
   __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-  const int n = gridDim.x * gridDim.y;
-  double a = 0.0;
-  for (int i = threadIdx.x; i < n; i += kThreads) a += __ldcg(loss_partial + i);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(kFull, a, o);
-  __syncthreads();
-  if (lane == 0) red[warp] = a;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-#pragma unroll
-    for (int w = 0; w < kWarps; ++w) t += red[w];
-    *fa.loss_sum = t;
-    if (fa.loss_slot) {
-      double l = t * (double)inv_n;
-      if (l != l) l = INFINITY;                                        // _nan2inf, dca/loss.py:148
-      if (fa.penalty) l += *fa.penalty;
-      const float lf32 = (float)l;
-      fa.loss_slot[0] = lf32;
-      fa.loss_slot[1] = (isfinite(lf32)) ? 0.f : 1.f;
-      if (fa.epoch_acc) { fa.epoch_acc[0] += l * (double)fa.batch; fa.epoch_acc[1] += (double)fa.batch; }
+  const CUtensorMap* mw[3] = {&map_w0, &map_w1, &map_w2};
+  auto load_h = [&](int blk) {
+    if ((tid & 127) == 0) { mbar_expect_tx(&h_bar[wg], kHBytes); tma_load_2d(h_buf, &map_h, 0, blk * 64, &h_bar[wg]); }
+  };
+  const long long u0 = (long long)blockIdx.x * p.units / gridDim.x, u1 = (long long)(blockIdx.x + 1) * p.units / gridDim.x;
+  uint32_t w_phase = 0, h_phase = 0;
+  float lsum_lg = 0.f, lsum_nb = 0.f, lsum_r = 0.f;
+  float tacc[kVec] = {0.f, 0.f, 0.f, 0.f};
+  for (long long u = u0; u < u1;) {
+    const int t = (int)(u / p.nblk);
+    const long long seg_end = min(u1, (long long)(t + 1) * p.nblk);
+    const int b_end = (int)(seg_end - (long long)t * p.nblk);
+    int blk = (int)(u - (long long)t * p.nblk) + wg;
+    __syncthreads();                                                      // every warpgroup is done with the previous tile
+    if (tid == 0) {
+      mbar_expect_tx(&w_bar, 3 * kWHeadBytes);
+      for (int h = 0; h < 3; ++h) {
+        tma_load_2d(smem + h * kWHeadBytes, mw[h], t * 128, 0, &w_bar);
+        tma_load_2d(smem + h * kWHeadBytes + kWHeadBytes / 2, mw[h], t * 128 + 64, 0, &w_bar);
+      }
     }
+    {
+      const int gcol = t * 128 + (tid & 127);                             // 384 threads: one bias of each head each
+      s_bias[tid] = gcol < p.G ? p.bias[tid >> 7][gcol] : 0.f;
+    }
+    if (blk < b_end) load_h(blk);
+    __syncthreads();
+    mbar_wait(&w_bar, w_phase); w_phase ^= 1;
+    // my four genes; lanes past G duplicate the last valid vector (as in the ring kernel) and only their results are dropped
+    const int gvalid = min(128, p.G - t * 128);
+    const bool active = 4 * lane < gvalid;
+    const int col = active ? 4 * lane : gvalid - kVec;
+    const int64_t gcol0 = (int64_t)t * 128 + col;
+    for (; blk < b_end; blk += kWG) {
+      mbar_wait(&h_bar[wg], h_phase); h_phase ^= 1;
+      for (int piece = 0; piece < 2; ++piece) {
+        const int r0 = blk * 64 + warp * 16 + piece * kRows;              // first of this warp's 8 rows in the piece
+        int my_yr = 0; float my_sf = 1.f;                                 // lane k < 8: count row / size factor of row r0 + k
+        if (lane < kRows && r0 + lane < p.B) {
+          my_yr = p.rows ? p.rows[r0 + lane] : r0 + lane;
+          my_sf = p.sf ? p.sf[my_yr] : 1.0f;
+        }
+        float acc[64];
+        float4 yv[kRows];
+        head_tile_mma(acc, smem_u32(h_buf), smem_u32(smem));
+        stage_head<EPI_MEAN_ACT>(acc, piece, s_bias, rows_base);
+#pragma unroll
+        for (int k = 0; k < kRows; ++k) {                                 // counts of the piece, in flight under the products
+          const int yr = __shfl_sync(0xffffffffu, my_yr, k);
+          yv[k] = (r0 + k < p.B) ? ld4_stream(p.Y + (int64_t)yr * p.ldy + gcol0) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        head_tile_mma(acc, smem_u32(h_buf), smem_u32(smem) + kWHeadBytes);
+        stage_head<EPI_DISP_ACT>(acc, piece, s_bias + 128, rows_base);
+        head_tile_mma(acc, smem_u32(h_buf), smem_u32(smem) + 2 * kWHeadBytes);
+        if (piece == 1) {                                                 // the warpgroup is done with this H3 block
+          named_barrier_sync(1 + wg, 128);
+          if (blk + kWG < b_end) load_h(blk + kWG);
+        }
+        stage_head<EPI_SIGMOID>(acc, piece, s_bias + 256, rows_base);
+        __syncwarp();
+        for (int k = 0; k < kRows; ++k) {
+          const int r = r0 + k;
+          if (r >= p.B) break;                                            // warp-uniform: the last block's tail
+          const float4 vy = yv[0];
+#pragma unroll
+          for (int j = 0; j + 1 < kRows; ++j) yv[j] = yv[j + 1];
+          const float row_sf = __shfl_sync(0xffffffffu, my_sf, k);
+          const uint8_t* src = rows_base + k * kRowBytes + slot16(col >> 2, k);
+          const float4 vm = *reinterpret_cast<const float4*>(src);
+          const float4 vd = *reinterpret_cast<const float4*>(src + 512);
+          const float4 vp = *reinterpret_cast<const float4*>(src + 1024);
+          __syncwarp();                                                   // row k's queue overwrites these operands
+          float4* q = reinterpret_cast<float4*>(wbase + k * kRowBytes);
+          const RowGrads g = zinb_row_ring<true>(vy, vm, vd, vp, row_sf, active, p.ridge, p.inv_n, q, lf, lsum_lg, lsum_nb,
+                                                 lsum_r, tacc, [] {});
+          if (active) {
+            const int64_t off = (int64_t)r * p.ldz + gcol0;
+            st4(p.dz[0] + off, g.gmA.x, g.gmA.y, g.gmB.x, g.gmB.y);
+            st4(p.dz[1] + off, g.gdA.x, g.gdA.y, g.gdB.x, g.gdB.y);
+            st4(p.dz[2] + off, g.gpA.x, g.gpA.y, g.gpB.x, g.gpB.y);
+          }
+        }
+      }
+    }
+    u = seg_end;
   }
+  block_loss_fold<kCtaThreads>((double)lsum_nb + (double)lsum_r - (double)zmath::kLn2 * (double)lsum_lg, red, &s_last,
+                            p.loss_partial, fa, p.inv_n);
 }
 
 __global__ void fold_partials_kernel(const double* __restrict__ part, int n, double* out, int accumulate,
@@ -922,6 +1171,41 @@ size_t loss_workspace_bytes(int B, int G) {
 int zinb_loss_fwd_bwd(const LossArgs& a, cudaStream_t s) { return launch<true>(a, s); }
 int zinb_loss_fwd(const LossArgs& a, cudaStream_t s) { return launch<false>(a, s); }
 
+int heads_loss_tc(const HeadsLossArgs& a, cudaStream_t s) {
+  using namespace hl;
+  const int B = a.B, G = a.G;
+  auto al = [](const void* q, uintptr_t n) { return (reinterpret_cast<uintptr_t>(q) & (n - 1)) == 0; };
+  if (B <= 0 || G <= 0 || G % 8 != 0 || a.ldy % 4 != 0 || !al(a.Y, 16) || a.ldz % 4 != 0 || a.ldz < G ||
+      !al(a.dz[0], 8) || !al(a.dz[1], 8) || !al(a.dz[2], 8)) {
+    set_error("heads_loss_tc: need G %% 8 == 0, a 16-byte aligned Y with ldy %% 4 == 0 and 8-byte aligned dZ with ldz %% 4 == 0 (>= G)");
+    return DCA_ERR_BAD_ARG;
+  }
+  const float* lf_dev = log_fact_table_device();
+  if (!lf_dev) return DCA_ERR_CUDA;
+  if (!a.ws || a.ws_bytes < loss_workspace_bytes(B, G)) { set_error("heads_loss_tc: workspace too small"); return DCA_ERR_BAD_ARG; }
+  CUtensorMap mh, mw[3];
+  DCA_TRY(tc::make_tensor_map_2d(&mh, a.H3, 2, 1, (uint64_t)B, 64, 64, 64, 64, 1));
+  for (int i = 0; i < 3; ++i) DCA_TRY(tc::make_tensor_map_2d(&mw[i], a.W[i], 2, 1, 64, (uint64_t)G, (uint64_t)G, 64, 64, 1));
+  Params p;
+  for (int i = 0; i < 3; ++i) { p.bias[i] = a.bias[i]; p.dz[i] = a.dz[i]; }
+  p.Y = a.Y; p.ldy = a.ldy; p.rows = a.rows; p.sf = a.sf; p.B = B; p.G = G; p.ldz = a.ldz;
+  p.nblk = cdiv(B, 64);
+  p.units = (long long)cdiv(G, 128) * p.nblk;
+  p.ridge = a.ridge; p.inv_n = a.inv_n;
+  p.loss_partial = reinterpret_cast<double*>(a.ws); p.lf = lf_dev;
+  FoldArgs fa{reinterpret_cast<unsigned*>(reinterpret_cast<char*>(a.ws) + sizeof(double) * (size_t)kMaxBlocks), a.loss_sum,
+              a.fin_penalty, a.fin_loss_slot, a.fin_epoch_acc, a.fin_batch};
+  if (!a.counter_ready) DCA_CUDA_OK(cudaMemsetAsync(fa.counter, 0, sizeof(unsigned), s));
+  static bool attr = false;
+  if (!attr) { DCA_CUDA_OK(cudaFuncSetAttribute(heads_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes)); attr = true; }
+  // one CTA per SM, each a contiguous range of the (gene tile, cell block) units; the grid follows the device, not the
+  // caller's SM budget, so that the loss is summed in the same order whatever the budget
+  const int grid = (int)std::min<long long>(p.units, sm_count_cached());
+  heads_loss_kernel<<<grid, kCtaThreads, kSmemBytes, s>>>(mh, mw[0], mw[1], mw[2], p, fa);
+  DCA_LAUNCH_CHECK();
+  return DCA_OK;
+}
+
 }  // namespace dca
 
 // ------------------------------------------------------------------------------------ C ABI
@@ -956,6 +1240,22 @@ extern "C" int dca_zinb_loss_fwd_bwd(const float* Y, int64_t ldy, const int32_t*
   LossArgs a{Y, ldy, rows, sf, m, d, pi, ld, batch, genes, ae_type, ridge, inv_n, dzm, dzd, dzp,
              grad_dtype == DCA_BF16 ? 1 : 0, dtheta, loss_sum, workspace, workspace_bytes};
   return zinb_loss_fwd_bwd(a, (cudaStream_t)stream);
+}
+
+extern "C" int dca_tc_heads_loss(const void* Hb, int32_t batch, const void* Wk, const float* bias, int32_t genes,
+                                 const float* Y, int64_t ldy, const int32_t* rows, const float* sf, float ridge, float inv_n,
+                                 void* dzm, void* dzd, void* dzp, int64_t ldz, double* loss_sum, void* workspace,
+                                 size_t workspace_bytes, void* stream) {
+  if (!Hb || !Wk || !bias || !Y || !dzm || !dzd || !dzp || !loss_sum || batch <= 0 || genes <= 0) {
+    set_error("dca_tc_heads_loss: bad argument"); return DCA_ERR_BAD_ARG;
+  }
+  HeadsLossArgs a{};
+  a.H3 = (const __nv_bfloat16*)Hb; a.B = batch; a.G = genes;
+  for (int i = 0; i < 3; ++i) { a.W[i] = (const __nv_bfloat16*)Wk + (size_t)i * 64 * genes; a.bias[i] = bias + (size_t)i * genes; }
+  a.Y = Y; a.ldy = ldy; a.rows = rows; a.sf = sf; a.ridge = ridge; a.inv_n = inv_n;
+  a.dz[0] = (__nv_bfloat16*)dzm; a.dz[1] = (__nv_bfloat16*)dzd; a.dz[2] = (__nv_bfloat16*)dzp; a.ldz = ldz;
+  a.loss_sum = loss_sum; a.ws = workspace; a.ws_bytes = workspace_bytes;
+  return heads_loss_tc(a, (cudaStream_t)stream);
 }
 
 extern "C" int dca_zinb_loss_fwd(const float* Y, int64_t ldy, const int32_t* rows, const float* sf,

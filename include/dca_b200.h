@@ -328,6 +328,17 @@ int dca_tc_heads_fwd(const void* Hb, int32_t batch, const void* Wk, const float*
                      int32_t n_heads, const int32_t kind[3], const float* row_scale,
                      float* out0, float* out1, float* out2, int64_t ld_out, void* stream);
 
+/* Heads forward + zinb-conddisp loss forward/backward in one kernel (the training step's path): Hb, Wk (3 heads:
+ * mean, dispersion, pi) and bias as in dca_tc_heads_fwd; Y, rows, sf, ridge, inv_n as in dca_zinb_loss_fwd_bwd.
+ * Writes the bf16 gradients dzm / dzd / dzp (leading dim ldz) and *loss_sum, bit-identical in dZ to
+ * dca_tc_heads_fwd (no row scale) followed by dca_zinb_loss_fwd_bwd with bf16 gradients; the fp32 head outputs are
+ * never stored.  Needs genes % 8 == 0, Y 16-byte aligned with ldy % 4 == 0, ldz % 4 == 0.  Workspace: as for
+ * dca_zinb_loss_fwd_bwd. */
+int dca_tc_heads_loss(const void* Hb, int32_t batch, const void* Wk, const float* bias, int32_t genes,
+                      const float* Y, int64_t ldy, const int32_t* rows, const float* sf, float ridge, float inv_n,
+                      void* dzm, void* dzd, void* dzp, int64_t ldz, double* loss_sum, void* workspace,
+                      size_t workspace_bytes, void* stream);
+
 /* The gene-wide tensor-core product kernel (one smem tile of Z = X or dZ feeds both products):
  * mode 1: out_b[B x 64] += Z . W (W = bf16 [genes x 64], Keras layout)             -- encoder forward
  * mode 2: dW += Z^T . H (H = bf16 [B x 64])                                       -- encoder backward
