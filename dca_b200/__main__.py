@@ -48,6 +48,9 @@ _OPTIONS = [
     (('--checkcounts',), dict(dest='checkcounts', action='store_true', help='Check that the matrix has raw counts (default: True)')),
     (('--nocheckcounts',), dict(dest='checkcounts', action='store_false', help='Do not check for raw counts')),
     (('--denoisesubset',), dict(dest='denoisesubset', type=str, help='Denoise only the genes listed (one per line) in this file')),
+    (('--preprocess',), dict(type=str, default='host', choices=('host', 'device'),
+                             help='Where size factors, log1p and scaling are computed: host (NumPy, default) or device '
+                                  '(on the GPU; the normalised matrix then stays in GPU memory for training and prediction)')),
 ]
 
 _DEFAULTS = dict(transpose=False, testsplit=False, saveweights=False, sizefactors=True, batchnorm=True,

@@ -120,6 +120,12 @@ PROTOTYPES = {
     "dca_pack_counts": (C.c_int, [_vp, _i32, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _i32]),
     "dca_sparse_counts": (C.c_int, [_vp, _i32, _i64, _i64, _i64, _vp, _vp, _i32]),
     "dca_pack_sparse": (C.c_int, [_vp, _i32, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i32]),
+    "dca_preprocess_workspace_bytes": (C.c_int, [_i64, _i32, C.POINTER(_sz)]),
+    "dca_counts_csr_to_dense": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _vp, _i64, _vp]),
+    "dca_count_totals": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "dca_gather_counts": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i32, _vp, _i64, _vp]),
+    "dca_log_moments": (C.c_int, [_vp, _i64, _i64, _i32, _vp, C.c_double, _i32, _vp, _vp, _vp, _sz, _vp]),
+    "dca_normalize_write": (C.c_int, [_vp, _i64, _i64, _i32, _vp, C.c_double, _i32, _vp, _vp, _vp, _i32, _i64, _vp]),
     "dca_launch_count": (C.c_int64, []),
     "dca_set_tunable": (C.c_int, [C.c_char_p, C.c_int64]),
 }

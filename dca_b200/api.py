@@ -41,16 +41,33 @@ def dca(adata, mode='denoise', ae_type='nb-conddisp', normalize_per_cell=True, s
     torch.manual_seed(random_state)
     os.environ['PYTHONHASHSEED'] = '0'
 
+    # 'preprocess': 'host' (default) | 'device' -- normalise on the GPU and keep X there (device_data.py); popped here
+    # like the other keywords train() does not take from the reference
+    training_kwds = dict(training_kwds)
+    preprocess = training_kwds.pop('preprocess', 'host')
+    if preprocess not in ('host', 'device'):
+        raise ValueError("training_kwds['preprocess'] must be 'host' or 'device', got %r" % (preprocess,))
+
     # raw counts go to adata.raw; the input object is copied only when copy=True  (dca/api.py:156-160)
     adata = read_dataset(adata, transpose=False, test_split=False, copy=copy, check_counts=check_counts)
 
-    # all-zero genes are an error, as in the reference                    (dca/api.py:163-164)
-    nonzero_genes, _ = filter_genes_mask(adata.X, min_counts=1)
-    assert nonzero_genes.all(), 'Please remove all-zero genes before using DCA.'
+    dd = None
+    if preprocess == 'device':
+        # the same steps on the device; adata.X keeps the raw counts until predict() overwrites it
+        from .device_data import DeviceDataset
+        from .io import apply_device_normalize
+        dd = DeviceDataset.from_counts(adata.X, None, network_kwds.get('x_dtype', 'float32'),
+                                       size_factors=normalize_per_cell, logtrans_input=log1p, normalize_input=scale)
+        assert (dd.input_gene_totals >= 1).all(), 'Please remove all-zero genes before using DCA.'
+        apply_device_normalize(adata, dd, filter_min_counts=False, set_x=False)
+    else:
+        # all-zero genes are an error, as in the reference                    (dca/api.py:163-164)
+        nonzero_genes, _ = filter_genes_mask(adata.X, min_counts=1)
+        assert nonzero_genes.all(), 'Please remove all-zero genes before using DCA.'
 
-    # no filtering here: cell and gene indices stay those of the caller    (dca/api.py:166-170)
-    adata = normalize(adata, filter_min_counts=False, size_factors=normalize_per_cell, normalize_input=scale,
-                      logtrans_input=log1p)
+        # no filtering here: cell and gene indices stay those of the caller    (dca/api.py:166-170)
+        adata = normalize(adata, filter_min_counts=False, size_factors=normalize_per_cell, normalize_input=scale,
+                          logtrans_input=log1p)
 
     net_args = dict(network_kwds, hidden_size=hidden_size, hidden_dropout=hidden_dropout, batchnorm=batchnorm,
                     activation=activation, init=init)
@@ -60,8 +77,14 @@ def dca(adata, mode='denoise', ae_type='nb-conddisp', normalize_per_cell=True, s
 
     fit_args = dict(training_kwds, epochs=epochs, reduce_lr=reduce_lr, early_stop=early_stop, batch_size=batch_size,
                     optimizer=optimizer, verbose=verbose, threads=threads, learning_rate=learning_rate)
-    hist = train(adata[adata.obs.dca_split == 'train'], net, **fit_args)
-    res = net.predict(adata, mode, return_info, copy)
+    if dd is None:
+        hist = train(adata[adata.obs.dca_split == 'train'], net, **fit_args)
+        res = net.predict(adata, mode, return_info, copy)
+    else:
+        train_mask = np.asarray(adata.obs.dca_split == 'train')
+        # no AnnData subset: train() reads everything from the dataset, and a subset would copy the raw counts
+        hist = train(None, net, device_data=dd.take(train_mask), **fit_args)
+        res = net.predict(adata, mode, return_info, copy, device_data=dd)
     adata = res if copy else adata
 
     if return_info:

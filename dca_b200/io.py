@@ -82,7 +82,31 @@ def _inplace_subset(adata, rows=None, cols=None):
         adata._inplace_subset_obs(np.asarray(rows))
 
 
-def normalize(adata, filter_min_counts=True, size_factors=True, normalize_input=True, logtrans_input=True):
+def apply_device_normalize(adata, dd, filter_min_counts, set_x=True):
+    """The AnnData mutations of normalize() from a DeviceDataset built with the same flags (device_data.py): in-place
+    filtering, raw, obs['n_counts'] / obs['size_factors'] and (set_x) X as a host fp32 copy of the device X."""
+    if filter_min_counts:
+        if not dd.gene_mask.all():
+            _inplace_subset(adata, cols=dd.gene_mask)
+        if not dd.cell_mask.all():
+            _inplace_subset(adata, rows=dd.cell_mask)
+    if dd.flags:
+        adata.raw = adata.copy()
+    else:
+        adata.raw = adata
+    if dd.flags & 1:
+        if not dd.sf_mask.all():
+            _inplace_subset(adata, rows=dd.sf_mask)
+        adata.obs['n_counts'] = dd.n_counts_host
+        adata.obs['size_factors'] = dd.size_factors_host
+    else:
+        adata.obs['size_factors'] = np.float32(1.0)
+    if set_x:
+        adata.X = np.ascontiguousarray(dd.host_x(), dtype=np.float32)
+    return adata
+
+
+def normalize(adata, filter_min_counts=True, size_factors=True, normalize_input=True, logtrans_input=True, device=None):
     """dca/io.py:88-111 with scanpy's arithmetic restated:
     filter_genes/filter_cells(min_counts=1); raw copy; normalize_per_cell (each cell scaled to the
     median total count; zero-count cells dropped as scanpy does); size_factors = n_counts/median;
@@ -90,7 +114,20 @@ def normalize(adata, filter_min_counts=True, size_factors=True, normalize_input=
 
     Like the reference, this MUTATES the object it is given -- X, obs['n_counts'], obs['size_factors'], raw and (when
     filtering) the set of cells / genes -- and returns the same object, for the lite stand-in and for a real
-    anndata.AnnData alike (only attribute assignment and the two in-place subsetting methods are used)."""
+    anndata.AnnData alike (only attribute assignment and the two in-place subsetting methods are used).
+
+    device (None: the NumPy path above): a CUDA device to compute all of this on (device_data.DeviceDataset, same
+    flags).  The AnnData is mutated the same way, X becomes a host fp32 copy of the device X, and the resident
+    dataset is returned in adata.uns['dca_device_data'] for train(device_data=...) and predict(device_data=...).
+    Size factors and n_counts are bit-identical to the host path; X agrees to a few fp32 ulp (device_data.py).  There
+    is no fallback: without a CUDA device this raises."""
+    if device is not None:
+        from .device_data import DeviceDataset
+        dd = DeviceDataset.from_counts(adata.X, device, "float32", size_factors=size_factors, logtrans_input=logtrans_input,
+                                       normalize_input=normalize_input, filter_min_counts=filter_min_counts)
+        apply_device_normalize(adata, dd, filter_min_counts)
+        adata.uns['dca_device_data'] = dd
+        return adata
     if filter_min_counts:
         gmask, _ = filter_genes_mask(adata.X, 1)                       # dca/io.py:90-92
         if not gmask.all():

@@ -155,7 +155,9 @@ class Autoencoder:
         self.encoder = self.engine
 
     # -- one fused inference pass instead of the reference's four Keras predict() calls
-    def _run_predict(self, adata, want_mean, want_disp, want_pi, want_latent):
+    def _run_predict(self, adata, want_mean, want_disp, want_pi, want_latent, device_data=None):
+        if device_data is not None:
+            return self._run_predict_device(adata, device_data, want_mean, want_disp, want_pi, want_latent)
         X = np.ascontiguousarray(np.asarray(adata.X), dtype=np.float32)
         eng = self.ensure_engine(max_batch=max(getattr(self, "_max_batch", 32), min(PREDICT_BATCH, X.shape[0])))
         dev = eng.device
@@ -190,11 +192,77 @@ class Autoencoder:
             out["dispersion"] = th.cpu().numpy()
         return out
 
+    def _run_predict_device(self, adata, dd, want_mean, want_disp, want_pi, want_latent):
+        """_run_predict with X and the size factors read from a DeviceDataset (device_data.py) of adata's cells.  Each
+        batch's outputs go to one of two device buffer sets and are copied to pinned host memory on a side stream, so
+        the copy of one batch overlaps the next batch."""
+        N = dd.n
+        if adata is not None and adata.n_obs != N:
+            raise ValueError("device_data covers %d cells, adata has %d" % (N, adata.n_obs))
+        eng = self.ensure_engine(max_batch=max(getattr(self, "_max_batch", 32), min(PREDICT_BATCH, N)))
+        dev = eng.device
+        if dd.X.device != dev or dd.x_dtype != eng.x_dtype:
+            raise ValueError("device_data X is %s on %s, the network expects %s on %s"
+                             % (dd.x_dtype, dd.X.device, eng.x_dtype, dev))
+        G = self.output_size
+        bs = min(PREDICT_BATCH, eng.max_batch)
+        cond = self.ae_type not in ("zinb", "nb", "poisson", "normal")
+        Gs = 1 if self.ae_type in ("nb-shared", "zinb-shared") else G
+        widths = {}
+        if want_mean: widths["mean"] = G
+        if want_disp and cond: widths["disp"] = Gs
+        if want_pi: widths["pi"] = Gs
+        if want_latent: widths["latent"] = eng.latent_dim
+        out = {k: np.empty((N, w), np.float32) for k, w in widths.items()}
+        bufs = [{k: torch.empty((bs, w), dtype=torch.float32, device=dev) for k, w in widths.items()} for _ in range(2)]
+        pins = [{k: torch.empty((bs, w), dtype=torch.float32, pin_memory=True) for k, w in widths.items()} for _ in range(2)]
+        pending = [None, None]
+        comp = torch.cuda.current_stream(dev)
+        side = torch.cuda.Stream(dev)
+
+        def drain(slot):
+            ev, s, e = pending[slot]
+            ev.synchronize()
+            for k in widths:
+                out[k][s:e] = pins[slot][k][: e - s].numpy()
+            pending[slot] = None
+
+        for i, s in enumerate(range(0, N, bs)):
+            e, slot = min(s + bs, N), i % 2
+            if pending[slot] is not None:
+                drain(slot)                  # its copy has finished: the device buffers of this slot are free again
+            b = bufs[slot]
+            eng.predict(dd.X, dd.sf, rows=dd.rows[s:e], mean=b.get("mean"), disp=b.get("disp"), pi=b.get("pi"),
+                        latent=b.get("latent"))
+            done = torch.cuda.Event()
+            done.record(comp)
+            side.wait_event(done)
+            with torch.cuda.stream(side):
+                for k in widths:
+                    pins[slot][k][: e - s].copy_(b[k][: e - s], non_blocking=True)
+            copied = torch.cuda.Event()
+            copied.record(side)
+            pending[slot] = (copied, s, e)
+        for slot in (0, 1):
+            if pending[slot] is not None:
+                drain(slot)
+        res = {"mean": out.get("mean"), "pi": out.get("pi"), "latent": out.get("latent")}
+        if want_disp:
+            if cond:
+                res["dispersion"] = out["disp"]
+            else:
+                th = torch.empty(G, dtype=torch.float32, device=dev)
+                eng.predict(dd.X, dd.sf, rows=dd.rows[:1], disp=th)
+                res["dispersion"] = th.cpu().numpy()
+        return res
+
     # -- dca/network.py:188-211
-    def predict(self, adata, mode='denoise', return_info=False, copy=False):
+    def predict(self, adata, mode='denoise', return_info=False, copy=False, device_data=None):
+        """device_data: a device_data.DeviceDataset of adata's cells; the input X and size factors are then read from
+        it instead of adata.X / obs['size_factors']."""
         assert mode in ('denoise', 'latent', 'full'), 'Unknown mode'
         adata = adata.copy() if copy else adata
-        res = self._run_predict(adata, mode in ('denoise', 'full'), False, False, mode in ('latent', 'full'))
+        res = self._run_predict(adata, mode in ('denoise', 'full'), False, False, mode in ('latent', 'full'), device_data)
         if mode in ('latent', 'full'):
             print('dca: Calculating low dimensional representations...')
             adata.obsm['X_dca'] = res["latent"]
@@ -227,11 +295,11 @@ class _InfoMixin:
     has_pi = False
     const_disp = False
 
-    def predict(self, adata, mode='denoise', return_info=False, copy=False, colnames=None):
+    def predict(self, adata, mode='denoise', return_info=False, copy=False, colnames=None, device_data=None):
         assert mode in ('denoise', 'latent', 'full'), 'Unknown mode'
         adata = adata.copy() if copy else adata
         res = self._run_predict(adata, mode in ('denoise', 'full'), return_info, return_info and self.has_pi,
-                                mode in ('latent', 'full'))
+                                mode in ('latent', 'full'), device_data)
         if return_info:
             if self.const_disp:
                 adata.var['X_dca_dispersion'] = res["dispersion"]

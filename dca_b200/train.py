@@ -82,9 +82,17 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
     one computes and normalises it on the device, dca/io.py:99-109 restated) -- for matrices that do not fit the GPU
     ('auto' switches when X + Y would exceed 60 % of the free device memory).  In streaming mode the training rows are
     shuffled ONCE and every epoch visits the batches in a new random order (documented deviation from Keras' per-epoch
-    row shuffle).  Other keywords of the reference's model.fit (e.g. shuffle=False) are honoured or rejected loudly."""
+    row shuffle).  Other keywords of the reference's model.fit (e.g. shuffle=False) are honoured or rejected loudly.
+
+    ``device_data``: a device_data.DeviceDataset of the cells of ``adata`` (in order), preprocessed in HBM.  X, the
+    raw-count target and the size factors are then read there (steps gather their rows through the dataset's
+    ``rows``) and adata's matrices are not used; the updates are those of the host arrays holding the same values.
+    Single process only, use_raw_as_output only, and with ``output_subset`` the dataset's Y must already hold those
+    genes (DeviceDataset.with_output_genes).  adata is then only read for ``raw.var_names`` (output_subset) and may be
+    None otherwise."""
     stream = kwds.pop('stream', False)
     shuffle = kwds.pop('shuffle', True)
+    device_data = kwds.pop('device_data', None)
     if kwds:
         raise TypeError("train() got keyword arguments the accelerated fit loop does not implement: %s" % sorted(kwds))
     from . import _lib as _L
@@ -95,6 +103,10 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
         raise NotImplementedError("tensorboard logging is not part of the accelerated path")
     if output_dir is not None:
         os.makedirs(output_dir, exist_ok=True)
+    if device_data is not None:
+        return _train_device_data(adata, network, device_data, stream, output_subset, use_raw_as_output, optimizer,
+                                  learning_rate, batch_size, validation_split, epochs, reduce_lr, early_stop, clip_grad,
+                                  verbose, save_weights, output_dir, shuffle)
 
     X = np.asarray(adata.X, dtype=np.float32)
     sf = np.asarray(adata.obs['size_factors'], dtype=np.float32).reshape(-1)
@@ -277,8 +289,63 @@ def _fit_stream(eng, network, X, Yh, sf, tr, va, batch_size, epochs, learning_ra
     return hist
 
 
+def _train_device_data(adata, network, dd, stream, output_subset, use_raw_as_output, optimizer, learning_rate, batch_size,
+                       validation_split, epochs, reduce_lr, early_stop, clip_grad, verbose, save_weights, output_dir, shuffle):
+    """train() on a DeviceDataset: the resident loop of train() with positions mapped through dd.rows."""
+    if stream:
+        raise ValueError("device_data is resident in HBM: it cannot be combined with stream=True")
+    if D.rank_world()[1] > 1:
+        raise NotImplementedError("device_data trains on one GPU; a torch.distributed world larger than 1 is not supported")
+    if not use_raw_as_output:
+        raise ValueError("device_data holds the raw counts as the target: use_raw_as_output=False is not supported")
+    if output_subset:
+        if adata is None:
+            raise ValueError("output_subset names genes of adata.raw: pass the AnnData with device_data")
+        raw_names = np.asarray(adata.raw.var_names)
+        gene_idx = [int(np.where(raw_names == x)[0][0]) for x in output_subset]
+        if dd.y_cols is None or list(dd.y_cols) != gene_idx:
+            raise ValueError("output_subset needs a dataset whose Y holds those genes: "
+                             "device_data.with_output_genes(<their positions in adata.raw.var_names>)")
+    elif dd.y_cols is not None:
+        raise ValueError("the dataset's Y holds a subset of the genes, but no output_subset was given")
+    if adata is not None and adata.n_obs != dd.n:
+        raise ValueError("device_data covers %d cells, adata has %d" % (dd.n, adata.n_obs))
+    eng = network.ensure_engine(max_batch=batch_size)
+    if dd.X.device != eng.device:
+        raise ValueError("device_data lives on %s, the network on %s" % (dd.X.device, eng.device))
+    if dd.x_dtype != eng.x_dtype:
+        raise ValueError("device_data X is %s, the network expects %s (network_kwds x_dtype)" % (dd.x_dtype, eng.x_dtype))
+    N = dd.n
+    n_tr = int(N * (1. - validation_split)) if validation_split and 0. < validation_split < 1. else N
+    n_va = N - n_tr
+    default_lr = eng.set_optimizer(optimizer)
+    if learning_rate is None:
+        learning_rate = default_lr
+    eng.reset_optimizer()
+    ctl = PlateauAndStop(float(learning_rate), reduce_lr, early_stop, verbose)
+    hist = History()
+    if verbose:
+        print(network.summary())
+    steps = (n_tr + batch_size - 1) // batch_size
+    dev = eng.device
+    torch.cuda.synchronize(dev)
+    prev_stream = torch.cuda.current_stream(dev)
+    torch.cuda.set_stream(torch.cuda.Stream(dev))
+    try:
+        hist = _fit_loop(eng, network, dd.X, dd.Y, dd.sf, n_tr, n_va, steps, batch_size, epochs, ctl, clip_grad, 1.0, 1, 0,
+                         dev, hist, verbose, save_weights, output_dir, shuffle, rows_map=dd.rows)
+    finally:
+        torch.cuda.synchronize(dev)
+        torch.cuda.set_stream(prev_stream)
+    if not hist.history["val_loss"]:
+        del hist.history["val_loss"]
+    return hist
+
+
 def _fit_loop(eng, network, Xd, Yd, sfd, n_tr, n_va, steps, batch_size, epochs, ctl, clip_grad, gscale, world, rank, dev, hist,
-              verbose, save_weights, output_dir, shuffle=True):
+              verbose, save_weights, output_dir, shuffle=True, rows_map=None):
+    """rows_map (int32 device tensor, n_tr + n_va entries): the storage row of each position in Xd / Yd / sfd; None:
+    position = row."""
     best_val = np.inf
     for epoch in range(epochs):
         # Keras: np.random.shuffle(index_array) with the global NumPy RNG (seeded in api.dca / CLI)
@@ -286,6 +353,8 @@ def _fit_loop(eng, network, Xd, Yd, sfd, n_tr, n_va, steps, batch_size, epochs, 
         if shuffle:
             np.random.shuffle(order)
         order_d = torch.from_numpy(order.astype(np.int32)).to(dev)
+        if rows_map is not None:
+            order_d = rows_map[order_d.long()]
         eng.read_epoch_acc(reset=True)
         for s in range(steps):
             rows = order_d[s * batch_size: min((s + 1) * batch_size, n_tr)]
@@ -297,7 +366,10 @@ def _fit_loop(eng, network, Xd, Yd, sfd, n_tr, n_va, steps, batch_size, epochs, 
         # validation pass: inference-mode BN over the held-out tail
         for s in range(n_tr, n_tr + n_va, batch_size):
             e = min(s + batch_size, n_tr + n_va)
-            eng.eval_step(Xd[s:e], Yd[s:e], sfd[s:e])
+            if rows_map is not None:
+                eng.eval_step(Xd, Yd, sfd, rows=rows_map[s:e])
+            else:
+                eng.eval_step(Xd[s:e], Yd[s:e], sfd[s:e])
         stop, best_val = _epoch_end(eng, network, hist, ctl, epoch, epochs, n_va, world, rank, dev, verbose, save_weights,
                                     output_dir, best_val)
         if stop:
@@ -324,10 +396,15 @@ def train_with_args(args):
                             check_counts=args.checkcounts,
                             test_split=args.testsplit)
 
+    preprocess = getattr(args, 'preprocess', 'host')
+    if preprocess not in ('host', 'device'):
+        raise ValueError("--preprocess must be 'host' or 'device'")
     adata = io.normalize(adata,
                          size_factors=args.sizefactors,
                          logtrans_input=args.loginput,
-                         normalize_input=args.norminput)
+                         normalize_input=args.norminput,
+                         device=torch.device('cuda', torch.cuda.current_device()) if preprocess == 'device' else None)
+    dd = adata.uns.pop('dca_device_data', None)
 
     if args.denoisesubset:
         genelist = list(set(io.read_genelist(args.denoisesubset)))
@@ -364,6 +441,14 @@ def train_with_args(args):
     net.save()
     net.build()
 
+    train_mask = np.asarray(adata.obs.dca_split == 'train')
+    extra = {}
+    if dd is not None:
+        dd_train = dd.take(train_mask)
+        if genelist:
+            raw_names = np.asarray(adata.raw.var_names)
+            dd_train = dd_train.with_output_genes([int(np.where(raw_names == x)[0][0]) for x in genelist])
+        extra['device_data'] = dd_train
     losses = train(adata[adata.obs.dca_split == 'train'], net,
                    output_dir=args.outputdir,
                    learning_rate=args.learningrate,
@@ -375,13 +460,13 @@ def train_with_args(args):
                    clip_grad=args.gradclip,
                    save_weights=args.saveweights,
                    tensorboard=args.tensorboard,
-                   verbose=True)
+                   verbose=True, **extra)
 
     if genelist:
         predict_columns = adata.var_names[[np.where(adata.var_names == x)[0][0] for x in genelist]]
     else:
         predict_columns = adata.var_names
 
-    net.predict(adata, mode='full', return_info=True)
+    net.predict(adata, mode='full', return_info=True, device_data=dd)
     net.write(adata, args.outputdir, mode='full', colnames=predict_columns)
     return losses

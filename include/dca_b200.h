@@ -357,6 +357,45 @@ int dca_tc_gene_gemm_sms(int32_t mode, const void* Z0, const void* Z1, const voi
                          float* dW0, float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed,
                          float* db0, float* db1, float* db2, void* stream, int32_t sm_count);
 
+/* ---- preprocessing of raw counts in HBM (csrc/preprocess.cu) ------------------------------------------------------
+ * dca/io.py:88-111 -- scanpy's pp.filter_genes / pp.filter_cells(min_counts=1), pp.normalize_per_cell, pp.log1p and
+ * pp.scale, restated on the host by dca_b200/io.py:normalize -- computed from the fp32 count matrix Y [n_cells x genes,
+ * leading dimension ldy] the training step reads.  No atomics: reductions over cells fold per-CTA workspace slots in
+ * slot order, so two calls are bit-identical.  The workspace of dca_count_totals / dca_log_moments is
+ * dca_preprocess_workspace_bytes(n_cells, genes).  Without a CUDA device every entry point returns DCA_ERR_NO_DEVICE.
+ *
+ * Arithmetic, per cell r and gene g (flags: DCA_PRE_*; a step whose flag is clear is skipped):
+ *   sf64 = n_counts[r] / median (fp64)                          normalize_per_cell (median of the fp64 totals)
+ *   q    = float((double)y / sf64)
+ *   l    = float(log1p((double)q))  -- rounded from double      pp.log1p
+ *   mean = sum_r l / N, std = sqrt(sum_r (l - mean)^2 / (N - 1)), fp64 sums, two passes as NumPy's var;
+ *          std = 1 for N = 1 and where it is 0                  pp.scale(zero_center=True), no clipping
+ *   X    = float(((double)l - mean) / std); a bf16 X is __float2bfloat16_rn of that float. */
+#define DCA_PRE_SIZE_FACTORS 1
+#define DCA_PRE_LOG1P 2
+#define DCA_PRE_SCALE 4
+int dca_preprocess_workspace_bytes(int64_t n_cells, int32_t genes, size_t* bytes);
+/* Y (zeros included) from a canonical CSR matrix (rows sorted, no duplicate entries, every index in [0, genes)):
+ * int64 indptr [n_cells + 1], int32 indices, float32 data. */
+int dca_counts_csr_to_dense(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_cells,
+                            int32_t genes, float* Y, int64_t ldy, void* stream);
+/* fp64 totals per cell (obs n_counts) and per gene (filter_genes' counts); either may be NULL.  *n_bad (device int64, or
+ * NULL) receives the number of entries that are negative, non-integer or not finite; they are not an error. */
+int dca_count_totals(const float* Y, int64_t ldy, int64_t n_cells, int32_t genes, double* cell_totals,
+                     double* gene_totals, int64_t* n_bad, void* workspace, size_t workspace_bytes, void* stream);
+/* out[i][j] = Y[rows[i]][cols[j]] (leading dimension ldo); rows / cols NULL: the identity.  Subsetting of AnnData's
+ * _inplace_subset_obs / _inplace_subset_var (filter_genes, filter_cells) and of the output genes of --denoisesubset. */
+int dca_gather_counts(const float* Y, int64_t ldy, const int32_t* rows, int64_t n_rows, const int32_t* cols,
+                      int32_t n_cols, float* out, int64_t ldo, void* stream);
+/* Gene mean and std of l (fp64, genes each).  Without DCA_PRE_SCALE: mean = 0, std = 1 and Y is not read.  n_counts
+ * (device fp64) and median are needed with DCA_PRE_SIZE_FACTORS only. */
+int dca_log_moments(const float* Y, int64_t ldy, int64_t n_cells, int32_t genes, const double* n_counts, double median,
+                    int32_t flags, double* mean, double* std, void* workspace, size_t workspace_bytes, void* stream);
+/* X [n_cells x genes, leading dimension ldx] in x_dtype (DCA_F32 | DCA_BF16); mean / std NULL: X = l. */
+int dca_normalize_write(const float* Y, int64_t ldy, int64_t n_cells, int32_t genes, const double* n_counts,
+                        double median, int32_t flags, const double* mean, const double* std, void* X, int32_t x_dtype,
+                        int64_t ldx, void* stream);
+
 /* Single-tile wgmma probe used by the tests to pin the operand descriptor conventions: D[128 x N] =
  * A . B with bf16 operands; a K-major operand is stored [MN x K], an MN-major one [K x MN].
  * *_lbo / *_sbo < 0 select the library's defaults for that layout. */
