@@ -112,7 +112,7 @@ namespace tc {
 int heads_fwd_tc(const __nv_bfloat16* Hb, int B, const __nv_bfloat16* const W[3], const float* const bias[3], int G,
                  int n_heads, const int kind[3], const float* row_scale, float* const out[3], int64_t ld_out, int sm_count,
                  cudaStream_t s);
-int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, int B, int G, int n_heads,
+int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, const int32_t* rows, int B, int G, int n_heads,
                  const __nv_bfloat16* H, const __nv_bfloat16* const W[3], float* out_b, float* const dW[3], int64_t dW_ld,
                  int dW_transposed, float* const db[3], void* ws, size_t ws_bytes, int sm_count, cudaStream_t s);
 size_t gene_gemm_workspace_bytes(int B);

@@ -196,7 +196,9 @@ int Engine::plan(const dca_config& c) {
   }
   if (tc_enc) {
     o_da1b = take(2 * B * 64);
-    o_xb = take(2 * B * (size_t)c.n_in);
+    // bf16 batches (stored X, the streamed batch, the dropped-out copy) are read in place by row index: only fp32 X is
+    // converted into this buffer
+    if (c.x_dtype != DCA_BF16) o_xb = take(2 * B * (size_t)c.n_in);
   }
   // double-buffered staging of raw uint16 counts streamed from the host + the input transform
   for (int k = 0; k < 2; ++k) { o_cnt[k] = take(sizeof(uint16_t) * B * (size_t)c.n_in); o_sfst[k] = take(sizeof(float) * B); }
@@ -264,15 +266,14 @@ int Engine::gemm_auto(GemmArgs g, cudaStream_t s) {
 
 int Engine::forward(const void* X, int64_t ldx, const int32_t* rows, int Bn, bool training, cudaStream_t s) {
   const void* hin = X; int64_t ldin = ldx; int in_bf16 = x_override_bf16 ? 1 : (cfg.x_dtype == DCA_BF16); const int32_t* gather = rows;
-  // tensor-core encoder: needs a contiguous bf16 batch (gathered / converted once, reused by the backward pass)
-  cur_xb = nullptr;
-  if (tc_enc) {
-    const bool direct = in_bf16 && !rows && (ldx % 8 == 0) && ((reinterpret_cast<uintptr_t>(X) & 15) == 0);
-    const bool can_gather = (ldx % (in_bf16 ? 8 : 4) == 0) && ((reinterpret_cast<uintptr_t>(X) & 15) == 0);
-    if (direct) { cur_xb = reinterpret_cast<const __nv_bfloat16*>(X); cur_ldxb = ldx; }
-    else if (can_gather) {
+  // tensor-core encoder (K1 here, K5 in the backward pass): reads bf16 X in place, the batch's rows by index; fp32 X is
+  // gathered and converted into a contiguous bf16 batch once per step
+  cur_x = XOperand{};
+  if (tc_enc && (reinterpret_cast<uintptr_t>(X) & 15) == 0) {
+    if (in_bf16 && ldx % 8 == 0) cur_x = XOperand{reinterpret_cast<const __nv_bfloat16*>(X), ldx, rows};
+    else if (!in_bf16 && ldx % 4 == 0) {
       DCA_TRY(gather_rows_bf16(X, in_bf16, ldx, rows, Bn, cfg.n_in, bf(o_xb), s));
-      cur_xb = bf(o_xb); cur_ldxb = cfg.n_in;
+      cur_x = XOperand{bf(o_xb), cfg.n_in, nullptr};
     }
   }
   const bool fused = use_mid(Bn);
@@ -280,10 +281,10 @@ int Engine::forward(const void* X, int64_t ldx, const int32_t* rows, int Bn, boo
     Layer& l = lay[i];
     float* a = f(l.o_a);
     DCA_TRY(fill_rows_with_bias(a, l.out, Bn, l.out, pp(l.b), s));
-    if (i == 0 && cur_xb) {
-      const __nv_bfloat16* Z[3] = {cur_xb, cur_xb, cur_xb};
+    if (i == 0 && cur_x.base) {
+      const __nv_bfloat16* Z[3] = {cur_x.base, cur_x.base, cur_x.base};
       const __nv_bfloat16* W1[3] = {bf(o_pbf) + lay[0].W, bf(o_pbf) + lay[0].W, bf(o_pbf) + lay[0].W};
-      DCA_TRY(tc::gene_gemm_tc(1, Z, cur_ldxb, Bn, cfg.n_in, 1, nullptr, W1, a, nullptr, 0, 0, nullptr, base + o_ggws, ggws_bytes, sm_count, s));
+      DCA_TRY(tc::gene_gemm_tc(1, Z, cur_x.ld, cur_x.rows, Bn, cfg.n_in, 1, nullptr, W1, a, nullptr, 0, 0, nullptr, base + o_ggws, ggws_bytes, sm_count, s));
     } else {
     GemmArgs g{};
     g.A = hin; g.lda = ldin; g.a_bf16 = in_bf16; g.transA = 0; g.a_rows = gather;
@@ -549,14 +550,14 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
       for (int k = 0; k < n_slots; ++k) {
         const __nv_bfloat16* Z1[3] = {Z[k], Z[k], Z[k]}; const __nv_bfloat16* W1[3] = {Wk[k], Wk[k], Wk[k]};
         float* dW1[3] = {dWp[k], dWp[k], dWp[k]}; float* db1[3] = {dbp[k], dbp[k], dbp[k]};
-        DCA_TRY(tc::gene_gemm_tc(3, Z1, G, Bn, G, 1, bf(o_h3b), W1, dh, dW1, G, 1, db1, base + o_ggws, ggws_bytes, sm_count, s));
+        DCA_TRY(tc::gene_gemm_tc(3, Z1, G, nullptr, Bn, G, 1, bf(o_h3b), W1, dh, dW1, G, 1, db1, base + o_ggws, ggws_bytes, sm_count, s));
         const int h = slot_head[k];
         DCA_CUDA_OK(cudaEventRecord(ev_fork, s));
         DCA_CUDA_OK(cudaStreamWaitEvent(comm_stream, ev_fork, 0));
         DCA_TRY(allreduce_range(head_W[h], head_b[h] + G, comm_stream));
       }
     } else
-    DCA_TRY(tc::gene_gemm_tc(3, Z, G, Bn, G, n_slots, bf(o_h3b), Wk, dh, dWp, G, 1, dbp, base + o_ggws, ggws_bytes, sm_count, s));
+    DCA_TRY(tc::gene_gemm_tc(3, Z, G, nullptr, Bn, G, n_slots, bf(o_h3b), Wk, dh, dWp, G, 1, dbp, base + o_ggws, ggws_bytes, sm_count, s));
   } else
   for (int k = 0; k < 3; ++k) {
     if (head_W[k] < 0 || !dz[k]) continue;
@@ -583,14 +584,14 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
   if (L > 0 && use_mid(Bn)) {
     mid::Params mp;
     mid_params(mp, Bn, true);
-    mp.dh_last = dh; mp.da0 = dh2; mp.da0_bf16 = cur_xb ? bf(o_da1b) : nullptr;
+    mp.dh_last = dh; mp.da0 = dh2; mp.da0_bf16 = cur_x.base ? bf(o_da1b) : nullptr;
     mp.max_ctas = dp_reserve_sms ? (sm_count - dp_reserve_sms) : 0;
     DCA_TRY(mid_backward(mp, s));
     Layer& l = lay[0];
-    if (cur_xb) {
-      const __nv_bfloat16* Z[3] = {cur_xb, cur_xb, cur_xb};
+    if (cur_x.base) {
+      const __nv_bfloat16* Z[3] = {cur_x.base, cur_x.base, cur_x.base};
       float* dWp[3] = {gp(l.W), gp(l.W), gp(l.W)};
-      DCA_TRY(tc::gene_gemm_tc(2, Z, cur_ldxb, Bn, cfg.n_in, 1, bf(o_da1b), nullptr, nullptr, dWp, l.out, 0, nullptr, nullptr, 0, sm_count - dp_reserve_sms, s));
+      DCA_TRY(tc::gene_gemm_tc(2, Z, cur_x.ld, cur_x.rows, Bn, cfg.n_in, 1, bf(o_da1b), nullptr, nullptr, dWp, l.out, 0, nullptr, nullptr, 0, sm_count - dp_reserve_sms, s));
     } else {
       GemmArgs g{};
       g.A = X; g.lda = ldx; g.a_bf16 = x_override_bf16 ? 1 : (cfg.x_dtype == DCA_BF16); g.transA = 1; g.a_rows = xrows;
@@ -611,11 +612,11 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
       } else
       DCA_TRY(bn_bwd_apply(dh, f(l.o_xhat), l.out, Bn, l.out, f(l.o_inv), d(o_dsum), d(o_dprod), gp(l.beta), s));
     }
-    if (i == 0 && cur_xb) {
+    if (i == 0 && cur_x.base) {
       DCA_TRY(cast_to_bf16(dh, bf(o_da1b), (int64_t)Bn * l.out, s));
-      const __nv_bfloat16* Z[3] = {cur_xb, cur_xb, cur_xb};
+      const __nv_bfloat16* Z[3] = {cur_x.base, cur_x.base, cur_x.base};
       float* dWp[3] = {gp(l.W), gp(l.W), gp(l.W)};
-      DCA_TRY(tc::gene_gemm_tc(2, Z, cur_ldxb, Bn, cfg.n_in, 1, bf(o_da1b), nullptr, nullptr, dWp, l.out, 0, nullptr, nullptr, 0, sm_count, s));
+      DCA_TRY(tc::gene_gemm_tc(2, Z, cur_x.ld, cur_x.rows, Bn, cfg.n_in, 1, bf(o_da1b), nullptr, nullptr, dWp, l.out, 0, nullptr, nullptr, 0, sm_count, s));
       DCA_TRY(col_sums(dh, nullptr, l.out, Bn, l.out, d(o_dsum), nullptr, d(o_scratch), s));
       DCA_TRY(col_sum_to_float(d(o_dsum), l.out, gp(l.b), s));
       continue;

@@ -98,7 +98,9 @@ struct Engine {
   int slot_head[3] = {0, -1, -1};          // packed head slot -> head index (0 mean, 1 dispersion, 2 pi)
   int slot_kind[3] = {0, 0, 0};
   size_t o_pbf = 0, o_h3b = 0, o_da1b = 0, o_xb = 0, o_dzb[3] = {0, 0, 0}, o_ggws = 0, ggws_bytes = 0;
-  const __nv_bfloat16* cur_xb = nullptr; int64_t cur_ldxb = 0;   // bf16 batch input of the current step
+  // bf16 encoder input of the current step (set by forward(), read again by the encoder backward): cell i of the batch
+  // is row rows[i] of base (row i when rows is null); base == null: the encoder runs on the generic path
+  struct XOperand { const __nv_bfloat16* base = nullptr; int64_t ld = 0; const int32_t* rows = nullptr; } cur_x;
   __nv_bfloat16* bf(size_t byte_off) const { return reinterpret_cast<__nv_bfloat16*>(base + byte_off); }
 
   // ---- remaining AE types (extra_types.cu): shape-general fp32 path, cfg.ae_type >= DCA_AE_POISSON

@@ -7,7 +7,9 @@
 //   encoder backward (K5)  dW1[G x 64] += X^T . dA1                                   (a)
 //
 // "Z" is the cells x genes bf16 operand (X or dZ), brought into shared memory by TMA as 128-cell x 128-gene tiles
-// (two SWIZZLE_128B boxes of 64 genes).  (b) reads a tile as a K-major A operand (M = 64 cells per warpgroup,
+// (two SWIZZLE_128B boxes of 64 genes).  K1 and K5 may instead name the batch's cells by row index into a larger X
+// (Params::rows): the tile rows are then copied by cp.async into the same shared-memory layout, so the batch is never
+// copied out of X.  (b) reads a tile as a K-major A operand (M = 64 cells per warpgroup,
 // K = genes), (a) as an MN-major A operand (M = 64 genes per warpgroup, K = cells) against H [cells x 64].  A CTA owns
 // one item = (head, range of gene blocks, range of cell blocks) and keeps its fp32 accumulators in registers.
 //
@@ -17,7 +19,8 @@
 //   (b) items span one cell block and a gene range; each writes its partial [128 x 64] into its own slot of a
 //       workspace, and gene_gemm_reduce_kernel adds the slots to the output in slot order.
 //
-// 256 threads = two warpgroups; thread 0 also issues the TMA loads, kStages - 1 tiles ahead.
+// 256 threads = two warpgroups; thread 0 also issues the TMA loads, kStages - 1 tiles ahead (gathered rows: every
+// thread also issues its share of the Z copies).
 #include "engine.h"
 #include "tc_common.cuh"
 
@@ -52,7 +55,18 @@ struct Params {
   int total_items;
   float* db[3];                   // column sums of Z per head (COLSUM)
   float* part; int64_t part_stride;   // (b): partial slot (head * gene_ranges + gene range) of part_stride floats
+  // cell i of the batch is row rows[i] of zsrc (ld ldz; one Z); rows == null: the tiles are rows of map_z*
+  const int32_t* rows; const __nv_bfloat16* zsrc; int64_t ldz;
 };
+
+// 16-byte global -> shared copy through the load path, zero-filling the bytes past src_bytes (cp.async groups are per
+// thread)
+__device__ __forceinline__ void cp_async_16(uint32_t smem_dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // MAXG: gene blocks per item held in registers (the (a) accumulators); WK: W is K-major (Keras [64 x G] head kernel)
 template <bool DO_A, bool DO_B, bool COLSUM, bool WK, int MAXG>
@@ -99,6 +113,17 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
   // CTA consumed in earlier items, so that stage and mbarrier phase continue across items (every issued tile is consumed
   // before the next item starts).
   uint32_t T0 = 0;
+  // Gathered rows (Params::rows; K1 / K5): the Z half of a stage is filled by all 256 threads with 16-byte cp.async
+  // copies instead of TMA boxes (a TMA box per 128-byte row half issues too slowly).  Thread (rh = tid / 8, c = tid % 8)
+  // copies chunk c (genes 8c .. 8c+7) of half rh % 2 of tile rows rh / 2 + 16 i, i < 8: each warp instruction reads
+  // four whole 128-byte row halves.  A chunk goes where SWIZZLE_128B puts it -- chunk c of row r at byte
+  // 16 * (c ^ (r % 8)) of the row -- so the tile is laid out exactly as the TMA lays out a contiguous batch; genes past
+  // G and rows past the batch are zero-filled.  Each thread waits for its own copies of a tile, makes them visible to
+  // the async proxy (wgmma), and a CTA barrier publishes them; the next tile's row indices load while copies run.
+  const bool gather = p.rows != nullptr;
+  const int g_rh = threadIdx.x >> 3, g_c = threadIdx.x & 7, g_h = g_rh & 1, g_r0 = g_rh >> 1;
+  const uint32_t g_dst = g_h * (kZBytes / 2) + g_r0 * 128 + ((g_c ^ (g_r0 & 7)) << 4);
+  int src_row[8];
   for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
     // item -> (head, gene blocks [gb0, gb1), cell blocks [cb0, cb1))
     const int cs = item % p.cell_splits, r = item / p.cell_splits;
@@ -114,9 +139,11 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
       const int st = (T0 + t) % kStages;
       const int cb = cb0 + t / ng, gb = gb0 + t % ng;
       uint8_t* dst = s_st + st * kStage;
-      mbar_expect_tx(&full[st], kStage);
-      tma_load_2d(dst, mz, gb * 128, cb * 128, &full[st]);
-      tma_load_2d(dst + kZBytes / 2, mz, gb * 128 + 64, cb * 128, &full[st]);
+      mbar_expect_tx(&full[st], gather ? kStage - kZBytes : kStage);
+      if (!gather) {
+        tma_load_2d(dst, mz, gb * 128, cb * 128, &full[st]);
+        tma_load_2d(dst + kZBytes / 2, mz, gb * 128 + 64, cb * 128, &full[st]);
+      }
       if (DO_B) {
         if (WK) {        // head backward: W = Keras [64 x G] (K-major B): two [64 feats x 64 genes] boxes
           tma_load_2d(dst + kZBytes, mw, gb * 128, 0, &full[st]);
@@ -127,8 +154,33 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
       }
       if (DO_A) tma_load_2d(dst + kZBytes + (DO_B ? kWBytes : 0), &map_h, 0, cb * 128, &full[st]);
     };
-    if (threadIdx.x == 0)
-      for (int t = 0; t < kStages - 1 && t < n_tiles; ++t) issue(t);
+    auto load_rows = [&](int t) {                   // gathered rows: source rows of this thread's rows of tile t
+      const int cb = cb0 + t / ng;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int r = cb * 128 + g_r0 + 16 * i;
+        src_row[i] = r < p.B ? __ldg(p.rows + r) : -1;
+      }
+    };
+    auto copy_rows = [&](int t) {                   // gathered rows: this thread's 8 chunks of the Z half of tile t
+      const int st = (T0 + t) % kStages, g0 = (gb0 + t % ng) * 128 + g_h * 64 + g_c * 8;
+      const uint32_t gbytes = g0 < p.G ? (uint32_t)min(16, 2 * (p.G - g0)) : 0u;
+      const uint32_t dst = smem_u32(s_st + st * kStage) + g_dst;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const bool ok = src_row[i] >= 0 && gbytes != 0;
+        cp_async_16(dst + i * 2048, ok ? p.zsrc + (int64_t)src_row[i] * p.ldz + g0 : p.zsrc, ok ? gbytes : 0u);
+      }
+      if (t + 1 < n_tiles) load_rows(t + 1);
+    };
+    if (gather) load_rows(0);
+    for (int t = 0; t < kStages - 1; ++t) {         // (gathered rows: one cp.async group per tile slot, empty or not)
+      if (t < n_tiles) {
+        if (threadIdx.x == 0) issue(t);
+        if (gather) copy_rows(t);
+      }
+      if (gather) cp_async_commit();
+    }
 
     float acc_b[DO_B ? 32 : 1];                                        // (b): cells 64*wg.. of the current cell block
     float acc_a[DO_A ? MAXG : 1][32];                                  // (a): genes 64*wg.. of each gene block of the item
@@ -152,7 +204,16 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
 #pragma unroll
       for (int jj = 0; jj < (DO_A ? MAXG : 1); ++jj)
       for (int j = jj; j < (DO_A ? min(jj + 1, ng) : ng); ++j) {
-        if (threadIdx.x == 0 && t + kStages - 1 < n_tiles) issue(t + kStages - 1);   // its stage was released at tile t-1
+        if (t + kStages - 1 < n_tiles) {            // its stage was released at tile t-1
+          if (threadIdx.x == 0) issue(t + kStages - 1);
+          if (gather) copy_rows(t + kStages - 1);
+        }
+        if (gather) {   // this thread's copies of tile t have landed (younger groups may still run); publish them all
+          cp_async_commit();
+          cp_async_wait<kStages - 1>();
+          fence_proxy_async_smem();
+          __syncthreads();
+        }
         const int st = (T0 + t) % kStages;
         mbar_wait(&full[st], ((T0 + t) / kStages) & 1);
         const uint32_t zb = smem_u32(s_st + st * kStage), wb = zb + kZBytes, hb = wb + (DO_B ? kWBytes : 0);
@@ -255,12 +316,14 @@ size_t gene_gemm_workspace_bytes(int B) { return sizeof(float) * (size_t)gg::kMa
 // encoder kernel), [64 x G] per head for mode 3; out_b: fp32 [B x 64] (+=).
 // mode: 1 = encoder forward (K1), 2 = encoder backward (K5), 3 = head backward (K4: dW / db pass, then the dH pass).
 // ws: gene_gemm_workspace_bytes(B) of device memory for the partial slots of modes 1 and 3.
-int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, int B, int G, int n_heads,
+// rows (modes 1 and 2, may be null): cell i of the batch is row rows[i] of Z[0]; every index must be a row of Z[0].
+int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, const int32_t* rows, int B, int G, int n_heads,
                  const __nv_bfloat16* H, const __nv_bfloat16* const W[3], float* out_b, float* const dW[3], int64_t dW_ld,
                  int dW_transposed, float* const db[3], void* ws, size_t ws_bytes, int sm_count, cudaStream_t s) {
   using namespace gg;
   if (ldz % 8 != 0) { set_error("gene_gemm_tc: ldz must be a multiple of 8 (16-byte TMA stride)"); return DCA_ERR_BAD_ARG; }
   if (mode < 1 || mode > 3) { set_error("gene_gemm_tc: bad mode %d", mode); return DCA_ERR_BAD_ARG; }
+  if (rows && (mode == 3 || n_heads != 1)) { set_error("gene_gemm_tc: row indices are for modes 1 and 2 (one Z)"); return DCA_ERR_BAD_ARG; }
   const bool do_a = mode & 2, do_b = mode & 1;
   if (do_b && (!ws || ws_bytes < gene_gemm_workspace_bytes(B))) { set_error("gene_gemm_tc: workspace too small"); return DCA_ERR_BAD_ARG; }
   CUtensorMap mz[3], mh, mw[3], mdw[3];
@@ -290,6 +353,7 @@ int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, int B, 
   base.n_cb = cdiv(B, 128); base.n_gb = cdiv(G, 128);
   for (int i = 0; i < 3; ++i) base.db[i] = db ? db[i] : nullptr;
   base.part = reinterpret_cast<float*>(ws); base.part_stride = (int64_t)base.n_cb * 128 * 64;
+  base.rows = rows; base.zsrc = Z[0]; base.ldz = ldz;
 
   // at most one CTA per SM (shared memory) and at most sm_count CTAs: a caller that passes fewer SMs than the device has
   // leaves the others free; the CTAs stride over the items
@@ -344,10 +408,10 @@ int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, int B, 
 
 // ------------------------------------------------------------------------------------ C ABI (tests / profiling)
 using namespace dca;
-extern "C" int dca_tc_gene_gemm_sms(int32_t mode, const void* Z0, const void* Z1, const void* Z2, int64_t ldz,
-                                    int32_t batch, int32_t genes, int32_t n_heads, const void* H, const void* W, float* out_b,
-                                    float* dW0, float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed, float* db0,
-                                    float* db1, float* db2, void* stream, int32_t sm_count) {
+extern "C" int dca_tc_gene_gemm_rows(int32_t mode, const void* Z0, const void* Z1, const void* Z2, int64_t ldz,
+                                     const int32_t* rows, int32_t batch, int32_t genes, int32_t n_heads, const void* H,
+                                     const void* W, float* out_b, float* dW0, float* dW1, float* dW2, int64_t dW_ld,
+                                     int32_t dW_transposed, float* db0, float* db1, float* db2, void* stream, int32_t sm_count) {
   if (!Z0 || batch <= 0 || genes <= 0 || n_heads < 1 || n_heads > 3) { set_error("dca_tc_gene_gemm: bad argument"); return DCA_ERR_BAD_ARG; }
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
@@ -362,10 +426,17 @@ extern "C" int dca_tc_gene_gemm_sms(int32_t mode, const void* Z0, const void* Z1
   const size_t ws_bytes = tc::gene_gemm_workspace_bytes(batch);
   void* ws = nullptr;
   DCA_CUDA_OK(cudaMallocAsync(&ws, ws_bytes, st));
-  const int rc = tc::gene_gemm_tc(mode, Z, ldz, batch, genes, n_heads, (const __nv_bfloat16*)H, Wp, out_b, dW,
+  const int rc = tc::gene_gemm_tc(mode, Z, ldz, rows, batch, genes, n_heads, (const __nv_bfloat16*)H, Wp, out_b, dW,
                                   dW_ld, dW_transposed, db, ws, ws_bytes, sms, st);
   DCA_CUDA_OK(cudaFreeAsync(ws, st));
   return rc;
+}
+extern "C" int dca_tc_gene_gemm_sms(int32_t mode, const void* Z0, const void* Z1, const void* Z2, int64_t ldz,
+                                    int32_t batch, int32_t genes, int32_t n_heads, const void* H, const void* W, float* out_b,
+                                    float* dW0, float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed, float* db0,
+                                    float* db1, float* db2, void* stream, int32_t sm_count) {
+  return dca_tc_gene_gemm_rows(mode, Z0, Z1, Z2, ldz, nullptr, batch, genes, n_heads, H, W, out_b, dW0, dW1, dW2, dW_ld,
+                               dW_transposed, db0, db1, db2, stream, sm_count);
 }
 extern "C" int dca_tc_gene_gemm(int32_t mode, const void* Z0, const void* Z1, const void* Z2, int64_t ldz, int32_t batch,
                                 int32_t genes, int32_t n_heads, const void* H, const void* W, float* out_b, float* dW0,

@@ -156,6 +156,9 @@ class Autoencoder:
 
     # -- one fused inference pass instead of the reference's four Keras predict() calls
     def _run_predict(self, adata, want_mean, want_disp, want_pi, want_latent, device_data=None):
+        # a model without a dropout head has no pi: the engine writes nothing there, so none is returned (not the
+        # uninitialised contents of the output buffer)
+        want_pi = want_pi and self.has_pi
         if device_data is not None:
             return self._run_predict_device(adata, device_data, want_mean, want_disp, want_pi, want_latent)
         X = np.ascontiguousarray(np.asarray(adata.X), dtype=np.float32)

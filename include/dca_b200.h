@@ -356,6 +356,13 @@ int dca_tc_gene_gemm_sms(int32_t mode, const void* Z0, const void* Z1, const voi
                          int32_t genes, int32_t n_heads, const void* H, const void* W, float* out_b,
                          float* dW0, float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed,
                          float* db0, float* db1, float* db2, void* stream, int32_t sm_count);
+/* The same for modes 1 and 2 with the batch named by row index: cell i is row rows[i] of Z0 (leading dim ldz, a
+ * multiple of 8; 16-byte aligned base), which may hold more rows than the batch.  Every index must be a row of Z0.
+ * Computes the same bits as dca_tc_gene_gemm_sms on the gathered contiguous Z0[rows].  rows == NULL: row i. */
+int dca_tc_gene_gemm_rows(int32_t mode, const void* Z0, const void* Z1, const void* Z2, int64_t ldz, const int32_t* rows,
+                          int32_t batch, int32_t genes, int32_t n_heads, const void* H, const void* W, float* out_b,
+                          float* dW0, float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed,
+                          float* db0, float* db1, float* db2, void* stream, int32_t sm_count);
 
 /* ---- preprocessing of raw counts in HBM (csrc/preprocess.cu) ------------------------------------------------------
  * dca/io.py:88-111 -- scanpy's pp.filter_genes / pp.filter_cells(min_counts=1), pp.normalize_per_cell, pp.log1p and
