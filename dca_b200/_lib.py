@@ -93,6 +93,10 @@ PROTOTYPES = {
     "dca_stream_begin_sparse": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp]),
     "dca_stream_step": (C.c_int, [_vp, _i64, _i64, _vp]),
     "dca_stream_end": (C.c_int, [_vp, _vp]),
+    "dca_expand_packed_counts": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp,
+                                           _vp]),
+    "dca_expand_sparse_counts": (C.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _i32, _vp, _vp,
+                                           _i32, _vp, _vp]),
     "dca_zinb_loss_fwd_bwd": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f, _f,
                                         _vp, _vp, _vp, _i32, _vp, _vp, _vp, _sz, _vp]),
     "dca_zinb_loss_workspace_bytes": (C.c_int, [_i32, _i32, C.POINTER(_sz)]),

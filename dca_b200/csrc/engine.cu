@@ -981,6 +981,8 @@ extern "C" int dca_train_step_host(dca_handle* h, const void* x_host, const floa
   Engine& e = h->e;
   if (!x_host || !y_host) { set_error("dca_train_step_host: NULL host buffer"); return DCA_ERR_BAD_ARG; }
   if (batch <= 0 || batch > e.cfg.max_batch) { set_error("dca_train_step_host: batch %d outside (0, max_batch=%d]", batch, e.cfg.max_batch); return DCA_ERR_BAD_ARG; }
+  // the staging buffers are the first expanded buffer of the streaming path: an expansion in flight there would race
+  if (e.hs.active) { set_error("dca_train_step_host: a host stream is active (call dca_stream_end first)"); return DCA_ERR_BAD_ARG; }
   cudaStream_t s = (cudaStream_t)stream;
   const size_t xb = (e.cfg.x_dtype == DCA_BF16) ? 2 : 4;
   DCA_CUDA_OK(cudaMemcpyAsync(e.base + e.o_stage_x, x_host, xb * (size_t)batch * e.cfg.n_in, cudaMemcpyHostToDevice, s));
@@ -1242,4 +1244,62 @@ extern "C" int dca_stream_end(dca_handle* h, void* stream) {
   }
   hs.active = false; hs.counts = nullptr; hs.ovf_indptr = nullptr; hs.ovf_entries = nullptr; hs.nib_indptr = nullptr; hs.nibbles = nullptr;
   return DCA_OK;
+}
+
+// stand-alone expansion of device-resident packed / sparse counts: the calls stream_prefetch makes, for the tests
+namespace {
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+int check_expand_args(const char* who, const void* src, int32_t n_rows, int32_t genes, const int64_t* ovf_indptr,
+                      const void* ovf_entries, const float* gene_mean, const float* gene_inv_std, const float* Y,
+                      const void* X, int32_t x_dtype) {
+  if (!src || !Y || !X || n_rows <= 0 || genes <= 0 || genes % 8 != 0) {
+    set_error("%s: bad argument (%d rows, %d genes: need rows > 0, genes a positive multiple of 8, non-NULL counts, Y, X)",
+              who, n_rows, genes);
+    return DCA_ERR_BAD_ARG;
+  }
+  if ((ovf_indptr == nullptr) != (ovf_entries == nullptr) || (gene_mean == nullptr) != (gene_inv_std == nullptr) ||
+      (x_dtype != DCA_F32 && x_dtype != DCA_BF16)) {
+    set_error("%s: bad argument (overflow arrays and mean / inv_std go in pairs; x_dtype %d)", who, x_dtype);
+    return DCA_ERR_BAD_ARG;
+  }
+  if (!aligned16(Y) || !aligned16(X) || (reinterpret_cast<uintptr_t>(ovf_entries) & 7)) {
+    set_error("%s: Y and X must be 16-byte aligned, the overflow entries 8-byte aligned", who);
+    return DCA_ERR_BAD_ARG;
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    (void)cudaGetLastError();
+    set_error("%s: no CUDA device available (this library has no CPU fallback)", who);
+    return DCA_ERR_NO_DEVICE;
+  }
+  return DCA_OK;
+}
+}  // namespace
+
+extern "C" int dca_expand_packed_counts(const void* packed, int32_t bits, const int64_t* ovf_indptr, const void* ovf_entries,
+                                        const float* sf, int32_t n_rows, int32_t genes, const float* gene_mean,
+                                        const float* gene_inv_std, int32_t use_size_factors, int32_t use_log1p, float* Y,
+                                        void* X, int32_t x_dtype, float* sf_out, void* stream) {
+  if (bits != 4 && bits != 8 && bits != 16) { set_error("dca_expand_packed_counts: bits must be 4, 8 or 16 (got %d)", bits); return DCA_ERR_BAD_ARG; }
+  if (!aligned16(packed)) { set_error("dca_expand_packed_counts: the packed matrix must be 16-byte aligned"); return DCA_ERR_BAD_ARG; }
+  DCA_TRY(check_expand_args("dca_expand_packed_counts", packed, n_rows, genes, ovf_indptr, ovf_entries, gene_mean,
+                            gene_inv_std, Y, X, x_dtype));
+  return expand_counts(packed, bits, sf, n_rows, genes, gene_mean, gene_inv_std, use_size_factors && sf, use_log1p, Y, X,
+                       x_dtype == DCA_BF16, sf_out, ovf_indptr, ovf_entries, (cudaStream_t)stream);
+}
+
+extern "C" int dca_expand_sparse_counts(const void* bitmap, const int64_t* nib_indptr, const void* nibbles,
+                                        int32_t max_row_nibble_bytes, const int64_t* ovf_indptr, const void* ovf_entries,
+                                        const float* sf, int32_t n_rows, int32_t genes, const float* gene_mean,
+                                        const float* gene_inv_std, int32_t use_size_factors, int32_t use_log1p, float* Y,
+                                        void* X, int32_t x_dtype, float* sf_out, void* stream) {
+  if (!nib_indptr || !nibbles) { set_error("dca_expand_sparse_counts: NULL nibble arrays"); return DCA_ERR_BAD_ARG; }
+  if (!aligned16(bitmap)) { set_error("dca_expand_sparse_counts: the bitmap must be 16-byte aligned"); return DCA_ERR_BAD_ARG; }
+  if (genes > 65536) { set_error("dca_expand_sparse_counts: at most 65536 genes in the sparse format (got %d)", genes); return DCA_ERR_UNSUPPORTED; }
+  DCA_TRY(check_expand_args("dca_expand_sparse_counts", bitmap, n_rows, genes, ovf_indptr, ovf_entries, gene_mean,
+                            gene_inv_std, Y, X, x_dtype));
+  return expand_sparse(bitmap, nib_indptr, nibbles, sf, n_rows, genes, gene_mean, gene_inv_std, use_size_factors && sf,
+                       use_log1p, Y, X, x_dtype == DCA_BF16, sf_out, ovf_indptr, ovf_entries, max_row_nibble_bytes,
+                       (cudaStream_t)stream);
 }

@@ -310,8 +310,10 @@ __global__ void cast_bf16_kernel(const float* __restrict__ in, __nv_bfloat16* __
 // packed counts (BITS = 4 / 8 / 16 per entry, row-major, gene c of a 4-bit row in byte c/2, low nibble = even c)
 // -> Y (fp32 target) and X = ((log1p)(y/sf) - mean_g) * inv_std_g (network input), 8 genes per thread.
 // With an overflow list the value 2^BITS-1 is an escape: the true count is looked up in the row's (short,
-// gene-sorted) segment of the CSR list.  log1p uses MUFU lg2 (relative error ~1e-6 for y/sf >= 1e-2, far
-// below the bf16 rounding of the encoder input and the 2e-5 parity tolerance of the fp32 path).
+// gene-sorted) segment of the CSR list.  log1p uses MUFU lg2: with its bound (2^-22 absolute on [0.5, 2], 2 ulp
+// elsewhere) and the roundings of y/sf, 1 + v and the ln2 product, |l - log1p(y/sf)| < 4e-7 + 4e-7 l, and
+// |X - X_exact| <= inv_std (4e-7 + 4e-7 l) + 2^-23 |X| (derived and checked in tests/test_gpu_stream.py), far below
+// the bf16 rounding of the encoder input.
 __device__ __forceinline__ float normalise_count(float y, float inv_s, int use_log1p, const float* mean,
                                                  const float* inv_std, int c) {
   float v = y * inv_s;                                    // sc.pp.normalize_per_cell   dca/io.py:99-100

@@ -309,8 +309,17 @@ class DeviceEngine:
 
     def train_step_host(self, x_host: torch.Tensor, y_host: torch.Tensor, sf_host: Optional[torch.Tensor],
                         lr: float, clip: float = 5.0) -> float:
-        """End-to-end step from HOST (pinned) buffers through dca_train_step_host."""
-        b = x_host.shape[0]
+        """End-to-end step from HOST (pinned) buffers through dca_train_step_host: x_host [b x n_in] of the engine's
+        x_dtype, y_host float32 [b x n_out], sf_host float32 [b] or None, all contiguous."""
+        def host(t, dtype, shape, what):
+            if t.is_cuda or t.dtype != dtype or tuple(t.shape) != shape or not t.is_contiguous():
+                raise ValueError("train_step_host: %s must be a contiguous %s HOST tensor of shape %s (got %s %s%s)"
+                                 % (what, dtype, shape, t.dtype, tuple(t.shape), " on the device" if t.is_cuda else ""))
+        b = x_host.shape[0] if x_host.dim() == 2 else -1
+        host(x_host, self.x_dtype, (b, self.n_in), "x_host")
+        host(y_host, torch.float32, (b, self.n_out), "y_host")
+        if sf_host is not None:
+            host(sf_host, torch.float32, (b,), "sf_host")
         out = C.c_float()
         check(self.lib.dca_train_step_host(self.handle, x_host.data_ptr(), y_host.data_ptr(),
                                            None if sf_host is None else sf_host.data_ptr(), b, lr, clip,

@@ -231,7 +231,8 @@ int dca_set_loss_ring(dca_handle* h, float* host_ring, int32_t n_slots);
 
 /* End-to-end variant with HOST buffers (pinned recommended): copies the batch
  * (x_host: batch x n_in of cfg.x_dtype, y_host: batch x n_out float, sf_host: batch float)
- * to the device, runs dca_train_step + dca_apply_update, copies the loss back and waits. */
+ * to the device, runs dca_train_step + dca_apply_update, copies the loss back and waits.  Its staging buffers are
+ * those of the streaming path below: between dca_stream_begin* and dca_stream_end it returns DCA_ERR_BAD_ARG. */
 int dca_train_step_host(dca_handle* h, const void* x_host, const float* y_host,
                         const float* sf_host, int32_t batch, float lr, float clip,
                         float* loss_host, void* stream);
@@ -270,6 +271,24 @@ int dca_stream_begin_sparse(dca_handle* h, const void* bitmap_host, const int64_
                             int64_t n_rows, int32_t batch, void* stream);
 int dca_stream_step(dca_handle* h, int64_t batch_index, int64_t next_batch_index /* -1: none */, void* stream);
 int dca_stream_end(dca_handle* h, void* stream);
+/* The expansion of one streamed batch on its own (parity tests): the same kernels dca_stream_step runs, on DEVICE
+ * arrays of n_rows contiguous rows in the formats above (overflow indptr int64[n_rows+1] and nib_indptr int64[n_rows+1]
+ * are offsets relative to their first entry).  Writes Y (float [n_rows x genes]), X = ((log1p)(y / sf) - mean_g) *
+ * inv_std_g in x_dtype (DCA_F32 | DCA_BF16, row stride genes) and sf_out[r] = sf[r] (1 when sf is NULL; sf_out may be
+ * NULL).  y / sf is taken only when use_size_factors is set and sf is given; gene_mean / gene_inv_std: device
+ * float[genes] or both NULL.  Sparse: max_row_nibble_bytes sizes the shared-memory copy of a row's codes; longer rows
+ * read them from global memory.  Returns DCA_ERR_BAD_ARG when genes % 8 != 0, bits is not 4, 8 or 16, or the counts,
+ * Y or X are not 16-byte aligned; DCA_ERR_UNSUPPORTED for a sparse matrix of more than 65536 genes; DCA_ERR_NO_DEVICE
+ * without a CUDA device. */
+int dca_expand_packed_counts(const void* packed, int32_t bits, const int64_t* ovf_indptr, const void* ovf_entries,
+                             const float* sf, int32_t n_rows, int32_t genes, const float* gene_mean,
+                             const float* gene_inv_std, int32_t use_size_factors, int32_t use_log1p,
+                             float* Y, void* X, int32_t x_dtype, float* sf_out, void* stream);
+int dca_expand_sparse_counts(const void* bitmap, const int64_t* nib_indptr, const void* nibbles,
+                             int32_t max_row_nibble_bytes, const int64_t* ovf_indptr, const void* ovf_entries,
+                             const float* sf, int32_t n_rows, int32_t genes, const float* gene_mean,
+                             const float* gene_inv_std, int32_t use_size_factors, int32_t use_log1p,
+                             float* Y, void* X, int32_t x_dtype, float* sf_out, void* stream);
 
 /* ---- stand-alone kernels (parity tests, profiling) -------------------------------------- */
 /* ZINB / NB negative log-likelihood forward + backward, one pass (dca/loss.py:72-156 and its

@@ -70,3 +70,32 @@ def test_entry_points_without_device_return_no_device():
     assert lib.dca_preprocess_workspace_bytes(100, 20, C.byref(ws)) == 0 and ws.value > 0
     st = lib.dca_count_totals(C.c_void_p(256), 20, 100, 20, None, None, None, C.c_void_p(256), ws.value, None)
     assert st == -5 and b"no CUDA device" in lib.dca_last_error()
+
+
+def test_expansion_entry_points_check_arguments_and_need_a_device():
+    """dca_expand_packed_counts / dca_expand_sparse_counts: malformed calls are refused before the device is looked
+    at (genes % 8, bits, 16-byte alignment, the sparse format's 65536 genes); a well-formed call without a device
+    returns DCA_ERR_NO_DEVICE."""
+    import ctypes as C
+    import torch
+    if torch.cuda.is_available():
+        pytest.skip("a CUDA device is present")
+    from dca_b200 import _lib
+    lib = _lib.load()
+    p, odd = C.c_void_p(4096), C.c_void_p(4104)          # stand-in device addresses: never dereferenced here
+
+    def packed(bits=4, genes=64, src=p, Y=p, X=p):
+        return lib.dca_expand_packed_counts(src, bits, None, None, None, 3, genes, None, None, 1, 1, Y, X, _lib.F32, None, None)
+
+    def sparse(genes=64, src=p, Y=p, X=p):
+        return lib.dca_expand_sparse_counts(src, p, p, 32, None, None, None, 3, genes, None, None, 1, 1, Y, X, _lib.BF16, None,
+                                            None)
+    for bits in (1, 2, 5, 12, 32):
+        assert packed(bits=bits) == -1 and b"bits" in lib.dca_last_error()
+    for call in (packed, sparse):
+        assert call(genes=60) == -1 and b"multiple of 8" in lib.dca_last_error()
+        for kw in ({"src": odd}, {"Y": odd}, {"X": odd}):
+            assert call(**kw) == -1 and b"aligned" in lib.dca_last_error(), kw
+        assert call() == -5 and b"no CUDA device" in lib.dca_last_error()
+    assert sparse(genes=65536 + 8) == -3 and b"65536" in lib.dca_last_error()
+    assert sparse(genes=65536) == -5
