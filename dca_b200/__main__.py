@@ -51,10 +51,15 @@ _OPTIONS = [
     (('--preprocess',), dict(type=str, default='host', choices=('host', 'device'),
                              help='Where size factors, log1p and scaling are computed: host (NumPy, default) or device '
                                   '(on the GPU; the normalised matrix then stays in GPU memory for training and prediction)')),
+    (('--stream',), dict(dest='stream', action='store_true',
+                         help='With --preprocess device: keep the raw counts packed in host memory and stream them '
+                              'through the GPU for preprocessing, training and prediction (data larger than GPU memory; '
+                              'same results)')),
 ]
 
 _DEFAULTS = dict(transpose=False, testsplit=False, saveweights=False, sizefactors=True, batchnorm=True,
-                 checkcounts=True, norminput=True, hyper=False, debug=False, tensorboard=False, loginput=True)
+                 checkcounts=True, norminput=True, hyper=False, debug=False, tensorboard=False, loginput=True,
+                 stream=False)
 
 
 def build_parser():

@@ -132,6 +132,22 @@ PROTOTYPES = {
     "dca_gather_counts": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i32, _vp, _i64, _vp]),
     "dca_log_moments": (C.c_int, [_vp, _i64, _i64, _i32, _vp, C.c_double, _i32, _vp, _vp, _vp, _sz, _vp]),
     "dca_normalize_write": (C.c_int, [_vp, _i64, _i64, _i32, _vp, C.c_double, _i32, _vp, _vp, _vp, _i32, _i64, _vp]),
+    "dca_stats_workspace_bytes": (C.c_int, [_i64, _i32, _i64, C.POINTER(_sz)]),
+    "dca_stats_begin": (C.c_int, [_i64, _i32, _vp, _sz, _vp]),
+    "dca_count_totals_rows": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _i32, _vp, _vp, _sz, _vp]),
+    "dca_count_totals_finish": (C.c_int, [_i64, _i32, _vp, _vp, _vp, _sz, _vp]),
+    "dca_log_moments_rows": (C.c_int, [_i32, _vp, _i64, _i64, _i64, _i64, _i32, _vp, C.c_double, _i32, _vp, _vp, _sz,
+                                       _vp]),
+    "dca_log_moments_finish": (C.c_int, [_i32, _i64, _i32, _i32, _vp, _vp, _sz, _vp]),
+    "dca_set_input_transform_exact": (C.c_int, [_vp, _vp, _vp, C.c_double, _i32, _vp]),
+    "dca_stream_row_totals": (C.c_int, [_vp, _vp]),
+    "dca_stream_predict": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _i64, _vp, _vp]),
+    "dca_stream_eval": (C.c_int, [_vp, _i64, _i64, _vp]),
+    "dca_stream_capacity": (C.c_int, [_vp, C.POINTER(_i64), C.POINTER(_i64)]),
+    "dca_expand_packed_counts_exact": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _i32, _i32, C.c_double, _i32, _vp, _vp, _vp,
+                                                 _vp, _i32, _vp, _vp]),
+    "dca_expand_sparse_counts_exact": (C.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _i32, C.c_double, _i32, _vp,
+                                                 _vp, _vp, _vp, _i32, _vp, _vp]),
     "dca_launch_count": (C.c_int64, []),
     "dca_set_tunable": (C.c_int, [C.c_char_p, C.c_int64]),
 }

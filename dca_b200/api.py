@@ -47,12 +47,29 @@ def dca(adata, mode='denoise', ae_type='nb-conddisp', normalize_per_cell=True, s
     preprocess = training_kwds.pop('preprocess', 'host')
     if preprocess not in ('host', 'device'):
         raise ValueError("training_kwds['preprocess'] must be 'host' or 'device', got %r" % (preprocess,))
+    # with 'preprocess': 'device', 'stream': True trains out of core (stream_data.StreamedDataset: packed counts in host
+    # memory, the same results as the resident dataset); 'auto' does so when the resident dataset would not fit
+    streamed = False
+    if preprocess == 'device' and training_kwds.get('stream', False) in (True, 'auto'):
+        streamed = training_kwds.pop('stream')
 
     # raw counts go to adata.raw; the input object is copied only when copy=True  (dca/api.py:156-160)
     adata = read_dataset(adata, transpose=False, test_split=False, copy=copy, check_counts=check_counts)
 
-    dd = None
-    if preprocess == 'device':
+    dd = sd = None
+    x_dtype = network_kwds.get('x_dtype', 'float32')
+    if streamed == 'auto':
+        from .device_data import DeviceDataset
+        dev = torch.device('cuda', torch.cuda.current_device())
+        streamed = DeviceDataset.device_bytes(adata.X, x_dtype, normalize_per_cell) > torch.cuda.mem_get_info(dev)[0]
+    if streamed:
+        from .stream_data import StreamedDataset
+        from .io import apply_device_normalize
+        sd = StreamedDataset.from_counts(adata.X, None, x_dtype, size_factors=normalize_per_cell, logtrans_input=log1p,
+                                         normalize_input=scale, batch=batch_size)
+        assert (sd.input_gene_totals >= 1).all(), 'Please remove all-zero genes before using DCA.'
+        apply_device_normalize(adata, sd, filter_min_counts=False, set_x=False)
+    elif preprocess == 'device':
         # the same steps on the device; adata.X keeps the raw counts until predict() overwrites it
         from .device_data import DeviceDataset
         from .io import apply_device_normalize
@@ -77,7 +94,11 @@ def dca(adata, mode='denoise', ae_type='nb-conddisp', normalize_per_cell=True, s
 
     fit_args = dict(training_kwds, epochs=epochs, reduce_lr=reduce_lr, early_stop=early_stop, batch_size=batch_size,
                     optimizer=optimizer, verbose=verbose, threads=threads, learning_rate=learning_rate)
-    if dd is None:
+    if sd is not None:
+        train_mask = np.asarray(adata.obs.dca_split == 'train')
+        hist = train(None, net, stream_data=sd.take(train_mask), **fit_args)
+        res = net.predict(adata, mode, return_info, copy, stream_data=sd)
+    elif dd is None:
         hist = train(adata[adata.obs.dca_split == 'train'], net, **fit_args)
         res = net.predict(adata, mode, return_info, copy)
     else:

@@ -98,12 +98,31 @@ int optimizer_update(float* params, const float* grads, float* s1, float* s2, in
 int glorot_fill(float* w, int64_t n, int fan_in, int fan_out, uint64_t seed, uint64_t stream_id, cudaStream_t s);
 int fill_value(float* p, int64_t n, float v, cudaStream_t s);
 int cast_to_bf16(const float* in, __nv_bfloat16* out, int64_t n, cudaStream_t s);
+
+// The exact input transform of the preprocessing (include/dca_b200.h, "preprocessing"), shared by the resident
+// normalisation (preprocess.cu) and the exact expansion of streamed batches (layers.cu): l of one count given the
+// row's fp64 size factor; flags are DCA_PRE_*.
+__device__ __forceinline__ float pre_log_value(float y, double sf64, int flags) {
+  float q = (flags & DCA_PRE_SIZE_FACTORS) ? (float)((double)y / sf64) : y;
+  if ((flags & DCA_PRE_LOG1P) && q != 0.f) q = (float)log1p((double)q);     // log1p(+-0) = +-0
+  return q;
+}
+// Arguments of the exact expansion: per-row fp64 totals of the batch (n_counts[r], r = row in the batch; needed with
+// DCA_PRE_SIZE_FACTORS), the median, fp64 gene mean / std (both non-NULL) and, optionally, x_zero[g] =
+// float((0 - mean_g) / std_g), the X of a zero count (NULL: computed per element).
+struct ExactXform {
+  const double* n_counts; double median; int flags;
+  const double* mean; const double* std; const float* x_zero;
+};
+int exact_zero_inputs(const double* mean, const double* std, int n, float* x_zero, cudaStream_t s);
+// ex != nullptr selects the exact transform (sf_in, mean, inv_std, use_sf and use_log1p are then not read)
 int expand_counts(const void* cnt, int bits, const float* sf_in, int M, int n, const float* mean, const float* inv_std, int use_sf,
                   int use_log1p, float* Yout, void* Xout, int x_bf16, float* sf_out, const int64_t* ovf_indptr,
-                  const void* ovf_entries, cudaStream_t s);
+                  const void* ovf_entries, cudaStream_t s, const ExactXform* ex = nullptr);
 int expand_sparse(const void* bitmap, const int64_t* nib_indptr, const void* nibbles, const float* sf_in, int M, int n,
                   const float* mean, const float* inv_std, int use_sf, int use_log1p, float* Yout, void* Xout, int x_bf16,
-                  float* sf_out, const int64_t* ovf_indptr, const void* ovf_entries, int max_row_nibble_bytes, cudaStream_t s);
+                  float* sf_out, const int64_t* ovf_indptr, const void* ovf_entries, int max_row_nibble_bytes, cudaStream_t s,
+                  const ExactXform* ex = nullptr);
 int gather_rows_bf16(const void* X, int x_bf16, int64_t ldx, const int32_t* rows, int M, int n, __nv_bfloat16* out,
                      cudaStream_t s);
 

@@ -207,6 +207,9 @@ int Engine::plan(const dca_config& c) {
   nib_cap = (int64_t)(B * (size_t)c.n_in / 4) + 64;       // sparse format: up to 50 % non-zero entries per batch
   for (int k = 0; k < 2; ++k) { o_nibp[k] = take(sizeof(int64_t) * (B + 1)); o_nib[k] = take((size_t)nib_cap); }
   o_gmean = take(sizeof(float) * (size_t)c.n_in); o_ginv = take(sizeof(float) * (size_t)c.n_in);
+  o_gmean64 = take(sizeof(double) * (size_t)c.n_in); o_gstd64 = take(sizeof(double) * (size_t)c.n_in);
+  o_gx0 = take(sizeof(float) * (size_t)c.n_in);
+  for (int k = 0; k < 2; ++k) o_ncst[k] = take(sizeof(double) * B);
   // staging for the host-buffer entry point
   const size_t xb = (c.x_dtype == DCA_BF16) ? 2 : 4;
   for (int k = 0; k < kExpBufs; ++k) {
@@ -1043,6 +1046,8 @@ int Engine::stream_prefetch(int64_t i, int b, int e) {
     DCA_CUDA_OK(cudaMemcpy2DAsync(base + o_cnt[b], tight, hs.counts + r0 * hs.row_bytes, (size_t)hs.row_bytes, tight, (size_t)nb,
                                   cudaMemcpyHostToDevice, hs.copy));
   if (hs.sf) DCA_CUDA_OK(cudaMemcpyAsync(base + o_sfst[b], hs.sf + r0, sizeof(float) * (size_t)nb, cudaMemcpyHostToDevice, hs.copy));
+  if (tf_exact && hs.n_counts)
+    DCA_CUDA_OK(cudaMemcpyAsync(base + o_ncst[b], hs.n_counts + r0, sizeof(double) * (size_t)nb, cudaMemcpyHostToDevice, hs.copy));
   if (sparse) {
     const int64_t n0 = hs.nib_indptr[r0], n1 = hs.nib_indptr[r0 + nb];
     DCA_CUDA_OK(cudaMemcpyAsync(base + o_nibp[b], hs.nib_indptr + r0, sizeof(int64_t) * (size_t)(nb + 1), cudaMemcpyHostToDevice, hs.copy));
@@ -1065,18 +1070,22 @@ int Engine::stream_prefetch(int64_t i, int b, int e) {
   const int x_bf16 = tc_enc ? 1 : (cfg.x_dtype == DCA_BF16);
   int max_nib = 0;                       // longest nibble run of a row of this batch (host CSR): sizes the expansion's smem
   if (sparse) for (int64_t r = r0; r < r0 + nb; ++r) { const int len = (int)(hs.nib_indptr[r + 1] - hs.nib_indptr[r]); if (len > max_nib) max_nib = len; }
+  const ExactXform ex{reinterpret_cast<const double*>(base + o_ncst[b]), tf_median, tf_flags,
+                      reinterpret_cast<const double*>(base + o_gmean64), reinterpret_cast<const double*>(base + o_gstd64),
+                      f(o_gx0)};
+  const ExactXform* exact = tf_exact ? &ex : nullptr;
   if (sparse)
     DCA_TRY(expand_sparse(base + o_cnt[b], reinterpret_cast<const int64_t*>(base + o_nibp[b]), base + o_nib[b],
                           hs.sf ? f(o_sfst[b]) : nullptr, (int)nb, cfg.n_in, tf_set == 2 ? f(o_gmean) : nullptr,
                           tf_set == 2 ? f(o_ginv) : nullptr, tf_use_sf && hs.sf, tf_use_log1p, f(o_sy[e]), base + o_sx[e], x_bf16,
                           f(o_ssf[e]), has_ovf ? reinterpret_cast<const int64_t*>(base + o_ovp[b]) : nullptr,
-                          has_ovf ? (const void*)(base + o_ove[b]) : nullptr, max_nib, hs.expand));
+                          has_ovf ? (const void*)(base + o_ove[b]) : nullptr, max_nib, hs.expand, exact));
   else
   DCA_TRY(expand_counts(base + o_cnt[b], hs.bits, hs.sf ? f(o_sfst[b]) : nullptr, (int)nb, cfg.n_in,
                         tf_set == 2 ? f(o_gmean) : nullptr, tf_set == 2 ? f(o_ginv) : nullptr, tf_use_sf && hs.sf,
                         tf_use_log1p, f(o_sy[e]), base + o_sx[e], x_bf16, f(o_ssf[e]),
                         has_ovf ? reinterpret_cast<const int64_t*>(base + o_ovp[b]) : nullptr,
-                        has_ovf ? (const void*)(base + o_ove[b]) : nullptr, hs.expand));
+                        has_ovf ? (const void*)(base + o_ove[b]) : nullptr, hs.expand, exact));
   DCA_CUDA_OK(cudaEventRecord(hs.cnt_free[b], hs.expand));
   DCA_CUDA_OK(cudaEventRecord(hs.ready[e], hs.expand));
   if (hs.tl_base && hs.tl.size() < 400) hs.tl_mark(hs.expand);
@@ -1110,6 +1119,39 @@ extern "C" int dca_set_input_transform(dca_handle* h, const float* gene_mean_hos
     DCA_CUDA_OK(cudaStreamSynchronize(s));
   }
   e.tf_set = gene_mean_host ? 2 : 1; e.tf_use_sf = use_size_factors != 0; e.tf_use_log1p = use_log1p != 0;
+  e.tf_exact = false;
+  return DCA_OK;
+}
+
+extern "C" int dca_set_input_transform_exact(dca_handle* h, const double* gene_mean_host, const double* gene_std_host,
+                                             double median, int32_t flags, void* stream) {
+  DCA_NEED_HANDLE(h);
+  Engine& e = h->e;
+  if (!gene_mean_host || !gene_std_host || flags < 0 || flags > 7 || ((flags & DCA_PRE_SIZE_FACTORS) && !(median > 0.0))) {
+    set_error("dca_set_input_transform_exact: bad argument (mean and std are required; flags %d; size factors need a "
+              "median > 0)", flags);
+    return DCA_ERR_BAD_ARG;
+  }
+  if (e.hs.active) { set_error("dca_set_input_transform_exact: a host stream is active (call dca_stream_end first)"); return DCA_ERR_BAD_ARG; }
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t n = (size_t)e.cfg.n_in;
+  DCA_CUDA_OK(cudaMemcpyAsync(e.base + e.o_gmean64, gene_mean_host, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+  DCA_CUDA_OK(cudaMemcpyAsync(e.base + e.o_gstd64, gene_std_host, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+  DCA_TRY(exact_zero_inputs(reinterpret_cast<const double*>(e.base + e.o_gmean64),
+                            reinterpret_cast<const double*>(e.base + e.o_gstd64), (int)n, e.f(e.o_gx0), s));
+  DCA_CUDA_OK(cudaStreamSynchronize(s));
+  e.tf_set = 3; e.tf_exact = true; e.tf_flags = flags; e.tf_median = (flags & DCA_PRE_SIZE_FACTORS) ? median : 1.0;
+  return DCA_OK;
+}
+
+extern "C" int dca_stream_row_totals(dca_handle* h, const double* n_counts_host) {
+  DCA_NEED_HANDLE(h);
+  auto& hs = h->e.hs;
+  if (!hs.active || hs.step_no != 0 || hs.pref_idx >= 0) {
+    set_error("dca_stream_row_totals: call it between dca_stream_begin* and the first step of the stream");
+    return DCA_ERR_BAD_ARG;
+  }
+  hs.n_counts = n_counts_host;
   return DCA_OK;
 }
 
@@ -1164,7 +1206,7 @@ extern "C" int dca_stream_begin_packed(dca_handle* h, const void* packed_host, i
   hs.ovf_indptr = ovf_indptr_host; hs.ovf_entries = reinterpret_cast<const unsigned char*>(ovf_entries_host);
   hs.sf = sf_host; hs.n_rows = n_rows; hs.batch = batch;
   if (bits != 1) { hs.nib_indptr = nullptr; hs.nibbles = nullptr; }
-  hs.pref_idx = -1; hs.step_no = 0; hs.active = true;
+  hs.pref_idx = -1; hs.step_no = 0; hs.active = true; hs.n_counts = nullptr;
   { const char* v = getenv("DCA_STREAM_DIAG");
     if (v && atoi(v) == 2) { hs.tl.clear(); if (!hs.tl_base) cudaEventCreate(&hs.tl_base); cudaEventRecord(hs.tl_base, s); } }
   return DCA_OK;
@@ -1196,12 +1238,21 @@ extern "C" int dca_stream_begin(dca_handle* h, const uint16_t* counts_host, int6
                                  batch, stream);
 }
 
-extern "C" int dca_stream_step(dca_handle* h, int64_t i, int64_t next, void* stream) {
+namespace {
+// One batch of the active host stream: wait for batch i (fetch it now when the previous call did not prefetch it), start
+// the copy + expansion of batch `next` and run `body` (the training step or the inference forward) on the expanded
+// buffers of batch i on `stream`.
+template <typename Body>
+int stream_run(dca_handle* h, const char* who, int64_t i, int64_t next, void* stream, Body body) {
   DCA_NEED_HANDLE(h);
   Engine& e = h->e; auto& hs = e.hs;
-  if (!hs.active) { set_error("dca_stream_step: no active stream (dca_stream_begin)"); return DCA_ERR_BAD_ARG; }
+  if (!hs.active) { set_error("%s: no active stream (dca_stream_begin)", who); return DCA_ERR_BAD_ARG; }
   if (i < 0 || i * (int64_t)hs.batch >= hs.n_rows || next * (int64_t)hs.batch >= hs.n_rows) {
-    set_error("dca_stream_step: batch index out of range (%lld, next %lld)", (long long)i, (long long)next); return DCA_ERR_BAD_ARG;
+    set_error("%s: batch index out of range (%lld, next %lld)", who, (long long)i, (long long)next); return DCA_ERR_BAD_ARG;
+  }
+  if (e.tf_exact && (e.tf_flags & DCA_PRE_SIZE_FACTORS) && !hs.n_counts) {
+    set_error("%s: the exact input transform with size factors needs the per-row totals (dca_stream_row_totals)", who);
+    return DCA_ERR_BAD_ARG;
   }
   cudaStream_t s = (cudaStream_t)stream;
   const int b = (int)(hs.step_no & 1), xb = (int)(hs.step_no % hs.exp_bufs);
@@ -1219,12 +1270,40 @@ extern "C" int dca_stream_step(dca_handle* h, int64_t i, int64_t next, void* str
   int st = DCA_OK;
   if (diag != 1) {                                  // (1 = diagnosis: copies + expansion only)
     e.x_override_bf16 = e.tc_enc ? 1 : 0;           // the tensor-core encoder reads the expanded bf16 batch in place
-    st = e.train_step(e.base + e.o_sx[xb], e.cfg.n_in, e.f(e.o_sy[xb]), e.cfg.n_out, e.f(e.o_ssf[xb]), nullptr, nb, s, 0);
+    st = body(e, xb, nb, s);
     e.x_override_bf16 = 0;
   }
   DCA_CUDA_OK(cudaEventRecord(hs.step_done[xb], s));
   if (tl_on) hs.tl_mark(s);
   return st;
+}
+}  // namespace
+
+extern "C" int dca_stream_step(dca_handle* h, int64_t i, int64_t next, void* stream) {
+  return stream_run(h, "dca_stream_step", i, next, stream, [](Engine& e, int xb, int nb, cudaStream_t s) {
+    return e.train_step(e.base + e.o_sx[xb], e.cfg.n_in, e.f(e.o_sy[xb]), e.cfg.n_out, e.f(e.o_ssf[xb]), nullptr, nb, s, 0);
+  });
+}
+
+extern "C" int dca_stream_eval(dca_handle* h, int64_t i, int64_t next, void* stream) {
+  return stream_run(h, "dca_stream_eval", i, next, stream, [](Engine& e, int xb, int nb, cudaStream_t s) {
+    return e.eval_step(e.base + e.o_sx[xb], e.cfg.n_in, e.f(e.o_sy[xb]), e.cfg.n_out, e.f(e.o_ssf[xb]), nullptr, nb, s);
+  });
+}
+
+extern "C" int dca_stream_capacity(const dca_handle* h, int64_t* ovf_entries, int64_t* nibble_bytes) {
+  DCA_NEED_HANDLE(h);
+  if (ovf_entries) *ovf_entries = h->e.ovf_cap;
+  if (nibble_bytes) *nibble_bytes = h->e.nib_cap;
+  return DCA_OK;
+}
+
+extern "C" int dca_stream_predict(dca_handle* h, int64_t i, int64_t next, float* mean_out, float* disp_out, float* pi_out,
+                                  int64_t ld_out, float* latent_out, void* stream) {
+  return stream_run(h, "dca_stream_predict", i, next, stream, [&](Engine& e, int xb, int nb, cudaStream_t s) {
+    return e.predict(e.base + e.o_sx[xb], e.cfg.n_in, e.f(e.o_ssf[xb]), nullptr, nb, mean_out, disp_out, pi_out, ld_out,
+                     latent_out, s);
+  });
 }
 
 extern "C" int dca_stream_end(dca_handle* h, void* stream) {
@@ -1242,7 +1321,7 @@ extern "C" int dca_stream_end(dca_handle* h, void* stream) {
     fprintf(stderr, "\n");
     hs.tl.clear();
   }
-  hs.active = false; hs.counts = nullptr; hs.ovf_indptr = nullptr; hs.ovf_entries = nullptr; hs.nib_indptr = nullptr; hs.nibbles = nullptr;
+  hs.active = false; hs.n_counts = nullptr; hs.counts = nullptr; hs.ovf_indptr = nullptr; hs.ovf_entries = nullptr; hs.nib_indptr = nullptr; hs.nibbles = nullptr;
   return DCA_OK;
 }
 
@@ -1302,4 +1381,47 @@ extern "C" int dca_expand_sparse_counts(const void* bitmap, const int64_t* nib_i
   return expand_sparse(bitmap, nib_indptr, nibbles, sf, n_rows, genes, gene_mean, gene_inv_std, use_size_factors && sf,
                        use_log1p, Y, X, x_dtype == DCA_BF16, sf_out, ovf_indptr, ovf_entries, max_row_nibble_bytes,
                        (cudaStream_t)stream);
+}
+
+namespace {
+int check_exact_args(const char* who, const double* n_counts, double median, int32_t flags, const double* gene_mean,
+                     const double* gene_std) {
+  if (!gene_mean || !gene_std || flags < 0 || flags > 7 ||
+      ((flags & DCA_PRE_SIZE_FACTORS) && (!n_counts || !(median > 0.0)))) {
+    set_error("%s: bad argument (gene mean and std are required; flags %d; size factors need n_counts and a median > 0)",
+              who, flags);
+    return DCA_ERR_BAD_ARG;
+  }
+  return DCA_OK;
+}
+}  // namespace
+
+extern "C" int dca_expand_packed_counts_exact(const void* packed, int32_t bits, const int64_t* ovf_indptr,
+                                              const void* ovf_entries, const double* n_counts, int32_t n_rows, int32_t genes,
+                                              double median, int32_t flags, const double* gene_mean, const double* gene_std,
+                                              float* Y, void* X, int32_t x_dtype, float* sf_out, void* stream) {
+  if (bits != 4 && bits != 8 && bits != 16) { set_error("dca_expand_packed_counts_exact: bits must be 4, 8 or 16 (got %d)", bits); return DCA_ERR_BAD_ARG; }
+  if (!aligned16(packed)) { set_error("dca_expand_packed_counts_exact: the packed matrix must be 16-byte aligned"); return DCA_ERR_BAD_ARG; }
+  DCA_TRY(check_expand_args("dca_expand_packed_counts_exact", packed, n_rows, genes, ovf_indptr, ovf_entries, nullptr,
+                            nullptr, Y, X, x_dtype));
+  DCA_TRY(check_exact_args("dca_expand_packed_counts_exact", n_counts, median, flags, gene_mean, gene_std));
+  const ExactXform ex{n_counts, median, flags, gene_mean, gene_std, nullptr};
+  return expand_counts(packed, bits, nullptr, n_rows, genes, nullptr, nullptr, 0, 0, Y, X, x_dtype == DCA_BF16, sf_out,
+                       ovf_indptr, ovf_entries, (cudaStream_t)stream, &ex);
+}
+
+extern "C" int dca_expand_sparse_counts_exact(const void* bitmap, const int64_t* nib_indptr, const void* nibbles,
+                                              int32_t max_row_nibble_bytes, const int64_t* ovf_indptr, const void* ovf_entries,
+                                              const double* n_counts, int32_t n_rows, int32_t genes, double median,
+                                              int32_t flags, const double* gene_mean, const double* gene_std, float* Y,
+                                              void* X, int32_t x_dtype, float* sf_out, void* stream) {
+  if (!nib_indptr || !nibbles) { set_error("dca_expand_sparse_counts_exact: NULL nibble arrays"); return DCA_ERR_BAD_ARG; }
+  if (!aligned16(bitmap)) { set_error("dca_expand_sparse_counts_exact: the bitmap must be 16-byte aligned"); return DCA_ERR_BAD_ARG; }
+  if (genes > 65536) { set_error("dca_expand_sparse_counts_exact: at most 65536 genes in the sparse format (got %d)", genes); return DCA_ERR_UNSUPPORTED; }
+  DCA_TRY(check_expand_args("dca_expand_sparse_counts_exact", bitmap, n_rows, genes, ovf_indptr, ovf_entries, nullptr,
+                            nullptr, Y, X, x_dtype));
+  DCA_TRY(check_exact_args("dca_expand_sparse_counts_exact", n_counts, median, flags, gene_mean, gene_std));
+  const ExactXform ex{n_counts, median, flags, gene_mean, gene_std, nullptr};
+  return expand_sparse(bitmap, nib_indptr, nibbles, nullptr, n_rows, genes, nullptr, nullptr, 0, 0, Y, X, x_dtype == DCA_BF16,
+                       sf_out, ovf_indptr, ovf_entries, max_row_nibble_bytes, (cudaStream_t)stream, &ex);
 }

@@ -53,13 +53,18 @@ struct Engine {
   int64_t ovf_cap = 0;                              // entries per staging buffer
   size_t o_nibp[2] = {0, 0}, o_nib[2] = {0, 0}; int64_t nib_cap = 0;   // sparse format: nibble indptr (int64[B+1]) + nibble bytes per staging buffer
   int tf_use_sf = 1, tf_use_log1p = 1, tf_set = 0, x_override_bf16 = 0;
+  // exact transform (dca_set_input_transform_exact): fp64 gene mean / std, X of a zero count, per-row fp64 totals of
+  // each staged batch
+  size_t o_gmean64 = 0, o_gstd64 = 0, o_gx0 = 0, o_ncst[2] = {0, 0};
+  bool tf_exact = false; int tf_flags = 0; double tf_median = 1.0;
   float* loss_ring = nullptr; int ring_n = 0; int64_t ring_pos = 0;   // mapped host mirror of the per-step loss
   struct HostStream {
     const unsigned char* counts = nullptr; int64_t row_bytes = 0; int bits = 16;       // packed host count matrix
     const int64_t* ovf_indptr = nullptr; const unsigned char* ovf_entries = nullptr;   // host CSR overflow list (or null)
     const int64_t* nib_indptr = nullptr; const unsigned char* nibbles = nullptr;       // bits == 1: sparse format (bitmap in `counts`)
     const float* sf = nullptr; int64_t n_rows = 0; int batch = 0;
-    cudaStream_t copy = nullptr;                      // host->device copies of the next batch
+    const double* n_counts = nullptr;                 // per-row fp64 totals of the exact transform (dca_stream_row_totals)
+    cudaStream_t copy = nullptr;                     // host->device copies of the next batch
     cudaStream_t expand = nullptr;                    // its expansion kernel (lowest priority: yields SMs to the step)
     cudaEvent_t h2d_done[2] = {nullptr, nullptr};     // copy stream: raw staging buffer b has arrived
     cudaEvent_t cnt_free[2] = {nullptr, nullptr};     // expand stream: raw staging buffer b has been consumed

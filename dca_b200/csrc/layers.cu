@@ -321,8 +321,8 @@ __device__ __forceinline__ float normalise_count(float y, float inv_s, int use_l
   return mean ? (v - mean[c]) * inv_std[c] : v;           // sc.pp.scale                dca/io.py:108-109
 }
 
-__device__ __noinline__ float overflow_lookup(const int64_t* __restrict__ indptr, const int2* __restrict__ entries, int r, int c,
-                                              float fallback) {
+__device__ __forceinline__ float overflow_find(const int64_t* __restrict__ indptr, const int2* __restrict__ entries, int r, int c,
+                                               float fallback) {
   const int64_t base = indptr[0];
   int64_t lo = indptr[r] - base, hi = indptr[r + 1] - base;
   while (lo < hi) {                                       // entries of a row are sorted by gene
@@ -333,17 +333,40 @@ __device__ __noinline__ float overflow_lookup(const int64_t* __restrict__ indptr
   }
   return fallback;
 }
+// out of line for the float transform (keeps its registers); the exact kernels inline it: a call there costs a spill
+__device__ __noinline__ float overflow_lookup(const int64_t* __restrict__ indptr, const int2* __restrict__ entries, int r, int c,
+                                              float fallback) {
+  return overflow_find(indptr, entries, r, c, fallback);
+}
 
-template <int BITS, typename XT>
+// The exact variant (EXACT = true, preprocess.cu's arithmetic): sf64 = n_counts[r] / median, X =
+// float(((double)l - mean_g) / std_g) with l = pre_log_value(y, sf64, flags).  Zero counts take the per-gene constant
+// x_zero, so the fp64 division and log1p run on non-zero entries only.
+__device__ __forceinline__ double exact_row_sf(const ExactXform& ex, int r) {
+  return (ex.flags & DCA_PRE_SIZE_FACTORS) ? ex.n_counts[r] / ex.median : 1.0;
+}
+__device__ __forceinline__ float exact_count(float y, double sf64, const ExactXform& ex, int c) {
+  if (y == 0.f) return ex.x_zero ? ex.x_zero[c] : (float)((0.0 - ex.mean[c]) / ex.std[c]);
+  return (float)(((double)pre_log_value(y, sf64, ex.flags) - ex.mean[c]) / ex.std[c]);
+}
+
+__global__ void exact_zero_kernel(const double* __restrict__ mean, const double* __restrict__ std, int n, float* __restrict__ out) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < n) out[g] = (float)((0.0 - mean[g]) / std[g]);
+}
+
+template <int BITS, typename XT, bool EXACT>
 __global__ void expand_counts_kernel(const unsigned char* __restrict__ cnt, const float* __restrict__ sf_in, int M, int n,
                                      const float* __restrict__ mean, const float* __restrict__ inv_std, int use_sf,
                                      int use_log1p, float* __restrict__ Yout, XT* __restrict__ Xout, float* __restrict__ sf_out,
-                                     const int64_t* __restrict__ ovf_indptr, const int2* __restrict__ ovf_entries) {
+                                     const int64_t* __restrict__ ovf_indptr, const int2* __restrict__ ovf_entries,
+                                     ExactXform ex) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int per_row = n / 8;
   if (i >= (int64_t)M * per_row) return;
   const int r = (int)(i / per_row), c = (int)(i % per_row) * 8;
-  const float s = sf_in ? sf_in[r] : 1.0f;
+  const double sf64 = EXACT ? exact_row_sf(ex, r) : 1.0;
+  const float s = EXACT ? (float)sf64 : (sf_in ? sf_in[r] : 1.0f);
   if (c == 0 && sf_out) sf_out[r] = s;
   const float inv_s = use_sf ? 1.0f / s : 1.0f;
   uint32_t q[8];
@@ -368,8 +391,9 @@ __global__ void expand_counts_kernel(const unsigned char* __restrict__ cnt, cons
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     y[k] = (float)q[k];
-    if (ovf_indptr && q[k] == kEsc) y[k] = overflow_lookup(ovf_indptr, ovf_entries, r, c + k, y[k]);
-    x[k] = normalise_count(y[k], inv_s, use_log1p, mean, inv_std, c + k);
+    if (ovf_indptr && q[k] == kEsc)
+      y[k] = EXACT ? overflow_find(ovf_indptr, ovf_entries, r, c + k, y[k]) : overflow_lookup(ovf_indptr, ovf_entries, r, c + k, y[k]);
+    x[k] = EXACT ? exact_count(y[k], sf64, ex, c + k) : normalise_count(y[k], inv_s, use_log1p, mean, inv_std, c + k);
   }
   float* yo = Yout + (int64_t)r * n + c;
   *reinterpret_cast<float4*>(yo) = make_float4(y[0], y[1], y[2], y[3]);
@@ -395,13 +419,14 @@ __global__ void expand_counts_kernel(const unsigned char* __restrict__ cnt, cons
 // scan gives every word the position of its first code in the row's nibble stream, then each thread expands its 32
 // genes (Y fp32, X normalised) with 128-bit stores.
 constexpr int kSparseMaxBytes = 8192;                    // bitmap bytes per row the kernel supports (65536 genes)
-template <typename XT>
+template <typename XT, bool EXACT>
 __global__ void __launch_bounds__(256)
 expand_sparse_kernel(const uint32_t* __restrict__ bitmap, const int64_t* __restrict__ nib_indptr,
                      const unsigned char* __restrict__ nibbles, const float* __restrict__ sf_in, int M, int n,
                      const float* __restrict__ mean, const float* __restrict__ inv_std, int use_sf, int use_log1p,
                      float* __restrict__ Yout, XT* __restrict__ Xout, float* __restrict__ sf_out,
-                     const int64_t* __restrict__ ovf_indptr, const int2* __restrict__ ovf_entries, int nib_cap) {
+                     const int64_t* __restrict__ ovf_indptr, const int2* __restrict__ ovf_entries, int nib_cap,
+                     ExactXform ex) {
   // One block per row.  Phase 0: the row's bitmap and its nibble bytes go to shared memory with thread-strided loads (all in
   // flight at once; the first version chased them from global memory, one dependent byte load after another: 0.25 ms per
   // 4096 x 20000 batch, 3 x what its 0.5 GB of stores need).  Phase 1: thread t popcounts S consecutive bitmap bytes and
@@ -427,7 +452,8 @@ expand_sparse_kernel(const uint32_t* __restrict__ bitmap, const int64_t* __restr
   if (nib_smem) for (int i = threadIdx.x; i < nib_len; i += 256) s_nib[i] = nibg[i];
   const unsigned char* bmb = s_bm;
   const unsigned char* nib = nib_smem ? s_nib : nibg;
-  const float s = sf_in ? sf_in[r] : 1.0f;
+  const double sf64 = EXACT ? exact_row_sf(ex, r) : 1.0;
+  const float s = EXACT ? (float)sf64 : (sf_in ? sf_in[r] : 1.0f);
   if (threadIdx.x == 0 && sf_out) sf_out[r] = s;
   const float inv_s = use_sf ? 1.0f / s : 1.0f;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -459,10 +485,11 @@ expand_sparse_kernel(const uint32_t* __restrict__ bitmap, const int64_t* __restr
         const unsigned code = (nib[pos >> 1] >> ((pos & 1) * 4)) & 0xfu;
         ++pos;
         yv = (float)code;
-        if (ovf_indptr && code == 15u) yv = overflow_lookup(ovf_indptr, ovf_entries, r, c0 + k, yv);
+        if (ovf_indptr && code == 15u)
+          yv = EXACT ? overflow_find(ovf_indptr, ovf_entries, r, c0 + k, yv) : overflow_lookup(ovf_indptr, ovf_entries, r, c0 + k, yv);
       }
       y[k] = yv;
-      x[k] = normalise_count(yv, inv_s, use_log1p, mean, inv_std, c0 + k);
+      x[k] = EXACT ? exact_count(yv, sf64, ex, c0 + k) : normalise_count(yv, inv_s, use_log1p, mean, inv_std, c0 + k);
     }
     float* yo = Yout + (int64_t)r * n + c0;
     *reinterpret_cast<float4*>(yo) = make_float4(y[0], y[1], y[2], y[3]);
@@ -488,7 +515,8 @@ inline int blocks_for(int64_t n, int t = 256) { return (int)((n + t - 1) / t); }
 
 int expand_sparse(const void* bitmap, const int64_t* nib_indptr, const void* nibbles, const float* sf_in, int M, int n,
                   const float* mean, const float* inv_std, int use_sf, int use_log1p, float* Yout, void* Xout, int x_bf16,
-                  float* sf_out, const int64_t* ovf_indptr, const void* ovf_entries, int max_row_nibble_bytes, cudaStream_t s) {
+                  float* sf_out, const int64_t* ovf_indptr, const void* ovf_entries, int max_row_nibble_bytes, cudaStream_t s,
+                  const ExactXform* ex) {
   if (M <= 0) return DCA_OK;
   if (n / 8 > kSparseMaxBytes) { set_error("expand_sparse: at most %d genes in the sparse format (got %d)", kSparseMaxBytes * 8, n); return DCA_ERR_UNSUPPORTED; }
   const int2* oe = ovf_indptr ? reinterpret_cast<const int2*>(ovf_entries) : nullptr;
@@ -500,15 +528,28 @@ int expand_sparse(const void* bitmap, const int64_t* nib_indptr, const void* nib
   if (nib_cap > n / 2) nib_cap = n / 2;
   nib_cap = (nib_cap + 15) & ~15;
   const size_t dyn = (size_t)((2 * nbytes + 15) & ~15) + (size_t)((nbytes + 15) & ~15) + (size_t)nib_cap;
-  static size_t attr_bf16 = 48 * 1024, attr_f32 = 48 * 1024;
-  size_t& attr = x_bf16 ? attr_bf16 : attr_f32;
-  if (dyn > attr) {
-    if (x_bf16) DCA_CUDA_OK(cudaFuncSetAttribute(expand_sparse_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-    else DCA_CUDA_OK(cudaFuncSetAttribute(expand_sparse_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-    attr = dyn;
-  }
-  if (x_bf16) expand_sparse_kernel<__nv_bfloat16><<<M, 256, dyn, s>>>((const uint32_t*)bitmap, nib_indptr, (const unsigned char*)nibbles, sf_in, M, n, mean, inv_std, use_sf, use_log1p, Yout, (__nv_bfloat16*)Xout, sf_out, ovf_indptr, oe, nib_cap);
-  else expand_sparse_kernel<float><<<M, 256, dyn, s>>>((const uint32_t*)bitmap, nib_indptr, (const unsigned char*)nibbles, sf_in, M, n, mean, inv_std, use_sf, use_log1p, Yout, (float*)Xout, sf_out, ovf_indptr, oe, nib_cap);
+  // one attribute value per instantiation (index: x_bf16 + 2 * exact)
+  static size_t attr[4] = {48 * 1024, 48 * 1024, 48 * 1024, 48 * 1024};
+  const int inst = (x_bf16 ? 1 : 0) + (ex ? 2 : 0);
+  const ExactXform e = ex ? *ex : ExactXform{};
+#define DCA_SPARSE_LAUNCH(XT, EX)                                                                                      \
+  do {                                                                                                                 \
+    if (dyn > attr[inst]) {                                                                                            \
+      DCA_CUDA_OK(cudaFuncSetAttribute(expand_sparse_kernel<XT, EX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn)); \
+      attr[inst] = dyn;                                                                                                \
+    }                                                                                                                  \
+    expand_sparse_kernel<XT, EX><<<M, 256, dyn, s>>>((const uint32_t*)bitmap, nib_indptr, (const unsigned char*)nibbles, \
+        sf_in, M, n, mean, inv_std, use_sf, use_log1p, Yout, (XT*)Xout, sf_out, ovf_indptr, oe, nib_cap, e);          \
+  } while (0)
+  if (x_bf16) { if (ex) DCA_SPARSE_LAUNCH(__nv_bfloat16, true); else DCA_SPARSE_LAUNCH(__nv_bfloat16, false); }
+  else { if (ex) DCA_SPARSE_LAUNCH(float, true); else DCA_SPARSE_LAUNCH(float, false); }
+#undef DCA_SPARSE_LAUNCH
+  DCA_LAUNCH_CHECK();
+  return DCA_OK;
+}
+
+int exact_zero_inputs(const double* mean, const double* std, int n, float* x_zero, cudaStream_t s) {
+  exact_zero_kernel<<<blocks_for(n), 256, 0, s>>>(mean, std, n, x_zero);
   DCA_LAUNCH_CHECK();
   return DCA_OK;
 }
@@ -651,21 +692,26 @@ int gather_rows_bf16(const void* X, int x_bf16, int64_t ldx, const int32_t* rows
 
 int expand_counts(const void* cnt, int bits, const float* sf_in, int M, int n, const float* mean, const float* inv_std, int use_sf,
                   int use_log1p, float* Yout, void* Xout, int x_bf16, float* sf_out, const int64_t* ovf_indptr,
-                  const void* ovf_entries, cudaStream_t s) {
+                  const void* ovf_entries, cudaStream_t s, const ExactXform* ex) {
   const int64_t tot = (int64_t)M * (n / 8);
   const unsigned char* src = reinterpret_cast<const unsigned char*>(cnt);
   const int2* oe = ovf_indptr ? reinterpret_cast<const int2*>(ovf_entries) : nullptr;
   if (!oe) ovf_indptr = nullptr;
+  const ExactXform e = ex ? *ex : ExactXform{};
+#define DCA_EXPAND_X(BITS, XT, EX)                                                                                   \
+  expand_counts_kernel<BITS, XT, EX><<<blocks_for(tot), 256, 0, s>>>(src, sf_in, M, n, mean, inv_std, use_sf, use_log1p, \
+                                                                     Yout, (XT*)Xout, sf_out, ovf_indptr, oe, e)
 #define DCA_EXPAND(BITS)                                                                                             \
   do {                                                                                                               \
-    if (x_bf16) expand_counts_kernel<BITS, __nv_bfloat16><<<blocks_for(tot), 256, 0, s>>>(src, sf_in, M, n, mean, inv_std, use_sf, use_log1p, Yout, (__nv_bfloat16*)Xout, sf_out, ovf_indptr, oe); \
-    else expand_counts_kernel<BITS, float><<<blocks_for(tot), 256, 0, s>>>(src, sf_in, M, n, mean, inv_std, use_sf, use_log1p, Yout, (float*)Xout, sf_out, ovf_indptr, oe); \
+    if (x_bf16) { if (ex) DCA_EXPAND_X(BITS, __nv_bfloat16, true); else DCA_EXPAND_X(BITS, __nv_bfloat16, false); } \
+    else { if (ex) DCA_EXPAND_X(BITS, float, true); else DCA_EXPAND_X(BITS, float, false); }                         \
   } while (0)
   if (bits == 16) DCA_EXPAND(16);
   else if (bits == 8) DCA_EXPAND(8);
   else if (bits == 4) DCA_EXPAND(4);
   else { set_error("expand_counts: bits must be 4, 8 or 16 (got %d)", bits); return DCA_ERR_BAD_ARG; }
 #undef DCA_EXPAND
+#undef DCA_EXPAND_X
   DCA_LAUNCH_CHECK();
   return DCA_OK;
 }

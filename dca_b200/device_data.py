@@ -121,15 +121,12 @@ class DeviceDataset:
             raise ValueError("at most 2**31 - 1 cells")
         ws_bytes = C.c_size_t()
         check(lib.dca_preprocess_workspace_bytes(N, G, C.byref(ws_bytes)), "dca_preprocess_workspace_bytes")
-        need = N * G * (4 + xdt.itemsize) + ws_bytes.value + N * 24
-        if filter_min_counts or size_factors:
-            need += N * G * 4                          # a filtered copy of Y exists next to the unfiltered one
-        if csr:
-            need += counts.nnz * 8 + (N + 1) * 8
+        need = cls.device_bytes(counts, xdt, size_factors, filter_min_counts)
         free = torch.cuda.mem_get_info(dev)[0]
         if need > free:
             raise MemoryError("preprocessing %d x %d counts on %s needs %.2f GB of device memory and %.2f GB are free; "
-                              "train from host memory instead: train(..., stream=True) or training_kwds={'stream': True}"
+                              "train from host memory instead: train(..., stream=True) or training_kwds={'stream': True} "
+                              "(with 'preprocess': 'device', stream_data.StreamedDataset: out of core, same results)"
                               % (N, G, dev, need / 1e9, free / 1e9))
         with torch.cuda.device(dev):
             Y = torch.empty((N, G), dtype=torch.float32, device=dev)
@@ -139,6 +136,21 @@ class DeviceDataset:
                 _upload_dense(counts, Y)
             ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
             return cls._normalize(lib, Y, ws, dev, xdt, size_factors, logtrans_input, normalize_input, filter_min_counts)
+
+    @staticmethod
+    def device_bytes(counts, x_dtype="float32", size_factors=True, filter_min_counts=False) -> int:
+        """Device memory from_counts needs for ``counts`` (cells x genes, dense or scipy CSR) with these flags."""
+        xdt = {"float32": torch.float32, "bfloat16": torch.bfloat16, torch.float32: torch.float32,
+               torch.bfloat16: torch.bfloat16}[x_dtype]
+        N, G = (int(s) for s in counts.shape)
+        ws_bytes = C.c_size_t()
+        check(_lib.load().dca_preprocess_workspace_bytes(N, G, C.byref(ws_bytes)), "dca_preprocess_workspace_bytes")
+        need = N * G * (4 + xdt.itemsize) + ws_bytes.value + N * 24
+        if filter_min_counts or size_factors:
+            need += N * G * 4                          # a filtered copy of Y exists next to the unfiltered one
+        if _is_csr(counts):
+            need += counts.nnz * 8 + (N + 1) * 8
+        return need
 
     @classmethod
     def _normalize(cls, lib, Y, ws, dev, xdt, size_factors, logtrans_input, normalize_input, filter_min_counts):

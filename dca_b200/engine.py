@@ -341,6 +341,24 @@ class DeviceEngine:
         check(self.lib.dca_set_input_transform(self.handle, mean.ctypes.data, inv.ctypes.data, int(use_size_factors),
                                                int(use_log1p), self._stream()), "dca_set_input_transform")
 
+    def set_input_transform_exact(self, gene_mean, gene_std, median: float, flags: int):
+        """The exact transform of the device preprocessing for streamed batches (dca_set_input_transform_exact): the X
+        DeviceDataset stores for the same counts.  gene_mean / gene_std: fp64 per gene; flags: device_data.PRE_*."""
+        mean = np.ascontiguousarray(gene_mean, dtype=np.float64)
+        std = np.ascontiguousarray(gene_std, dtype=np.float64)
+        if mean.size != self.n_in or std.size != self.n_in:
+            raise ValueError("gene_mean / gene_std must have %d entries" % self.n_in)
+        check(self.lib.dca_set_input_transform_exact(self.handle, mean.ctypes.data, std.ctypes.data, float(median),
+                                                     int(flags), self._stream()), "dca_set_input_transform_exact")
+
+    def stream_row_totals(self, n_counts: torch.Tensor):
+        """Per-row fp64 totals of the active stream's rows for the exact transform: a pinned HOST float64 tensor, kept
+        until stream_end."""
+        if n_counts.is_cuda or n_counts.dtype != torch.float64 or not n_counts.is_contiguous():
+            raise ValueError("the row totals must be a contiguous float64 HOST tensor")
+        self._stream_keep = tuple(self._stream_keep or ()) + (n_counts,)
+        check(self.lib.dca_stream_row_totals(self.handle, n_counts.data_ptr()), "dca_stream_row_totals")
+
     def stream_begin(self, counts, sf: Optional[torch.Tensor], batch: int):
         """Train from HOST memory.  counts: a HOST uint16 tensor [n_rows x n_in] (pin it, hostmem.pin_near_gpu), or an
         io.PackedCounts (4/8/16 bits per entry + overflow list, see io.pack_counts) whose arrays are pinned
@@ -361,16 +379,8 @@ class DeviceEngine:
         if pc.n_genes != self.n_in:
             raise ValueError("packed counts have %d genes, the engine %d" % (pc.n_genes, self.n_in))
 
-        from .hostmem import pin_near_gpu
-
-        def pinned(a, view):                      # pinned pages on the GPU's NUMA node (hostmem.py)
-            return pin_near_gpu(np.ascontiguousarray(a).view(view), self.device.index or 0)
-        if getattr(pc, "_pinned", None) is None:      # pin once per PackedCounts (cudaHostAlloc costs milliseconds)
-            pc._pinned = (pinned(pc.packed, np.uint8), pinned(pc.indptr, np.int64),
-                          pinned(pc.entries if len(pc.entries) else np.zeros(1, dtype=pc.entries.dtype), np.uint8))
-            if pc.bits == 1:
-                pc._pinned += (pinned(pc.nib_indptr, np.int64), pinned(pc.nibbles, np.uint8))
-        packed, indptr, entries = pc._pinned[:3]
+        from .stream_data import pin_packed
+        packed, indptr, entries = pin_packed(pc, self.device.index or 0)[:3]
         self._stream_keep = pc._pinned + (sf,)
         if pc.bits == 1:                              # sparse format: bitmap + nibble stream (dca_stream_begin_sparse)
             check(self.lib.dca_stream_begin_sparse(self.handle, packed.data_ptr(), pc._pinned[3].data_ptr(), pc._pinned[4].data_ptr(),
@@ -395,6 +405,29 @@ class DeviceEngine:
     def stream_step(self, batch_index: int, next_batch_index: int = -1):
         """Forward + loss + backward of host batch `batch_index`; the copy of `next_batch_index` overlaps it."""
         check(self.lib.dca_stream_step(self.handle, batch_index, next_batch_index, self._stream()), "dca_stream_step")
+
+    def stream_eval(self, batch_index: int, next_batch_index: int = -1):
+        """eval_step on host batch `batch_index` of the active stream (validation pass); the copy and expansion of
+        `next_batch_index` overlap it."""
+        check(self.lib.dca_stream_eval(self.handle, batch_index, next_batch_index, self._stream()), "dca_stream_eval")
+
+    def stream_capacity(self):
+        """(overflow entries, bytes of sparse non-zero codes) one streamed batch may carry (dca_stream_capacity)."""
+        ovf, nib = C.c_int64(), C.c_int64()
+        check(self.lib.dca_stream_capacity(self.handle, C.byref(ovf), C.byref(nib)), "dca_stream_capacity")
+        return int(ovf.value), int(nib.value)
+
+    def stream_predict(self, batch_index: int, next_batch_index: int = -1, mean=None, disp=None, pi=None, latent=None):
+        """predict() on host batch `batch_index` of the active stream (outputs as there); the copy and expansion of
+        `next_batch_index` overlap it."""
+        ld = None
+        for t in (mean, disp, pi):
+            if t is not None and t.dim() == 2 and t.shape[1] > 1:
+                ld = t.stride(0) if ld is None else ld
+                if t.stride(0) != ld:
+                    raise ValueError("outputs must share a leading dimension")
+        check(self.lib.dca_stream_predict(self.handle, batch_index, next_batch_index, _ptr(mean), _ptr(disp), _ptr(pi),
+                                          ld or self.n_out, _ptr(latent), self._stream()), "dca_stream_predict")
 
     def stream_end(self):
         check(self.lib.dca_stream_end(self.handle, self._stream()), "dca_stream_end")

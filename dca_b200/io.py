@@ -106,7 +106,8 @@ def apply_device_normalize(adata, dd, filter_min_counts, set_x=True):
     return adata
 
 
-def normalize(adata, filter_min_counts=True, size_factors=True, normalize_input=True, logtrans_input=True, device=None):
+def normalize(adata, filter_min_counts=True, size_factors=True, normalize_input=True, logtrans_input=True, device=None,
+              stream=False):
     """dca/io.py:88-111 with scanpy's arithmetic restated:
     filter_genes/filter_cells(min_counts=1); raw copy; normalize_per_cell (each cell scaled to the
     median total count; zero-count cells dropped as scanpy does); size_factors = n_counts/median;
@@ -120,7 +121,22 @@ def normalize(adata, filter_min_counts=True, size_factors=True, normalize_input=
     flags).  The AnnData is mutated the same way, X becomes a host fp32 copy of the device X, and the resident
     dataset is returned in adata.uns['dca_device_data'] for train(device_data=...) and predict(device_data=...).
     Size factors and n_counts are bit-identical to the host path; X agrees to a few fp32 ulp (device_data.py).  There
-    is no fallback: without a CUDA device this raises."""
+    is no fallback: without a CUDA device this raises.
+
+    stream=True (with a device): out of core instead (stream_data.StreamedDataset, same flags, same bits as the resident
+    dataset): the raw counts stay packed in host memory, adata.X keeps the (filtered) raw counts -- no normalised matrix
+    exists on the host -- and the dataset is returned in adata.uns['dca_stream_data'] for train(stream_data=...) and
+    predict(stream_data=...)."""
+    if stream:
+        if device is None:
+            raise ValueError("stream=True preprocesses on a device: give device=")
+        from .stream_data import StreamedDataset
+        sd = StreamedDataset.from_counts(adata.X, device, "float32", size_factors=size_factors,
+                                         logtrans_input=logtrans_input, normalize_input=normalize_input,
+                                         filter_min_counts=filter_min_counts)
+        apply_device_normalize(adata, sd, filter_min_counts, set_x=False)
+        adata.uns['dca_stream_data'] = sd
+        return adata
     if device is not None:
         from .device_data import DeviceDataset
         dd = DeviceDataset.from_counts(adata.X, device, "float32", size_factors=size_factors, logtrans_input=logtrans_input,
@@ -246,6 +262,169 @@ class PackedCounts:
             b += 8 * (r1 - r0 + 1) + int(self.nib_indptr[r1] - self.nib_indptr[r0])
         return b
 
+    def take_rows(self, idx, block=65536):
+        """The rows ``idx`` (integer positions, in that order) as a new PackedCounts, copied on the packed arrays without
+        unpacking: the bytes pack_counts writes for the selected rows at the same width.  Works in blocks of rows so
+        that the index arrays stay small."""
+        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+        if idx.size and (idx.min() < 0 or idx.max() >= self.n_rows):
+            raise IndexError("row index out of range for %d rows" % self.n_rows)
+        if idx.size <= block:
+            return self._take_block(idx)
+        return concat_packed([self._take_block(idx[i:i + block]) for i in range(0, idx.size, block)])
+
+    def _take_block(self, idx):
+        indptr, entries = _gather_segments(self.indptr, self.entries, idx)
+        if self.bits != 1:
+            return PackedCounts(np.ascontiguousarray(self.packed[idx]), self.bits, self.n_genes, indptr, entries)
+        nib_indptr, nib = _gather_segments(self.nib_indptr, self.nibbles, idx)
+        nibbles = np.zeros(nib.size + 16, dtype=np.uint8)            # + slack: the device reads whole bytes
+        nibbles[:nib.size] = nib
+        return PackedCounts(np.ascontiguousarray(self.packed[idx]), 1, self.n_genes, indptr, entries, nib_indptr, nibbles)
+
+
+def _gather_segments(indptr, data, idx):
+    """CSR row selection: (new indptr, data of rows idx concatenated in that order)."""
+    lens = indptr[idx + 1] - indptr[idx]
+    out_ptr = np.zeros(idx.size + 1, dtype=np.int64)
+    np.cumsum(lens, out=out_ptr[1:])
+    row = np.repeat(np.arange(idx.size, dtype=np.int64), lens)
+    src = indptr[idx][row] + np.arange(int(out_ptr[-1]), dtype=np.int64) - out_ptr[:-1][row]
+    return out_ptr, data[src]
+
+
+def concat_packed(parts):
+    """Row concatenation of PackedCounts of one format (same width and gene count): the bytes pack_counts writes for
+    the stacked matrix at that width."""
+    parts = list(parts)
+    if not parts:
+        raise ValueError("nothing to concatenate")
+    bits, g = parts[0].bits, parts[0].n_genes
+    if any(p.bits != bits or p.n_genes != g for p in parts):
+        raise ValueError("packed parts differ in width or gene count")
+
+    def cat_ptr(ptrs):
+        out = [np.zeros(1, dtype=np.int64)]
+        off = 0
+        for p in ptrs:
+            out.append(p[1:] - p[0] + off)
+            off += int(p[-1] - p[0])
+        return np.concatenate(out)
+    packed = np.concatenate([p.packed for p in parts])
+    indptr = cat_ptr([p.indptr for p in parts])
+    entries = np.concatenate([p.entries for p in parts]) if parts else np.empty(0, OVERFLOW_ENTRY)
+    if bits != 1:
+        return PackedCounts(packed, bits, g, indptr, entries)
+    nib_indptr = cat_ptr([p.nib_indptr for p in parts])
+    nibbles = np.zeros(int(nib_indptr[-1]) + 16, dtype=np.uint8)
+    for p, o in zip(parts, nib_indptr[np.cumsum([0] + [p.n_rows for p in parts[:-1]])]):
+        n = int(p.nib_indptr[-1] - p.nib_indptr[0])
+        nibbles[o:o + n] = p.nibbles[:n]
+    return PackedCounts(packed, 1, g, indptr, entries, nib_indptr, nibbles)
+
+
+def pack_rows(counts, bits="auto", batch=None, chunk_rows=16384, threads=0):
+    """pack_counts of a dense matrix or a scipy.sparse CSR matrix, ``chunk_rows`` rows at a time (a CSR matrix is
+    never dense on the host as a whole), concatenated with concat_packed: the bytes pack_counts writes for the whole
+    matrix.  bits='auto' / 'sparse' / 'dense' decide the format once, from the whole matrix as pack_counts does."""
+    csr = hasattr(counts, "tocsr") and getattr(counts, "format", None) == "csr"
+    n, g = (int(s) for s in counts.shape)
+    if g % 8 != 0:
+        raise ValueError("the number of genes must be a multiple of 8 for the packed format (got %d)" % g)
+    if n <= chunk_rows and not csr:
+        return pack_counts(counts, bits, batch=batch, threads=threads)
+    if bits in ("auto", "sparse", "dense"):
+        bits = _choose_format(counts, csr, bits, batch, chunk_rows)
+
+    def rows(r0, r1):
+        m = counts[r0:r1]
+        return m.toarray() if csr else np.asarray(m)
+    return concat_packed([pack_counts(rows(r0, min(n, r0 + chunk_rows)), bits, threads=threads)
+                          for r0 in range(0, n, chunk_rows)])
+
+
+def _choose_format(counts, csr, bits, batch, chunk_rows):
+    """The width pack_counts(counts, bits, batch) would choose (1 = sparse), from per-row statistics gathered chunk by
+    chunk (the native escape counter; non-integer or negative counts raise)."""
+    n, g = counts.shape
+    nnz = np.zeros(n, dtype=np.int64)
+    per_row = np.zeros((3, n), dtype=np.int64)
+    for r0 in range(0, n, chunk_rows):
+        r1 = min(n, r0 + chunk_rows)
+        m = counts[r0:r1]
+        m = m.toarray() if csr else np.asarray(m)
+        nnz[r0:r1] = np.count_nonzero(m, axis=1)
+        per_row[:, r0:r1] = _escapes_native(m)
+    if bits in ("sparse", "auto") and n > 0:
+        if bits == "sparse" or _prefer_sparse(int(nnz.sum()), n * g):
+            nib = np.zeros(n + 1, dtype=np.int64)
+            np.cumsum((nnz + 1) // 2, out=nib[1:])
+            if _worst_batch(nib, batch) <= _nibble_cap(batch, g):
+                return "sparse"
+            if bits == "sparse":
+                raise ValueError("more than 50 % non-zero entries in a batch: use a dense width (bits=4)")
+    return _choose_bits(per_row, n, g, batch)
+
+
+def _prefer_sparse(nnz, size):
+    """pack_counts' choice of the sparse over the dense formats: fewer than 45 % non-zeros, and 1 bit per entry + 4 bits
+    per non-zero at least 20 % below the 4 bits per entry of the dense 4-bit width."""
+    return nnz < 0.45 * size and size / 8.0 + nnz / 2.0 < 0.8 * size / 2.0
+
+
+def _worst_batch(indptr, batch):
+    """Largest span of a CSR indptr over consecutive batches of `batch` rows (0 without a batch)."""
+    n = len(indptr) - 1
+    if not batch or n <= 0:
+        return 0
+    return int(np.max(np.diff(indptr[np.r_[np.arange(0, n, batch), n]])))
+
+
+def _nibble_cap(batch, g):
+    """Bytes of non-zero codes a streamed batch of the sparse format may carry (50 % non-zeros; engine.cu nib_cap)."""
+    return batch * g // 4 + 64 if batch else 0
+
+
+def _escapes_native(C, threads=0):
+    """int64 [3][rows]: entries of each row that need the overflow list at 4, 8 and 16 bits (dca_count_escapes)."""
+    from . import _lib
+    lib = _lib.load()
+    if C.dtype not in _NATIVE_DTYPES:
+        C = C.astype(np.float64 if C.dtype.kind == "f" else np.int64)
+    C = np.ascontiguousarray(C)
+    n, g = C.shape
+    per_row = np.zeros((3, n), dtype=np.int64)
+    if n == 0:
+        return per_row
+    st = lib.dca_count_escapes(C.ctypes.data, _NATIVE_DTYPES[C.dtype], n, g, g, per_row.ctypes.data, int(threads))
+    if st != 0:
+        msg = lib.dca_last_error().decode("utf-8", "replace")
+        raise ValueError("counts must be non-negative integers" if "non-negative" in msg else msg)
+    return per_row
+
+
+def fit_batches(pc, batch, ovf_cap, nib_cap, chunk_rows=16384):
+    """``pc`` when every batch of ``batch`` consecutive rows carries at most ``ovf_cap`` overflow entries (and, in the
+    sparse format, at most ``nib_cap`` bytes of non-zero codes) -- what a streaming engine can stage
+    (DeviceEngine.stream_capacity); otherwise the same counts repacked, chunk by chunk, at the narrowest dense width
+    whose batches fit.  The counts are the same, so the expanded Y and X are the same bits."""
+    if (_worst_batch(pc.indptr, batch) <= ovf_cap
+            and (pc.bits != 1 or _worst_batch(pc.nib_indptr, batch) <= nib_cap)):
+        return pc
+    n = pc.n_rows
+    per_row = np.zeros((3, n), dtype=np.int64)
+    for r0 in range(0, n, chunk_rows):
+        r1 = min(n, r0 + chunk_rows)
+        per_row[:, r0:r1] = _escapes_native(unpack_counts(pc.take_rows(np.arange(r0, r1))))
+    for w, b in enumerate((4, 8, 16)):
+        ptr = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(per_row[w], out=ptr[1:])
+        if _worst_batch(ptr, batch) <= ovf_cap:
+            return concat_packed([pack_counts(unpack_counts(pc.take_rows(np.arange(r0, min(n, r0 + chunk_rows)))), b)
+                                  for r0 in range(0, n, chunk_rows)])
+    raise ValueError("a batch of %d rows holds more than %d counts >= 65535 (the overflow capacity of one streamed batch)"
+                     % (batch, ovf_cap))
+
 
 OVERFLOW_ENTRY = np.dtype([("gene", "<i4"), ("count", "<f4")])
 
@@ -291,10 +470,8 @@ def _pack_sparse_native(C, batch, threads=0):
         raise ValueError("counts must be non-negative integers" if "non-negative" in msg else msg)
     nib_indptr = np.zeros(n + 1, dtype=np.int64); np.cumsum((nnz + 1) // 2, out=nib_indptr[1:])
     indptr = np.zeros(n + 1, dtype=np.int64); np.cumsum(esc, out=indptr[1:])
-    if batch:
-        worst = max(int(nib_indptr[min(i + batch, n)] - nib_indptr[i]) for i in range(0, max(n, 1), batch)) if n else 0
-        if worst > batch * g // 4 + 64:
-            raise ValueError("more than 50 % non-zero entries in a batch: use a dense width (bits=4)")
+    if _worst_batch(nib_indptr, batch) > _nibble_cap(batch, g):
+        raise ValueError("more than 50 % non-zero entries in a batch: use a dense width (bits=4)")
     bitmap = np.empty((n, g // 8), dtype=np.uint8)
     nibbles = np.zeros(int(nib_indptr[-1]) + 16, dtype=np.uint8)
     entries = np.empty(int(indptr[-1]), dtype=OVERFLOW_ENTRY)
@@ -329,10 +506,8 @@ def _pack_sparse(C, batch):
     np.cumsum(np.bincount(orow, minlength=n), out=indptr[1:])
     entries = np.empty(orow.shape[0], dtype=OVERFLOW_ENTRY)
     entries["gene"] = ocol; entries["count"] = vals[over]
-    if batch:
-        worst = max(int(nib_indptr[min(i + batch, n)] - nib_indptr[i]) for i in range(0, max(n, 1), batch)) if n else 0
-        if worst > batch * g // 4 + 64:
-            raise ValueError("more than 50 % non-zero entries in a batch: use a dense width (bits=4)")
+    if _worst_batch(nib_indptr, batch) > _nibble_cap(batch, g):
+        raise ValueError("more than 50 % non-zero entries in a batch: use a dense width (bits=4)")
     return PackedCounts(np.ascontiguousarray(bitmap), 1, g, indptr, entries, nib_indptr, nibbles)
 
 
@@ -357,7 +532,7 @@ def pack_counts(counts, bits="auto", batch=None, native=True, threads=0):
             raise ValueError("counts must be non-negative integers")
         nnz = int(np.count_nonzero(C))
         # sparse: 1 bit per entry + 4 bits per non-zero (+ 8 B per count >= 15); dense 4-bit: 4 bits per entry
-        if bits == "sparse" or (nnz < 0.45 * C.size and C.size / 8.0 + nnz / 2.0 < 0.8 * C.size / 2.0):
+        if bits == "sparse" or _prefer_sparse(nnz, C.size):
             try:
                 return _pack_sparse_native(C, batch, threads) if native else _pack_sparse(C, batch)
             except ValueError:
@@ -396,11 +571,7 @@ def _pack_counts_native(C, bits, batch, threads):
     C = np.ascontiguousarray(C)
     n, g = C.shape
     dt = _NATIVE_DTYPES[C.dtype]
-    per_row = np.zeros((3, n), dtype=np.int64)
-    st = lib.dca_count_escapes(C.ctypes.data, dt, n, g, g, per_row.ctypes.data, int(threads))
-    if st != 0:
-        msg = lib.dca_last_error().decode("utf-8", "replace")
-        raise ValueError("counts must be non-negative integers" if "non-negative" in msg else msg)
+    per_row = _escapes_native(C, threads)
     if bits == "auto":
         bits = _choose_bits(per_row, n, g, batch)
     w = (4, 8, 16).index(bits)

@@ -155,10 +155,14 @@ class Autoencoder:
         self.encoder = self.engine
 
     # -- one fused inference pass instead of the reference's four Keras predict() calls
-    def _run_predict(self, adata, want_mean, want_disp, want_pi, want_latent, device_data=None):
+    def _run_predict(self, adata, want_mean, want_disp, want_pi, want_latent, device_data=None, stream_data=None):
         # a model without a dropout head has no pi: the engine writes nothing there, so none is returned (not the
         # uninitialised contents of the output buffer)
         want_pi = want_pi and self.has_pi
+        if stream_data is not None:
+            if device_data is not None:
+                raise ValueError("give device_data or stream_data, not both")
+            return self._run_predict_stream(adata, stream_data, want_mean, want_disp, want_pi, want_latent)
         if device_data is not None:
             return self._run_predict_device(adata, device_data, want_mean, want_disp, want_pi, want_latent)
         X = np.ascontiguousarray(np.asarray(adata.X), dtype=np.float32)
@@ -207,8 +211,49 @@ class Autoencoder:
         if dd.X.device != dev or dd.x_dtype != eng.x_dtype:
             raise ValueError("device_data X is %s on %s, the network expects %s on %s"
                              % (dd.x_dtype, dd.X.device, eng.x_dtype, dev))
-        G = self.output_size
         bs = min(PREDICT_BATCH, eng.max_batch)
+
+        def run(i, s, e, b):
+            eng.predict(dd.X, dd.sf, rows=dd.rows[s:e], mean=b.get("mean"), disp=b.get("disp"), pi=b.get("pi"),
+                        latent=b.get("latent"))
+
+        def theta(th):
+            eng.predict(dd.X, dd.sf, rows=dd.rows[:1], disp=th)
+        return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
+
+    def _run_predict_stream(self, adata, sd, want_mean, want_disp, want_pi, want_latent):
+        """_run_predict with the input batches streamed from a stream_data.StreamedDataset of adata's cells: each batch
+        is copied from the packed host counts and expanded with the exact transform while the previous one runs
+        (dca_stream_predict); the outputs travel to the host as in _run_predict_device."""
+        N = sd.n
+        if adata is not None and adata.n_obs != N:
+            raise ValueError("stream_data covers %d cells, adata has %d" % (N, adata.n_obs))
+        eng = self.ensure_engine(max_batch=max(getattr(self, "_max_batch", 32), min(PREDICT_BATCH, N)))
+        dev = eng.device
+        if sd.device != dev or sd.x_dtype != eng.x_dtype:
+            raise ValueError("stream_data X is %s for %s, the network expects %s on %s" % (sd.x_dtype, sd.device, eng.x_dtype, dev))
+        if eng.n_in != sd.n_genes:
+            raise ValueError("stream_data has %d genes, the network %d inputs" % (sd.n_genes, eng.n_in))
+        bs = min(PREDICT_BATCH, eng.max_batch)
+        nb = (N + bs - 1) // bs
+        sd.stream_batches(eng, bs)
+        try:
+            def run(i, s, e, b):
+                eng.stream_predict(i, i + 1 if i + 1 < nb else -1, mean=b.get("mean"), disp=b.get("disp"),
+                                   pi=b.get("pi"), latent=b.get("latent"))
+
+            def theta(th):
+                eng.stream_predict(0, -1, disp=th)
+            return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
+        finally:
+            eng.stream_end()
+
+    def _predict_batches(self, eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta):
+        """The outputs of run(i, s, e, buffers) -- the inference of batch i, rows [s, e), into one of two device buffer
+        sets -- gathered on the host: each batch's outputs are copied to pinned host memory on a side stream, so the
+        copy of one batch overlaps the next batch.  theta(th) writes the per-gene dispersion of the const-disp types."""
+        dev = eng.device
+        G = self.output_size
         cond = self.ae_type not in ("zinb", "nb", "poisson", "normal")
         Gs = 1 if self.ae_type in ("nb-shared", "zinb-shared") else G
         widths = {}
@@ -235,8 +280,7 @@ class Autoencoder:
             if pending[slot] is not None:
                 drain(slot)                  # its copy has finished: the device buffers of this slot are free again
             b = bufs[slot]
-            eng.predict(dd.X, dd.sf, rows=dd.rows[s:e], mean=b.get("mean"), disp=b.get("disp"), pi=b.get("pi"),
-                        latent=b.get("latent"))
+            run(i, s, e, b)
             done = torch.cuda.Event()
             done.record(comp)
             side.wait_event(done)
@@ -255,17 +299,19 @@ class Autoencoder:
                 res["dispersion"] = out["disp"]
             else:
                 th = torch.empty(G, dtype=torch.float32, device=dev)
-                eng.predict(dd.X, dd.sf, rows=dd.rows[:1], disp=th)
+                theta(th)
                 res["dispersion"] = th.cpu().numpy()
         return res
 
     # -- dca/network.py:188-211
-    def predict(self, adata, mode='denoise', return_info=False, copy=False, device_data=None):
+    def predict(self, adata, mode='denoise', return_info=False, copy=False, device_data=None, stream_data=None):
         """device_data: a device_data.DeviceDataset of adata's cells; the input X and size factors are then read from
-        it instead of adata.X / obs['size_factors']."""
+        it instead of adata.X / obs['size_factors'].  stream_data: a stream_data.StreamedDataset of adata's cells; the
+        input batches are then streamed from its packed counts (the same outputs as from the DeviceDataset)."""
         assert mode in ('denoise', 'latent', 'full'), 'Unknown mode'
         adata = adata.copy() if copy else adata
-        res = self._run_predict(adata, mode in ('denoise', 'full'), False, False, mode in ('latent', 'full'), device_data)
+        res = self._run_predict(adata, mode in ('denoise', 'full'), False, False, mode in ('latent', 'full'), device_data,
+                                stream_data)
         if mode in ('latent', 'full'):
             print('dca: Calculating low dimensional representations...')
             adata.obsm['X_dca'] = res["latent"]
@@ -298,11 +344,12 @@ class _InfoMixin:
     has_pi = False
     const_disp = False
 
-    def predict(self, adata, mode='denoise', return_info=False, copy=False, colnames=None, device_data=None):
+    def predict(self, adata, mode='denoise', return_info=False, copy=False, colnames=None, device_data=None,
+                stream_data=None):
         assert mode in ('denoise', 'latent', 'full'), 'Unknown mode'
         adata = adata.copy() if copy else adata
         res = self._run_predict(adata, mode in ('denoise', 'full'), return_info, return_info and self.has_pi,
-                                mode in ('latent', 'full'), device_data)
+                                mode in ('latent', 'full'), device_data, stream_data)
         if return_info:
             if self.const_disp:
                 adata.var['X_dca_dispersion'] = res["dispersion"]

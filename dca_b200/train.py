@@ -93,6 +93,7 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
     stream = kwds.pop('stream', False)
     shuffle = kwds.pop('shuffle', True)
     device_data = kwds.pop('device_data', None)
+    stream_data = kwds.pop('stream_data', None)
     if kwds:
         raise TypeError("train() got keyword arguments the accelerated fit loop does not implement: %s" % sorted(kwds))
     from . import _lib as _L
@@ -103,6 +104,12 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
         raise NotImplementedError("tensorboard logging is not part of the accelerated path")
     if output_dir is not None:
         os.makedirs(output_dir, exist_ok=True)
+    if stream_data is not None:
+        if device_data is not None:
+            raise ValueError("give device_data or stream_data, not both")
+        return _train_stream_data(adata, network, stream_data, output_subset, use_raw_as_output, optimizer, learning_rate,
+                                  batch_size, validation_split, epochs, reduce_lr, early_stop, clip_grad, verbose,
+                                  save_weights, output_dir, shuffle)
     if device_data is not None:
         return _train_device_data(adata, network, device_data, stream, output_subset, use_raw_as_output, optimizer,
                                   learning_rate, batch_size, validation_split, epochs, reduce_lr, early_stop, clip_grad,
@@ -289,6 +296,76 @@ def _fit_stream(eng, network, X, Yh, sf, tr, va, batch_size, epochs, learning_ra
     return hist
 
 
+def _train_stream_data(adata, network, sd, output_subset, use_raw_as_output, optimizer, learning_rate, batch_size,
+                       validation_split, epochs, reduce_lr, early_stop, clip_grad, verbose, save_weights, output_dir, shuffle):
+    """train() on a stream_data.StreamedDataset: the split and stream semantics of _fit_stream (the training rows shuffled
+    once, every epoch permuting whole batches; in order with shuffle=False), with batches normalised by the exact transform
+    of the device preprocessing.  The validation rows are streamed as well (dca_stream_eval), so device memory does not
+    grow with the dataset."""
+    if D.rank_world()[1] > 1:
+        raise NotImplementedError("stream_data trains on one GPU; a torch.distributed world larger than 1 is not supported")
+    if not use_raw_as_output:
+        raise ValueError("stream_data holds the raw counts as the target: use_raw_as_output=False is not supported")
+    if output_subset:
+        raise NotImplementedError("stream_data needs the raw counts of the input genes as the target (no output_subset)")
+    if adata is not None and adata.n_obs != sd.n:
+        raise ValueError("stream_data covers %d cells, adata has %d" % (sd.n, adata.n_obs))
+    eng = network.ensure_engine(max_batch=batch_size)
+    if eng.n_in != sd.n_genes or eng.n_out != sd.n_genes:
+        raise ValueError("stream_data has %d genes, the network %d inputs and %d outputs" % (sd.n_genes, eng.n_in, eng.n_out))
+    if sd.device != eng.device:
+        raise ValueError("stream_data is for %s, the network on %s" % (sd.device, eng.device))
+    if sd.x_dtype != eng.x_dtype:
+        raise ValueError("stream_data X is %s, the network expects %s (network_kwds x_dtype)" % (sd.x_dtype, eng.x_dtype))
+    dev = eng.device
+    N = sd.n
+    n_tr = int(N * (1. - validation_split)) if validation_split and 0. < validation_split < 1. else N
+    n_va = N - n_tr
+    order0 = np.arange(n_tr)
+    if shuffle:
+        np.random.shuffle(order0)                 # ONE row shuffle; the epochs permute whole batches (as _fit_stream)
+    tr = sd.take(order0)
+    va = sd.rows(n_tr, N) if n_va else None
+    nb_va = (n_va + batch_size - 1) // batch_size
+    default_lr = eng.set_optimizer(optimizer)
+    if learning_rate is None:
+        learning_rate = default_lr
+    eng.reset_optimizer()
+    ctl = PlateauAndStop(float(learning_rate), reduce_lr, early_stop, verbose)
+    hist = History()
+    if verbose:
+        print(network.summary())
+    nb = (n_tr + batch_size - 1) // batch_size
+    torch.cuda.synchronize(dev)
+    prev_stream = torch.cuda.current_stream(dev)
+    torch.cuda.set_stream(torch.cuda.Stream(dev))
+    best_val = np.inf
+    try:
+        for epoch in range(epochs):
+            border = np.random.permutation(nb) if shuffle else np.arange(nb)
+            eng.read_epoch_acc(reset=True)
+            tr.stream_batches(eng, batch_size)
+            for k in range(nb):
+                eng.stream_step(int(border[k]), int(border[k + 1]) if k + 1 < nb else -1)
+                eng.apply_update(ctl.lr, clip_grad, 1.0)
+            eng.stream_end()
+            if n_va:
+                va.stream_batches(eng, batch_size)
+                for k in range(nb_va):
+                    eng.stream_eval(k, k + 1 if k + 1 < nb_va else -1)
+                eng.stream_end()
+            stop, best_val = _epoch_end(eng, network, hist, ctl, epoch, epochs, n_va, 1, 0, dev, verbose, save_weights,
+                                        output_dir, best_val)
+            if stop:
+                break
+    finally:
+        torch.cuda.synchronize(dev)
+        torch.cuda.set_stream(prev_stream)
+    if not hist.history["val_loss"]:
+        del hist.history["val_loss"]
+    return hist
+
+
 def _train_device_data(adata, network, dd, stream, output_subset, use_raw_as_output, optimizer, learning_rate, batch_size,
                        validation_split, epochs, reduce_lr, early_stop, clip_grad, verbose, save_weights, output_dir, shuffle):
     """train() on a DeviceDataset: the resident loop of train() with positions mapped through dd.rows."""
@@ -399,12 +476,20 @@ def train_with_args(args):
     preprocess = getattr(args, 'preprocess', 'host')
     if preprocess not in ('host', 'device'):
         raise ValueError("--preprocess must be 'host' or 'device'")
+    stream = bool(getattr(args, 'stream', False))
+    if stream and preprocess != 'device':
+        raise ValueError("--stream needs --preprocess device")
+    if stream and args.denoisesubset:
+        raise NotImplementedError("--stream trains on every input gene (the streamed batches need n_in == n_out): "
+                                  "--denoisesubset is not supported with it")
     adata = io.normalize(adata,
                          size_factors=args.sizefactors,
                          logtrans_input=args.loginput,
                          normalize_input=args.norminput,
-                         device=torch.device('cuda', torch.cuda.current_device()) if preprocess == 'device' else None)
+                         device=torch.device('cuda', torch.cuda.current_device()) if preprocess == 'device' else None,
+                         stream=stream)
     dd = adata.uns.pop('dca_device_data', None)
+    sd = adata.uns.pop('dca_stream_data', None)
 
     if args.denoisesubset:
         genelist = list(set(io.read_genelist(args.denoisesubset)))
@@ -449,6 +534,8 @@ def train_with_args(args):
             raw_names = np.asarray(adata.raw.var_names)
             dd_train = dd_train.with_output_genes([int(np.where(raw_names == x)[0][0]) for x in genelist])
         extra['device_data'] = dd_train
+    if sd is not None:
+        extra['stream_data'] = sd.take(train_mask)
     losses = train(adata[adata.obs.dca_split == 'train'], net,
                    output_dir=args.outputdir,
                    learning_rate=args.learningrate,
@@ -467,6 +554,6 @@ def train_with_args(args):
     else:
         predict_columns = adata.var_names
 
-    net.predict(adata, mode='full', return_info=True, device_data=dd)
+    net.predict(adata, mode='full', return_info=True, device_data=dd, stream_data=sd)
     net.write(adata, args.outputdir, mode='full', colnames=predict_columns)
     return losses

@@ -271,6 +271,27 @@ int dca_stream_begin_sparse(dca_handle* h, const void* bitmap_host, const int64_
                             int64_t n_rows, int32_t batch, void* stream);
 int dca_stream_step(dca_handle* h, int64_t batch_index, int64_t next_batch_index /* -1: none */, void* stream);
 int dca_stream_end(dca_handle* h, void* stream);
+/* The exact transform of the device preprocessing (see "preprocessing" below; dca/io.py:88-111) for streamed batches,
+ * instead of the float one of dca_set_input_transform: sf = float(n_counts[r] / median), X = float(((double)l -
+ * mean_g) / std_g) with l = float(log1p((double)float((double)y / sf64))) per the DCA_PRE_* flags -- the bits
+ * dca_normalize_write stores for the same cell.  gene_mean_host / gene_std_host: HOST fp64 [n_in] (copied; mean 0
+ * and std 1 without DCA_PRE_SCALE).  With DCA_PRE_SIZE_FACTORS every stream needs its per-row fp64 totals:
+ * dca_stream_row_totals(h, n_counts_host [n_rows], pinned, kept until dca_stream_end), called between
+ * dca_stream_begin* and the first step; sf_host is then not read.  dca_set_input_transform switches back. */
+int dca_set_input_transform_exact(dca_handle* h, const double* gene_mean_host, const double* gene_std_host, double median,
+                                  int32_t flags, void* stream);
+int dca_stream_row_totals(dca_handle* h, const double* n_counts_host);
+/* Inference on the host stream (dca/network.py:188-211 on data that does not fit the GPU): dca_predict on batch
+ * batch_index (outputs as there, batch rows), while the copy and expansion of next_batch_index overlap it -- the
+ * batch bookkeeping of dca_stream_step, which it may follow or precede within one stream. */
+int dca_stream_predict(dca_handle* h, int64_t batch_index, int64_t next_batch_index, float* mean_out, float* disp_out,
+                       float* pi_out, int64_t ld_out, float* latent_out, void* stream);
+/* The validation pass of fit (dca/train.py:96) on the host stream: dca_eval_step on batch batch_index, with the batch
+ * bookkeeping of dca_stream_step. */
+int dca_stream_eval(dca_handle* h, int64_t batch_index, int64_t next_batch_index, void* stream);
+/* What one streamed batch may carry (fixed by max_batch and n_in at dca_create): overflow entries (dca_stream_begin_packed)
+ * and bytes of non-zero codes (dca_stream_begin_sparse).  dca_stream_begin* rejects a dataset with a batch above either. */
+int dca_stream_capacity(const dca_handle* h, int64_t* ovf_entries, int64_t* nibble_bytes);
 /* The expansion of one streamed batch on its own (parity tests): the same kernels dca_stream_step runs, on DEVICE
  * arrays of n_rows contiguous rows in the formats above (overflow indptr int64[n_rows+1] and nib_indptr int64[n_rows+1]
  * are offsets relative to their first entry).  Writes Y (float [n_rows x genes]), X = ((log1p)(y / sf) - mean_g) *
@@ -289,6 +310,18 @@ int dca_expand_sparse_counts(const void* bitmap, const int64_t* nib_indptr, cons
                              const float* sf, int32_t n_rows, int32_t genes, const float* gene_mean,
                              const float* gene_inv_std, int32_t use_size_factors, int32_t use_log1p,
                              float* Y, void* X, int32_t x_dtype, float* sf_out, void* stream);
+/* The same with the exact transform of dca_set_input_transform_exact (dca/io.py:99-109 as dca_normalize_write computes
+ * it): n_counts = device fp64 [n_rows] totals of these rows (needed with DCA_PRE_SIZE_FACTORS), gene_mean / gene_std =
+ * device fp64 [genes].  sf_out[r] = float(n_counts[r] / median) (1 without DCA_PRE_SIZE_FACTORS). */
+int dca_expand_packed_counts_exact(const void* packed, int32_t bits, const int64_t* ovf_indptr, const void* ovf_entries,
+                                   const double* n_counts, int32_t n_rows, int32_t genes, double median, int32_t flags,
+                                   const double* gene_mean, const double* gene_std, float* Y, void* X, int32_t x_dtype,
+                                   float* sf_out, void* stream);
+int dca_expand_sparse_counts_exact(const void* bitmap, const int64_t* nib_indptr, const void* nibbles,
+                                   int32_t max_row_nibble_bytes, const int64_t* ovf_indptr, const void* ovf_entries,
+                                   const double* n_counts, int32_t n_rows, int32_t genes, double median, int32_t flags,
+                                   const double* gene_mean, const double* gene_std, float* Y, void* X, int32_t x_dtype,
+                                   float* sf_out, void* stream);
 
 /* ---- stand-alone kernels (parity tests, profiling) -------------------------------------- */
 /* ZINB / NB negative log-likelihood forward + backward, one pass (dca/loss.py:72-156 and its
@@ -421,6 +454,28 @@ int dca_log_moments(const float* Y, int64_t ldy, int64_t n_cells, int32_t genes,
 int dca_normalize_write(const float* Y, int64_t ldy, int64_t n_cells, int32_t genes, const double* n_counts,
                         double median, int32_t flags, const double* mean, const double* std, void* X, int32_t x_dtype,
                         int64_t ldx, void* stream);
+/* The statistics of dca_count_totals and dca_log_moments over an n_cells-row matrix fed in row chunks (out-of-core
+ * preprocessing of dca/io.py:88-111: the matrix never exists whole in device memory).  Every chunking gives the same
+ * bits as the whole-matrix call: the chunk kernels run the CTA plan of the whole matrix and carry each warp's fp64
+ * sums in the workspace from one chunk to the next.  A pass is dca_stats_begin, then the *_rows call for rows
+ * [row0, row0 + n_rows) of every chunk -- in row order, without gaps or overlaps, Y holding those rows -- then the
+ * *_finish call.  Pass 0 (totals): cell_totals (device fp64 [n_cells], or NULL) receives the chunk's per-cell totals
+ * at [row0, row0 + n_rows); the finish writes gene_totals and *n_bad (either may be NULL).  Passes 1 and 2 (moments):
+ * n_counts (device fp64 [n_cells], indexed by row) and median with DCA_PRE_SIZE_FACTORS; pass 2 reads the mean pass 1
+ * finished; finish(1) writes the mean, finish(2) the std (without DCA_PRE_SCALE: 0 and 1; the rows calls then do
+ * nothing).  The workspace (dca_stats_workspace_bytes; about slices x 8 x genes doubles, 18 MB at 20000 genes, plus
+ * 8 bytes per gene block and row of the largest chunk) belongs to one pass at a time.  No atomics. */
+int dca_stats_workspace_bytes(int64_t n_cells, int32_t genes, int64_t max_chunk_rows, size_t* bytes);
+int dca_stats_begin(int64_t n_cells, int32_t genes, void* workspace, size_t workspace_bytes, void* stream);
+int dca_count_totals_rows(const float* Y, int64_t ldy, int64_t row0, int64_t n_rows, int64_t n_cells, int32_t genes,
+                          double* cell_totals, void* workspace, size_t workspace_bytes, void* stream);
+int dca_count_totals_finish(int64_t n_cells, int32_t genes, double* gene_totals, int64_t* n_bad, void* workspace,
+                            size_t workspace_bytes, void* stream);
+int dca_log_moments_rows(int32_t pass, const float* Y, int64_t ldy, int64_t row0, int64_t n_rows, int64_t n_cells,
+                         int32_t genes, const double* n_counts, double median, int32_t flags, const double* mean,
+                         void* workspace, size_t workspace_bytes, void* stream);
+int dca_log_moments_finish(int32_t pass, int64_t n_cells, int32_t genes, int32_t flags, double* out, void* workspace,
+                           size_t workspace_bytes, void* stream);
 
 /* Single-tile wgmma probe used by the tests to pin the operand descriptor conventions: D[128 x N] =
  * A . B with bf16 operands; a K-major operand is stored [MN x K], an MN-major one [K x MN].
