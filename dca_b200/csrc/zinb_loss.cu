@@ -844,53 +844,68 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
 // computed, so the fp32 mean / dispersion / pi never reach HBM.  Per element the kernel moves the count (4 B in) and the
 // three bf16 gradients (6 B out); H3 and the head weights are re-read from L2.
 //
-// One CTA = three warpgroups sharing the bf16 weights of one 128-gene tile (3 x 16 KB, TMA).  A CTA owns a contiguous range
+// One CTA = four warpgroups sharing the bf16 weights of one 128-gene tile (3 x 16 KB, TMA).  A CTA owns a contiguous range
 // of (gene tile, 64-cell block) units, tile-major; its warpgroups take the blocks of a tile in turn.  Per block a warpgroup
-// loads H3 (TMA, 8 KB) and, for each of the two 8-row halves of its warps' accumulator fragments ("pieces"), runs the three
-// m64n128 products of head_tile_mma (the same products and epilogue as heads_fwd_kernel, so the activations are bit-identical
-// to K2's outputs), keeps the fragment rows of the piece and stages their activations in warp-private shared memory
-// (8 rows x 128 genes x 3 heads, fp32).  The warp then walks its 8 rows with zinb_row_ring -- the per-row body of the ring
-// kernel, with the same warp / lane / 128-gene mapping -- and stores bf16 dZ.  Recomputing the products for the second
-// piece costs tensor time the kernel has to spare and halves the staging, which is what fits three warpgroups on an SM.
+// loads H3 (TMA, 8 KB) and, for each of the four 4-row quarters of its warps' accumulator fragments ("pieces"), runs the
+// three m64n128 products of head_tile_mma (the same products as heads_fwd_kernel, so the accumulators are bit-identical to
+// K2's) and stages the raw fp32 accumulators of the piece's rows in warp-private shared memory (4 rows x 128 genes x
+// 3 heads); the counts of those rows stream into the warp's slot by cp.async under the products, so that no registers
+// hold them next to the accumulators.  The warp then walks its 4 rows: each lane applies K2's epilogue (head_out, same
+// inputs, so m, theta and pi carry K2's bits) to its own 4 genes x 3 heads and runs zinb_row_ring -- the per-row body of
+// the ring kernel, with the same warp / lane / 128-gene mapping -- and stores bf16 dZ.  Recomputing the products for
+// every piece costs tensor time but quarters the staging, which with at most 128 registers per thread is what fits four
+// warpgroups (16 warps to hide the latency of the row walk) on an SM.
 namespace hl {
-constexpr int kWG = 3;                                       // warpgroups per CTA
+constexpr int kWG = 4;                                       // warpgroups per CTA
 constexpr int kCtaThreads = 128 * kWG;
-constexpr int kRows = 8;                                     // rows per warp and piece
+constexpr int kRows = 4;                                     // rows per warp and piece
+constexpr int kPieces = 16 / kRows;                          // pieces per 16-row warp fragment
 constexpr uint32_t kWHeadBytes = 64 * 128 * 2;               // one head's W tile: two 64-gene boxes of [64 k][64 genes] bf16
 constexpr uint32_t kHBytes = 64 * 64 * 2;                    // one 64-cell H3 block
-constexpr uint32_t kRowBytes = 3 * 128 * 4;                  // m | d | pi of one row's 128 genes
+constexpr uint32_t kRowBytes = 3 * 128 * 4;                  // m | d | pi accumulators of one row's 128 genes
 constexpr uint32_t kQPad = 512;                              // the NB queue of row k (2 KB) starts 512 B ahead of row k's
-constexpr uint32_t kWarpBytes = kQPad + kRows * kRowBytes;   // operands and overwrites them once they are in registers
+                                                             // operands and overwrites them once they are in registers
+constexpr uint32_t kOffY = kQPad + kRows * kRowBytes;        // the piece's count rows (cp.async, 16 B per lane and row)
+constexpr uint32_t kWarpBytes = kOffY + kRows * 128 * 4;
 constexpr uint32_t kOffH = 3 * kWHeadBytes;
 constexpr uint32_t kOffStage = kOffH + kWG * kHBytes;
 constexpr uint32_t kOffBias = kOffStage + kWG * 4 * kWarpBytes;
 constexpr uint32_t kSmemBytes = kOffBias + 3 * 128 * 4 + 1024;   // + alignment of the swizzled TMA destinations
+static_assert(kSmemBytes + 1024 <= 227 * 1024, "heads_loss_kernel: dynamic + 1 KB static shared memory over the sm_90 limit");
 
 struct Params {
   const float* bias[3];
   const float* Y; int64_t ldy; const int32_t* rows; const float* sf;
-  int B, G, nblk; long long units;
+  int B, G, nblk, units;                                     // units < 2^31 (checked on the host)
   float ridge, inv_n;
   __nv_bfloat16* dz[3]; int64_t ldz;
   double* loss_partial; const float* lf;
 };
 
-// float4 slot of genes 4i..4i+3 in staged row k: XOR-swizzled so that the fragment stores of the 8 rows of a piece spread
+// float4 slot of genes 4i..4i+3 in staged row k: XOR-swizzled so that the fragment stores of the 4 rows of a piece spread
 // over all banks (rows are 1536 B apart, a multiple of 128 B)
 __device__ __forceinline__ uint32_t slot16(int i, int k) { return (uint32_t)((i ^ ((2 * k) & 6)) * 16); }
 
-template <int KIND>
-__device__ __forceinline__ void stage_head(const float (&acc)[64], int piece, const float* s_bias, uint8_t* rows_base) {
-  const int lane = threadIdx.x & 31, k = lane >> 2;
-  uint8_t* dst = rows_base + k * kRowBytes + (KIND == EPI_MEAN_ACT ? 0 : (KIND == EPI_DISP_ACT ? 512 : 1024)) + (lane & 1) * 8;
+// Rows 4 piece .. 4 piece + 3 of the warp's 16 fragment rows are held by lanes 16 (piece & 1) .. + 15, in acc[4c], acc[4c+1]
+// (pieces 0, 1) or acc[4c+2], acc[4c+3] (pieces 2, 3).  Those lanes store them, raw, at head offset `head_base`.
+__device__ __forceinline__ void stage_acc(const float (&acc)[64], int piece, uint8_t* head_base) {
+  const int lane = threadIdx.x & 31, k = (lane >> 2) & 3;
+  if ((lane >> 4) != (piece & 1)) return;
+  const bool hi = piece >= 2;
+  uint8_t* dst = head_base + k * kRowBytes + (lane & 1) * 8;
 #pragma unroll
   for (int c = 0; c < 16; ++c) {
     const int g = 8 * c + 2 * (lane & 3);
-    const float2 b = *reinterpret_cast<const float2*>(s_bias + g);
     *reinterpret_cast<float2*>(dst + slot16(g >> 2, k)) =
-        make_float2(tc::head_out<KIND>(piece ? acc[4 * c + 2] : acc[4 * c], b.x, 1.0f),
-                    tc::head_out<KIND>(piece ? acc[4 * c + 3] : acc[4 * c + 1], b.y, 1.0f));
+        make_float2(hi ? acc[4 * c + 2] : acc[4 * c], hi ? acc[4 * c + 3] : acc[4 * c + 1]);
   }
+}
+
+// K2's epilogue of one head on a lane's 4 genes
+template <int KIND>
+__device__ __forceinline__ float4 head_out4(const float4 a, const float4 b) {
+  return make_float4(tc::head_out<KIND>(a.x, b.x, 1.0f), tc::head_out<KIND>(a.y, b.y, 1.0f),
+                     tc::head_out<KIND>(a.z, b.z, 1.0f), tc::head_out<KIND>(a.w, b.w, 1.0f));
 }
 }  // namespace hl
 
@@ -909,8 +924,9 @@ heads_loss_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_consta
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
   float* s_bias = reinterpret_cast<float*>(smem + kOffBias);
   uint8_t* h_buf = smem + kOffH + wg * kHBytes;
-  uint8_t* wbase = smem + kOffStage + (wg * 4 + warp) * kWarpBytes;       // this warp's queue pad + 8 staged rows
+  uint8_t* wbase = smem + kOffStage + (wg * 4 + warp) * kWarpBytes;       // this warp's queue pad + 4 staged rows + counts
   uint8_t* rows_base = wbase + kQPad;
+  const uint32_t my_y = smem_u32(wbase + kOffY) + lane * 16;             // my 16 bytes of the piece's count row 0
   if (tid < zmath::kLogFactN) lf[tid] = p.lf[tid];
   if (tid == 0) {
     mbar_init(&w_bar, 1);
@@ -922,15 +938,15 @@ heads_loss_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_consta
   auto load_h = [&](int blk) {
     if ((tid & 127) == 0) { mbar_expect_tx(&h_bar[wg], kHBytes); tma_load_2d(h_buf, &map_h, 0, blk * 64, &h_bar[wg]); }
   };
-  const long long u0 = (long long)blockIdx.x * p.units / gridDim.x, u1 = (long long)(blockIdx.x + 1) * p.units / gridDim.x;
+  const int u0 = (int)((long long)blockIdx.x * p.units / gridDim.x), u1 = (int)((long long)(blockIdx.x + 1) * p.units / gridDim.x);
   uint32_t w_phase = 0, h_phase = 0;
   float lsum_lg = 0.f, lsum_nb = 0.f, lsum_r = 0.f;
   float tacc[kVec] = {0.f, 0.f, 0.f, 0.f};
-  for (long long u = u0; u < u1;) {
-    const int t = (int)(u / p.nblk);
-    const long long seg_end = min(u1, (long long)(t + 1) * p.nblk);
-    const int b_end = (int)(seg_end - (long long)t * p.nblk);
-    int blk = (int)(u - (long long)t * p.nblk) + wg;
+  for (int u = u0; u < u1;) {
+    const int t = u / p.nblk;
+    const int seg_end = min(u1, (t + 1) * p.nblk);
+    const int b_end = seg_end - t * p.nblk;
+    int blk = u - t * p.nblk + wg;
     __syncthreads();                                                      // every warpgroup is done with the previous tile
     if (tid == 0) {
       mbar_expect_tx(&w_bar, 3 * kWHeadBytes);
@@ -939,9 +955,10 @@ heads_loss_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_consta
         tma_load_2d(smem + h * kWHeadBytes + kWHeadBytes / 2, mw[h], t * 128 + 64, 0, &w_bar);
       }
     }
-    {
+    if (tid < 3 * 128) {
       const int gcol = t * 128 + (tid & 127);                             // 384 threads: one bias of each head each
-      s_bias[tid] = gcol < p.G ? p.bias[tid >> 7][gcol] : 0.f;
+      const float* bias = wg == 0 ? p.bias[0] : (wg == 1 ? p.bias[1] : p.bias[2]);   // (no local copy of p for p.bias[wg])
+      s_bias[tid] = gcol < p.G ? bias[gcol] : 0.f;
     }
     if (blk < b_end) load_h(blk);
     __syncthreads();
@@ -953,43 +970,49 @@ heads_loss_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_consta
     const int64_t gcol0 = (int64_t)t * 128 + col;
     for (; blk < b_end; blk += kWG) {
       mbar_wait(&h_bar[wg], h_phase); h_phase ^= 1;
-      for (int piece = 0; piece < 2; ++piece) {
-        const int r0 = blk * 64 + warp * 16 + piece * kRows;              // first of this warp's 8 rows in the piece
-        int my_yr = 0; float my_sf = 1.f;                                 // lane k < 8: count row / size factor of row r0 + k
+      for (int piece = 0; piece < kPieces; ++piece) {
+        const int r0 = blk * 64 + warp * 16 + piece * kRows;              // first of this warp's 4 rows in the piece
+        int my_yr = 0; float my_sf = 1.f;                                 // lane k < 4: count row / size factor of row r0 + k
         if (lane < kRows && r0 + lane < p.B) {
           my_yr = p.rows ? p.rows[r0 + lane] : r0 + lane;
           my_sf = p.sf ? p.sf[my_yr] : 1.0f;
         }
         float acc[64];
-        float4 yv[kRows];
         head_tile_mma(acc, smem_u32(h_buf), smem_u32(smem));
-        stage_head<EPI_MEAN_ACT>(acc, piece, s_bias, rows_base);
+        stage_acc(acc, piece, rows_base);
 #pragma unroll
         for (int k = 0; k < kRows; ++k) {                                 // counts of the piece, in flight under the products
-          const int yr = __shfl_sync(0xffffffffu, my_yr, k);
-          yv[k] = (r0 + k < p.B) ? ld4_stream(p.Y + (int64_t)yr * p.ldy + gcol0) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const int yr = __shfl_sync(0xffffffffu, my_yr, k);              // (through shared memory: no registers held)
+          if (r0 + k < p.B)
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(my_y + k * 512), "l"(p.Y + (int64_t)yr * p.ldy + gcol0)
+                         : "memory");
         }
+        cp_async_commit();
         head_tile_mma(acc, smem_u32(h_buf), smem_u32(smem) + kWHeadBytes);
-        stage_head<EPI_DISP_ACT>(acc, piece, s_bias + 128, rows_base);
+        stage_acc(acc, piece, rows_base + 512);
         head_tile_mma(acc, smem_u32(h_buf), smem_u32(smem) + 2 * kWHeadBytes);
-        if (piece == 1) {                                                 // the warpgroup is done with this H3 block
+        if (piece == kPieces - 1) {                                       // the warpgroup is done with this H3 block
           named_barrier_sync(1 + wg, 128);
           if (blk + kWG < b_end) load_h(blk + kWG);
         }
-        stage_head<EPI_SIGMOID>(acc, piece, s_bias + 256, rows_base);
+        stage_acc(acc, piece, rows_base + 1024);
+        cp_async_wait<0>();                                               // my count copies have landed (I read only those)
         __syncwarp();
         for (int k = 0; k < kRows; ++k) {
           const int r = r0 + k;
           if (r >= p.B) break;                                            // warp-uniform: the last block's tail
-          const float4 vy = yv[0];
-#pragma unroll
-          for (int j = 0; j + 1 < kRows; ++j) yv[j] = yv[j + 1];
+          float4 vy;
+          asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(vy.x), "=f"(vy.y), "=f"(vy.z), "=f"(vy.w) : "r"(my_y + k * 512)
+                       : "memory");
           const float row_sf = __shfl_sync(0xffffffffu, my_sf, k);
           const uint8_t* src = rows_base + k * kRowBytes + slot16(col >> 2, k);
-          const float4 vm = *reinterpret_cast<const float4*>(src);
-          const float4 vd = *reinterpret_cast<const float4*>(src + 512);
-          const float4 vp = *reinterpret_cast<const float4*>(src + 1024);
+          const float4 am = *reinterpret_cast<const float4*>(src);
+          const float4 ad = *reinterpret_cast<const float4*>(src + 512);
+          const float4 ap = *reinterpret_cast<const float4*>(src + 1024);
           __syncwarp();                                                   // row k's queue overwrites these operands
+          const float4 vm = head_out4<EPI_MEAN_ACT>(am, *reinterpret_cast<const float4*>(s_bias + col));
+          const float4 vd = head_out4<EPI_DISP_ACT>(ad, *reinterpret_cast<const float4*>(s_bias + 128 + col));
+          const float4 vp = head_out4<EPI_SIGMOID>(ap, *reinterpret_cast<const float4*>(s_bias + 256 + col));
           float4* q = reinterpret_cast<float4*>(wbase + k * kRowBytes);
           const RowGrads g = zinb_row_ring<true>(vy, vm, vd, vp, row_sf, active, p.ridge, p.inv_n, q, lf, lsum_lg, lsum_nb,
                                                  lsum_r, tacc, [] {});
@@ -1190,7 +1213,9 @@ int heads_loss_tc(const HeadsLossArgs& a, cudaStream_t s) {
   for (int i = 0; i < 3; ++i) { p.bias[i] = a.bias[i]; p.dz[i] = a.dz[i]; }
   p.Y = a.Y; p.ldy = a.ldy; p.rows = a.rows; p.sf = a.sf; p.B = B; p.G = G; p.ldz = a.ldz;
   p.nblk = cdiv(B, 64);
-  p.units = (long long)cdiv(G, 128) * p.nblk;
+  const long long units = (long long)cdiv(G, 128) * p.nblk;         // 2^31 units would be over 2^44 counts
+  if (units > INT_MAX) { set_error("heads_loss_tc: %lld (gene tile, cell block) units, over 2^31 - 1", units); return DCA_ERR_BAD_ARG; }
+  p.units = (int)units;
   p.ridge = a.ridge; p.inv_n = a.inv_n;
   p.loss_partial = reinterpret_cast<double*>(a.ws); p.lf = lf_dev;
   FoldArgs fa{reinterpret_cast<unsigned*>(reinterpret_cast<char*>(a.ws) + sizeof(double) * (size_t)kMaxBlocks), a.loss_sum,
