@@ -20,27 +20,148 @@ def _dense(X):
 
 
 def read_text_or_h5ad(path: str):
-    """sc.read(path, first_column_names=True) -- dca/io.py:59."""
+    """sc.read(path, first_column_names=True) -- dca/io.py:59.  Text tables go through the GPU reader when it can take
+    them (read_counts_text), otherwise through pandas; both give the same AnnData."""
+    return _read_path(path, False)[0]
+
+
+_TEXT_EXTS = (".tsv", ".txt", ".csv")
+# magic numbers of the compressed formats pandas would decompress (or choke on) under a plain text extension
+_COMPRESSED_MAGIC = (b"\x1f\x8b", b"BZh", b"\xfd7zXZ\x00", b"\x28\xb5\x2f\xfd", b"PK\x03\x04")
+
+
+def _read_path(path, transpose):
+    """(AnnData, transposed): transposed is True when the GPU reader already returned the cells x genes orientation."""
     ext = os.path.splitext(path)[1].lower()
     if ext == ".h5ad":
         try:
             import anndata  # type: ignore
         except ImportError as e:
             raise ImportError("reading .h5ad needs the anndata package, which is not installed") from e
-        return anndata.read_h5ad(path)
+        return anndata.read_h5ad(path), False
     sep = "," if ext == ".csv" else "\t"
+    if ext in _TEXT_EXTS and _cuda_available():
+        ad = read_counts_text(path, sep, transpose)
+        if ad is not None:
+            return ad, transpose
+    return _read_text_pandas(path, sep), False
+
+
+def _read_text_pandas(path, sep):
+    """The pandas reader of a text table (genes x cells as in the file)."""
     tab = pd.read_csv(path, sep=sep, index_col=0)
     return AnnData(tab.values.astype(np.float32), obs=pd.DataFrame(index=tab.index.astype(str)),
                    var=pd.DataFrame(index=tab.columns.astype(str)))
 
 
+def _cuda_available():
+    try:
+        import torch
+        return torch.cuda.is_available()
+    except Exception:
+        return False
+
+
+def read_counts_text(path, sep, transpose=False, chunk_bytes=0, device=None):
+    """The AnnData _read_text_pandas(path, sep) gives (its .transpose() with transpose=True), parsed on a CUDA device
+    by dca_read_text_counts (csrc/read_text.cu), bit for bit; None when the file is not one the GPU reader takes
+    exactly (include/dca_b200.h lists them), is compressed, or its matrix does not fit in free device memory.
+
+    The file's bytes go to the device in chunks of chunk_bytes (0: 64 MB) and the float32 matrix comes back.  Column
+    labels come from pandas reading the header alone; row labels from pandas reading a two-column table made of the
+    header's first field and every line's first field, in the row chunks pandas' own reader infers types in, so they
+    are the same strings (numeric-looking labels, NA tokens, booleans, duplicates, the index name, a BOM)."""
+    import ctypes as C
+    import torch
+    from . import _lib
+    with open(path, "rb") as f:
+        if any(f.read(6).startswith(m) for m in _COMPRESSED_MAGIC):
+            return None
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.type != "cuda":
+        raise ValueError("read_counts_text parses on a CUDA device (got %s)" % dev)
+    lib = _lib.load()
+    sep_b = sep.encode()
+    if len(sep_b) != 1:
+        return None
+    info = np.zeros(4, dtype=np.int64)
+    stream = torch.cuda.current_stream(dev)
+    with torch.cuda.device(dev):
+        st = lib.dca_read_text_counts(os.fsencode(path), sep_b[0], int(bool(transpose)), int(chunk_bytes), dev.index,
+                                      C.c_void_p(stream.cuda_stream), None, 0, None, None, 0, info.ctypes.data)
+        if st == -3:
+            return None
+        _lib.check(st, "dca_read_text_counts")
+        rows, cols, nlab, work = (int(v) for v in info)
+        if rows * cols * 4 + work > torch.cuda.mem_get_info(dev)[0]:
+            return None
+        columns = pd.read_csv(path, sep=sep, index_col=0, nrows=0).columns
+        if len(columns) != cols:
+            return None
+        out = torch.empty((cols, rows) if transpose else (rows, cols), dtype=torch.float32, device=dev)
+        offsets = np.zeros(rows + 1, dtype=np.int64)
+        labels = np.zeros(max(nlab, 1), dtype=np.uint8)
+        st = lib.dca_read_text_counts(os.fsencode(path), sep_b[0], int(bool(transpose)), int(chunk_bytes), dev.index,
+                                      C.c_void_p(stream.cuda_stream), C.c_void_p(out.data_ptr()), out.numel(),
+                                      offsets.ctypes.data, labels.ctypes.data, nlab, info.ctypes.data)
+        if st == -3:                 # the file changed between the two passes
+            return None
+        _lib.check(st, "dca_read_text_counts")
+        X = out.cpu().numpy()
+    del out
+    index = _row_labels(path, sep_b, labels[:nlab].tobytes(), offsets, cols + 1)
+    if index is None:
+        return None
+    obs = pd.DataFrame(index=index.astype(str))
+    var = pd.DataFrame(index=columns.astype(str))
+    return AnnData(X, obs=var, var=obs) if transpose else AnnData(X, obs=obs, var=var)
+
+
+def _pandas_chunk_rows(width):
+    """Rows per chunk in which pandas' C reader (low_memory=True) infers column types for a table of `width` fields:
+    the largest power of two below half of 2**20 // width."""
+    heuristic = 2 ** 20 // width
+    n = 1
+    while n * 2 < heuristic:
+        n *= 2
+    return n
+
+
+def _row_labels(path, sep, labels, offsets, width):
+    """The index pd.read_csv(path, sep=sep, index_col=0) gives, from the header's first field and the first field of
+    every data line: pandas reads them as a two-column table (a second column keeps an empty label from being a blank
+    line), chunk by chunk in the chunks its reader of the `width`-field file infers types in.  None when the chunks
+    infer different types (pandas then mixes them into one object column, which this does not restate)."""
+    import io as _io
+    with open(path, "rb") as f:
+        header = f.readline()
+    head = header.split(sep, 1)[0]
+    n = len(offsets) - 1
+    starts, ends = offsets[:-1], offsets[1:]
+    body = b"".join([labels[a:b] + sep + b"0\n" for a, b in zip(starts.tolist(), ends.tolist())])
+    text = head + sep + b"x\n" + body
+    try:
+        whole = pd.read_csv(_io.BytesIO(text), sep=sep.decode(), index_col=0, low_memory=False).index
+        step = _pandas_chunk_rows(width)
+        if n > step and whole.dtype != np.int64:
+            kinds = {c.index.dtype for c in pd.read_csv(_io.BytesIO(text), sep=sep.decode(), index_col=0, chunksize=step,
+                                                        low_memory=False)}
+            if len(kinds) != 1:
+                return None
+    except Exception:
+        return None
+    return whole
+
+
 def read_dataset(adata, transpose=False, test_split=False, copy=False, check_counts=True):
-    """dca/io.py:53-85."""
+    """dca/io.py:53-85.  A path to a text table is read on the GPU when read_counts_text takes it, which transposes on
+    the device; it only returns integer counts, so the check below passes in either orientation."""
+    transposed = False
     if is_anndata(adata):
         if copy:
             adata = adata.copy()
     elif isinstance(adata, str):
-        adata = read_text_or_h5ad(adata)
+        adata, transposed = _read_path(adata, transpose)
     else:
         raise NotImplementedError
 
@@ -50,7 +171,7 @@ def read_dataset(adata, transpose=False, test_split=False, copy=False, check_cou
         norm_error = 'Make sure that the dataset (adata.X) contains unnormalized count data.'
         assert np.all(X_subset.astype(int) == X_subset), norm_error
 
-    if transpose:
+    if transpose and not transposed:
         adata = adata.transpose()
 
     if test_split:

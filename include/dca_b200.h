@@ -508,6 +508,29 @@ int dca_write_text_matrix(const char* path, const void* matrix, int32_t is_float
                           int64_t ld, const char* const* row_names, const char* const* col_names,
                           int32_t transpose, int32_t threads);
 
+/* GPU reader of a count table in text form (dca_b200/io.py:read_counts_text): a header line, then one line per gene
+ * whose first field is its label and whose other fields are counts, separated by `sep` (',' or '\t').  It gives the
+ * matrix pandas.read_csv(path, sep=sep, index_col=0).values.astype(numpy.float32) gives, bit for bit, for exactly the
+ * files whose
+ *   - header line has as many fields as every data line, and no quote, NUL or carriage return before its line end;
+ *   - lines end in '\n' or "\r\n" (the final one may have no line end), none is blank and none holds a quote or NUL;
+ *   - value fields are non-empty [0-9]+ or [0-9]+\.0* with at most 18 digits (and no value above 2^53 when some
+ *     field has a '.'), at most 64 bytes long;
+ *   - data lines each fit in chunk_bytes.
+ * Any other file returns DCA_ERR_UNSUPPORTED with the first reason in file order in dca_last_error(), and nothing is
+ * returned.  Two calls with the same arguments:
+ *   1. out == NULL: reads and checks the file; info[0..3] = data lines, value columns, total label bytes, device bytes
+ *      the chunk buffers of the second call take besides `out`.
+ *   2. out: device float32 [rows x cols] (row = data line), or [cols x rows] with transpose != 0; info as the first
+ *      call returned it; label_offsets: host int64 [rows + 1]; label_bytes: host char [info[2]]: the first field of data
+ *      line r is label_bytes[label_offsets[r] .. label_offsets[r + 1]), raw bytes.
+ * Each call reads the file once through two pinned chunk buffers (chunk_bytes each, 0 = 64 MB), overlapping the disk
+ * read with the copy and the kernels on `stream` (of `device`), and returns when they are done.  Without a CUDA
+ * device it returns DCA_ERR_NO_DEVICE. */
+int dca_read_text_counts(const char* path, int32_t sep, int32_t transpose, int64_t chunk_bytes, int32_t device,
+                         void* stream, float* out, int64_t out_elems, int64_t* label_offsets, char* label_bytes,
+                         int64_t label_cap, int64_t* info);
+
 /* Host-side packer for dca_stream_begin_packed (multi-threaded counterpart of dca_b200/io.py:pack_counts; no
  * reference counterpart).  counts: HOST matrix rows x cols (ld elements per row) of dtype 0 float32, 1 float64,
  * 2 uint16, 3 int32, 4 int64 holding non-negative integers.  dca_count_escapes fills per_row[w*rows + r] with the
