@@ -55,11 +55,14 @@ _OPTIONS = [
                          help='With --preprocess device: keep the raw counts packed in host memory and stream them '
                               'through the GPU for preprocessing, training and prediction (data larger than GPU memory; '
                               'same results)')),
+    (('--packed',), dict(dest='packed', action='store_true',
+                         help='With --preprocess device: keep the raw counts packed in GPU memory (several times more '
+                              'cells than the normalised matrix; every batch is expanded on the GPU; same results)')),
 ]
 
 _DEFAULTS = dict(transpose=False, testsplit=False, saveweights=False, sizefactors=True, batchnorm=True,
                  checkcounts=True, norminput=True, hyper=False, debug=False, tensorboard=False, loginput=True,
-                 stream=False)
+                 stream=False, packed=False)
 
 
 def build_parser():

@@ -54,6 +54,15 @@ class TensorInfo(C.Structure):
                 ("rows", C.c_int32), ("cols", C.c_int32)]
 
 
+class PackedCountsDesc(C.Structure):
+    """dca_packed_counts: device pointers of one packed count matrix (include/dca_b200.h)."""
+    _fields_ = [
+        ("struct_bytes", C.c_int32), ("bits", C.c_int32), ("n_rows", C.c_int64), ("genes", C.c_int32),
+        ("max_row_nibble_bytes", C.c_int32), ("packed", C.c_void_p), ("ovf_indptr", C.c_void_p),
+        ("ovf_entries", C.c_void_p), ("nib_indptr", C.c_void_p), ("nibbles", C.c_void_p), ("n_counts", C.c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); every symbol declared in include/dca_b200.h
 _vp, _i32, _i64, _f, _sz = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t
 PROTOTYPES = {
@@ -149,6 +158,13 @@ PROTOTYPES = {
                                                  _vp, _i32, _vp, _vp]),
     "dca_expand_sparse_counts_exact": (C.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _i32, C.c_double, _i32, _vp,
                                                  _vp, _vp, _vp, _i32, _vp, _vp]),
+    "dca_pack_count_rows": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _i64, _vp]),
+    "dca_pack_rows_device": (C.c_int, [_vp, _i64, _i64, _i64, C.POINTER(PackedCountsDesc), _vp]),
+    "dca_expand_rows_exact": (C.c_int, [C.POINTER(PackedCountsDesc), _vp, _i32, C.c_double, _i32, _vp, _vp, _vp, _vp, _i32,
+                                        _vp, _vp]),
+    "dca_packed_train_step": (C.c_int, [_vp, C.POINTER(PackedCountsDesc), _vp, _i32, _vp]),
+    "dca_packed_eval_step": (C.c_int, [_vp, C.POINTER(PackedCountsDesc), _vp, _i32, _vp]),
+    "dca_packed_predict": (C.c_int, [_vp, C.POINTER(PackedCountsDesc), _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp]),
     "dca_launch_count": (C.c_int64, []),
     "dca_set_tunable": (C.c_int, [C.c_char_p, C.c_int64]),
 }

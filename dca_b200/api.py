@@ -49,6 +49,14 @@ def dca(adata, mode='denoise', ae_type='nb-conddisp', normalize_per_cell=True, s
         raise ValueError("training_kwds['preprocess'] must be 'host' or 'device', got %r" % (preprocess,))
     # with 'preprocess': 'device', 'stream': True trains out of core (stream_data.StreamedDataset: packed counts in host
     # memory, the same results as the resident dataset); 'auto' does so when the resident dataset would not fit
+    # 'packed': True keeps the raw counts packed in device memory (packed_data.PackedDeviceDataset: several times the
+    # cells of the resident dataset, the same results)
+    packed = training_kwds.pop('packed', False)
+    if packed and preprocess != 'device':
+        raise ValueError("training_kwds['packed'] needs 'preprocess': 'device'")
+    if packed and training_kwds.get('stream', False):
+        raise ValueError("training_kwds 'packed' and 'stream' exclude each other: the counts stay packed in device or "
+                         "in host memory")
     streamed = False
     if preprocess == 'device' and training_kwds.get('stream', False) in (True, 'auto'):
         streamed = training_kwds.pop('stream')
@@ -56,7 +64,7 @@ def dca(adata, mode='denoise', ae_type='nb-conddisp', normalize_per_cell=True, s
     # raw counts go to adata.raw; the input object is copied only when copy=True  (dca/api.py:156-160)
     adata = read_dataset(adata, transpose=False, test_split=False, copy=copy, check_counts=check_counts)
 
-    dd = sd = None
+    dd = sd = pd_ = None
     x_dtype = network_kwds.get('x_dtype', 'float32')
     if streamed == 'auto':
         from .device_data import DeviceDataset
@@ -69,6 +77,13 @@ def dca(adata, mode='denoise', ae_type='nb-conddisp', normalize_per_cell=True, s
                                          normalize_input=scale, batch=batch_size)
         assert (sd.input_gene_totals >= 1).all(), 'Please remove all-zero genes before using DCA.'
         apply_device_normalize(adata, sd, filter_min_counts=False, set_x=False)
+    elif packed:
+        from .packed_data import PackedDeviceDataset
+        from .io import apply_device_normalize
+        pd_ = PackedDeviceDataset.from_counts(adata.X, None, x_dtype, size_factors=normalize_per_cell,
+                                              logtrans_input=log1p, normalize_input=scale)
+        assert (pd_.input_gene_totals >= 1).all(), 'Please remove all-zero genes before using DCA.'
+        apply_device_normalize(adata, pd_, filter_min_counts=False, set_x=False)
     elif preprocess == 'device':
         # the same steps on the device; adata.X keeps the raw counts until predict() overwrites it
         from .device_data import DeviceDataset
@@ -98,6 +113,10 @@ def dca(adata, mode='denoise', ae_type='nb-conddisp', normalize_per_cell=True, s
         train_mask = np.asarray(adata.obs.dca_split == 'train')
         hist = train(None, net, stream_data=sd.take(train_mask), **fit_args)
         res = net.predict(adata, mode, return_info, copy, stream_data=sd)
+    elif pd_ is not None:
+        train_mask = np.asarray(adata.obs.dca_split == 'train')
+        hist = train(None, net, packed_data=pd_.take(train_mask), **fit_args)
+        res = net.predict(adata, mode, return_info, copy, packed_data=pd_)
     elif dd is None:
         hist = train(adata[adata.obs.dca_split == 'train'], net, **fit_args)
         res = net.predict(adata, mode, return_info, copy)

@@ -115,14 +115,20 @@ struct ExactXform {
   const double* mean; const double* std; const float* x_zero;
 };
 int exact_zero_inputs(const double* mean, const double* std, int n, float* x_zero, cudaStream_t s);
-// ex != nullptr selects the exact transform (sf_in, mean, inv_std, use_sf and use_log1p are then not read)
+// ex != nullptr selects the exact transform (sf_in, mean, inv_std, use_sf and use_log1p are then not read).
+// rows == nullptr: the M rows are the contiguous rows of a batch, with overflow / nibble offsets relative to their first
+// row and sf_in / ex->n_counts indexed by batch row.  rows != nullptr: output row r is source row rows[r] of a whole
+// packed matrix whose offsets are absolute (they index ovf_entries / nibbles directly) and sf_in / ex->n_counts are
+// indexed by source row.
 int expand_counts(const void* cnt, int bits, const float* sf_in, int M, int n, const float* mean, const float* inv_std, int use_sf,
                   int use_log1p, float* Yout, void* Xout, int x_bf16, float* sf_out, const int64_t* ovf_indptr,
-                  const void* ovf_entries, cudaStream_t s, const ExactXform* ex = nullptr);
+                  const void* ovf_entries, cudaStream_t s, const ExactXform* ex = nullptr, const int32_t* rows = nullptr);
 int expand_sparse(const void* bitmap, const int64_t* nib_indptr, const void* nibbles, const float* sf_in, int M, int n,
                   const float* mean, const float* inv_std, int use_sf, int use_log1p, float* Yout, void* Xout, int x_bf16,
                   float* sf_out, const int64_t* ovf_indptr, const void* ovf_entries, int max_row_nibble_bytes, cudaStream_t s,
-                  const ExactXform* ex = nullptr);
+                  const ExactXform* ex = nullptr, const int32_t* rows = nullptr);
+// validity of a dca_packed_counts (pack.cu): DCA_OK, or the status with the message set
+int check_packed_counts(const char* who, const dca_packed_counts* p);
 int gather_rows_bf16(const void* X, int x_bf16, int64_t ldx, const int32_t* rows, int M, int n, __nv_bfloat16* out,
                      cudaStream_t s);
 

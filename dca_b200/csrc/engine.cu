@@ -1425,3 +1425,76 @@ extern "C" int dca_expand_sparse_counts_exact(const void* bitmap, const int64_t*
   return expand_sparse(bitmap, nib_indptr, nibbles, nullptr, n_rows, genes, nullptr, nullptr, 0, 0, Y, X, x_dtype == DCA_BF16,
                        sf_out, ovf_indptr, ovf_entries, max_row_nibble_bytes, (cudaStream_t)stream, &ex);
 }
+
+// ------------------------------------------------------------------------------ packed counts resident in device memory
+namespace {
+// rows[0..n) of src (NULL: rows 0..n-1) -> Y, X, sf with the exact transform ex (ex.n_counts = src->n_counts)
+int expand_packed_rows(const dca_packed_counts* src, const int32_t* rows, int n, const ExactXform& ex, float* Y, void* X,
+                       int x_bf16, float* sf_out, cudaStream_t s) {
+  if (src->bits == 1)
+    return expand_sparse(src->packed, src->nib_indptr, src->nibbles, nullptr, n, src->genes, nullptr, nullptr, 0, 0, Y, X,
+                         x_bf16, sf_out, src->ovf_indptr, src->ovf_entries, src->max_row_nibble_bytes, s, &ex, rows);
+  return expand_counts(src->packed, src->bits, nullptr, n, src->genes, nullptr, nullptr, 0, 0, Y, X, x_bf16, sf_out,
+                       src->ovf_indptr, src->ovf_entries, s, &ex, rows);
+}
+
+// One batch named by row index: expand it into the first expanded-batch buffer on `stream` (the step that follows on the
+// same stream is its only reader), then run `body` (training step, validation or inference forward) on it.
+template <typename Body>
+int packed_run(dca_handle* h, const char* who, const dca_packed_counts* src, const int32_t* rows, int32_t batch,
+               void* stream, Body body) {
+  DCA_NEED_HANDLE(h);
+  Engine& e = h->e;
+  if (e.hs.active) { set_error("%s: a host stream is active (call dca_stream_end first)", who); return DCA_ERR_BAD_ARG; }
+  if (e.cfg.n_in != e.cfg.n_out) { set_error("%s: needs n_in == n_out", who); return DCA_ERR_UNSUPPORTED; }
+  if (e.cfg.n_in % 8 != 0) { set_error("%s: n_in must be a multiple of 8", who); return DCA_ERR_UNSUPPORTED; }
+  DCA_TRY(check_packed_counts(who, src));
+  if (src->genes != e.cfg.n_in) { set_error("%s: the packed counts have %d genes, the engine %d", who, src->genes, e.cfg.n_in); return DCA_ERR_BAD_ARG; }
+  if (batch <= 0 || batch > e.cfg.max_batch) { set_error("%s: batch %d outside (0, max_batch=%d]", who, batch, e.cfg.max_batch); return DCA_ERR_BAD_ARG; }
+  if (!e.tf_exact) { set_error("%s: call dca_set_input_transform_exact first", who); return DCA_ERR_BAD_ARG; }
+  if ((e.tf_flags & DCA_PRE_SIZE_FACTORS) && !src->n_counts) { set_error("%s: size factors need the row totals (n_counts)", who); return DCA_ERR_BAD_ARG; }
+  cudaStream_t s = (cudaStream_t)stream;
+  const ExactXform ex{src->n_counts, e.tf_median, e.tf_flags, reinterpret_cast<const double*>(e.base + e.o_gmean64),
+                      reinterpret_cast<const double*>(e.base + e.o_gstd64), e.f(e.o_gx0)};
+  const int x_bf16 = e.tc_enc ? 1 : (e.cfg.x_dtype == DCA_BF16);
+  DCA_TRY(expand_packed_rows(src, rows, batch, ex, e.f(e.o_sy[0]), e.base + e.o_sx[0], x_bf16, e.f(e.o_ssf[0]), s));
+  e.x_override_bf16 = e.tc_enc ? 1 : 0;             // the tensor-core encoder reads the expanded bf16 batch in place
+  const int st = body(e, batch, s);
+  e.x_override_bf16 = 0;
+  return st;
+}
+}  // namespace
+
+extern "C" int dca_expand_rows_exact(const dca_packed_counts* src, const int32_t* rows, int32_t n, double median,
+                                     int32_t flags, const double* gene_mean, const double* gene_std, float* Y, void* X,
+                                     int32_t x_dtype, float* sf_out, void* stream) {
+  DCA_TRY(check_packed_counts("dca_expand_rows_exact", src));
+  DCA_TRY(check_expand_args("dca_expand_rows_exact", src->packed, n, src->genes, src->ovf_indptr, src->ovf_entries, nullptr,
+                            nullptr, Y, X, x_dtype));
+  DCA_TRY(check_exact_args("dca_expand_rows_exact", src->n_counts, median, flags, gene_mean, gene_std));
+  const ExactXform ex{src->n_counts, median, flags, gene_mean, gene_std, nullptr};
+  return expand_packed_rows(src, rows, n, ex, Y, X, x_dtype == DCA_BF16, sf_out, (cudaStream_t)stream);
+}
+
+extern "C" int dca_packed_train_step(dca_handle* h, const dca_packed_counts* src, const int32_t* rows, int32_t batch,
+                                     void* stream) {
+  return packed_run(h, "dca_packed_train_step", src, rows, batch, stream, [](Engine& e, int nb, cudaStream_t s) {
+    return e.train_step(e.base + e.o_sx[0], e.cfg.n_in, e.f(e.o_sy[0]), e.cfg.n_out, e.f(e.o_ssf[0]), nullptr, nb, s, 0);
+  });
+}
+
+extern "C" int dca_packed_eval_step(dca_handle* h, const dca_packed_counts* src, const int32_t* rows, int32_t batch,
+                                    void* stream) {
+  return packed_run(h, "dca_packed_eval_step", src, rows, batch, stream, [](Engine& e, int nb, cudaStream_t s) {
+    return e.eval_step(e.base + e.o_sx[0], e.cfg.n_in, e.f(e.o_sy[0]), e.cfg.n_out, e.f(e.o_ssf[0]), nullptr, nb, s);
+  });
+}
+
+extern "C" int dca_packed_predict(dca_handle* h, const dca_packed_counts* src, const int32_t* rows, int32_t batch,
+                                  float* mean_out, float* disp_out, float* pi_out, int64_t ld_out, float* latent_out,
+                                  void* stream) {
+  return packed_run(h, "dca_packed_predict", src, rows, batch, stream, [&](Engine& e, int nb, cudaStream_t s) {
+    return e.predict(e.base + e.o_sx[0], e.cfg.n_in, e.f(e.o_ssf[0]), nullptr, nb, mean_out, disp_out, pi_out, ld_out,
+                     latent_out, s);
+  });
+}

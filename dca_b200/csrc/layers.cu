@@ -321,9 +321,11 @@ __device__ __forceinline__ float normalise_count(float y, float inv_s, int use_l
   return mean ? (v - mean[c]) * inv_std[c] : v;           // sc.pp.scale                dca/io.py:108-109
 }
 
-__device__ __forceinline__ float overflow_find(const int64_t* __restrict__ indptr, const int2* __restrict__ entries, int r, int c,
-                                               float fallback) {
-  const int64_t base = indptr[0];
+// r: the source row; absolute: the offsets of indptr index `entries` directly (a row-indexed expansion of a whole packed
+// matrix), else they are relative to indptr[0] (a contiguous batch whose entries start at `entries`)
+__device__ __forceinline__ float overflow_find(const int64_t* __restrict__ indptr, const int2* __restrict__ entries, int64_t r,
+                                               int c, float fallback, bool absolute = false) {
+  const int64_t base = absolute ? 0 : indptr[0];
   int64_t lo = indptr[r] - base, hi = indptr[r + 1] - base;
   while (lo < hi) {                                       // entries of a row are sorted by gene
     const int64_t mid = (lo + hi) >> 1;
@@ -334,15 +336,15 @@ __device__ __forceinline__ float overflow_find(const int64_t* __restrict__ indpt
   return fallback;
 }
 // out of line for the float transform (keeps its registers); the exact kernels inline it: a call there costs a spill
-__device__ __noinline__ float overflow_lookup(const int64_t* __restrict__ indptr, const int2* __restrict__ entries, int r, int c,
-                                              float fallback) {
-  return overflow_find(indptr, entries, r, c, fallback);
+__device__ __noinline__ float overflow_lookup(const int64_t* __restrict__ indptr, const int2* __restrict__ entries, int64_t r,
+                                              int c, float fallback, bool absolute) {
+  return overflow_find(indptr, entries, r, c, fallback, absolute);
 }
 
 // The exact variant (EXACT = true, preprocess.cu's arithmetic): sf64 = n_counts[r] / median, X =
 // float(((double)l - mean_g) / std_g) with l = pre_log_value(y, sf64, flags).  Zero counts take the per-gene constant
 // x_zero, so the fp64 division and log1p run on non-zero entries only.
-__device__ __forceinline__ double exact_row_sf(const ExactXform& ex, int r) {
+__device__ __forceinline__ double exact_row_sf(const ExactXform& ex, int64_t r) {
   return (ex.flags & DCA_PRE_SIZE_FACTORS) ? ex.n_counts[r] / ex.median : 1.0;
 }
 __device__ __forceinline__ float exact_count(float y, double sf64, const ExactXform& ex, int c) {
@@ -360,17 +362,18 @@ __global__ void expand_counts_kernel(const unsigned char* __restrict__ cnt, cons
                                      const float* __restrict__ mean, const float* __restrict__ inv_std, int use_sf,
                                      int use_log1p, float* __restrict__ Yout, XT* __restrict__ Xout, float* __restrict__ sf_out,
                                      const int64_t* __restrict__ ovf_indptr, const int2* __restrict__ ovf_entries,
-                                     ExactXform ex) {
+                                     ExactXform ex, const int32_t* __restrict__ rows) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int per_row = n / 8;
   if (i >= (int64_t)M * per_row) return;
   const int r = (int)(i / per_row), c = (int)(i % per_row) * 8;
-  const double sf64 = EXACT ? exact_row_sf(ex, r) : 1.0;
-  const float s = EXACT ? (float)sf64 : (sf_in ? sf_in[r] : 1.0f);
+  const int64_t sr = rows ? (int64_t)rows[r] : (int64_t)r;        // source row (ROWS: any row of the whole matrix)
+  const double sf64 = EXACT ? exact_row_sf(ex, sr) : 1.0;
+  const float s = EXACT ? (float)sf64 : (sf_in ? sf_in[sr] : 1.0f);
   if (c == 0 && sf_out) sf_out[r] = s;
   const float inv_s = use_sf ? 1.0f / s : 1.0f;
   uint32_t q[8];
-  const unsigned char* src = cnt + ((int64_t)r * n + c) * BITS / 8;
+  const unsigned char* src = cnt + (sr * n + c) * BITS / 8;
   if (BITS == 16) {
     const uint4 raw = *reinterpret_cast<const uint4*>(src);
     const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
@@ -392,7 +395,8 @@ __global__ void expand_counts_kernel(const unsigned char* __restrict__ cnt, cons
   for (int k = 0; k < 8; ++k) {
     y[k] = (float)q[k];
     if (ovf_indptr && q[k] == kEsc)
-      y[k] = EXACT ? overflow_find(ovf_indptr, ovf_entries, r, c + k, y[k]) : overflow_lookup(ovf_indptr, ovf_entries, r, c + k, y[k]);
+      y[k] = EXACT ? overflow_find(ovf_indptr, ovf_entries, sr, c + k, y[k], rows != nullptr)
+                   : overflow_lookup(ovf_indptr, ovf_entries, sr, c + k, y[k], rows != nullptr);
     x[k] = EXACT ? exact_count(y[k], sf64, ex, c + k) : normalise_count(y[k], inv_s, use_log1p, mean, inv_std, c + k);
   }
   float* yo = Yout + (int64_t)r * n + c;
@@ -426,7 +430,7 @@ expand_sparse_kernel(const uint32_t* __restrict__ bitmap, const int64_t* __restr
                      const float* __restrict__ mean, const float* __restrict__ inv_std, int use_sf, int use_log1p,
                      float* __restrict__ Yout, XT* __restrict__ Xout, float* __restrict__ sf_out,
                      const int64_t* __restrict__ ovf_indptr, const int2* __restrict__ ovf_entries, int nib_cap,
-                     ExactXform ex) {
+                     ExactXform ex, const int32_t* __restrict__ rows) {
   // One block per row.  Phase 0: the row's bitmap and its nibble bytes go to shared memory with thread-strided loads (all in
   // flight at once; the first version chased them from global memory, one dependent byte load after another: 0.25 ms per
   // 4096 x 20000 batch, 3 x what its 0.5 GB of stores need).  Phase 1: thread t popcounts S consecutive bitmap bytes and
@@ -439,21 +443,24 @@ expand_sparse_kernel(const uint32_t* __restrict__ bitmap, const int64_t* __restr
   __shared__ int warp_tot[8];
   const int r = blockIdx.x;
   if (r >= M) return;
+  // source row: rows[r] of the whole matrix (offsets absolute), else row r of a contiguous batch (offsets relative to
+  // its first row)
+  const int64_t sr = rows ? (int64_t)rows[r] : (int64_t)r;
   const int nbytes = n / 8;
   unsigned short* pre = reinterpret_cast<unsigned short*>(sp_dyn);
   unsigned char* s_bm = sp_dyn + ((2 * nbytes + 15) & ~15);
   unsigned char* s_nib = s_bm + ((nbytes + 15) & ~15);
-  const unsigned char* bmg = reinterpret_cast<const unsigned char*>(bitmap) + (int64_t)r * nbytes;
-  const int64_t nib0 = nib_indptr[r] - nib_indptr[0];
-  const int nib_len = (int)(nib_indptr[r + 1] - nib_indptr[r]);
+  const unsigned char* bmg = reinterpret_cast<const unsigned char*>(bitmap) + sr * nbytes;
+  const int64_t nib0 = nib_indptr[sr] - (rows ? 0 : nib_indptr[0]);
+  const int nib_len = (int)(nib_indptr[sr + 1] - nib_indptr[sr]);
   const unsigned char* nibg = nibbles + nib0;
   for (int i = threadIdx.x; i < nbytes; i += 256) s_bm[i] = bmg[i];
   const bool nib_smem = nib_len <= nib_cap;                 // (always, when the host sized the launch from this batch)
   if (nib_smem) for (int i = threadIdx.x; i < nib_len; i += 256) s_nib[i] = nibg[i];
   const unsigned char* bmb = s_bm;
   const unsigned char* nib = nib_smem ? s_nib : nibg;
-  const double sf64 = EXACT ? exact_row_sf(ex, r) : 1.0;
-  const float s = EXACT ? (float)sf64 : (sf_in ? sf_in[r] : 1.0f);
+  const double sf64 = EXACT ? exact_row_sf(ex, sr) : 1.0;
+  const float s = EXACT ? (float)sf64 : (sf_in ? sf_in[sr] : 1.0f);
   if (threadIdx.x == 0 && sf_out) sf_out[r] = s;
   const float inv_s = use_sf ? 1.0f / s : 1.0f;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -486,7 +493,8 @@ expand_sparse_kernel(const uint32_t* __restrict__ bitmap, const int64_t* __restr
         ++pos;
         yv = (float)code;
         if (ovf_indptr && code == 15u)
-          yv = EXACT ? overflow_find(ovf_indptr, ovf_entries, r, c0 + k, yv) : overflow_lookup(ovf_indptr, ovf_entries, r, c0 + k, yv);
+          yv = EXACT ? overflow_find(ovf_indptr, ovf_entries, sr, c0 + k, yv, rows != nullptr)
+                     : overflow_lookup(ovf_indptr, ovf_entries, sr, c0 + k, yv, rows != nullptr);
       }
       y[k] = yv;
       x[k] = EXACT ? exact_count(yv, sf64, ex, c0 + k) : normalise_count(yv, inv_s, use_log1p, mean, inv_std, c0 + k);
@@ -516,7 +524,7 @@ inline int blocks_for(int64_t n, int t = 256) { return (int)((n + t - 1) / t); }
 int expand_sparse(const void* bitmap, const int64_t* nib_indptr, const void* nibbles, const float* sf_in, int M, int n,
                   const float* mean, const float* inv_std, int use_sf, int use_log1p, float* Yout, void* Xout, int x_bf16,
                   float* sf_out, const int64_t* ovf_indptr, const void* ovf_entries, int max_row_nibble_bytes, cudaStream_t s,
-                  const ExactXform* ex) {
+                  const ExactXform* ex, const int32_t* rows) {
   if (M <= 0) return DCA_OK;
   if (n / 8 > kSparseMaxBytes) { set_error("expand_sparse: at most %d genes in the sparse format (got %d)", kSparseMaxBytes * 8, n); return DCA_ERR_UNSUPPORTED; }
   const int2* oe = ovf_indptr ? reinterpret_cast<const int2*>(ovf_entries) : nullptr;
@@ -539,7 +547,7 @@ int expand_sparse(const void* bitmap, const int64_t* nib_indptr, const void* nib
       attr[inst] = dyn;                                                                                                \
     }                                                                                                                  \
     expand_sparse_kernel<XT, EX><<<M, 256, dyn, s>>>((const uint32_t*)bitmap, nib_indptr, (const unsigned char*)nibbles, \
-        sf_in, M, n, mean, inv_std, use_sf, use_log1p, Yout, (XT*)Xout, sf_out, ovf_indptr, oe, nib_cap, e);          \
+        sf_in, M, n, mean, inv_std, use_sf, use_log1p, Yout, (XT*)Xout, sf_out, ovf_indptr, oe, nib_cap, e, rows);    \
   } while (0)
   if (x_bf16) { if (ex) DCA_SPARSE_LAUNCH(__nv_bfloat16, true); else DCA_SPARSE_LAUNCH(__nv_bfloat16, false); }
   else { if (ex) DCA_SPARSE_LAUNCH(float, true); else DCA_SPARSE_LAUNCH(float, false); }
@@ -692,7 +700,7 @@ int gather_rows_bf16(const void* X, int x_bf16, int64_t ldx, const int32_t* rows
 
 int expand_counts(const void* cnt, int bits, const float* sf_in, int M, int n, const float* mean, const float* inv_std, int use_sf,
                   int use_log1p, float* Yout, void* Xout, int x_bf16, float* sf_out, const int64_t* ovf_indptr,
-                  const void* ovf_entries, cudaStream_t s, const ExactXform* ex) {
+                  const void* ovf_entries, cudaStream_t s, const ExactXform* ex, const int32_t* rows) {
   const int64_t tot = (int64_t)M * (n / 8);
   const unsigned char* src = reinterpret_cast<const unsigned char*>(cnt);
   const int2* oe = ovf_indptr ? reinterpret_cast<const int2*>(ovf_entries) : nullptr;
@@ -700,7 +708,7 @@ int expand_counts(const void* cnt, int bits, const float* sf_in, int M, int n, c
   const ExactXform e = ex ? *ex : ExactXform{};
 #define DCA_EXPAND_X(BITS, XT, EX)                                                                                   \
   expand_counts_kernel<BITS, XT, EX><<<blocks_for(tot), 256, 0, s>>>(src, sf_in, M, n, mean, inv_std, use_sf, use_log1p, \
-                                                                     Yout, (XT*)Xout, sf_out, ovf_indptr, oe, e)
+                                                                     Yout, (XT*)Xout, sf_out, ovf_indptr, oe, e, rows)
 #define DCA_EXPAND(BITS)                                                                                             \
   do {                                                                                                               \
     if (x_bf16) { if (ex) DCA_EXPAND_X(BITS, __nv_bfloat16, true); else DCA_EXPAND_X(BITS, __nv_bfloat16, false); } \

@@ -391,6 +391,39 @@ class DeviceEngine:
                                                indptr.data_ptr(), entries.data_ptr(), None if sf is None else sf.data_ptr(),
                                                pc.n_rows, batch, self._stream()), "dca_stream_begin_packed")
 
+    # ------------------------------------------------------------------ packed counts resident in device memory
+    def _packed_rows(self, pd, rows):
+        if pd.device != self.device or pd.x_dtype != self.x_dtype:
+            raise ValueError("packed_data X is %s on %s, the engine expects %s on %s"
+                             % (pd.x_dtype, pd.device, self.x_dtype, self.device))
+        if rows.dtype != torch.int32 or not rows.is_contiguous() or not rows.is_cuda:
+            raise ValueError("rows must be a contiguous int32 device tensor")
+        if rows.numel() > self.max_batch:
+            raise ValueError("batch %d > max_batch %d" % (rows.numel(), self.max_batch))
+        return C.byref(pd.desc), rows.data_ptr(), int(rows.numel())
+
+    def packed_train_step(self, pd, rows):
+        """train_step on rows ``rows`` (int32 device tensor of storage rows) of a packed_data.PackedDeviceDataset: the
+        rows are expanded on the device with the transform of set_input_transform_exact (dca_packed_train_step)."""
+        src, r, b = self._packed_rows(pd, rows)
+        check(self.lib.dca_packed_train_step(self.handle, src, r, b, self._stream()), "dca_packed_train_step")
+
+    def packed_eval_step(self, pd, rows):
+        src, r, b = self._packed_rows(pd, rows)
+        check(self.lib.dca_packed_eval_step(self.handle, src, r, b, self._stream()), "dca_packed_eval_step")
+
+    def packed_predict(self, pd, rows, mean=None, disp=None, pi=None, latent=None):
+        """predict() on rows ``rows`` of a PackedDeviceDataset (outputs as there)."""
+        src, r, b = self._packed_rows(pd, rows)
+        ld = None
+        for t in (mean, disp, pi):
+            if t is not None and t.dim() == 2 and t.shape[1] > 1:
+                ld = t.stride(0) if ld is None else ld
+                if t.stride(0) != ld:
+                    raise ValueError("outputs must share a leading dimension")
+        check(self.lib.dca_packed_predict(self.handle, src, r, b, _ptr(mean), _ptr(disp), _ptr(pi), ld or self.n_out,
+                                          _ptr(latent), self._stream()), "dca_packed_predict")
+
     def set_loss_ring(self, ring: Optional[torch.Tensor]):
         """Mirror every step's loss into the pinned host float32 tensor `ring` (slot k % len for the k-th
         apply_update after this call); None switches it off."""

@@ -228,7 +228,7 @@ def apply_device_normalize(adata, dd, filter_min_counts, set_x=True):
 
 
 def normalize(adata, filter_min_counts=True, size_factors=True, normalize_input=True, logtrans_input=True, device=None,
-              stream=False):
+              stream=False, packed=False):
     """dca/io.py:88-111 with scanpy's arithmetic restated:
     filter_genes/filter_cells(min_counts=1); raw copy; normalize_per_cell (each cell scaled to the
     median total count; zero-count cells dropped as scanpy does); size_factors = n_counts/median;
@@ -247,7 +247,23 @@ def normalize(adata, filter_min_counts=True, size_factors=True, normalize_input=
     stream=True (with a device): out of core instead (stream_data.StreamedDataset, same flags, same bits as the resident
     dataset): the raw counts stay packed in host memory, adata.X keeps the (filtered) raw counts -- no normalised matrix
     exists on the host -- and the dataset is returned in adata.uns['dca_stream_data'] for train(stream_data=...) and
-    predict(stream_data=...)."""
+    predict(stream_data=...).
+
+    packed=True (with a device): the raw counts are packed on the device and stay there, packed
+    (packed_data.PackedDeviceDataset, same flags): adata.X keeps the (filtered) raw counts and the dataset is returned in
+    adata.uns['dca_packed_data'] for train(packed_data=...) and predict(packed_data=...)."""
+    if packed:
+        if device is None:
+            raise ValueError("packed=True preprocesses on a device: give device=")
+        if stream:
+            raise ValueError("give stream=True or packed=True, not both")
+        from .packed_data import PackedDeviceDataset
+        pd_ = PackedDeviceDataset.from_counts(adata.X, device, "float32", size_factors=size_factors,
+                                              logtrans_input=logtrans_input, normalize_input=normalize_input,
+                                              filter_min_counts=filter_min_counts)
+        apply_device_normalize(adata, pd_, filter_min_counts, set_x=False)
+        adata.uns['dca_packed_data'] = pd_
+        return adata
     if stream:
         if device is None:
             raise ValueError("stream=True preprocesses on a device: give device=")

@@ -155,10 +155,15 @@ class Autoencoder:
         self.encoder = self.engine
 
     # -- one fused inference pass instead of the reference's four Keras predict() calls
-    def _run_predict(self, adata, want_mean, want_disp, want_pi, want_latent, device_data=None, stream_data=None):
+    def _run_predict(self, adata, want_mean, want_disp, want_pi, want_latent, device_data=None, stream_data=None,
+                     packed_data=None):
         # a model without a dropout head has no pi: the engine writes nothing there, so none is returned (not the
         # uninitialised contents of the output buffer)
         want_pi = want_pi and self.has_pi
+        if packed_data is not None:
+            if device_data is not None or stream_data is not None:
+                raise ValueError("give one of device_data, stream_data and packed_data")
+            return self._run_predict_packed(adata, packed_data, want_mean, want_disp, want_pi, want_latent)
         if stream_data is not None:
             if device_data is not None:
                 raise ValueError("give device_data or stream_data, not both")
@@ -248,6 +253,26 @@ class Autoencoder:
         finally:
             eng.stream_end()
 
+    def _run_predict_packed(self, adata, pd, want_mean, want_disp, want_pi, want_latent):
+        """_run_predict with every batch expanded by row index from a packed_data.PackedDeviceDataset of adata's cells
+        (dca_packed_predict); the outputs travel to the host as in _run_predict_device."""
+        N = pd.n
+        if adata is not None and adata.n_obs != N:
+            raise ValueError("packed_data covers %d cells, adata has %d" % (N, adata.n_obs))
+        eng = self.ensure_engine(max_batch=max(getattr(self, "_max_batch", 32), min(PREDICT_BATCH, N)))
+        if eng.n_in != pd.n_genes:
+            raise ValueError("packed_data has %d genes, the network %d inputs" % (pd.n_genes, eng.n_in))
+        bs = min(PREDICT_BATCH, eng.max_batch)
+        eng.set_input_transform_exact(pd.mean, pd.std, pd.median, pd.flags)
+
+        def run(i, s, e, b):
+            eng.packed_predict(pd, pd.rows[s:e], mean=b.get("mean"), disp=b.get("disp"), pi=b.get("pi"),
+                               latent=b.get("latent"))
+
+        def theta(th):
+            eng.packed_predict(pd, pd.rows[:1], disp=th)
+        return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
+
     def _predict_batches(self, eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta):
         """The outputs of run(i, s, e, buffers) -- the inference of batch i, rows [s, e), into one of two device buffer
         sets -- gathered on the host: each batch's outputs are copied to pinned host memory on a side stream, so the
@@ -304,14 +329,17 @@ class Autoencoder:
         return res
 
     # -- dca/network.py:188-211
-    def predict(self, adata, mode='denoise', return_info=False, copy=False, device_data=None, stream_data=None):
+    def predict(self, adata, mode='denoise', return_info=False, copy=False, device_data=None, stream_data=None,
+                packed_data=None):
         """device_data: a device_data.DeviceDataset of adata's cells; the input X and size factors are then read from
         it instead of adata.X / obs['size_factors'].  stream_data: a stream_data.StreamedDataset of adata's cells; the
-        input batches are then streamed from its packed counts (the same outputs as from the DeviceDataset)."""
+        input batches are then streamed from its packed counts (the same outputs as from the DeviceDataset).
+        packed_data: a packed_data.PackedDeviceDataset of adata's cells; the input batches are then expanded from its
+        packed counts in device memory (the same outputs again)."""
         assert mode in ('denoise', 'latent', 'full'), 'Unknown mode'
         adata = adata.copy() if copy else adata
         res = self._run_predict(adata, mode in ('denoise', 'full'), False, False, mode in ('latent', 'full'), device_data,
-                                stream_data)
+                                stream_data, packed_data)
         if mode in ('latent', 'full'):
             print('dca: Calculating low dimensional representations...')
             adata.obsm['X_dca'] = res["latent"]
@@ -345,11 +373,11 @@ class _InfoMixin:
     const_disp = False
 
     def predict(self, adata, mode='denoise', return_info=False, copy=False, colnames=None, device_data=None,
-                stream_data=None):
+                stream_data=None, packed_data=None):
         assert mode in ('denoise', 'latent', 'full'), 'Unknown mode'
         adata = adata.copy() if copy else adata
         res = self._run_predict(adata, mode in ('denoise', 'full'), return_info, return_info and self.has_pi,
-                                mode in ('latent', 'full'), device_data, stream_data)
+                                mode in ('latent', 'full'), device_data, stream_data, packed_data)
         if return_info:
             if self.const_disp:
                 adata.var['X_dca_dispersion'] = res["dispersion"]

@@ -327,8 +327,10 @@ def _workspace(lib, N, G, chunk, dev):
     return torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
 
 
-def _totals(pc, dev, chunk_rows=None):
-    """(n_counts fp64 [N], gene totals fp64 [G], number of bad entries) on the host."""
+def _totals(pc, dev, chunk_rows=None, chunks=None):
+    """(n_counts fp64 [N], gene totals fp64 [G], number of bad entries) on the host.  chunks(chunk, fn) feeds the row
+    chunks of the matrix to fn(r0, n, Y) (default: for_each_chunk over the packed host counts pc); pc then only needs
+    n_rows and n_genes."""
     lib = _lib.load()
     N, G = pc.n_rows, pc.n_genes
     chunk = min(N, chunk_rows or _chunk_rows(G))
@@ -341,14 +343,15 @@ def _totals(pc, dev, chunk_rows=None):
     def rows(r0, n, Y):
         check(lib.dca_count_totals_rows(Y.data_ptr(), G, r0, n, N, G, n_counts.data_ptr(), ws.data_ptr(), ws.numel(),
                                         _stream(dev)), "dca_count_totals_rows")
-    for_each_chunk(pc, dev, chunk, rows)
+    (chunks or (lambda c, fn: for_each_chunk(pc, dev, c, fn)))(chunk, rows)
     check(lib.dca_count_totals_finish(N, G, gene_tot.data_ptr(), n_bad.data_ptr(), ws.data_ptr(), ws.numel(),
                                       _stream(dev)), "dca_count_totals_finish")
     return n_counts.cpu().numpy(), gene_tot.cpu().numpy(), int(n_bad.item())
 
 
-def _moments(pc, nc_host, median, flags, dev, chunk_rows=None):
-    """Gene mean and std (fp64, host) of l over the rows of pc: passes 1 and 2 of dca_log_moments."""
+def _moments(pc, nc_host, median, flags, dev, chunk_rows=None, chunks=None):
+    """Gene mean and std (fp64, host) of l over the rows of pc: passes 1 and 2 of dca_log_moments (chunks: as for
+    _totals)."""
     lib = _lib.load()
     N, G = pc.n_rows, pc.n_genes
     chunk = min(N, chunk_rows or _chunk_rows(G))
@@ -362,7 +365,7 @@ def _moments(pc, nc_host, median, flags, dev, chunk_rows=None):
             def rows(r0, n, Y, p=p):
                 check(lib.dca_log_moments_rows(p, Y.data_ptr(), G, r0, n, N, G, ncp, median, flags, out[0].data_ptr(),
                                                ws.data_ptr(), ws.numel(), _stream(dev)), "dca_log_moments_rows")
-            for_each_chunk(pc, dev, chunk, rows)
+            (chunks or (lambda c, fn: for_each_chunk(pc, dev, c, fn)))(chunk, rows)
         check(lib.dca_log_moments_finish(p, N, G, flags, out[p - 1].data_ptr(), ws.data_ptr(), ws.numel(), _stream(dev)),
               "dca_log_moments_finish")
     return out[0].cpu().numpy(), out[1].cpu().numpy()

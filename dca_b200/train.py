@@ -89,11 +89,16 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
     ``rows``) and adata's matrices are not used; the updates are those of the host arrays holding the same values.
     Single process only, use_raw_as_output only, and with ``output_subset`` the dataset's Y must already hold those
     genes (DeviceDataset.with_output_genes).  adata is then only read for ``raw.var_names`` (output_subset) and may be
-    None otherwise."""
+    None otherwise.
+
+    ``packed_data``: a packed_data.PackedDeviceDataset of the cells of ``adata`` (in order): raw counts packed in HBM,
+    every batch expanded on the device by row index.  The resident loop as with device_data (rows reshuffled every
+    epoch exactly like Keras) and the same updates; single process only, use_raw_as_output only, no output_subset."""
     stream = kwds.pop('stream', False)
     shuffle = kwds.pop('shuffle', True)
     device_data = kwds.pop('device_data', None)
     stream_data = kwds.pop('stream_data', None)
+    packed_data = kwds.pop('packed_data', None)
     if kwds:
         raise TypeError("train() got keyword arguments the accelerated fit loop does not implement: %s" % sorted(kwds))
     from . import _lib as _L
@@ -104,6 +109,13 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
         raise NotImplementedError("tensorboard logging is not part of the accelerated path")
     if output_dir is not None:
         os.makedirs(output_dir, exist_ok=True)
+    if packed_data is not None:
+        if device_data is not None or stream_data is not None or stream:
+            raise ValueError("packed_data is resident in HBM: it cannot be combined with stream, device_data or "
+                             "stream_data")
+        return _train_packed_data(adata, network, packed_data, output_subset, use_raw_as_output, optimizer,
+                                  learning_rate, batch_size, validation_split, epochs, reduce_lr, early_stop, clip_grad,
+                                  verbose, save_weights, output_dir, shuffle)
     if stream_data is not None:
         if device_data is not None:
             raise ValueError("give device_data or stream_data, not both")
@@ -419,10 +431,58 @@ def _train_device_data(adata, network, dd, stream, output_subset, use_raw_as_out
     return hist
 
 
+def _train_packed_data(adata, network, pd, output_subset, use_raw_as_output, optimizer, learning_rate, batch_size,
+                       validation_split, epochs, reduce_lr, early_stop, clip_grad, verbose, save_weights, output_dir, shuffle):
+    """train() on a PackedDeviceDataset: the resident loop of train() with every batch expanded from the packed counts
+    by row index (dca_packed_train_step / dca_packed_eval_step) with the exact transform of the device preprocessing."""
+    if D.rank_world()[1] > 1:
+        raise NotImplementedError("packed_data trains on one GPU; a torch.distributed world larger than 1 is not supported")
+    if not use_raw_as_output:
+        raise ValueError("packed_data holds the raw counts as the target: use_raw_as_output=False is not supported")
+    if output_subset:
+        raise NotImplementedError("packed_data needs the raw counts of the input genes as the target (no output_subset)")
+    if adata is not None and adata.n_obs != pd.n:
+        raise ValueError("packed_data covers %d cells, adata has %d" % (pd.n, adata.n_obs))
+    eng = network.ensure_engine(max_batch=batch_size)
+    if eng.n_in != pd.n_genes or eng.n_out != pd.n_genes:
+        raise ValueError("packed_data has %d genes, the network %d inputs and %d outputs" % (pd.n_genes, eng.n_in, eng.n_out))
+    if pd.device != eng.device:
+        raise ValueError("packed_data lives on %s, the network on %s" % (pd.device, eng.device))
+    if pd.x_dtype != eng.x_dtype:
+        raise ValueError("packed_data X is %s, the network expects %s (network_kwds x_dtype)" % (pd.x_dtype, eng.x_dtype))
+    N = pd.n
+    n_tr = int(N * (1. - validation_split)) if validation_split and 0. < validation_split < 1. else N
+    n_va = N - n_tr
+    default_lr = eng.set_optimizer(optimizer)
+    if learning_rate is None:
+        learning_rate = default_lr
+    eng.reset_optimizer()
+    eng.set_input_transform_exact(pd.mean, pd.std, pd.median, pd.flags)
+    ctl = PlateauAndStop(float(learning_rate), reduce_lr, early_stop, verbose)
+    hist = History()
+    if verbose:
+        print(network.summary())
+    steps = (n_tr + batch_size - 1) // batch_size
+    dev = eng.device
+    torch.cuda.synchronize(dev)
+    prev_stream = torch.cuda.current_stream(dev)
+    torch.cuda.set_stream(torch.cuda.Stream(dev))
+    try:
+        hist = _fit_loop(eng, network, None, None, None, n_tr, n_va, steps, batch_size, epochs, ctl, clip_grad, 1.0, 1, 0,
+                         dev, hist, verbose, save_weights, output_dir, shuffle, rows_map=pd.rows, packed=pd)
+    finally:
+        torch.cuda.synchronize(dev)
+        torch.cuda.set_stream(prev_stream)
+    if not hist.history["val_loss"]:
+        del hist.history["val_loss"]
+    return hist
+
+
 def _fit_loop(eng, network, Xd, Yd, sfd, n_tr, n_va, steps, batch_size, epochs, ctl, clip_grad, gscale, world, rank, dev, hist,
-              verbose, save_weights, output_dir, shuffle=True, rows_map=None):
+              verbose, save_weights, output_dir, shuffle=True, rows_map=None, packed=None):
     """rows_map (int32 device tensor, n_tr + n_va entries): the storage row of each position in Xd / Yd / sfd; None:
-    position = row."""
+    position = row.  packed: a PackedDeviceDataset whose storage rows rows_map names (Xd, Yd, sfd unused): every batch
+    is expanded from its packed counts."""
     best_val = np.inf
     for epoch in range(epochs):
         # Keras: np.random.shuffle(index_array) with the global NumPy RNG (seeded in api.dca / CLI)
@@ -435,7 +495,9 @@ def _fit_loop(eng, network, Xd, Yd, sfd, n_tr, n_va, steps, batch_size, epochs, 
         eng.read_epoch_acc(reset=True)
         for s in range(steps):
             rows = order_d[s * batch_size: min((s + 1) * batch_size, n_tr)]
-            if world > 1:
+            if packed is not None:
+                eng.packed_train_step(packed, rows)
+            elif world > 1:
                 eng.train_step_allreduce(Xd, Yd, sfd, rows=rows)     # NCCL all-reduce overlapped with the backward tail
             else:
                 eng.train_step(Xd, Yd, sfd, rows=rows)
@@ -443,7 +505,9 @@ def _fit_loop(eng, network, Xd, Yd, sfd, n_tr, n_va, steps, batch_size, epochs, 
         # validation pass: inference-mode BN over the held-out tail
         for s in range(n_tr, n_tr + n_va, batch_size):
             e = min(s + batch_size, n_tr + n_va)
-            if rows_map is not None:
+            if packed is not None:
+                eng.packed_eval_step(packed, rows_map[s:e])
+            elif rows_map is not None:
                 eng.eval_step(Xd, Yd, sfd, rows=rows_map[s:e])
             else:
                 eng.eval_step(Xd[s:e], Yd[s:e], sfd[s:e])
@@ -479,6 +543,14 @@ def train_with_args(args):
     stream = bool(getattr(args, 'stream', False))
     if stream and preprocess != 'device':
         raise ValueError("--stream needs --preprocess device")
+    packed = bool(getattr(args, 'packed', False))
+    if packed and preprocess != 'device':
+        raise ValueError("--packed needs --preprocess device")
+    if packed and stream:
+        raise ValueError("--packed and --stream exclude each other: the counts stay packed in GPU or in host memory")
+    if packed and args.denoisesubset:
+        raise NotImplementedError("--packed trains on every input gene (the expanded batches need n_in == n_out): "
+                                  "--denoisesubset is not supported with it")
     if stream and args.denoisesubset:
         raise NotImplementedError("--stream trains on every input gene (the streamed batches need n_in == n_out): "
                                   "--denoisesubset is not supported with it")
@@ -487,9 +559,10 @@ def train_with_args(args):
                          logtrans_input=args.loginput,
                          normalize_input=args.norminput,
                          device=torch.device('cuda', torch.cuda.current_device()) if preprocess == 'device' else None,
-                         stream=stream)
+                         stream=stream, packed=packed)
     dd = adata.uns.pop('dca_device_data', None)
     sd = adata.uns.pop('dca_stream_data', None)
+    pdd = adata.uns.pop('dca_packed_data', None)
 
     if args.denoisesubset:
         genelist = list(set(io.read_genelist(args.denoisesubset)))
@@ -536,6 +609,8 @@ def train_with_args(args):
         extra['device_data'] = dd_train
     if sd is not None:
         extra['stream_data'] = sd.take(train_mask)
+    if pdd is not None:
+        extra['packed_data'] = pdd.take(train_mask)
     losses = train(adata[adata.obs.dca_split == 'train'], net,
                    output_dir=args.outputdir,
                    learning_rate=args.learningrate,
@@ -554,6 +629,6 @@ def train_with_args(args):
     else:
         predict_columns = adata.var_names
 
-    net.predict(adata, mode='full', return_info=True, device_data=dd, stream_data=sd)
+    net.predict(adata, mode='full', return_info=True, device_data=dd, stream_data=sd, packed_data=pdd)
     net.write(adata, args.outputdir, mode='full', colnames=predict_columns)
     return losses

@@ -323,6 +323,52 @@ int dca_expand_sparse_counts_exact(const void* bitmap, const int64_t* nib_indptr
                                    const double* gene_mean, const double* gene_std, float* Y, void* X, int32_t x_dtype,
                                    float* sf_out, void* stream);
 
+/* ---- packed counts resident in device memory -------------------------------------------------------------------
+ * The formats of dca_stream_begin_packed / dca_stream_begin_sparse, held whole in DEVICE memory with absolute offsets:
+ * a dataset several times larger than the fp32 Y + X of the resident path, with no host traffic per step.  The rows of
+ * a batch are named by index and expanded into the engine's expanded-batch staging with the exact transform
+ * (dca_set_input_transform_exact), so every X, Y and size factor is the one dca_normalize_write stores for that cell. */
+typedef struct dca_packed_counts {
+  int32_t struct_bytes;           /* sizeof(dca_packed_counts), ABI guard */
+  int32_t bits;                   /* 1 (sparse: bitmap + 4-bit codes of the non-zeros), 4, 8 or 16 bits per entry */
+  int64_t n_rows;
+  int32_t genes;                  /* a multiple of 8 */
+  int32_t max_row_nibble_bytes;   /* sparse: the longest row's code bytes (sizes the expansion's shared memory) */
+  const void* packed;             /* [n_rows x genes*bits/8] bytes, 16-byte aligned (sparse: the bitmap) */
+  const int64_t* ovf_indptr;      /* int64 [n_rows + 1], absolute offsets into ovf_entries; NULL: no overflow entries */
+  const void* ovf_entries;        /* {int32 gene; float count} sorted by row, then gene */
+  const int64_t* nib_indptr;      /* sparse: int64 [n_rows + 1], absolute byte offsets into nibbles */
+  const void* nibbles;            /* sparse: the codes, each row on a byte boundary, 16 readable bytes of slack */
+  const double* n_counts;         /* fp64 [n_rows] row totals (needed with DCA_PRE_SIZE_FACTORS) */
+} dca_packed_counts;
+
+/* The GPU packer.  Count pass: for n_rows rows of fp32 counts Y (device, leading dim ldy) stats[k * ld_stats + r]
+ * (device int64) receives, per row r: k = 0 the non-zero entries, 1..3 the entries >= 15, >= 255 and >= 65535 (the
+ * overflow entries of the 4, 8 and 16-bit widths, dca_count_escapes), 4 the entries that are negative, not an
+ * integer or not finite.  Pack pass: rows [0, n_rows) of Y become rows row0 .. row0 + n_rows of the arrays of `dst`
+ * (its pointers are the whole matrix's, its ovf_indptr / nib_indptr the exclusive prefix sums of the chosen width's
+ * per-row escapes / (non-zeros + 1) / 2 over all rows): the bytes dca_pack_counts / dca_pack_sparse write for the same
+ * counts.  dst->n_counts is not read.  No atomics: the output is a function of the counts. */
+int dca_pack_count_rows(const float* Y, int64_t ldy, int64_t n_rows, int32_t genes, int64_t* stats, int64_t ld_stats,
+                        void* stream);
+int dca_pack_rows_device(const float* Y, int64_t ldy, int64_t n_rows, int64_t row0, const dca_packed_counts* dst,
+                         void* stream);
+/* Y [n x genes] (fp32), X (x_dtype, row stride genes) and sf_out [n] of rows rows[0..n) of src (device int32, each
+ * < src->n_rows; NULL: rows 0..n-1) with the exact transform: the rows dca_normalize_write and the resident dataset
+ * hold for the same cells.  gene_mean / gene_std: device fp64 [genes]. */
+int dca_expand_rows_exact(const dca_packed_counts* src, const int32_t* rows, int32_t n, double median, int32_t flags,
+                          const double* gene_mean, const double* gene_std, float* Y, void* X, int32_t x_dtype,
+                          float* sf_out, void* stream);
+/* dca_train_step / dca_eval_step / dca_predict on the batch rows[0..batch) of src: the rows are expanded with the
+ * transform of dca_set_input_transform_exact (which must come first) into the engine's expanded-batch staging (bf16 X
+ * for the tensor-core encoder) on `stream`, then the step runs on that contiguous batch.  The same bits as the step on
+ * a resident dataset of the same cells.  DCA_ERR_BAD_ARG while a host stream is active (dca_stream_begin*);
+ * DCA_ERR_UNSUPPORTED when n_in != n_out or n_in % 8 != 0. */
+int dca_packed_train_step(dca_handle* h, const dca_packed_counts* src, const int32_t* rows, int32_t batch, void* stream);
+int dca_packed_eval_step(dca_handle* h, const dca_packed_counts* src, const int32_t* rows, int32_t batch, void* stream);
+int dca_packed_predict(dca_handle* h, const dca_packed_counts* src, const int32_t* rows, int32_t batch, float* mean_out,
+                       float* disp_out, float* pi_out, int64_t ld_out, float* latent_out, void* stream);
+
 /* ---- stand-alone kernels (parity tests, profiling) -------------------------------------- */
 /* ZINB / NB negative log-likelihood forward + backward, one pass (dca/loss.py:72-156 and its
  * autodiff).  Inputs are POST-activation head outputs: m = MeanAct(zm) (not yet multiplied by
