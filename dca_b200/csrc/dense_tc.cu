@@ -64,7 +64,8 @@ struct ProbeParams {
 template <int NC, int TA, int TB>
 __device__ __forceinline__ void probe_mma(float (&acc)[NC / 2], uint64_t da, uint64_t db) {
   if constexpr (NC == 128) wgmma_m64n128k16<TA, TB>(acc, da, db, 1u);
-  else wgmma_m64n64k16<TA, TB>(acc, da, db, 1u);
+  else if constexpr (NC == 64) wgmma_m64n64k16<TA, TB>(acc, da, db, 1u);
+  else wgmma_m64n16k16<TA, TB>(acc, da, db, 1u);
 }
 
 // one warpgroup: D[rows m0.., cols n0..n0+NC) of the 128 x N product, K / 16 wgmma steps
@@ -110,10 +111,12 @@ tc_probe_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
     for (int i = 0; i < p.b_boxes; ++i) tma_load_2d(sb + (size_t)i * p.b_box_bytes, &map_b, i * p.b_box_c0, i * p.b_box_c1, &bar_load);
   }
   mbar_wait(&bar_load, 0);
-  // N chunks of 128 where possible: an MN-major B operand then spans two 64-wide blocks (exercises its LBO)
+  // N chunks of 128 where possible: an MN-major B operand then spans two 64-wide blocks (exercises its LBO).  N = 16:
+  // the m64n16 product of the heads + loss kernel (A = the weights MN-major, B = 16 rows of H K-major)
   for (int m0 = 0; m0 < p.M; m0 += 64)
     for (int n0 = 0; n0 < p.N;) {
-      if (p.N - n0 >= 128) { probe_chunk<128>(p, smem_u32(sa), smem_u32(sb), m0, n0, D); n0 += 128; }
+      if (p.N == 16) { probe_chunk<16>(p, smem_u32(sa), smem_u32(sb), m0, n0, D); n0 += 16; }
+      else if (p.N - n0 >= 128) { probe_chunk<128>(p, smem_u32(sa), smem_u32(sb), m0, n0, D); n0 += 128; }
       else { probe_chunk<64>(p, smem_u32(sa), smem_u32(sb), m0, n0, D); n0 += 64; }
     }
 }
@@ -252,8 +255,8 @@ extern "C" int dca_tc_probe(const void* A, int32_t a_rows, int32_t a_cols, const
                             int32_t a_mn_major, int32_t b_mn_major, int32_t M, int32_t N, int32_t K,
                             int32_t a_lbo, int32_t a_sbo, int32_t b_lbo, int32_t b_sbo, float* D, void* stream) {
   using namespace tc;
-  if (M != 128 || N % 64 != 0 || N < 64 || N > 256 || K % 64 != 0 || K <= 0 || K > 256) {
-    set_error("dca_tc_probe: need M=128, N%%64==0 (64..256), K%%64==0 (<=256)"); return DCA_ERR_BAD_ARG;
+  if (M != 128 || (N != 16 && (N % 64 != 0 || N < 64 || N > 256)) || K % 64 != 0 || K <= 0 || K > 256) {
+    set_error("dca_tc_probe: need M=128, N=16 or N%%64==0 (64..256), K%%64==0 (<=256)"); return DCA_ERR_BAD_ARG;
   }
   ProbeParams p{};
   p.a_mn = a_mn_major; p.b_mn = b_mn_major; p.M = M; p.N = N; p.K = K;

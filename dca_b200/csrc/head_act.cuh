@@ -22,8 +22,8 @@ __device__ __forceinline__ float act_sigmoid(float z) { return rcpf(1.0f + ex2f(
 
 // Pre-activations of one 64-cell x 128-gene head tile, issued by one warpgroup: H (K-major, 64 rows of 128 B, SWIZZLE_128B,
 // 32 B per k16 step) times W (MN-major, the Keras [64 k][genes] layout as two 64-gene boxes 8 KB apart, 2 KB per k16 step),
-// four k16 steps from a zero accumulator.  Shared by the head-forward kernel (dense_tc.cu) and the head+loss kernel
-// (zinb_loss.cu) so that both see the same accumulators bit for bit.
+// four k16 steps from a zero accumulator.  The head-forward kernel's product (dense_tc.cu); the heads + loss kernel
+// (zinb_loss.cu) computes the same products gene-major with head_piece_mma.
 __device__ __forceinline__ void head_tile_mma(float (&acc)[64], uint32_t h_smem, uint32_t w_smem) {
   wgmma_fence();
 #pragma unroll
@@ -32,6 +32,23 @@ __device__ __forceinline__ void head_tile_mma(float (&acc)[64], uint32_t h_smem,
   wgmma_commit();
   wgmma_wait<0>();
   acc_fence(acc);
+}
+
+// Gene-major pre-activations of one head for 16 cells, issued by one warpgroup: D[128 genes x 16 cells] = Wᵀ . Hᵀ as two
+// m64n16 m-blocks (genes 0-63 | 64-127, acc[0] | acc[1]) of four k16 steps from a zero accumulator.  A = W, MN-major (the
+// same two 64-gene boxes as head_tile_mma's B operand, one box per m-block); B = 16 consecutive rows of H (K-major,
+// h_smem 1024-byte aligned, i.e. a multiple of 8 rows into the swizzled block).  Commits one wgmma group and does not
+// wait: the caller waits (wgmma_wait) and fences the accumulators before reading them.  Thread t holds acc[mb][i] at
+// gene 64 mb + 16 (t/32 % 4) + (t%32)/4 + 8 ((i/2)%2), cell 8 (i/4) + 2 (t%4) + i%2.
+__device__ __forceinline__ void head_piece_mma(float (&acc)[2][8], uint32_t h_smem, uint32_t w_smem) {
+  wgmma_fence();
+#pragma unroll
+  for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wgmma_m64n16k16<1, 0>(acc[mb], make_smem_desc(w_smem + mb * 8192 + k * 2048, 8192, 1024),
+                            make_smem_desc(h_smem + k * 32, 0, 1024), k > 0);
+  wgmma_commit();
 }
 
 // Epilogue of one head output: activation of (accumulator + bias), MeanAct scaled by the row's scale (1 in training).

@@ -846,27 +846,30 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
 //
 // One CTA = four warpgroups sharing the bf16 weights of one 128-gene tile (3 x 16 KB, TMA).  A CTA owns a contiguous range
 // of (gene tile, 64-cell block) units, tile-major; its warpgroups take the blocks of a tile in turn.  Per block a warpgroup
-// loads H3 (TMA, 8 KB) and, for each of the four 4-row quarters of its warps' accumulator fragments ("pieces"), runs the
-// three m64n128 products of head_tile_mma (the same products as heads_fwd_kernel, so the accumulators are bit-identical to
-// K2's) and stages the raw fp32 accumulators of the piece's rows in warp-private shared memory (4 rows x 128 genes x
-// 3 heads); the counts of those rows stream into the warp's slot by cp.async under the products, so that no registers
-// hold them next to the accumulators.  The warp then walks its 4 rows: each lane applies K2's epilogue (head_out, same
-// inputs, so m, theta and pi carry K2's bits) to its own 4 genes x 3 heads and runs zinb_row_ring -- the per-row body of
-// the ring kernel, with the same warp / lane / 128-gene mapping -- and stores bf16 dZ.  Recomputing the products for
-// every piece costs tensor time but quarters the staging, which with at most 128 registers per thread is what fits four
-// warpgroups (16 warps to hide the latency of the row walk) on an SM.
+// loads H3 (TMA, 8 KB) and walks it in four pieces of 16 consecutive cells; warp w walks cells 4w .. 4w + 3 of a piece.
+// Per piece the warpgroup computes each head's products once, gene-major (head_piece_mma: 128 genes x 16 cells, the three
+// heads committed back to back), and every thread stores its raw fp32 accumulators into the staging rows of the warp that
+// walks that cell (warp-private areas, 4 rows x 128 genes x 3 heads each); the counts of a warp's rows stream into its
+// slot by cp.async under the products, so that no registers hold them next to the accumulators.  The warp then walks its
+// 4 rows: each lane applies K2's epilogue (head_out, same inputs, so m, theta and pi carry K2's bits when the gene-major
+// accumulators equal K2's cell-major ones) to its own 4 genes x 3 heads and runs zinb_row_ring -- the per-row body of the
+// ring kernel, with the same warp / lane / 128-gene mapping -- and stores bf16 dZ.  Two warpgroup barriers per piece
+// order the staging stores against the walks of the previous and the current piece.  The staging of one piece is what fits
+// four warpgroups (16 warps to hide the latency of the row walk) on an SM with at most 128 registers per thread.
 namespace hl {
 constexpr int kWG = 4;                                       // warpgroups per CTA
 constexpr int kCtaThreads = 128 * kWG;
 constexpr int kRows = 4;                                     // rows per warp and piece
-constexpr int kPieces = 16 / kRows;                          // pieces per 16-row warp fragment
+constexpr int kPieceCells = 4 * kRows;                       // cells per piece (the four warps of a warpgroup)
+constexpr int kPieces = 64 / kPieceCells;                    // pieces per 64-cell block
 constexpr uint32_t kWHeadBytes = 64 * 128 * 2;               // one head's W tile: two 64-gene boxes of [64 k][64 genes] bf16
 constexpr uint32_t kHBytes = 64 * 64 * 2;                    // one 64-cell H3 block
 constexpr uint32_t kRowBytes = 3 * 128 * 4;                  // m | d | pi accumulators of one row's 128 genes
 constexpr uint32_t kQPad = 512;                              // the NB queue of row k (2 KB) starts 512 B ahead of row k's
                                                              // operands and overwrites them once they are in registers
 constexpr uint32_t kOffY = kQPad + kRows * kRowBytes;        // the piece's count rows (cp.async, 16 B per lane and row)
-constexpr uint32_t kWarpBytes = kOffY + kRows * 128 * 4;
+constexpr uint32_t kWarpBytes = kOffY + kRows * 128 * 4 + 32;   // + 32: consecutive warps' areas 32 B apart modulo 128 B
+static_assert(kWarpBytes % 128 == 32, "stage_head's stores are conflict-free only with warp areas 32 B apart modulo 128 B");
 constexpr uint32_t kOffH = 3 * kWHeadBytes;
 constexpr uint32_t kOffStage = kOffH + kWG * kHBytes;
 constexpr uint32_t kOffBias = kOffStage + kWG * 4 * kWarpBytes;
@@ -886,19 +889,24 @@ struct Params {
 // over all banks (rows are 1536 B apart, a multiple of 128 B)
 __device__ __forceinline__ uint32_t slot16(int i, int k) { return (uint32_t)((i ^ ((2 * k) & 6)) * 16); }
 
-// Rows 4 piece .. 4 piece + 3 of the warp's 16 fragment rows are held by lanes 16 (piece & 1) .. + 15, in acc[4c], acc[4c+1]
-// (pieces 0, 1) or acc[4c+2], acc[4c+3] (pieces 2, 3).  Those lanes store them, raw, at head offset `head_base`.
-__device__ __forceinline__ void stage_acc(const float (&acc)[64], int piece, uint8_t* head_base) {
-  const int lane = threadIdx.x & 31, k = (lane >> 2) & 3;
-  if ((lane >> 4) != (piece & 1)) return;
-  const bool hi = piece >= 2;
-  uint8_t* dst = head_base + k * kRowBytes + (lane & 1) * 8;
+// Stores head h's gene-major accumulators of a piece (head_piece_mma), raw, into the staging rows of the warps that walk
+// them: cell c of the piece is row c % 4 of warp c / 4 of the warpgroup (`wg_stage`: its first warp's area).  In the
+// fragment, acc[mb][i] of lane l is gene 64 mb + 16 warp + l / 4 + 8 (i / 2 % 2) and cell 8 (i / 4) + 2 (l % 4) + i % 2,
+// i.e. row 2 (l & 1) + (i & 1) of warp 2 (i / 4) + (l >> 1 & 1).  Its 16-byte slot (slot16) is gene / 4 XOR 4 (l & 1) + 2
+// (i & 1), and these bit fields do not overlap, so the address is a per-lane base plus a constant per (mb, i):
+//   slot = (4 warp ^ 4 (l & 1)) | l >> 4   |   16 mb | 2 ((i / 2 ^ i) & 1).
+// Each store instruction writes 32 distinct banks: lane bit 0 flips 16 banks (slot bit 2), bit 1 moves 8 (the next warp's
+// area, 32 B further modulo 128 B), bits 2-3 pick the word and bit 4 moves 4 (slot bit 0).
+__device__ __forceinline__ void stage_head(const float (&acc)[2][8], uint8_t* wg_stage, int h) {
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  uint8_t* base = wg_stage + ((lane >> 1) & 1) * kWarpBytes + kQPad + 2 * (lane & 1) * kRowBytes + h * 512 + ((lane >> 2) & 3) * 4 +
+                  ((((4 * warp) ^ (4 * (lane & 1))) | (lane >> 4)) * 16);
 #pragma unroll
-  for (int c = 0; c < 16; ++c) {
-    const int g = 8 * c + 2 * (lane & 3);
-    *reinterpret_cast<float2*>(dst + slot16(g >> 2, k)) =
-        make_float2(hi ? acc[4 * c + 2] : acc[4 * c], hi ? acc[4 * c + 3] : acc[4 * c + 1]);
-  }
+  for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      *reinterpret_cast<float*>(base + 2 * (i >> 2) * kWarpBytes + (i & 1) * kRowBytes + (16 * mb | (2 * (((i >> 1) ^ i) & 1))) * 16) =
+          acc[mb][i];
 }
 
 // K2's epilogue of one head on a lane's 4 genes
@@ -924,7 +932,8 @@ heads_loss_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_consta
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
   float* s_bias = reinterpret_cast<float*>(smem + kOffBias);
   uint8_t* h_buf = smem + kOffH + wg * kHBytes;
-  uint8_t* wbase = smem + kOffStage + (wg * 4 + warp) * kWarpBytes;       // this warp's queue pad + 4 staged rows + counts
+  uint8_t* wg_stage = smem + kOffStage + wg * 4 * kWarpBytes;             // the warpgroup's four warp areas
+  uint8_t* wbase = wg_stage + warp * kWarpBytes;                          // this warp's queue pad + 4 staged rows + counts
   uint8_t* rows_base = wbase + kQPad;
   const uint32_t my_y = smem_u32(wbase + kOffY) + lane * 16;             // my 16 bytes of the piece's count row 0
   if (tid < zmath::kLogFactN) lf[tid] = p.lf[tid];
@@ -970,16 +979,20 @@ heads_loss_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_consta
     const int64_t gcol0 = (int64_t)t * 128 + col;
     for (; blk < b_end; blk += kWG) {
       mbar_wait(&h_bar[wg], h_phase); h_phase ^= 1;
-      for (int piece = 0; piece < kPieces; ++piece) {
-        const int r0 = blk * 64 + warp * 16 + piece * kRows;              // first of this warp's 4 rows in the piece
+      // pieces wholly past the batch are skipped (the same for the whole warpgroup)
+      const int last_piece = min(kPieces, (p.B - blk * 64 + kPieceCells - 1) / kPieceCells) - 1;
+      for (int piece = 0; piece <= last_piece; ++piece) {
+        float acc[3][2][8];                                               // [head][gene m-block][fragment]
+        const uint32_t h_piece = smem_u32(h_buf) + piece * kPieceCells * 128;
+        head_piece_mma(acc[0], h_piece, smem_u32(smem));
+        head_piece_mma(acc[1], h_piece, smem_u32(smem) + kWHeadBytes);
+        head_piece_mma(acc[2], h_piece, smem_u32(smem) + 2 * kWHeadBytes);
+        const int r0 = blk * 64 + piece * kPieceCells + warp * kRows;     // first of this warp's 4 rows in the piece
         int my_yr = 0; float my_sf = 1.f;                                 // lane k < 4: count row / size factor of row r0 + k
         if (lane < kRows && r0 + lane < p.B) {
           my_yr = p.rows ? p.rows[r0 + lane] : r0 + lane;
           my_sf = p.sf ? p.sf[my_yr] : 1.0f;
         }
-        float acc[64];
-        head_tile_mma(acc, smem_u32(h_buf), smem_u32(smem));
-        stage_acc(acc, piece, rows_base);
 #pragma unroll
         for (int k = 0; k < kRows; ++k) {                                 // counts of the piece, in flight under the products
           const int yr = __shfl_sync(0xffffffffu, my_yr, k);              // (through shared memory: no registers held)
@@ -988,14 +1001,15 @@ heads_loss_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_consta
                          : "memory");
         }
         cp_async_commit();
-        head_tile_mma(acc, smem_u32(h_buf), smem_u32(smem) + kWHeadBytes);
-        stage_acc(acc, piece, rows_base + 512);
-        head_tile_mma(acc, smem_u32(h_buf), smem_u32(smem) + 2 * kWHeadBytes);
-        if (piece == kPieces - 1) {                                       // the warpgroup is done with this H3 block
-          named_barrier_sync(1 + wg, 128);
-          if (blk + kWG < b_end) load_h(blk + kWG);
-        }
-        stage_acc(acc, piece, rows_base + 1024);
+        named_barrier_sync(1 + wg, 128);                                  // every warp has walked the previous piece's rows
+        wgmma_wait<2>(); acc_fence(acc[0][0]); acc_fence(acc[0][1]);
+        stage_head(acc[0], wg_stage, 0);
+        wgmma_wait<1>(); acc_fence(acc[1][0]); acc_fence(acc[1][1]);
+        stage_head(acc[1], wg_stage, 1);
+        wgmma_wait<0>(); acc_fence(acc[2][0]); acc_fence(acc[2][1]);
+        stage_head(acc[2], wg_stage, 2);
+        named_barrier_sync(1 + wg, 128);                                  // the piece is staged and every product is done
+        if (piece == last_piece && blk + kWG < b_end) load_h(blk + kWG);  // the warpgroup is done with this H3 block
         cp_async_wait<0>();                                               // my count copies have landed (I read only those)
         __syncwarp();
         for (int k = 0; k < kRows; ++k) {
