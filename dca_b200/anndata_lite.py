@@ -4,6 +4,10 @@ Implements only what the DCA surface touches (dca/io.py, dca/api.py, dca/network
 X, obs, var, obsm, uns, raw, n_obs, n_vars, obs_names, var_names, copy(), transpose(),
 boolean row subsetting, obsm_keys(), var_keys(), uns_keys().  When the real ``anndata``
 package is importable the host code accepts its objects as well (duck typing).
+
+X is a dense ndarray, or a scipy.sparse CSR matrix when the constructor is asked to keep one
+(``keep_sparse=True``, as the Matrix Market readers do); copies, the transpose, raw and every
+subset of a CSR AnnData stay CSR.
 """
 from __future__ import annotations
 
@@ -24,11 +28,24 @@ class _Raw:
         return _Raw(self.X[idx], self.var)
 
 
+def _is_sparse(X):
+    return hasattr(X, "toarray")
+
+
+def _copy_x(X):
+    return X.copy() if _is_sparse(X) else np.array(X, copy=True)
+
+
 class AnnData:
-    def __init__(self, X, obs=None, var=None, obsm=None, uns=None, raw=None, dtype=np.float32):
-        if hasattr(X, "toarray"):
-            X = X.toarray()
-        self.X = np.asarray(X, dtype=dtype)
+    def __init__(self, X, obs=None, var=None, obsm=None, uns=None, raw=None, dtype=np.float32, *, keep_sparse=False):
+        """A sparse X is densified unless keep_sparse=True, which keeps it as a CSR matrix of `dtype`."""
+        if _is_sparse(X) and keep_sparse:
+            X = X.tocsr()
+            self.X = X if X.dtype == dtype else X.astype(dtype)
+        else:
+            if _is_sparse(X):
+                X = X.toarray()
+            self.X = np.asarray(X, dtype=dtype)
         if self.X.ndim != 2:
             raise ValueError("X must be 2-dimensional (cells x genes)")
         n, g = self.X.shape
@@ -60,7 +77,7 @@ class AnnData:
         if value is None or isinstance(value, _Raw):
             self._raw = value
         else:   # anndata semantics: adata.raw = adata  freezes X and var
-            self._raw = _Raw(np.array(value.X, copy=True), value.var.copy())
+            self._raw = _Raw(_copy_x(value.X), value.var.copy())
 
     def obsm_keys(self): return list(self.obsm.keys())
     def var_keys(self): return list(self.var.columns)
@@ -70,10 +87,11 @@ class AnnData:
     def copy(self):
         raw = None if self._raw is None else _Raw(self._raw.X.copy(), self._raw.var.copy())
         return AnnData(self.X.copy(), self.obs, self.var, {k: np.array(v, copy=True) for k, v in self.obsm.items()},
-                       dict(self.uns), raw, dtype=self.X.dtype)
+                       dict(self.uns), raw, dtype=self.X.dtype, keep_sparse=True)
 
     def transpose(self):
-        return AnnData(self.X.T.copy(), self.var, self.obs, None, dict(self.uns), None, dtype=self.X.dtype)
+        X = self.X.T.tocsr() if _is_sparse(self.X) else self.X.T.copy()
+        return AnnData(X, self.var, self.obs, None, dict(self.uns), None, dtype=self.X.dtype, keep_sparse=True)
 
     T = property(transpose)
 
@@ -100,7 +118,8 @@ class AnnData:
         idx = np.asarray(idx)
         raw = None if self._raw is None else self._raw[idx]
         return AnnData(self.X[idx], self.obs.iloc[idx] if idx.dtype != bool else self.obs[idx], self.var,
-                       {k: np.asarray(v)[idx] for k, v in self.obsm.items()}, dict(self.uns), raw, dtype=self.X.dtype)
+                       {k: np.asarray(v)[idx] for k, v in self.obsm.items()}, dict(self.uns), raw, dtype=self.X.dtype,
+                       keep_sparse=True)
 
     def __repr__(self):
         return "AnnData(lite) n_obs x n_vars = %d x %d" % self.shape

@@ -2,17 +2,14 @@
 // labels pd.read_csv(path, sep=sep, index_col=0).values.astype(np.float32) gives, bit for bit, for the files whose
 // every value field is [0-9]+ or [0-9]+\.0* (anything else is reported as DCA_ERR_UNSUPPORTED and read by pandas).
 //
-// The host reads the file in chunks into two pinned staging buffers; a chunk ends at its last '\n' and the partial
-// line carries over to the next one.  Per chunk, on the caller's stream:
-//   tile_count    per 4 KB tile: '\n' and separator counts; flags quotes, NUL bytes and a '\r' without '\n'
-//   scan_tiles    one CTA: exclusive prefix of both counts over the tiles; the chunk's line count and first row
-//   line_ends     position of every '\n' and the number of separators before it
+// The file goes through the chunked reader of text_chunks.cuh (two pinned staging buffers; per chunk the tile count,
+// the tile scan and the line ends).  Then per chunk, on the caller's stream:
 //   parse_values  every separator starts a value field: line = '\n' rank, column = separator rank - the line's first
 //                 separator rank; digits go into a uint64 and __ull2float_rn (NumPy's int64 -> float32 cast)
 //   line_check    field count of every line; label extents into mapped host memory for the host to copy
 //   transpose     (transpose != 0) the chunk's rows, staged in file order, into columns of the output by 32 x 32 tiles
 // Problems are recorded as min((file offset << 8) | reason), so the first one in file order is reported.
-#include "dca_internal.cuh"
+#include "text_chunks.cuh"
 
 #include <fcntl.h>
 #include <unistd.h>
@@ -25,16 +22,12 @@
 namespace dca {
 namespace {
 
-constexpr int kThreads = 256;
-constexpr int kBytesPerThread = 16;
-constexpr int kTile = kThreads * kBytesPerThread;      // 4096 bytes per CTA
+using namespace chunked;
+
 constexpr int kMaxDigits = 18;                         // < 2^63: pandas parses the column as int64
 constexpr int kMaxToken = 64;                          // longer value fields ("1.000...") go to pandas
-constexpr int64_t kDefaultChunk = 64ll << 20;
 
-enum Reason : int {
-  R_NONE = 0, R_QUOTE, R_NUL, R_CR, R_FIELDS, R_EMPTY, R_CHAR, R_DIGITS, R_ROWS, R_LINES, R_BIG_DOT
-};
+enum Reason : int { R_FIELDS = 4, R_EMPTY, R_CHAR, R_DIGITS, R_ROWS, R_BIG_DOT = 10 };   // R_QUOTE..R_CR, R_LINES: chunked
 const char* reason_text(int r) {
   switch (r) {
     case R_QUOTE: return "a quote character in a data line";
@@ -52,142 +45,10 @@ const char* reason_text(int r) {
 }
 
 // device state of one read (zeroed / set by the host before the first chunk)
-struct ReadState {
-  unsigned long long err;        // min((file offset << 8) | reason), ~0 when clean
+struct ReadState : ChunkState {
   unsigned long long max_val;    // largest value field
   int any_dot;                   // some value field has a '.'
-  int pad;
-  long long lines_done;          // data lines of the chunks before the current one
-  long long chunk_base;          // first data line of the current chunk
-  int chunk_lines;               // lines of the current chunk (including an unterminated last line)
-  int chunk_seps;
 };
-
-__device__ __forceinline__ void flag(ReadState* st, long long pos, int reason) {
-  atomicMin(&st->err, ((unsigned long long)pos << 8) | (unsigned)reason);
-}
-
-// exclusive block scan of one int per thread (kThreads threads); returns the block total in *total
-__device__ __forceinline__ int block_exclusive_scan(int v, int* smem_warp, int* total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-  if (lane == 31) smem_warp[warp] = x;
-  __syncthreads();
-  if (warp == 0) {
-    int w = lane < kThreads / 32 ? smem_warp[lane] : 0;
-#pragma unroll
-    for (int o = 1; o < kThreads / 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
-    if (lane < kThreads / 32) smem_warp[lane] = w;          // inclusive warp totals
-  }
-  __syncthreads();
-  const int before = (warp ? smem_warp[warp - 1] : 0) + x - v;
-  *total = smem_warp[kThreads / 32 - 1];
-  return before;
-}
-
-// the 16 bytes of this thread (the buffer is padded to whole tiles), and byte i of them without a local array
-__device__ __forceinline__ uint4 load16(const unsigned char* buf, long long p) {
-  return *reinterpret_cast<const uint4*>(buf + p);
-}
-__device__ __forceinline__ unsigned byte_at(const uint4& q, int i) {
-  const unsigned w = i < 8 ? (i < 4 ? q.x : q.y) : (i < 12 ? q.z : q.w);
-  return (w >> ((i & 3) * 8)) & 0xffu;
-}
-
-// packed ('\n' count << 16) | separator count of 16 bytes from p (bytes at or beyond n do not count)
-__device__ __forceinline__ int count16(const uint4& q, long long p, long long n, unsigned char sep) {
-  int nl = 0, sp = 0;
-#pragma unroll
-  for (int i = 0; i < kBytesPerThread; ++i) {
-    const bool in = p + i < n;
-    const unsigned x = byte_at(q, i);
-    nl += in && x == '\n';
-    sp += in && x == sep;
-  }
-  return (nl << 16) | sp;
-}
-
-__global__ void __launch_bounds__(kThreads) tile_count_kernel(const unsigned char* __restrict__ buf, long long n,
-                                                              unsigned char sep, int* tile_nl, int* tile_sep,
-                                                              ReadState* st, long long file_off) {
-  __shared__ int sw[kThreads / 32];
-  const long long p = (long long)blockIdx.x * kTile + threadIdx.x * kBytesPerThread;
-  const uint4 q = load16(buf, p);
-  const int c = count16(q, p, n, sep);
-#pragma unroll
-  for (int i = 0; i < kBytesPerThread; ++i) {
-    if (p + i >= n) break;
-    const unsigned x = byte_at(q, i);
-    if (x == '"') flag(st, file_off + p + i, R_QUOTE);
-    else if (x == 0) flag(st, file_off + p + i, R_NUL);
-    else if (x == '\r' && (p + i + 1 >= n || buf[p + i + 1] != '\n')) flag(st, file_off + p + i, R_CR);
-  }
-  int total;
-  (void)block_exclusive_scan(c, sw, &total);
-  if (threadIdx.x == 0) { tile_nl[blockIdx.x] = total >> 16; tile_sep[blockIdx.x] = total & 0xffff; }
-}
-
-// one CTA: exclusive prefixes of the tile counts, the chunk's line count (+1 for an unterminated last line, which
-// gets a virtual '\n' at n) and its first row
-__global__ void __launch_bounds__(1024) scan_tiles_kernel(int* tile_nl, int* tile_sep, int tiles, long long n, int tail_line,
-                                                          int max_lines, int* nl_pos, int* nl_seprank, ReadState* st,
-                                                          int* h_count, long long file_off) {
-  __shared__ int s_nl[1024], s_sep[1024];
-  __shared__ int carry_nl, carry_sep;
-  if (threadIdx.x == 0) { carry_nl = 0; carry_sep = 0; }
-  __syncthreads();
-  for (int base = 0; base < tiles; base += 1024) {
-    const int i = base + threadIdx.x;
-    const int a = i < tiles ? tile_nl[i] : 0, b = i < tiles ? tile_sep[i] : 0;
-    s_nl[threadIdx.x] = a; s_sep[threadIdx.x] = b;
-    __syncthreads();
-    for (int o = 1; o < 1024; o <<= 1) {          // Hillis-Steele inclusive scan
-      const int x = threadIdx.x >= o ? s_nl[threadIdx.x - o] : 0, y = threadIdx.x >= o ? s_sep[threadIdx.x - o] : 0;
-      __syncthreads();
-      s_nl[threadIdx.x] += x; s_sep[threadIdx.x] += y;
-      __syncthreads();
-    }
-    if (i < tiles) { tile_nl[i] = carry_nl + s_nl[threadIdx.x] - a; tile_sep[i] = carry_sep + s_sep[threadIdx.x] - b; }
-    __syncthreads();
-    if (threadIdx.x == 0) { carry_nl += s_nl[1023]; carry_sep += s_sep[1023]; }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    int lines = carry_nl + tail_line;
-    if (lines > max_lines) { flag(st, file_off, R_LINES); lines = max_lines; }
-    if (tail_line && carry_nl < max_lines) { nl_pos[carry_nl] = (int)n; nl_seprank[carry_nl] = carry_sep; }
-    st->chunk_base = st->lines_done;
-    st->lines_done += lines;
-    st->chunk_lines = lines;
-    st->chunk_seps = carry_sep;
-    *h_count = lines;
-  }
-}
-
-__global__ void __launch_bounds__(kThreads) line_ends_kernel(const unsigned char* __restrict__ buf, long long n,
-                                                             unsigned char sep, const int* __restrict__ tile_nl,
-                                                             const int* __restrict__ tile_sep, int max_lines, int* nl_pos,
-                                                             int* nl_seprank) {
-  __shared__ int sw[kThreads / 32];
-  const long long p = (long long)blockIdx.x * kTile + threadIdx.x * kBytesPerThread;
-  const uint4 q = load16(buf, p);
-  int total;
-  const int before = block_exclusive_scan(count16(q, p, n, sep), sw, &total);
-  int nl = tile_nl[blockIdx.x] + (before >> 16), sp = tile_sep[blockIdx.x] + (before & 0xffff);
-#pragma unroll
-  for (int i = 0; i < kBytesPerThread; ++i) {
-    if (p + i >= n) break;
-    const unsigned x = byte_at(q, i);
-    if (x == '\n') {
-      if (nl < max_lines) { nl_pos[nl] = (int)(p + i); nl_seprank[nl] = sp; }
-      ++nl;
-    } else if (x == sep) {
-      ++sp;
-    }
-  }
-}
 
 // Value fields.  Every separator starts one; its line is the number of '\n' before it and its column the number of
 // separators between the line's start and it.  out: row-major [rows x cols] (row = file line) when stage == NULL,
@@ -287,18 +148,12 @@ __global__ void __launch_bounds__(1024) transpose_kernel(const float* __restrict
 }
 
 // ---------------------------------------------------------------------------------------------------------- host
-struct Buffers {
-  unsigned char* h_buf = nullptr;      // pinned staging
+// a staging buffer with the label and transpose arrays of this reader
+struct Buffers : ChunkBuffers {
   int* h_lab = nullptr;                // mapped: 2 ints per line
-  int* h_count = nullptr;              // mapped
-  unsigned char* d_buf = nullptr;
-  int *tile_nl = nullptr, *tile_sep = nullptr, *nl_pos = nullptr, *nl_seprank = nullptr, *label_end = nullptr;
-  float* stage = nullptr;
   int* d_lab = nullptr;                // device view of h_lab
-  int* d_count = nullptr;
-  cudaEvent_t done = nullptr;
-  long long bytes = 0, file_off = 0;   // chunk in flight: length and offset in the file
-  bool busy = false;
+  int* label_end = nullptr;
+  float* stage = nullptr;
 };
 
 struct Reader {
@@ -313,25 +168,12 @@ struct Reader {
   void release() {
     if (fd >= 0) close(fd);
     for (Buffers& x : b) {
-      if (x.done) { cudaEventSynchronize(x.done); cudaEventDestroy(x.done); }
-      cudaFreeHost(x.h_buf); cudaFreeHost(x.h_lab); cudaFreeHost(x.h_count);
-      cudaFree(x.d_buf); cudaFree(x.tile_nl); cudaFree(x.tile_sep); cudaFree(x.nl_pos); cudaFree(x.nl_seprank);
-      cudaFree(x.label_end); cudaFree(x.stage);
+      x.release();
+      cudaFreeHost(x.h_lab); cudaFree(x.label_end); cudaFree(x.stage);
     }
     cudaFree(d_state);
   }
 };
-
-long long read_full(int fd, unsigned char* dst, long long want) {
-  long long got = 0;
-  while (got < want) {
-    const ssize_t r = ::read(fd, dst + got, (size_t)std::min<long long>(want - got, 1ll << 30));
-    if (r < 0) return -1;
-    if (r == 0) break;
-    got += r;
-  }
-  return got;
-}
 
 // The header line: its byte length (with the line end) and field count; DCA_ERR_UNSUPPORTED for a header pandas would
 // read differently from a plain split (quotes, NUL, a lone '\r') or a file without data lines.
@@ -402,29 +244,19 @@ extern "C" int dca_read_text_counts(const char* path, int32_t sep, int32_t trans
   const int cols = fields - 1;
   if (lseek(rd.fd, header_bytes, SEEK_SET) != header_bytes) { set_error("dca_read_text_counts: seek failed"); return DCA_ERR_BAD_ARG; }
 
-  const long long cap = chunk_bytes ? chunk_bytes : kDefaultChunk;
+  const ChunkGeometry geo = chunk_geometry(chunk_bytes, fields);
+  const long long cap = geo.cap, padded = geo.padded;
   if (cap > (1ll << 30)) { set_error("dca_read_text_counts: chunk_bytes above 1 GB"); return DCA_ERR_BAD_ARG; }
-  const long long padded = (cap + 16 + kTile - 1) / kTile * kTile;       // whole tiles + the byte after the last one
-  const int tiles_cap = (int)(padded / kTile);
-  // a line with `fields` non-empty fields has at least 2 * fields - 1 bytes besides its '\n'
-  const int max_lines = (int)std::min<long long>(cap / (2ll * fields) + 2, INT32_MAX / 2);
+  const int tiles_cap = geo.tiles_cap, max_lines = geo.max_lines;
   const bool staged = fill && transpose;
 
   DCA_CUDA_OK(cudaMalloc(&rd.d_state, sizeof(ReadState)));
   for (Buffers& x : rd.b) {
-    DCA_CUDA_OK(cudaHostAlloc(&x.h_buf, (size_t)padded, cudaHostAllocDefault));
+    DCA_TRY(x.alloc(geo));
     DCA_CUDA_OK(cudaHostAlloc(&x.h_lab, (size_t)max_lines * 2 * sizeof(int), cudaHostAllocMapped));
-    DCA_CUDA_OK(cudaHostAlloc(&x.h_count, sizeof(int), cudaHostAllocMapped));
     DCA_CUDA_OK(cudaHostGetDevicePointer((void**)&x.d_lab, x.h_lab, 0));
-    DCA_CUDA_OK(cudaHostGetDevicePointer((void**)&x.d_count, x.h_count, 0));
-    DCA_CUDA_OK(cudaMalloc(&x.d_buf, (size_t)padded));
-    DCA_CUDA_OK(cudaMalloc(&x.tile_nl, (size_t)tiles_cap * sizeof(int)));
-    DCA_CUDA_OK(cudaMalloc(&x.tile_sep, (size_t)tiles_cap * sizeof(int)));
-    DCA_CUDA_OK(cudaMalloc(&x.nl_pos, (size_t)max_lines * sizeof(int)));
-    DCA_CUDA_OK(cudaMalloc(&x.nl_seprank, (size_t)max_lines * sizeof(int)));
     DCA_CUDA_OK(cudaMalloc(&x.label_end, (size_t)max_lines * sizeof(int)));
     if (staged) DCA_CUDA_OK(cudaMalloc(&x.stage, (size_t)max_lines * cols * sizeof(float)));
-    DCA_CUDA_OK(cudaEventCreateWithFlags(&x.done, cudaEventDisableTiming));
   }
   {
     ReadState init{};
@@ -433,12 +265,9 @@ extern "C" int dca_read_text_counts(const char* path, int32_t sep, int32_t trans
   }
 
   long long rows = 0, labels = 0;
-  std::string err_once;
   // labels of a finished chunk, from its staging bytes (the buffer is reused only after this)
-  auto collect = [&](Buffers& x) -> int {
-    if (!x.busy) return DCA_OK;
-    DCA_CUDA_OK(cudaEventSynchronize(x.done));
-    x.busy = false;
+  auto collect = [&](ChunkBuffers& cb) -> int {
+    const Buffers& x = static_cast<const Buffers&>(cb);
     const int n = *x.h_count;
     for (int k = 0; k < n; ++k) {
       const int a = x.h_lab[2 * k], e = x.h_lab[2 * k + 1];
@@ -452,41 +281,8 @@ extern "C" int dca_read_text_counts(const char* path, int32_t sep, int32_t trans
     }
     return DCA_OK;
   };
-
-  long long file_off = header_bytes, carry = 0;
-  int cur = 0;
-  for (;;) {
-    Buffers& x = rd.b[cur];
-    const long long got = read_full(rd.fd, x.h_buf + carry, cap - carry);
-    if (got < 0) { set_error("dca_read_text_counts: read of %s failed", path); return DCA_ERR_BAD_ARG; }
-    const long long len = carry + got;
-    if (len == 0) break;
-    const bool eof = got < cap - carry;
-    long long end = len;
-    if (!eof) {
-      const void* q = nullptr;
-      for (long long i = len - 1; i >= 0 && !q; --i) if (x.h_buf[i] == '\n') q = x.h_buf + i;
-      if (!q) {
-        set_error("dca_read_text_counts: unsupported file: a line longer than chunk_bytes (%lld) at byte %lld", cap, file_off);
-        return DCA_ERR_UNSUPPORTED;
-      }
-      end = (const unsigned char*)q - x.h_buf + 1;
-    }
-    Buffers& y = rd.b[cur ^ 1];
-    DCA_TRY(collect(y));                       // the other buffer's chunk is done: its labels, then its staging is free
-    carry = len - end;
-    if (carry) memcpy(y.h_buf, x.h_buf + end, (size_t)carry);
-    const int tail_line = x.h_buf[end - 1] != '\n';
-    const int tiles = (int)((end + kTile - 1) / kTile);
-    DCA_CUDA_OK(cudaMemcpyAsync(x.d_buf, x.h_buf, (size_t)end, cudaMemcpyHostToDevice, s));
-    DCA_CUDA_OK(cudaMemsetAsync(x.d_buf + end, 0, (size_t)(padded - end), s));
-    tile_count_kernel<<<tiles, kThreads, 0, s>>>(x.d_buf, end, sp, x.tile_nl, x.tile_sep, rd.d_state, file_off);
-    DCA_LAUNCH_CHECK();
-    scan_tiles_kernel<<<1, 1024, 0, s>>>(x.tile_nl, x.tile_sep, tiles, end, tail_line, max_lines, x.nl_pos, x.nl_seprank,
-                                         rd.d_state, x.d_count, file_off);
-    DCA_LAUNCH_CHECK();
-    line_ends_kernel<<<tiles, kThreads, 0, s>>>(x.d_buf, end, sp, x.tile_nl, x.tile_sep, max_lines, x.nl_pos, x.nl_seprank);
-    DCA_LAUNCH_CHECK();
+  auto launch = [&](ChunkBuffers& cb, long long, long long end, long long file_off, int tiles) -> int {
+    Buffers& x = static_cast<Buffers&>(cb);
     parse_values_kernel<<<tiles, kThreads, 0, s>>>(x.d_buf, end, sp, x.tile_nl, x.tile_sep, x.nl_seprank, x.label_end,
                                                    max_lines, cols, rows_expect, staged ? nullptr : out, x.stage,
                                                    rd.d_state, file_off);
@@ -499,14 +295,11 @@ extern "C" int dca_read_text_counts(const char* path, int32_t sep, int32_t trans
       transpose_kernel<<<grid, 1024, 0, s>>>(x.stage, cols, rows_expect, out, rd.d_state);
       DCA_LAUNCH_CHECK();
     }
-    DCA_CUDA_OK(cudaEventRecord(x.done, s));
-    x.busy = true;
-    file_off += end;
-    cur ^= 1;
-    if (eof && carry == 0) break;
-  }
-  DCA_TRY(collect(rd.b[0]));
-  DCA_TRY(collect(rd.b[1]));
+    return DCA_OK;
+  };
+  DCA_TRY(for_each_chunk("dca_read_text_counts", rd.fd, header_bytes, geo, rd.b[0], rd.b[1], sp, rd.d_state, s, launch,
+                         collect));
+  const long long file_off = lseek(rd.fd, 0, SEEK_CUR);
 
   ReadState fin;
   DCA_CUDA_OK(cudaMemcpyAsync(&fin, rd.d_state, sizeof(fin), cudaMemcpyDeviceToHost, s));

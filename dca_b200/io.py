@@ -21,7 +21,8 @@ def _dense(X):
 
 def read_text_or_h5ad(path: str):
     """sc.read(path, first_column_names=True) -- dca/io.py:59.  Text tables go through the GPU reader when it can take
-    them (read_counts_text), otherwise through pandas; both give the same AnnData."""
+    them (read_counts_text), otherwise through pandas; Matrix Market files through read_counts_mtx, otherwise through
+    scipy; both give the same AnnData."""
     return _read_path(path, False)[0]
 
 
@@ -39,6 +40,14 @@ def _read_path(path, transpose):
         except ImportError as e:
             raise ImportError("reading .h5ad needs the anndata package, which is not installed") from e
         return anndata.read_h5ad(path), False
+    if path.lower().endswith(".mtx.gz"):         # Cell Ranger >= 3 writes its matrix gzipped: scipy decompresses it
+        return _read_mtx_scipy(path), False
+    if ext == ".mtx":
+        if _cuda_available():
+            ad = read_counts_mtx(path, transpose)
+            if ad is not None:
+                return ad, transpose
+        return _read_mtx_scipy(path), False
     sep = "," if ext == ".csv" else "\t"
     if ext in _TEXT_EXTS and _cuda_available():
         ad = read_counts_text(path, sep, transpose)
@@ -117,6 +126,68 @@ def read_counts_text(path, sep, transpose=False, chunk_bytes=0, device=None):
     return AnnData(X, obs=var, var=obs) if transpose else AnnData(X, obs=obs, var=var)
 
 
+def _read_mtx_scipy(path):
+    """scanpy's reader of a .mtx path (anndata.read_mtx): csr_matrix(scipy.io.mmread(path).astype('float32')), with
+    the names '0', '1', ... of both axes."""
+    import warnings
+    import scipy.io
+    import scipy.sparse as sp
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore", DeprecationWarning)        # scipy >= 1.15: spmatrix -> sparse array default
+        X = sp.csr_matrix(scipy.io.mmread(path).astype(np.float32))
+    return AnnData(X, keep_sparse=True)
+
+
+def read_counts_mtx(path, transpose=False, chunk_bytes=0, device=None):
+    """The AnnData _read_mtx_scipy(path) gives (its .transpose() with transpose=True), parsed on a CUDA device by
+    dca_read_mtx_counts (csrc/read_mtx.cu): X is a float32 scipy.sparse.csr_matrix whose indptr, indices and data equal
+    scipy's in dtype and bytes.  None when the GPU reader does not take the file (include/dca_b200.h lists the files it
+    takes: entries in CSR order of the output, as Cell Ranger writes them for transpose=True), the file is compressed,
+    or the arrays do not fit in free device memory.
+
+    The file's bytes go to the device in chunks of chunk_bytes (0: 64 MB) in one pass, and the CSR arrays come back.
+    The index arrays are int32 unless NNZ or a dimension reaches 2^31, as scipy chooses."""
+    import ctypes as C
+    import torch
+    import scipy.sparse as sp
+    from . import _lib
+    with open(path, "rb") as f:
+        if any(f.read(6).startswith(m) for m in _COMPRESSED_MAGIC):
+            return None
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.type != "cuda":
+        raise ValueError("read_counts_mtx parses on a CUDA device (got %s)" % dev)
+    if dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    lib = _lib.load()
+    info = np.zeros(4, dtype=np.int64)
+    stream = torch.cuda.current_stream(dev)
+    with torch.cuda.device(dev):
+        args = (os.fsencode(path), int(bool(transpose)), int(chunk_bytes), dev.index, C.c_void_p(stream.cuda_stream))
+        st = lib.dca_read_mtx_counts(*args, None, None, None, info.ctypes.data)
+        if st == -3:
+            return None
+        _lib.check(st, "dca_read_mtx_counts")
+        rows, cols, nnz, work = (int(v) for v in info)
+        if 8 * (rows + 1) + 8 * nnz + work > torch.cuda.mem_get_info(dev)[0]:
+            return None
+        indptr = torch.empty(rows + 1, dtype=torch.int64, device=dev)
+        indices = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
+        data = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
+        st = lib.dca_read_mtx_counts(*args, C.c_void_p(indptr.data_ptr()), C.c_void_p(indices.data_ptr()),
+                                     C.c_void_p(data.data_ptr()), info.ctypes.data)
+        if st == -3:
+            return None
+        _lib.check(st, "dca_read_mtx_counts")
+        indptr, indices, data = indptr.cpu().numpy(), indices[:nnz].cpu().numpy(), data[:nnz].cpu().numpy()
+    if max(rows, cols, nnz) < 2 ** 31:
+        indptr = indptr.astype(np.int32)
+    else:
+        indices = indices.astype(np.int64)
+    X = sp.csr_matrix((data, indices, indptr), shape=(rows, cols), copy=False)
+    return AnnData(X, keep_sparse=True)
+
+
 def _pandas_chunk_rows(width):
     """Rows per chunk in which pandas' C reader (low_memory=True) infers column types for a table of `width` fields:
     the largest power of two below half of 2**20 // width."""
@@ -154,8 +225,9 @@ def _row_labels(path, sep, labels, offsets, width):
 
 
 def read_dataset(adata, transpose=False, test_split=False, copy=False, check_counts=True):
-    """dca/io.py:53-85.  A path to a text table is read on the GPU when read_counts_text takes it, which transposes on
-    the device; it only returns integer counts, so the check below passes in either orientation."""
+    """dca/io.py:53-85.  A path to a text table is read on the GPU when read_counts_text takes it, and a Matrix Market
+    file when read_counts_mtx takes it; both transpose on the device and only return integer counts, so the check below
+    passes in either orientation.  A .mtx file gives a CSR X (as the reference's AnnData has)."""
     transposed = False
     if is_anndata(adata):
         if copy:

@@ -577,6 +577,29 @@ int dca_read_text_counts(const char* path, int32_t sep, int32_t transpose, int64
                          void* stream, float* out, int64_t out_elems, int64_t* label_offsets, char* label_bytes,
                          int64_t label_cap, int64_t* info);
 
+/* GPU reader of a Matrix Market coordinate file of counts (dca_b200/io.py:read_counts_mtx).  It gives the CSR arrays of
+ * scipy.sparse.csr_matrix(scipy.io.mmread(path).astype(numpy.float32)) (of its .T.tocsr() with transpose != 0), bit for
+ * bit, for exactly the files whose
+ *   - first line is "%%MatrixMarket matrix coordinate integer general" or "... real general", followed by zero or more
+ *     lines starting with '%' and the size line "M N NNZ" (single spaces, digits only, 1 <= M, N < 2^31);
+ *   - NNZ entry lines follow, each "i j v": single spaces, 1 <= i <= M, 1 <= j <= N, v = [0-9]+ of at most 18 digits
+ *     (integer) or 15 digits (real); lines end in '\n' or "\r\n", the last one may have no line end;
+ *   - entries are in strictly increasing (row, column) order of the output, whose entry (row, column) is (i, j), or
+ *     (j, i) with transpose: the CSR order, so there are no duplicates.  Cell Ranger's genes x cells matrix.mtx read
+ *     with transpose, and scipy.io.mmwrite of a CSR cells x genes matrix read without, are in this order;
+ *   - lines each fit in chunk_bytes.
+ * Explicit zeros are kept.  Any other file returns DCA_ERR_UNSUPPORTED with the first reason in file order in
+ * dca_last_error(), and the outputs hold nothing defined.  Two calls with the same arguments:
+ *   1. indptr == NULL: reads the header only; info[0..3] = output rows, output columns, NNZ, device bytes the chunk
+ *      buffers of the second call take besides the outputs.
+ *   2. info as the first call returned it; device int64 indptr[rows + 1], int32 indices[NNZ], float32 data[NNZ]:
+ *      one pass over the entries through two pinned chunk buffers (chunk_bytes each, 0 = 64 MB), overlapping the disk
+ *      read with the copy and the kernels on `stream` (of `device`); it returns when they are done, and stops at the
+ *      first chunk with a problem.  Entry k of the file goes to slot k; indptr is written without atomics.
+ * File offsets, entry ordinals and indptr are 64-bit.  Without a CUDA device it returns DCA_ERR_NO_DEVICE. */
+int dca_read_mtx_counts(const char* path, int32_t transpose, int64_t chunk_bytes, int32_t device, void* stream,
+                        int64_t* indptr, int32_t* indices, float* data, int64_t* info);
+
 /* Host-side packer for dca_stream_begin_packed (multi-threaded counterpart of dca_b200/io.py:pack_counts; no
  * reference counterpart).  counts: HOST matrix rows x cols (ld elements per row) of dtype 0 float32, 1 float64,
  * 2 uint16, 3 int32, 4 int64 holding non-negative integers.  dca_count_escapes fills per_row[w*rows + r] with the
