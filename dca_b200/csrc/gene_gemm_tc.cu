@@ -21,12 +21,21 @@
 //
 // 256 threads = two warpgroups; thread 0 also issues the TMA loads, kStages - 1 tiles ahead (gathered rows: every
 // thread also issues its share of the Z copies).
+//
+// The head backward runs both item kinds in one launch (BANDED; dca_set_tunable("head_bwd_banded", 0) gives the two
+// launches of one kind each).  The items are the same as in the two launches, so every sum keeps its order and its bits;
+// only their order changes.  A band is (head, (b) gene range): its (a) items (one gene block each, over all cell
+// blocks) and its (b) items (one cell block each, over the band's gene blocks) alternate in the item order, so they
+// run at about the same time and most tiles of dZ are read from HBM once, the second read hitting L2.
 #include "engine.h"
 #include "tc_common.cuh"
 
 namespace dca {
 namespace tc {
 int g_gg_profile = 0;       // dca_set_tunable("gg_profile", 1): phase timeline of the hidden-stack kernels (mid_stack.cu)
+int g_head_bwd_banded = 1;  // dca_set_tunable("head_bwd_banded", 0 | 1): head backward as one band-ordered launch
+int g_head_bwd_stagger = 1300;  // dca_set_tunable("head_bwd_stagger", SM cycles): its start delay per band position
+                                // (tests/diag_head_bwd.py sweep, DESIGN §8)
 namespace gg {
 
 constexpr int kThreads = 256;
@@ -38,13 +47,37 @@ constexpr uint32_t kOnesBytes = 16 * 128;            // [16 x 64] bf16 ones, K-m
 constexpr int kMaxGb = 4;                            // (a): gene blocks per item held in registers
 constexpr int kMaxSlots = 16;                        // (b): partial slots (heads x gene ranges)
 
-template <bool DO_A, bool DO_B>
-constexpr int stages() { return DO_A && DO_B ? 2 : 3; }
-template <bool DO_A, bool DO_B>
-constexpr uint32_t stage_bytes() { return kZBytes + (DO_B ? kWBytes : 0) + (DO_A ? kHBytes : 0); }
-template <bool DO_A, bool DO_B, bool COLSUM>
+// BANDED: a stage holds Z and the W tile ((b) item) or the H tile ((a) item) at the same offset
+static_assert(kWBytes == kHBytes, "the two item kinds of the banded launch share one stage shape");
+template <bool DO_A, bool DO_B, bool BANDED>
+constexpr int stages() { return DO_A && DO_B && !BANDED ? 2 : 3; }
+template <bool DO_A, bool DO_B, bool BANDED>
+constexpr uint32_t stage_bytes() { return BANDED ? kZBytes + kWBytes : kZBytes + (DO_B ? kWBytes : 0) + (DO_A ? kHBytes : 0); }
+template <bool DO_A, bool DO_B, bool COLSUM, bool BANDED>
 constexpr uint32_t smem_bytes() {
-  return stages<DO_A, DO_B>() * stage_bytes<DO_A, DO_B>() + (DO_A ? kOutBytes : 0) + (COLSUM ? kOnesBytes : 0) + 1024;
+  return stages<DO_A, DO_B, BANDED>() * stage_bytes<DO_A, DO_B, BANDED>() + (DO_A ? kOutBytes : 0) + (COLSUM ? kOnesBytes : 0) + 1024;
+}
+
+// One item of the banded head backward.  kind 0: (a) item = gene block gb0 of head `head` over all cell blocks;
+// kind 1: (b) item = cell block cb0 over gene blocks [gb0, gb0 + ng) = (b) gene range gr, partial slot
+// head * ranges + gr.
+struct BandItem { int kind, head, gr, gb0, ng, cb0, ncb; };
+
+// Item k of the band order: bands (head, gene range of gpr gene blocks; only the last range of a head may be shorter)
+// head-major; within a band (a) and (b) items alternate, (a) first, and the longer kind's remaining items follow.  Tile
+// (gb0 + i, cell block j) of a band is read by its (a) item i at step j and by its (b) item j at step i.
+__host__ __device__ inline BandItem band_item(int k, int n_gb, int n_cb, int gpr, int ranges) {
+  const int per_head = n_gb + ranges * n_cb, full_band = gpr + n_cb;
+  BandItem it;
+  it.head = k / per_head; k -= it.head * per_head;
+  it.gr = min(k / full_band, ranges - 1); k -= it.gr * full_band;
+  const int gb0 = it.gr * gpr, ng = min(n_gb, gb0 + gpr) - gb0, m = min(ng, n_cb);
+  int idx;
+  if (k < 2 * m) { it.kind = k & 1; idx = k >> 1; }
+  else { it.kind = ng > n_cb ? 0 : 1; idx = k - m; }
+  if (it.kind == 0) { it.gb0 = gb0 + idx; it.ng = 1; it.cb0 = 0; it.ncb = n_cb; }
+  else { it.gb0 = gb0; it.ng = ng; it.cb0 = idx; it.ncb = 1; }
+  return it;
 }
 
 struct Params {
@@ -53,7 +86,8 @@ struct Params {
   int gb_per_item, cb_per_item;
   int gene_ranges, cell_splits;   // per head
   int total_items;
-  float* db[3];                   // column sums of Z per head (COLSUM)
+  int stagger;                    // BANDED: start delay per band position, SM cycles (0: none)
+  float* db[3];                  // column sums of Z per head (COLSUM)
   float* part; int64_t part_stride;   // (b): partial slot (head * gene_ranges + gene range) of part_stride floats
   // cell i of the batch is row rows[i] of zsrc (ld ldz; one Z); rows == null: the tiles are rows of map_z*
   const int32_t* rows; const __nv_bfloat16* zsrc; int64_t ldz;
@@ -68,16 +102,19 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// MAXG: gene blocks per item held in registers (the (a) accumulators); WK: W is K-major (Keras [64 x G] head kernel)
-template <bool DO_A, bool DO_B, bool COLSUM, bool WK, int MAXG>
+// MAXG: gene blocks per item held in registers (the (a) accumulators); WK: W is K-major (Keras [64 x G] head kernel);
+// BANDED (with DO_A, DO_B): each item is one kind, (a) or (b), in band order (band_item)
+template <bool DO_A, bool DO_B, bool COLSUM, bool WK, int MAXG, bool BANDED>
 __global__ void __launch_bounds__(kThreads, 1)
 gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_constant__ CUtensorMap map_z1,
                  const __grid_constant__ CUtensorMap map_z2, const __grid_constant__ CUtensorMap map_h,
                  const __grid_constant__ CUtensorMap map_w0, const __grid_constant__ CUtensorMap map_w1,
                  const __grid_constant__ CUtensorMap map_w2, const __grid_constant__ CUtensorMap map_dw0, const __grid_constant__ CUtensorMap map_dw1,
                  const __grid_constant__ CUtensorMap map_dw2, const int dw_transposed, const Params p) {
-  constexpr int kStages = stages<DO_A, DO_B>();
-  constexpr uint32_t kStage = stage_bytes<DO_A, DO_B>();
+  static_assert(!BANDED || (DO_A && DO_B && MAXG == 1), "banded items hold one gene block of (a) accumulators");
+  constexpr int kStages = stages<DO_A, DO_B, BANDED>();
+  constexpr uint32_t kStage = stage_bytes<DO_A, DO_B, BANDED>();
+  constexpr uint32_t kHOff = kZBytes + (DO_B && !BANDED ? kWBytes : 0);   // H tile within a stage
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* s_st = smem;                                                  // [kStages][Z | W | H]
@@ -124,12 +161,34 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
   const int g_rh = threadIdx.x >> 3, g_c = threadIdx.x & 7, g_h = g_rh & 1, g_r0 = g_rh >> 1;
   const uint32_t g_dst = g_h * (kZBytes / 2) + g_r0 * 128 + ((g_c ^ (g_r0 & 7)) << 4);
   int src_row[8];
+  if constexpr (BANDED) {
+    // Start stagger: the CTA whose first item is a band's item i (of either kind) starts i x p.stagger SM cycles late,
+    // about i tile steps.  (a) item i then reads tile (i, j) at about the time (b) item j does, so the second read of a
+    // tile follows the first closely; later items keep the offset (equal item lengths, grid of whole bands).
+    if (p.stagger > 0 && blockIdx.x < p.total_items) {
+      const BandItem it = band_item(blockIdx.x, p.n_gb, p.n_cb, p.gb_per_item, p.gene_ranges);
+      const long long wait = (long long)(it.kind ? it.cb0 : it.gb0 - it.gr * p.gb_per_item) * p.stagger;
+      if (threadIdx.x == 0) {
+        const long long c0 = clock64();
+        while (clock64() - c0 < wait) __nanosleep(100);
+      }
+      __syncthreads();
+    }
+  }
   for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
-    // item -> (head, gene blocks [gb0, gb1), cell blocks [cb0, cb1))
-    const int cs = item % p.cell_splits, r = item / p.cell_splits;
-    const int gr = r % p.gene_ranges, head = r / p.gene_ranges;
-    const int gb0 = gr * p.gb_per_item, ng = min(p.n_gb, gb0 + p.gb_per_item) - gb0;
-    const int cb0 = cs * p.cb_per_item, ncb = min(p.n_cb, cb0 + p.cb_per_item) - cb0;
+    // item -> (head, gene blocks [gb0, gb1), cell blocks [cb0, cb1)); ia / ib: the item computes (a) / (b)
+    int head, gr, gb0, ng, cb0, ncb;
+    bool ia = DO_A, ib = DO_B;
+    if constexpr (BANDED) {
+      const BandItem it = band_item(item, p.n_gb, p.n_cb, p.gb_per_item, p.gene_ranges);
+      head = it.head; gr = it.gr; gb0 = it.gb0; ng = it.ng; cb0 = it.cb0; ncb = it.ncb;
+      ia = it.kind == 0; ib = !ia;
+    } else {
+      const int cs = item % p.cell_splits, r = item / p.cell_splits;
+      gr = r % p.gene_ranges; head = r / p.gene_ranges;
+      gb0 = gr * p.gb_per_item; ng = min(p.n_gb, gb0 + p.gb_per_item) - gb0;
+      cb0 = cs * p.cb_per_item; ncb = min(p.n_cb, cb0 + p.cb_per_item) - cb0;
+    }
     const int n_tiles = ng * ncb;
     const CUtensorMap* mz = head == 0 ? &map_z0 : (head == 1 ? &map_z1 : &map_z2);
     const CUtensorMap* mw = head == 0 ? &map_w0 : (head == 1 ? &map_w1 : &map_w2);
@@ -144,7 +203,7 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
         tma_load_2d(dst, mz, gb * 128, cb * 128, &full[st]);
         tma_load_2d(dst + kZBytes / 2, mz, gb * 128 + 64, cb * 128, &full[st]);
       }
-      if (DO_B) {
+      if (DO_B && ib) {
         if (WK) {        // head backward: W = Keras [64 x G] (K-major B): two [64 feats x 64 genes] boxes
           tma_load_2d(dst + kZBytes, mw, gb * 128, 0, &full[st]);
           tma_load_2d(dst + kZBytes + kWBytes / 2, mw, gb * 128 + 64, 0, &full[st]);
@@ -152,7 +211,7 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
           tma_load_2d(dst + kZBytes, mw, 0, gb * 128, &full[st]);
         }
       }
-      if (DO_A) tma_load_2d(dst + kZBytes + (DO_B ? kWBytes : 0), &map_h, 0, cb * 128, &full[st]);
+      if (DO_A && ia) tma_load_2d(dst + kHOff, &map_h, 0, cb * 128, &full[st]);
     };
     auto load_rows = [&](int t) {                   // gathered rows: source rows of this thread's rows of tile t
       const int cb = cb0 + t / ng;
@@ -203,7 +262,7 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
       // whole gene range with one accumulator
 #pragma unroll
       for (int jj = 0; jj < (DO_A ? MAXG : 1); ++jj)
-      for (int j = jj; j < (DO_A ? min(jj + 1, ng) : ng); ++j) {
+      for (int j = jj; j < (DO_A && ia ? min(jj + 1, ng) : ng); ++j) {
         if (t + kStages - 1 < n_tiles) {            // its stage was released at tile t-1
           if (threadIdx.x == 0) issue(t + kStages - 1);
           if (gather) copy_rows(t + kStages - 1);
@@ -216,9 +275,10 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
         }
         const int st = (T0 + t) % kStages;
         mbar_wait(&full[st], ((T0 + t) / kStages) & 1);
-        const uint32_t zb = smem_u32(s_st + st * kStage), wb = zb + kZBytes, hb = wb + (DO_B ? kWBytes : 0);
+        const uint32_t zb = smem_u32(s_st + st * kStage), wb = zb + kZBytes, hb = zb + kHOff;
         wgmma_fence();
         if constexpr (DO_B) {
+          if (ib)
 #pragma unroll
           for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -229,6 +289,7 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
             }
         }
         if constexpr (DO_A) {
+          if (ia)
 #pragma unroll
           for (int k = 0; k < 8; ++k) {
             const uint64_t da = make_smem_desc(zb + wg * (kZBytes / 2) + k * 2048, 0, 1024);
@@ -250,7 +311,7 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
         __syncthreads();                            // every warpgroup is done with stage st
         ++t;
       }
-      if constexpr (DO_B) {  // (b) of this cell block -> this item's partial slot (rows padded to whole cell blocks)
+      if constexpr (DO_B) if (ib) {  // (b) of this cell block -> this item's partial slot (rows padded to whole cell blocks)
         float* dst = p.part + (int64_t)(head * p.gene_ranges + gr) * p.part_stride + (int64_t)cb * 128 * 64;
 #pragma unroll
         for (int i = 0; i < 32; i += 2) {
@@ -260,7 +321,7 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
       }
     }
     T0 += n_tiles;
-    if constexpr (DO_A) {  // (a) of the item: one [128 genes x 64] block per gene block
+    if (DO_A && ia) {      // (a) of the item: one [128 genes x 64] block per gene block
 #pragma unroll
       for (int j = 0; j < MAXG; ++j) {
         if (j >= ng) break;
@@ -308,13 +369,48 @@ __global__ void gene_gemm_reduce_kernel(const float* __restrict__ part, int slot
   *reinterpret_cast<float4*>(out + i) = acc;
 }
 
+// Item plans; p holds n_cb and n_gb.  The (b) gene ranges fix the partial slots and so the bits of the Z.W products:
+// the banded head backward takes them from plan_b.
+// (a): items = (head, gene range) over all cells.  gpi (gene blocks per item, <= kMaxGb for the registers) by the
+// shortest makespan in tile units: rounds x (tiles per item + a flush term per gene block)
+void plan_a(Params& p, int n_heads, int sm_count) {
+  int best_gpi = 1; long long best_cost = -1;
+  for (int gpi = 1; gpi <= kMaxGb; ++gpi) {
+    const long long items = (long long)cdiv(p.n_gb, gpi) * n_heads, rounds = (items + sm_count - 1) / sm_count;
+    const long long cost = rounds * ((long long)gpi * p.n_cb + 2ll * gpi);
+    if (best_cost < 0 || cost < best_cost) { best_cost = cost; best_gpi = gpi; }
+  }
+  p.gb_per_item = best_gpi; p.gene_ranges = cdiv(p.n_gb, best_gpi);
+  p.cb_per_item = p.n_cb; p.cell_splits = 1;
+  p.total_items = p.gene_ranges * n_heads;
+}
+// (b): items = (head, gene range, cell block), ~4 per SM, at most kMaxSlots partial slots
+void plan_b(Params& p, int n_heads, int sm_count) {
+  p.cb_per_item = 1; p.cell_splits = p.n_cb;
+  int gsplits = cdiv(4 * sm_count, p.n_cb * n_heads); if (gsplits < 1) gsplits = 1;
+  if (gsplits > kMaxSlots / n_heads) gsplits = kMaxSlots / n_heads;
+  if (gsplits > p.n_gb) gsplits = p.n_gb;
+  while (gsplits > 1 && cdiv(p.n_gb, gsplits) < 4) --gsplits;
+  p.gb_per_item = cdiv(p.n_gb, gsplits); p.gene_ranges = cdiv(p.n_gb, p.gb_per_item);
+  p.total_items = p.gene_ranges * p.cell_splits * n_heads;
+}
+// Banded head backward: plan_b's gene ranges, (a) items of one gene block (their bits do not depend on the item size).
+// The grid is a whole number of full bands when the SM budget holds one, so that the bands of a wave start together.
+void plan_banded(Params& p, int n_heads, int sm_count, int* grid) {
+  plan_b(p, n_heads, sm_count);
+  p.total_items = n_heads * (p.n_gb + p.gene_ranges * p.n_cb);
+  const int band = p.gb_per_item + p.n_cb;
+  *grid = min(p.total_items, sm_count >= band ? sm_count / band * band : sm_count);
+}
+
 }  // namespace gg
 
 size_t gene_gemm_workspace_bytes(int B) { return sizeof(float) * (size_t)gg::kMaxSlots * cdiv(B, 128) * 128 * 64; }
 
 // Z: bf16 [B x G] per head (ldz elements); H: bf16 [B x 64]; W[i]: bf16 Keras-layout kernels -- [G x 64] for mode 1 (the
 // encoder kernel), [64 x G] per head for mode 3; out_b: fp32 [B x 64] (+=).
-// mode: 1 = encoder forward (K1), 2 = encoder backward (K5), 3 = head backward (K4: dW / db pass, then the dH pass).
+// mode: 1 = encoder forward (K1), 2 = encoder backward (K5), 3 = head backward (K4: one band-ordered launch of the dW /
+// db and dH items, or with head_bwd_banded = 0 the dW / db pass, then the dH pass).
 // ws: gene_gemm_workspace_bytes(B) of device memory for the partial slots of modes 1 and 3.
 // rows (modes 1 and 2, may be null): cell i of the batch is row rows[i] of Z[0]; every index must be a row of Z[0].
 int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, const int32_t* rows, int B, int G, int n_heads,
@@ -357,44 +453,40 @@ int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, const i
 
   // at most one CTA per SM (shared memory) and at most sm_count CTAs: a caller that passes fewer SMs than the device has
   // leaves the others free; the CTAs stride over the items
-#define DCA_GG_LAUNCH(P, A, Bb, Cc, WKk, MG)                                                                           \
+#define DCA_GG_LAUNCH(P, GRID, A, Bb, Cc, WKk, MG, BND)                                                                \
   do {                                                                                                                 \
     static bool attr = false;                                                                                          \
-    constexpr uint32_t sm = smem_bytes<A, Bb, Cc>();                                                                       \
-    if (!attr) { DCA_CUDA_OK(cudaFuncSetAttribute(gene_gemm_kernel<A, Bb, Cc, WKk, MG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); attr = true; } \
-    gene_gemm_kernel<A, Bb, Cc, WKk, MG><<<min(P.total_items, sm_count), kThreads, sm, s>>>(mz[0], mz[1], mz[2], mh, mw[0], mw[1], mw[2],      \
+    constexpr uint32_t sm = smem_bytes<A, Bb, Cc, BND>();                                                              \
+    if (!attr) { DCA_CUDA_OK(cudaFuncSetAttribute(gene_gemm_kernel<A, Bb, Cc, WKk, MG, BND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); attr = true; } \
+    gene_gemm_kernel<A, Bb, Cc, WKk, MG, BND><<<GRID, kThreads, sm, s>>>(mz[0], mz[1], mz[2], mh, mw[0], mw[1], mw[2],  \
                                                                           mdw[0], mdw[1], mdw[2], dW_transposed, P);  \
     DCA_LAUNCH_CHECK();                                                                                                \
   } while (0)
 
-  if (do_a) {
-    // (a): items = (head, gene range) over all cells.  gpi (gene blocks per item, <= kMaxGb for the registers) by the
-    // shortest makespan in tile units: rounds x (tiles per item + a flush term per gene block)
+  if (mode == 3 && g_head_bwd_banded) {
     Params p = base;
-    int best_gpi = 1; long long best_cost = -1;
-    for (int gpi = 1; gpi <= kMaxGb; ++gpi) {
-      const long long items = (long long)cdiv(p.n_gb, gpi) * n_heads, rounds = (items + sm_count - 1) / sm_count;
-      const long long cost = rounds * ((long long)gpi * p.n_cb + 2ll * gpi);
-      if (best_cost < 0 || cost < best_cost) { best_cost = cost; best_gpi = gpi; }
-    }
-    p.gb_per_item = best_gpi; p.gene_ranges = cdiv(p.n_gb, best_gpi);
-    p.cb_per_item = p.n_cb; p.cell_splits = 1;
-    p.total_items = p.gene_ranges * n_heads;
-    if (mode == 3) DCA_GG_LAUNCH(p, true, false, true, false, kMaxGb);
-    else DCA_GG_LAUNCH(p, true, false, false, false, kMaxGb);
+    int grid = 0;
+    plan_banded(p, n_heads, sm_count, &grid);
+    p.stagger = g_head_bwd_stagger;
+    DCA_GG_LAUNCH(p, grid, true, true, true, true, 1, true);
+    const int64_t n = (int64_t)B * 64;
+    gene_gemm_reduce_kernel<<<(unsigned)cdiv(n / 4, 256), 256, 0, s>>>(p.part, p.gene_ranges * n_heads, p.part_stride, out_b, n);
+    DCA_LAUNCH_CHECK();
+    return DCA_OK;
+  }
+  if (do_a) {
+    Params p = base;
+    plan_a(p, n_heads, sm_count);
+    const int grid = min(p.total_items, sm_count);
+    if (mode == 3) DCA_GG_LAUNCH(p, grid, true, false, true, false, kMaxGb, false);
+    else DCA_GG_LAUNCH(p, grid, true, false, false, false, kMaxGb, false);
   }
   if (do_b) {
-    // (b): items = (head, gene range, cell block), ~4 per SM, at most kMaxSlots partial slots
     Params p = base;
-    p.cb_per_item = 1; p.cell_splits = p.n_cb;
-    int gsplits = cdiv(4 * sm_count, p.n_cb * n_heads); if (gsplits < 1) gsplits = 1;
-    if (gsplits > kMaxSlots / n_heads) gsplits = kMaxSlots / n_heads;
-    if (gsplits > p.n_gb) gsplits = p.n_gb;
-    while (gsplits > 1 && cdiv(p.n_gb, gsplits) < 4) --gsplits;
-    p.gb_per_item = cdiv(p.n_gb, gsplits); p.gene_ranges = cdiv(p.n_gb, p.gb_per_item);
-    p.total_items = p.gene_ranges * p.cell_splits * n_heads;
-    if (mode == 3) DCA_GG_LAUNCH(p, false, true, false, true, 1);
-    else DCA_GG_LAUNCH(p, false, true, false, false, 1);
+    plan_b(p, n_heads, sm_count);
+    const int grid = min(p.total_items, sm_count);
+    if (mode == 3) DCA_GG_LAUNCH(p, grid, false, true, false, true, 1, false);
+    else DCA_GG_LAUNCH(p, grid, false, true, false, false, 1, false);
     const int64_t n = (int64_t)B * 64;
     gene_gemm_reduce_kernel<<<(unsigned)cdiv(n / 4, 256), 256, 0, s>>>(p.part, p.gene_ranges * n_heads, p.part_stride, out_b, n);
     DCA_LAUNCH_CHECK();
@@ -444,4 +536,45 @@ extern "C" int dca_tc_gene_gemm(int32_t mode, const void* Z0, const void* Z1, co
                                 float* db2, void* stream) {
   return dca_tc_gene_gemm_sms(mode, Z0, Z1, Z2, ldz, batch, genes, n_heads, H, W, out_b, dW0, dW1, dW2, dW_ld,
                               dW_transposed, db0, db1, db2, stream, 0);
+}
+extern "C" int dca_head_bwd_schedule(int32_t batch, int32_t genes, int32_t n_heads, int32_t sm_count, int32_t banded,
+                                     int32_t* items, int64_t cap, int64_t* n_items, int32_t* grid) {
+  if (batch <= 0 || genes <= 0 || n_heads < 1 || n_heads > 3 || sm_count < 1 || !n_items || !grid) {
+    set_error("dca_head_bwd_schedule: bad argument"); return DCA_ERR_BAD_ARG;
+  }
+  tc::gg::Params base{};
+  base.n_cb = cdiv(batch, 128); base.n_gb = cdiv(genes, 128);
+  int64_t k = 0;
+  auto put = [&](int launch, int kind, int head, int gb0, int ng, int cb0, int ncb, int slot) {
+    if (items && k < cap) {
+      int32_t* r = items + 8 * k;
+      r[0] = launch; r[1] = kind; r[2] = head; r[3] = gb0; r[4] = ng; r[5] = cb0; r[6] = ncb; r[7] = slot;
+    }
+    ++k;
+  };
+  if (banded) {
+    tc::gg::Params p = base;
+    plan_banded(p, n_heads, sm_count, &grid[0]);
+    grid[1] = 0;
+    for (int i = 0; i < p.total_items; ++i) {
+      const tc::gg::BandItem it = tc::gg::band_item(i, p.n_gb, p.n_cb, p.gb_per_item, p.gene_ranges);
+      put(0, it.kind, it.head, it.gb0, it.ng, it.cb0, it.ncb, it.kind ? it.head * p.gene_ranges + it.gr : -1);
+    }
+  } else {   // the kernel's item decoding of the two launches
+    tc::gg::Params pa = base, pb = base;
+    plan_a(pa, n_heads, sm_count);
+    plan_b(pb, n_heads, sm_count);
+    grid[0] = std::min(pa.total_items, (int)sm_count); grid[1] = std::min(pb.total_items, (int)sm_count);
+    for (int pass = 0; pass < 2; ++pass) {
+      const tc::gg::Params& p = pass ? pb : pa;
+      for (int i = 0; i < p.total_items; ++i) {
+        const int cs = i % p.cell_splits, r = i / p.cell_splits, gr = r % p.gene_ranges, head = r / p.gene_ranges;
+        const int gb0 = gr * p.gb_per_item, cb0 = cs * p.cb_per_item;
+        put(pass, pass, head, gb0, std::min(p.n_gb, gb0 + p.gb_per_item) - gb0, cb0, std::min(p.n_cb, cb0 + p.cb_per_item) - cb0,
+            pass ? head * p.gene_ranges + gr : -1);
+      }
+    }
+  }
+  *n_items = k;
+  return DCA_OK;
 }

@@ -15,7 +15,7 @@
 #include <cstdlib>
 
 namespace dca {
-namespace tc { extern int g_gg_profile; }
+namespace tc { extern int g_gg_profile; extern int g_head_bwd_banded; extern int g_head_bwd_stagger; }
 
 namespace {
 
@@ -1260,6 +1260,8 @@ extern "C" int dca_set_tunable(const char* name, int64_t value) {
   else if (n == "loss_branch_free" && (value == 0 || value == 1)) g_tune.branch_free = (int)value;
   else if (n == "loss_ring" && value >= 0 && value <= 2) g_tune.ring = (int)value;
   else if (n == "gg_profile" && (value == 0 || value == 1)) tc::g_gg_profile = (int)value;
+  else if (n == "head_bwd_banded" && (value == 0 || value == 1)) tc::g_head_bwd_banded = (int)value;
+  else if (n == "head_bwd_stagger" && value >= 0 && value <= 100000) tc::g_head_bwd_stagger = (int)value;
   else { set_error("dca_set_tunable: unknown name or value out of range (%s = %lld)", name, (long long)value); return DCA_ERR_BAD_ARG; }
   return DCA_OK;
 }

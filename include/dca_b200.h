@@ -461,6 +461,15 @@ int dca_tc_gene_gemm_rows(int32_t mode, const void* Z0, const void* Z1, const vo
                           int32_t batch, int32_t genes, int32_t n_heads, const void* H, const void* W, float* out_b,
                           float* dW0, float* dW1, float* dW2, int64_t dW_ld, int32_t dW_transposed,
                           float* db0, float* db1, float* db2, void* stream, int32_t sm_count);
+/* The item schedule of mode 3 (host only, no device needed) for a batch of `batch` cells, `genes` genes, n_heads heads
+ * and a grid of at most sm_count CTAs.  banded = 1: the one band-ordered launch (tunable "head_bwd_banded" = 1);
+ * 0: the dW / db launch, then the dH launch.  Writes *n_items and grid[0..1] (CTAs of launch 0 and 1; 0 = no launch);
+ * items (may be NULL) receives min(*n_items, cap) rows of 8 int32 in launch order: (launch, kind, head, first gene
+ * block, gene blocks, first cell block, cell blocks, partial slot).  kind 0: dW / db over the item's 128-gene blocks and
+ * all cells (slot -1); kind 1: dH over the item's gene blocks into its partial slot.  CTA c of a launch runs the
+ * launch's items c, c + grid, c + 2 grid, ... */
+int dca_head_bwd_schedule(int32_t batch, int32_t genes, int32_t n_heads, int32_t sm_count, int32_t banded,
+                          int32_t* items, int64_t cap, int64_t* n_items, int32_t* grid);
 
 /* ---- preprocessing of raw counts in HBM (csrc/preprocess.cu) ------------------------------------------------------
  * dca/io.py:88-111 -- scanpy's pp.filter_genes / pp.filter_cells(min_counts=1), pp.normalize_per_cell, pp.log1p and
@@ -624,7 +633,9 @@ int64_t dca_launch_count(void);
  * a captured step graph keeps the values it was recorded with): "loss_target_blocks",
  * "loss_producer_sleep_ns", "loss_consumer_sleep_ns", "loss_branch_free" (0 | 1, default 1); "fused_heads" (0 | 1, default 0): engines created afterwards
  * run head forward + loss + head backward of a zinb-conddisp training step as one fused kernel (flash_zinb.cu)
- * instead of three (environment override DCA_FUSED_HEADS).  Profiling aid -- no reference counterpart. */
+ * instead of three (environment override DCA_FUSED_HEADS); "head_bwd_banded" (0 | 1, default 1): the head backward
+ * as one band-ordered launch instead of two (same bits); "head_bwd_stagger" (SM cycles, default 1300): the start delay
+ * of that launch's CTAs per position in their band.  Profiling aid -- no reference counterpart. */
 int dca_set_tunable(const char* name, int64_t value);
 
 #ifdef __cplusplus
