@@ -132,6 +132,9 @@ PROTOTYPES = {
     "dca_profile_read": (C.c_int, [_vp, C.POINTER(C.c_double * 6), C.POINTER(C.c_int64 * 6), _i32]),
     "dca_engine_info": (C.c_int, [_vp, C.POINTER(_i32 * 8)]),
     "dca_write_text_matrix": (C.c_int, [C.c_char_p, _vp, _i32, _i64, _i64, _i64, _vp, _vp, _i32, _i32]),
+    "dca_write_text_device": (C.c_int, [C.c_char_p, _i32, _vp, _i64, _i64, _i64, _i32, _vp, _i64, _vp, _vp, _i64, _i32, _vp,
+                                        _vp]),
+    "dca_format_fixed6_host": (C.c_int, [_vp, _i64, _vp, _vp]),
     "dca_read_text_counts": (C.c_int, [C.c_char_p, _i32, _i32, _i64, _i32, _vp, _vp, _i64, _vp, _vp, _i64, _vp]),
     "dca_read_mtx_counts": (C.c_int, [C.c_char_p, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
     "dca_count_escapes": (C.c_int, [_vp, _i32, _i64, _i64, _i64, _vp, _i32]),

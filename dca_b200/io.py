@@ -435,6 +435,81 @@ def write_text_matrix(matrix, filename, rownames=None, colnames=None, transpose=
                "dca_write_text_matrix")
 
 
+def quote_label(name):
+    """The bytes of one label in the files write_text_matrix writes: str(name) in UTF-8, quoted csv.QUOTE_MINIMAL style
+    (inside '"', quotes doubled) only when it holds a tab, a quote, '\\n' or '\\r'."""
+    b = str(name).encode()
+    if any(c in b for c in b'\t"\n\r'):
+        return b'"' + b.replace(b'"', b'""') + b'"'
+    return b
+
+
+def label_bytes(names, n):
+    """(bytes, int64 offsets[n + 1]) of the quoted labels `names` back to back: the label block dca_write_text_device
+    takes."""
+    vals = [quote_label(v) for v in list(names)]
+    if len(vals) != n:
+        raise ValueError("got %d labels for %d rows/columns" % (len(vals), n))
+    offsets = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum([len(v) for v in vals], out=offsets[1:])
+    return b"".join(vals), offsets
+
+
+def header_bytes(colnames, has_rownames):
+    """The header line of write_text_matrix: the quoted column labels joined by tabs, after an empty cell when the
+    lines have labels."""
+    return (b"\t" if has_rownames else b"") + b"\t".join(quote_label(v) for v in list(colnames)) + b"\n"
+
+
+def write_text_matrix_device(tensor, filename, rownames=None, colnames=None, transpose=False, append=False,
+                             header=True, chunk_bytes=0, info=None):
+    """write_text_matrix(tensor.cpu().numpy(), filename, rownames, colnames, transpose) byte for byte, formatted on the
+    tensor's CUDA device (dca_write_text_device, csrc/write_text.cu): a float32 matrix in device memory becomes text
+    without a host copy of it.  The text reaches the file in pinned pieces of chunk_bytes (0: 16 MB), the write of one
+    overlapping the formatting of the next.
+
+    append=True appends to the file instead of creating it, and header=False leaves out the header line, so that a
+    matrix can be written in blocks of output lines.  info: an int64 array of 4, filled with the bytes written, line
+    groups, microseconds of formatting kernels and microseconds waiting for the file writes.  An empty matrix goes
+    through write_text_matrix."""
+    import ctypes as C
+    import torch
+    from . import _lib
+    t = tensor
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or t.dim() != 2:
+        raise ValueError("write_text_matrix_device takes a 2-d float32 CUDA tensor")
+    if t.numel() == 0:
+        if append or not header:
+            raise ValueError("an empty matrix is written whole")
+        write_text_matrix(t.cpu().numpy(), filename, rownames, colnames, transpose)
+        return
+    if t.stride(1) != 1 or t.stride(0) < t.shape[1]:
+        t = t.contiguous()
+    rows, cols = t.shape
+    line_names, head_names = (colnames, rownames) if transpose else (rownames, colnames)
+    out_rows, out_cols = (cols, rows) if transpose else (rows, cols)
+    labels, offsets = label_bytes(line_names, out_rows) if line_names is not None else (None, None)
+    if head_names is not None:
+        names = list(head_names)
+        if len(names) != out_cols:
+            raise ValueError("got %d labels for %d rows/columns" % (len(names), out_cols))
+        head = header_bytes(names, line_names is not None) if header else b""
+    else:
+        head = b""
+    lib = _lib.load()
+    dev = t.device
+    info_arr = np.zeros(4, dtype=np.int64)
+    stream = torch.cuda.current_stream(dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.dca_write_text_device(os.fsencode(filename), int(bool(append)), C.c_void_p(t.data_ptr()), rows, cols,
+                                             t.stride(0), int(bool(transpose)), head, len(head), labels,
+                                             None if offsets is None else offsets.ctypes.data, int(chunk_bytes), dev.index,
+                                             C.c_void_p(stream.cuda_stream), info_arr.ctypes.data),
+                   "dca_write_text_device")
+    if info is not None:
+        info[:] = info_arr
+
+
 def read_pickle(inputfile):
     return pickle.load(open(inputfile, "rb"))
 

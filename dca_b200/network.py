@@ -10,6 +10,7 @@ kernel and run on the shape-general fp32 path of the engine (csrc/extra_types.cu
 """
 from __future__ import annotations
 
+import contextlib
 import os
 import pickle
 from typing import Optional
@@ -18,9 +19,20 @@ import numpy as np
 import torch
 
 from .engine import DeviceEngine
-from .io import write_text_matrix
+from .io import write_text_matrix, write_text_matrix_device
 
 PREDICT_BATCH = 4096      # rows per dca_predict call (Keras predict uses 32; result is identical)
+
+
+def gene_block(n_cells, n_genes, n_heads, free_bytes, max_block_bytes=None):
+    """Genes per block of write_predictions: the device holds n_cells x block float32 per gene-major head, within half
+    of free_bytes (the rest is left to the batch buffers and the text writer) and within max_block_bytes (all heads
+    together) when given; at least one gene, at most n_genes."""
+    budget = free_bytes // 2
+    if max_block_bytes is not None:
+        budget = min(budget, int(max_block_bytes))
+    per_gene = 4 * max(int(n_cells), 1) * max(int(n_heads), 1)
+    return int(max(1, min(int(n_genes), budget // per_gene)))
 
 
 class Autoencoder:
@@ -208,6 +220,47 @@ class Autoencoder:
         """_run_predict with X and the size factors read from a DeviceDataset (device_data.py) of adata's cells.  Each
         batch's outputs go to one of two device buffer sets and are copied to pinned host memory on a side stream, so
         the copy of one batch overlaps the next batch."""
+        eng, N, bs, run, theta, session = self._device_source(adata, dd)
+        with session():
+            return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
+
+    def _run_predict_stream(self, adata, sd, want_mean, want_disp, want_pi, want_latent):
+        """_run_predict with the input batches streamed from a stream_data.StreamedDataset of adata's cells: each batch
+        is copied from the packed host counts and expanded with the exact transform while the previous one runs
+        (dca_stream_predict); the outputs travel to the host as in _run_predict_device."""
+        eng, N, bs, run, theta, session = self._stream_source(adata, sd)
+        with session():
+            return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
+
+    def _run_predict_packed(self, adata, pd, want_mean, want_disp, want_pi, want_latent):
+        """_run_predict with every batch expanded by row index from a packed_data.PackedDeviceDataset of adata's cells
+        (dca_packed_predict); the outputs travel to the host as in _run_predict_device."""
+        eng, N, bs, run, theta, session = self._packed_source(adata, pd)
+        with session():
+            return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
+
+    # -- input sources of the batched inference: (engine, cells, batch rows, run, theta, session).  run(i, s, e, buffers)
+    # is the inference of batch i, rows [s, e), into the device buffers {"mean", "disp", "pi", "latent"} (any subset);
+    # theta(th) writes the per-gene dispersion of the const-disp types; a pass of run over the batches, and theta, go
+    # inside `with session():`.
+    def _host_source(self, adata):
+        X = np.ascontiguousarray(np.asarray(adata.X), dtype=np.float32)
+        eng = self.ensure_engine(max_batch=max(getattr(self, "_max_batch", 32), min(PREDICT_BATCH, X.shape[0])))
+        dev = eng.device
+        sf = np.asarray(adata.obs['size_factors'], dtype=np.float32).reshape(-1)
+
+        def run(i, s, e, b):
+            xd = torch.from_numpy(X[s:e]).to(dev).to(eng.x_dtype)
+            sd = torch.from_numpy(sf[s:e]).to(dev)
+            eng.predict(xd, sd, mean=b.get("mean"), disp=b.get("disp"), pi=b.get("pi"), latent=b.get("latent"))
+
+        def theta(th):
+            xd = torch.from_numpy(X[:1]).to(dev).to(eng.x_dtype)
+            sd = torch.from_numpy(sf[:1]).to(dev)
+            eng.predict(xd, sd, disp=th)
+        return eng, X.shape[0], min(PREDICT_BATCH, eng.max_batch), run, theta, contextlib.nullcontext
+
+    def _device_source(self, adata, dd):
         N = dd.n
         if adata is not None and adata.n_obs != N:
             raise ValueError("device_data covers %d cells, adata has %d" % (N, adata.n_obs))
@@ -224,12 +277,9 @@ class Autoencoder:
 
         def theta(th):
             eng.predict(dd.X, dd.sf, rows=dd.rows[:1], disp=th)
-        return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
+        return eng, N, bs, run, theta, contextlib.nullcontext
 
-    def _run_predict_stream(self, adata, sd, want_mean, want_disp, want_pi, want_latent):
-        """_run_predict with the input batches streamed from a stream_data.StreamedDataset of adata's cells: each batch
-        is copied from the packed host counts and expanded with the exact transform while the previous one runs
-        (dca_stream_predict); the outputs travel to the host as in _run_predict_device."""
+    def _stream_source(self, adata, sd):
         N = sd.n
         if adata is not None and adata.n_obs != N:
             raise ValueError("stream_data covers %d cells, adata has %d" % (N, adata.n_obs))
@@ -241,21 +291,24 @@ class Autoencoder:
             raise ValueError("stream_data has %d genes, the network %d inputs" % (sd.n_genes, eng.n_in))
         bs = min(PREDICT_BATCH, eng.max_batch)
         nb = (N + bs - 1) // bs
-        sd.stream_batches(eng, bs)
-        try:
-            def run(i, s, e, b):
-                eng.stream_predict(i, i + 1 if i + 1 < nb else -1, mean=b.get("mean"), disp=b.get("disp"),
-                                   pi=b.get("pi"), latent=b.get("latent"))
 
-            def theta(th):
-                eng.stream_predict(0, -1, disp=th)
-            return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
-        finally:
-            eng.stream_end()
+        def run(i, s, e, b):
+            eng.stream_predict(i, i + 1 if i + 1 < nb else -1, mean=b.get("mean"), disp=b.get("disp"),
+                               pi=b.get("pi"), latent=b.get("latent"))
 
-    def _run_predict_packed(self, adata, pd, want_mean, want_disp, want_pi, want_latent):
-        """_run_predict with every batch expanded by row index from a packed_data.PackedDeviceDataset of adata's cells
-        (dca_packed_predict); the outputs travel to the host as in _run_predict_device."""
+        def theta(th):
+            eng.stream_predict(0, -1, disp=th)
+
+        @contextlib.contextmanager
+        def session():
+            sd.stream_batches(eng, bs)
+            try:
+                yield
+            finally:
+                eng.stream_end()
+        return eng, N, bs, run, theta, session
+
+    def _packed_source(self, adata, pd):
         N = pd.n
         if adata is not None and adata.n_obs != N:
             raise ValueError("packed_data covers %d cells, adata has %d" % (N, adata.n_obs))
@@ -271,7 +324,7 @@ class Autoencoder:
 
         def theta(th):
             eng.packed_predict(pd, pd.rows[:1], disp=th)
-        return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
+        return eng, N, bs, run, theta, contextlib.nullcontext
 
     def _predict_batches(self, eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta):
         """The outputs of run(i, s, e, buffers) -- the inference of batch i, rows [s, e), into one of two device buffer
@@ -364,6 +417,105 @@ class Autoencoder:
             print('dca: Saving latent representations...')
             write_text_matrix(adata.obsm['X_dca'], os.path.join(file_path, 'latent.tsv'),
                               rownames=rownames, transpose=False)
+
+    def write_predictions(self, file_path, rownames, colnames, mode='full', return_info=True, device_data=None,
+                          stream_data=None, packed_data=None, adata=None, max_block_bytes=None, chunk_bytes=0):
+        """The files predict(adata, mode, return_info, ...) followed by write(adata, file_path, mode, colnames) write,
+        byte for byte and with the same messages, without the cells x genes outputs ever on the host.  rownames: the
+        cell labels (adata.obs_names), colnames: the output gene labels.  The input comes from device_data,
+        stream_data or packed_data as in predict, else from adata (X and obs['size_factors']).
+
+        mean.tsv, dispersion.tsv and dropout.tsv hold one line per gene, so they are written in gene blocks: per block,
+        one inference pass over all cells keeps the block's columns of each of these heads on the device (cells x block
+        float32 each, sized from free device memory and capped by max_block_bytes for all heads together), and
+        io.write_text_matrix_device appends the block's lines to each file.  Every pass runs the same batches as
+        predict, so the values are the ones predict returns; a model whose outputs fit one block is run once.
+        latent.tsv comes from the first pass; the per-gene dispersion of 'nb' / 'zinb' from the same call as in
+        predict, written by write_text_matrix.  The per-cell dispersion and dropout of 'nb-shared' / 'zinb-shared'
+        are not cells x genes: with return_info those models go through predict(adata, ...) and write(...) unchanged,
+        which needs adata.  chunk_bytes: the pinned text pieces of the writer (0: 16 MB)."""
+        assert mode in ('denoise', 'latent', 'full'), 'Unknown mode'
+        info = return_info and isinstance(self, _InfoMixin)
+        if info and self.ae_type in ("nb-shared", "zinb-shared"):
+            if adata is None:
+                raise ValueError("%s writes its per-cell dispersion and dropout through predict and write: give adata"
+                                 % self.ae_type)
+            self.predict(adata, mode=mode, return_info=return_info, device_data=device_data, stream_data=stream_data,
+                         packed_data=packed_data)
+            self.write(adata, file_path, mode=mode, colnames=colnames)
+            return
+        if packed_data is not None:
+            if device_data is not None or stream_data is not None:
+                raise ValueError("give one of device_data, stream_data and packed_data")
+            eng, N, bs, run, theta, session = self._packed_source(adata, packed_data)
+        elif stream_data is not None:
+            if device_data is not None:
+                raise ValueError("give device_data or stream_data, not both")
+            eng, N, bs, run, theta, session = self._stream_source(adata, stream_data)
+        elif device_data is not None:
+            eng, N, bs, run, theta, session = self._device_source(adata, device_data)
+        elif adata is not None:
+            eng, N, bs, run, theta, session = self._host_source(adata)
+        else:
+            raise ValueError("give adata, device_data, stream_data or packed_data")
+        rownames, colnames = list(rownames), list(colnames)
+        G = self.output_size
+        if len(rownames) != N or len(colnames) != G:
+            raise ValueError("got %d row and %d column labels for %d cells and %d output genes"
+                             % (len(rownames), len(colnames), N, G))
+        dev = eng.device
+        cond = self.ae_type not in ("zinb", "nb", "poisson", "normal")
+        want_mean, want_latent = mode in ('denoise', 'full'), mode in ('latent', 'full')
+        want_pi = info and self.has_pi
+        # the heads predict asks the engine for, and the gene-major ones written block by block
+        widths = {}
+        if want_mean: widths["mean"] = G
+        if info and cond: widths["disp"] = G
+        if want_pi: widths["pi"] = G
+        if want_latent: widths["latent"] = eng.latent_dim
+        files = [(k, f) for k, f in (("mean", "mean.tsv"), ("disp", "dispersion.tsv"), ("pi", "dropout.tsv"))
+                 if k in widths]
+        bufs = {k: torch.empty((bs, w), dtype=torch.float32, device=dev) for k, w in widths.items()}
+        free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+        block = gene_block(N, G, len(files), free, max_block_bytes)
+        blk = {k: torch.empty((N, block), dtype=torch.float32, device=dev) for k, _ in files}
+        latent = torch.empty((N, eng.latent_dim), dtype=torch.float32, device=dev) if want_latent else None
+
+        if want_latent:
+            print('dca: Calculating low dimensional representations...')
+        if want_mean:
+            print('dca: Calculating reconstructions...')
+        print('dca: Saving output(s)...')
+        os.makedirs(file_path, exist_ok=True)
+        if want_mean:
+            print('dca: Saving denoised expression...')
+        for b, g0 in enumerate(range(0, G, block) if files else [0]):
+            g1 = min(G, g0 + block)
+            with session():
+                for i, s in enumerate(range(0, N, bs)):
+                    e = min(s + bs, N)
+                    run(i, s, e, bufs)
+                    for k, _ in files:
+                        blk[k][s:e, :g1 - g0].copy_(bufs[k][:e - s, g0:g1])
+                    if latent is not None and b == 0:
+                        latent[s:e].copy_(bufs["latent"][:e - s])
+            for k, f in files:
+                # mean.tsv starts with the header of cell labels; dispersion.tsv and dropout.tsv have none
+                write_text_matrix_device(blk[k][:, :g1 - g0], os.path.join(file_path, f),
+                                         rownames=rownames if (k == "mean" and b == 0) else None,
+                                         colnames=colnames[g0:g1], transpose=True, append=b > 0,
+                                         chunk_bytes=chunk_bytes)
+        del blk, bufs
+        if want_latent:
+            print('dca: Saving latent representations...')
+            write_text_matrix_device(latent, os.path.join(file_path, 'latent.tsv'), rownames=rownames,
+                                     chunk_bytes=chunk_bytes)
+        if info and not cond:
+            th = torch.empty(G, dtype=torch.float32, device=dev)
+            with session():
+                theta(th)
+            write_text_matrix(th.cpu().numpy().reshape(1, -1), os.path.join(file_path, 'dispersion.tsv'),
+                              colnames=colnames, transpose=True)
 
 
 class _InfoMixin:

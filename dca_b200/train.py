@@ -629,6 +629,8 @@ def train_with_args(args):
     else:
         predict_columns = adata.var_names
 
-    net.predict(adata, mode='full', return_info=True, device_data=dd, stream_data=sd, packed_data=pdd)
-    net.write(adata, args.outputdir, mode='full', colnames=predict_columns)
+    # the files of net.predict(adata, mode='full', return_info=True, ...) + net.write(...), written in gene blocks
+    # from the device: host memory holds the labels and the text buffers, never a cells x genes output
+    net.write_predictions(args.outputdir, adata.obs_names.values, predict_columns, mode='full', return_info=True,
+                          device_data=dd, stream_data=sd, packed_data=pdd, adata=adata)
     return losses

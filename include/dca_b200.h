@@ -13,7 +13,7 @@
  *     (parameters, gradients, optimizer state, BatchNorm state, fixed workspace).  No
  *     allocation happens inside step / predict calls.
  *   - all work is enqueued on the caller's stream (a cudaStream_t passed as void*); no
- *     hidden synchronisation except in the *_host entry points and dca_read_*.
+ *     hidden synchronisation except in the *_host entry points, dca_read_* and dca_write_text_device.
  *   - a handle is bound to the device that was current at dca_create and is not thread safe.
  *   - matrices are row-major (cells x genes), leading dimensions in ELEMENTS.
  */
@@ -562,6 +562,27 @@ int dca_engine_info(const dca_handle* h, int32_t info[8]);
 int dca_write_text_matrix(const char* path, const void* matrix, int32_t is_float64, int64_t rows, int64_t cols,
                           int64_t ld, const char* const* row_names, const char* const* col_names,
                           int32_t transpose, int32_t threads);
+
+/* GPU writer of the same bytes (dca_b200/io.py:write_text_matrix_device) from a DEVICE float32 matrix rows x cols,
+ * leading dimension ld (rows, cols >= 1): output line i holds row i, or column i with transpose != 0.  The file is
+ * created (append == 0) or appended to; header_len bytes of `header` are written first as given (the caller quotes the
+ * labels).  label_offsets: NULL for lines without labels, else HOST int64[out_lines + 1] into the HOST bytes `labels`
+ * (already quoted): line i starts with labels[label_offsets[i] .. label_offsets[i + 1]) and a tab.  Values are
+ * printf's '%.6f' of the float32 value (correctly rounded, ties to even, the sign of -0.0 and of negatives that round to
+ * zero kept), NaN an empty field, infinities "inf" / "-inf", all formatted with integer arithmetic on `device`.
+ * Whole lines are formatted in groups on `stream` (a length pass, one fixed-order scan, a write pass), so the bytes
+ * do not depend on scheduling; the text goes to the file in pieces of at most chunk_bytes (0 = 16 MB) through two
+ * pinned buffers, the write of one piece overlapping the formatting and copy of the next by a helper thread that is
+ * joined before the call returns.  info (NULL or int64[4]): bytes written, line groups, microseconds of the
+ * formatting kernels, microseconds spent waiting for the file writes.  Without a CUDA device it returns
+ * DCA_ERR_NO_DEVICE. */
+int dca_write_text_device(const char* path, int32_t append, const float* matrix, int64_t rows, int64_t cols, int64_t ld,
+                          int32_t transpose, const char* header, int64_t header_len, const char* labels,
+                          const int64_t* label_offsets, int64_t chunk_bytes, int32_t device, void* stream,
+                          int64_t* info);
+/* The number formatter of dca_write_text_device run on the CPU, for tests: the '%.6f' text of the float32 bit patterns
+ * bits[0..n) back to back in out (at least 47 * n bytes), that of bits[i] at out[offsets[i] .. offsets[i + 1]). */
+int dca_format_fixed6_host(const uint32_t* bits, int64_t n, char* out, int64_t* offsets);
 
 /* GPU reader of a count table in text form (dca_b200/io.py:read_counts_text): a header line, then one line per gene
  * whose first field is its label and whose other fields are counts, separated by `sep` (',' or '\t').  It gives the
