@@ -64,34 +64,19 @@ def dca(adata, mode='denoise', ae_type='nb-conddisp', normalize_per_cell=True, s
     # raw counts go to adata.raw; the input object is copied only when copy=True  (dca/api.py:156-160)
     adata = read_dataset(adata, transpose=False, test_split=False, copy=copy, check_counts=check_counts)
 
-    dd = sd = pd_ = None
+    ds = None
     x_dtype = network_kwds.get('x_dtype', 'float32')
-    if streamed == 'auto':
-        from .device_data import DeviceDataset
-        dev = torch.device('cuda', torch.cuda.current_device())
-        streamed = DeviceDataset.device_bytes(adata.X, x_dtype, normalize_per_cell) > torch.cuda.mem_get_info(dev)[0]
-    if streamed:
-        from .stream_data import StreamedDataset
-        from .io import apply_device_normalize
-        sd = StreamedDataset.from_counts(adata.X, None, x_dtype, size_factors=normalize_per_cell, logtrans_input=log1p,
-                                         normalize_input=scale, batch=batch_size)
-        assert (sd.input_gene_totals >= 1).all(), 'Please remove all-zero genes before using DCA.'
-        apply_device_normalize(adata, sd, filter_min_counts=False, set_x=False)
-    elif packed:
-        from .packed_data import PackedDeviceDataset
-        from .io import apply_device_normalize
-        pd_ = PackedDeviceDataset.from_counts(adata.X, None, x_dtype, size_factors=normalize_per_cell,
-                                              logtrans_input=log1p, normalize_input=scale)
-        assert (pd_.input_gene_totals >= 1).all(), 'Please remove all-zero genes before using DCA.'
-        apply_device_normalize(adata, pd_, filter_min_counts=False, set_x=False)
-    elif preprocess == 'device':
+    if preprocess == 'device':
         # the same steps on the device; adata.X keeps the raw counts until predict() overwrites it
-        from .device_data import DeviceDataset
+        from .device_data import DeviceDataset, build_dataset
         from .io import apply_device_normalize
-        dd = DeviceDataset.from_counts(adata.X, None, network_kwds.get('x_dtype', 'float32'),
-                                       size_factors=normalize_per_cell, logtrans_input=log1p, normalize_input=scale)
-        assert (dd.input_gene_totals >= 1).all(), 'Please remove all-zero genes before using DCA.'
-        apply_device_normalize(adata, dd, filter_min_counts=False, set_x=False)
+        if streamed == 'auto':
+            dev = torch.device('cuda', torch.cuda.current_device())
+            streamed = DeviceDataset.device_bytes(adata.X, x_dtype, normalize_per_cell) > torch.cuda.mem_get_info(dev)[0]
+        ds = build_dataset(adata.X, None, x_dtype, stream=streamed, packed=packed, batch=batch_size,
+                           size_factors=normalize_per_cell, logtrans_input=log1p, normalize_input=scale)
+        assert (ds.input_gene_totals >= 1).all(), 'Please remove all-zero genes before using DCA.'
+        apply_device_normalize(adata, ds, filter_min_counts=False, set_x=False)
     else:
         # all-zero genes are an error, as in the reference                    (dca/api.py:163-164)
         nonzero_genes, _ = filter_genes_mask(adata.X, min_counts=1)
@@ -109,22 +94,14 @@ def dca(adata, mode='denoise', ae_type='nb-conddisp', normalize_per_cell=True, s
 
     fit_args = dict(training_kwds, epochs=epochs, reduce_lr=reduce_lr, early_stop=early_stop, batch_size=batch_size,
                     optimizer=optimizer, verbose=verbose, threads=threads, learning_rate=learning_rate)
-    if sd is not None:
-        train_mask = np.asarray(adata.obs.dca_split == 'train')
-        hist = train(None, net, stream_data=sd.take(train_mask), **fit_args)
-        res = net.predict(adata, mode, return_info, copy, stream_data=sd)
-    elif pd_ is not None:
-        train_mask = np.asarray(adata.obs.dca_split == 'train')
-        hist = train(None, net, packed_data=pd_.take(train_mask), **fit_args)
-        res = net.predict(adata, mode, return_info, copy, packed_data=pd_)
-    elif dd is None:
+    if ds is None:
         hist = train(adata[adata.obs.dca_split == 'train'], net, **fit_args)
         res = net.predict(adata, mode, return_info, copy)
     else:
         train_mask = np.asarray(adata.obs.dca_split == 'train')
         # no AnnData subset: train() reads everything from the dataset, and a subset would copy the raw counts
-        hist = train(None, net, device_data=dd.take(train_mask), **fit_args)
-        res = net.predict(adata, mode, return_info, copy, device_data=dd)
+        hist = train(None, net, **{ds.kind: ds.take(train_mask)}, **fit_args)
+        res = net.predict(adata, mode, return_info, copy, **{ds.kind: ds})
     adata = res if copy else adata
 
     if return_info:

@@ -11,6 +11,7 @@ ulp).
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 
 import numpy as np
@@ -60,28 +61,154 @@ def _is_csr(counts):
     return hasattr(counts, "tocsr") and getattr(counts, "format", None) == "csr"
 
 
-class DeviceDataset:
+def _device(device):
+    """The CUDA device a dataset is built on (None or an index-less 'cuda': the current one)."""
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    return torch.device("cuda", torch.cuda.current_device()) if dev.index is None else dev
+
+
+_X_DTYPES = {"float32": torch.float32, "bfloat16": torch.bfloat16, torch.float32: torch.float32,
+             torch.bfloat16: torch.bfloat16}
+
+
+def _counts_matrix(counts):
+    """counts as a scipy CSR matrix or a dense ndarray, checked to be a non-empty cells x genes matrix."""
+    if not _is_csr(counts):
+        counts = np.asarray(counts.toarray() if hasattr(counts, "toarray") else counts)
+    if counts.ndim != 2 or counts.shape[0] < 1 or counts.shape[1] < 1:
+        raise ValueError("counts must be a non-empty cells x genes matrix")
+    if counts.shape[0] >= 2 ** 31:
+        raise ValueError("at most 2**31 - 1 cells")
+    return counts
+
+
+def _size_factors(nc, size_factors):
+    """(median, fp32 size factors) of the row totals nc: n_counts / median, or (1, ones) without size factors."""
+    if not size_factors:
+        return 1.0, np.ones(nc.shape[0], np.float32)
+    med = float(np.median(nc))
+    return med, (nc / med).astype(np.float32)
+
+
+def build_dataset(counts, device=None, x_dtype="float32", stream=False, packed=False, batch=32, **flags):
+    """The dataset of the device preprocessing of ``counts`` with the flags of io.normalize (``flags``): resident
+    (DeviceDataset), out of core from packed host counts (stream: stream_data.StreamedDataset, packed for a training
+    batch of ``batch`` rows) or packed in device memory (packed: packed_data.PackedDeviceDataset)."""
+    if packed:
+        from .packed_data import PackedDeviceDataset
+        return PackedDeviceDataset.from_counts(counts, device, x_dtype, **flags)
+    if stream:
+        from .stream_data import StreamedDataset
+        return StreamedDataset.from_counts(counts, device, x_dtype, batch=batch, **flags)
+    return DeviceDataset.from_counts(counts, device, x_dtype, **flags)
+
+
+def _one_dataset(device_data=None, stream_data=None, packed_data=None, stream=False):
+    """The dataset given to train / predict / write_predictions through its keyword, or None (input from the AnnData).
+    stream: train()'s host-streaming switch, which only a StreamedDataset goes with."""
+    given = [d for d in (device_data, stream_data, packed_data) if d is not None]
+    if packed_data is not None and (len(given) > 1 or stream):
+        raise ValueError("packed_data is resident in HBM: it cannot be combined with stream, device_data or "
+                         "stream_data")
+    if len(given) > 1:
+        raise ValueError("give device_data or stream_data, not both")
+    if device_data is not None and stream:
+        raise ValueError("device_data is resident in HBM: it cannot be combined with stream=True")
+    return given[0] if given else None
+
+
+def _resident_fit(eng, n_tr, n, batch, shuffle, step, evaluate, rows_map=None):
+    """(epoch, validate) over n cells of which the first n_tr train: every epoch reshuffles the training rows with the
+    global NumPy RNG as Keras does (np.random.shuffle of the index array) and runs step(rows) on each batch, rows an
+    int32 device tensor of storage rows (positions mapped through rows_map when given); validate runs evaluate(s, e)
+    over the held-out positions [n_tr, n) in batches."""
+    def epoch(update):
+        order = np.arange(n_tr)
+        if shuffle:
+            np.random.shuffle(order)
+        order_d = torch.from_numpy(order.astype(np.int32)).to(eng.device)
+        if rows_map is not None:
+            order_d = rows_map[order_d.long()]
+        for s in range(0, n_tr, batch):
+            step(order_d[s:s + batch])
+            update()
+
+    def validate():
+        for s in range(n_tr, n, batch):             # inference-mode BN over the held-out tail
+            evaluate(s, min(s + batch, n))
+    return epoch, validate
+
+
+class _Dataset:
+    """What train() and predict() know of a dataset kind, the same on DeviceDataset, stream_data.StreamedDataset and
+    packed_data.PackedDeviceDataset:
+      ``kind``: the keyword of train / predict / write_predictions that takes it and the suffix of its adata.uns key;
+      ``_bind(eng)``: its checks against the engine and, where the kind needs it, the exact input transform;
+      ``_fit(eng, n_tr, batch, shuffle)`` -> (epoch, validate): epoch(update) runs one epoch's training steps over the
+      first n_tr cells, calling update() after each, and validate() the validation pass over the others;
+      ``_predictor(eng, bs)`` -> (run, theta, session): run(i, s, e, buffers) is the inference of batch i, cells
+      [s, e), into the device buffers {"mean", "disp", "pi", "latent"} (any subset); theta(th) writes the per-gene
+      dispersion of the const-disp types; a pass of run over the batches, and theta, go inside ``with session():``."""
+    kind = None
+    _on = "lives on"
+
+    # the buffers are never written after from_counts: copies of an AnnData share them instead of duplicating memory
+    def __copy__(self):
+        return self
+
+    def __deepcopy__(self, memo):
+        return self
+
+    def _positions(self, mask_or_index):
+        """int64 positions in [0, n) of the cells ``mask_or_index`` selects (a boolean mask over this dataset's cells
+        or integer positions, negative ones counting from the end), in that order."""
+        idx = np.asarray(mask_or_index)
+        if idx.dtype == bool:
+            if idx.shape != (self.n,):
+                raise ValueError("a mask must have one entry per cell (%d), got shape %s" % (self.n, idx.shape))
+            idx = np.flatnonzero(idx)
+        idx = idx.astype(np.int64).reshape(-1)
+        if idx.size and (idx.min() < -self.n or idx.max() >= self.n):
+            raise IndexError("cell index out of range for %d cells" % self.n)
+        return idx % max(self.n, 1)
+
+    def _cover(self, adata):
+        if adata is not None and adata.n_obs != self.n:
+            raise ValueError("%s covers %d cells, adata has %d" % (self.kind, self.n, adata.n_obs))
+
+    def _check_genes(self, eng):
+        if eng.n_in != self.n_genes or eng.n_out != self.n_genes:
+            raise ValueError("%s has %d genes, the network %d inputs and %d outputs"
+                             % (self.kind, self.n_genes, eng.n_in, eng.n_out))
+
+    def _bind(self, eng):
+        if self.device != eng.device:
+            raise ValueError("%s %s %s, the network on %s" % (self.kind, self._on, self.device, eng.device))
+        if self.x_dtype != eng.x_dtype:
+            raise ValueError("%s X is %s, the network expects %s (network_kwds x_dtype)"
+                             % (self.kind, self.x_dtype, eng.x_dtype))
+
+    def host_size_factors(self) -> np.ndarray:
+        return self.size_factors_host
+
+
+class DeviceDataset(_Dataset):
     """Resident Y (fp32 raw counts), X (fp32 or bf16 normalised input), sf (fp32 size factors), n_counts, gene mean /
     std (fp64) and ``rows``, the int32 storage rows of the cells this dataset covers, in order.  ``take`` makes a
     dataset over a subset of them without copying a matrix.  ``y_cols`` names the input genes Y holds when it holds a
-    subset of them (``with_output_genes``), otherwise None.
+    subset of them (``with_output_genes``), otherwise None.  Training and prediction gather their batches through
+    ``rows`` (the interface of _Dataset, keyword ``device_data``).
 
     Host copies of the per-cell and per-gene results (``n_counts_host``, ``size_factors_host``, ``gene_totals_host``)
     and the masks of the filtering steps (``gene_mask``, ``cell_mask``, ``sf_mask``) are what ``io.normalize`` needs to
     mutate an AnnData the way the host path does."""
+    kind = "device_data"
 
     def __init__(self, Y, X, sf, n_counts, mean, std, rows, y_cols=None):
         self.Y, self.X, self.sf, self.n_counts, self.mean, self.std = Y, X, sf, n_counts, mean, std
         self.rows = rows
         self.y_cols = y_cols
         self.device = X.device
-
-    # the buffers are never written after from_counts: copies of an AnnData share them instead of duplicating HBM
-    def __copy__(self):
-        return self
-
-    def __deepcopy__(self, memo):
-        return self
 
     @property
     def n(self) -> int:
@@ -104,21 +231,10 @@ class DeviceDataset:
         lib = _lib.load()
         if not torch.cuda.is_available():
             raise _lib.DcaError("DeviceDataset needs a CUDA device (H100); there is no CPU fallback")
-        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        if dev.index is None:
-            dev = torch.device("cuda", torch.cuda.current_device())
-        xdt = {"float32": torch.float32, "bfloat16": torch.bfloat16, torch.float32: torch.float32,
-               torch.bfloat16: torch.bfloat16}[x_dtype]
+        dev, xdt = _device(device), _X_DTYPES[x_dtype]
+        counts = _counts_matrix(counts)
         csr = _is_csr(counts)
-        if not csr and hasattr(counts, "toarray"):
-            counts = counts.toarray()
-        if not csr:
-            counts = np.asarray(counts)
-        if counts.ndim != 2 or counts.shape[0] < 1 or counts.shape[1] < 1:
-            raise ValueError("counts must be a non-empty cells x genes matrix")
         N, G = (int(s) for s in counts.shape)
-        if N >= 2 ** 31:
-            raise ValueError("at most 2**31 - 1 cells")
         ws_bytes = C.c_size_t()
         check(lib.dca_preprocess_workspace_bytes(N, G, C.byref(ws_bytes)), "dca_preprocess_workspace_bytes")
         need = cls.device_bytes(counts, xdt, size_factors, filter_min_counts)
@@ -140,8 +256,7 @@ class DeviceDataset:
     @staticmethod
     def device_bytes(counts, x_dtype="float32", size_factors=True, filter_min_counts=False) -> int:
         """Device memory from_counts needs for ``counts`` (cells x genes, dense or scipy CSR) with these flags."""
-        xdt = {"float32": torch.float32, "bfloat16": torch.bfloat16, torch.float32: torch.float32,
-               torch.bfloat16: torch.bfloat16}[x_dtype]
+        xdt = _X_DTYPES[x_dtype]
         N, G = (int(s) for s in counts.shape)
         ws_bytes = C.c_size_t()
         check(_lib.load().dca_preprocess_workspace_bytes(N, G, C.byref(ws_bytes)), "dca_preprocess_workspace_bytes")
@@ -176,11 +291,7 @@ class DeviceDataset:
                 Y = _gather(lib, Y, np.flatnonzero(sf_mask), None, dev)
                 n_counts, gene_tot, _ = _totals(lib, Y, ws, dev)
                 nc = n_counts.cpu().numpy()
-            med = float(np.median(nc))
-            sf_h = (nc / med).astype(np.float32)
-        else:
-            med = 1.0
-            sf_h = np.ones(nc.shape[0], np.float32)
+        med, sf_h = _size_factors(nc, size_factors)
         N, G = Y.shape
         flags = preprocess_flags(size_factors, logtrans_input, normalize_input)
         s = _stream(dev)
@@ -214,15 +325,7 @@ class DeviceDataset:
     def take(self, mask_or_index):
         """The cells ``mask_or_index`` (a boolean mask over this dataset's cells or integer positions) selects, in
         that order: only ``rows`` is composed, the matrices are shared."""
-        idx = np.asarray(mask_or_index)
-        if idx.dtype == bool:
-            if idx.shape != (self.n,):
-                raise ValueError("a mask must have one entry per cell (%d), got shape %s" % (self.n, idx.shape))
-            idx = np.flatnonzero(idx)
-        idx = idx.astype(np.int64).reshape(-1)
-        if idx.size and (idx.min() < -self.n or idx.max() >= self.n):
-            raise IndexError("cell index out of range for %d cells" % self.n)
-        sel = torch.from_numpy(idx % max(self.n, 1)).to(self.device)
+        sel = torch.from_numpy(self._positions(mask_or_index)).to(self.device)
         return self._derive(rows=self.rows[sel].contiguous())
 
     def with_output_genes(self, cols):
@@ -242,6 +345,21 @@ class DeviceDataset:
 
     def host_size_factors(self) -> np.ndarray:
         return self.sf[self.rows.long()].cpu().numpy()
+
+    # ------------------------------------------------------------------ training and prediction
+    def _fit(self, eng, n_tr, batch, shuffle):
+        return _resident_fit(eng, n_tr, self.n, batch, shuffle,
+                             lambda rows: eng.train_step(self.X, self.Y, self.sf, rows=rows),
+                             lambda s, e: eng.eval_step(self.X, self.Y, self.sf, rows=self.rows[s:e]), self.rows)
+
+    def _predictor(self, eng, bs):
+        def run(i, s, e, b):
+            eng.predict(self.X, self.sf, rows=self.rows[s:e], mean=b.get("mean"), disp=b.get("disp"), pi=b.get("pi"),
+                        latent=b.get("latent"))
+
+        def theta(th):
+            eng.predict(self.X, self.sf, rows=self.rows[:1], disp=th)
+        return run, theta, contextlib.nullcontext
 
 
 # ---------------------------------------------------------------------- helpers

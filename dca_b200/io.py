@@ -324,34 +324,17 @@ def normalize(adata, filter_min_counts=True, size_factors=True, normalize_input=
     packed=True (with a device): the raw counts are packed on the device and stay there, packed
     (packed_data.PackedDeviceDataset, same flags): adata.X keeps the (filtered) raw counts and the dataset is returned in
     adata.uns['dca_packed_data'] for train(packed_data=...) and predict(packed_data=...)."""
-    if packed:
+    if device is not None or stream or packed:
         if device is None:
-            raise ValueError("packed=True preprocesses on a device: give device=")
-        if stream:
+            raise ValueError("%s=True preprocesses on a device: give device=" % ("packed" if packed else "stream"))
+        if stream and packed:
             raise ValueError("give stream=True or packed=True, not both")
-        from .packed_data import PackedDeviceDataset
-        pd_ = PackedDeviceDataset.from_counts(adata.X, device, "float32", size_factors=size_factors,
-                                              logtrans_input=logtrans_input, normalize_input=normalize_input,
-                                              filter_min_counts=filter_min_counts)
-        apply_device_normalize(adata, pd_, filter_min_counts, set_x=False)
-        adata.uns['dca_packed_data'] = pd_
-        return adata
-    if stream:
-        if device is None:
-            raise ValueError("stream=True preprocesses on a device: give device=")
-        from .stream_data import StreamedDataset
-        sd = StreamedDataset.from_counts(adata.X, device, "float32", size_factors=size_factors,
-                                         logtrans_input=logtrans_input, normalize_input=normalize_input,
-                                         filter_min_counts=filter_min_counts)
-        apply_device_normalize(adata, sd, filter_min_counts, set_x=False)
-        adata.uns['dca_stream_data'] = sd
-        return adata
-    if device is not None:
-        from .device_data import DeviceDataset
-        dd = DeviceDataset.from_counts(adata.X, device, "float32", size_factors=size_factors, logtrans_input=logtrans_input,
-                                       normalize_input=normalize_input, filter_min_counts=filter_min_counts)
-        apply_device_normalize(adata, dd, filter_min_counts)
-        adata.uns['dca_device_data'] = dd
+        from .device_data import build_dataset
+        ds = build_dataset(adata.X, device, "float32", stream=stream, packed=packed, size_factors=size_factors,
+                           logtrans_input=logtrans_input, normalize_input=normalize_input,
+                           filter_min_counts=filter_min_counts)
+        apply_device_normalize(adata, ds, filter_min_counts, set_x=not (stream or packed))
+        adata.uns['dca_' + ds.kind] = ds
         return adata
     if filter_min_counts:
         gmask, _ = filter_genes_mask(adata.X, 1)                       # dca/io.py:90-92

@@ -18,6 +18,7 @@ from typing import Optional
 import numpy as np
 import torch
 
+from .device_data import _one_dataset
 from .engine import DeviceEngine
 from .io import write_text_matrix, write_text_matrix_device
 
@@ -172,77 +173,23 @@ class Autoencoder:
         # a model without a dropout head has no pi: the engine writes nothing there, so none is returned (not the
         # uninitialised contents of the output buffer)
         want_pi = want_pi and self.has_pi
-        if packed_data is not None:
-            if device_data is not None or stream_data is not None:
-                raise ValueError("give one of device_data, stream_data and packed_data")
-            return self._run_predict_packed(adata, packed_data, want_mean, want_disp, want_pi, want_latent)
-        if stream_data is not None:
-            if device_data is not None:
-                raise ValueError("give device_data or stream_data, not both")
-            return self._run_predict_stream(adata, stream_data, want_mean, want_disp, want_pi, want_latent)
-        if device_data is not None:
-            return self._run_predict_device(adata, device_data, want_mean, want_disp, want_pi, want_latent)
-        X = np.ascontiguousarray(np.asarray(adata.X), dtype=np.float32)
-        eng = self.ensure_engine(max_batch=max(getattr(self, "_max_batch", 32), min(PREDICT_BATCH, X.shape[0])))
-        dev = eng.device
-        sf = np.asarray(adata.obs['size_factors'], dtype=np.float32).reshape(-1)
-        N, G = X.shape[0], self.output_size
+        eng, N, bs, run, theta, session = self._source(adata, _one_dataset(device_data, stream_data, packed_data))
+        with session():
+            return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
+
+    # -- the input of the batched inference: (engine, cells, batch rows, run, theta, session) as
+    # device_data._Dataset._predictor describes them, from a dataset or else from adata (X and obs['size_factors'])
+    def _source(self, adata, data):
+        if data is None:
+            if adata is None:
+                raise ValueError("give adata, device_data, stream_data or packed_data")
+            return self._host_source(adata)
+        data._cover(adata)
+        eng = self.ensure_engine(max_batch=max(getattr(self, "_max_batch", 32), min(PREDICT_BATCH, data.n)))
+        data._bind(eng)
         bs = min(PREDICT_BATCH, eng.max_batch)
-        cond = self.ae_type not in ("zinb", "nb", "poisson", "normal")     # a dispersion head (vs per-gene theta / none)
-        Gs = 1 if self.ae_type in ("nb-shared", "zinb-shared") else G       # per-cell heads: Dense(1)
-        out = {}
-        if want_mean: out["mean"] = np.empty((N, G), np.float32)
-        if want_disp: out["dispersion"] = np.empty((N, Gs), np.float32) if cond else None
-        if want_pi: out["pi"] = np.empty((N, Gs), np.float32)
-        if want_latent: out["latent"] = np.empty((N, eng.latent_dim), np.float32)
-        mean_d = torch.empty((bs, G), dtype=torch.float32, device=dev) if want_mean else None
-        disp_d = torch.empty((bs, Gs), dtype=torch.float32, device=dev) if (want_disp and cond) else None
-        pi_d = torch.empty((bs, Gs), dtype=torch.float32, device=dev) if want_pi else None
-        lat_d = torch.empty((bs, eng.latent_dim), dtype=torch.float32, device=dev) if want_latent else None
-        for s in range(0, N, bs):
-            e = min(s + bs, N)
-            xd = torch.from_numpy(X[s:e]).to(dev).to(eng.x_dtype)
-            sd = torch.from_numpy(sf[s:e]).to(dev)
-            eng.predict(xd, sd, mean=mean_d, disp=disp_d, pi=pi_d, latent=lat_d)
-            if want_mean: out["mean"][s:e] = mean_d[: e - s].cpu().numpy()
-            if disp_d is not None: out["dispersion"][s:e] = disp_d[: e - s].cpu().numpy()
-            if want_pi: out["pi"][s:e] = pi_d[: e - s].cpu().numpy()
-            if want_latent: out["latent"][s:e] = lat_d[: e - s].cpu().numpy()
-        if want_disp and not cond:
-            th = torch.empty(G, dtype=torch.float32, device=dev)
-            xd = torch.from_numpy(X[:1]).to(dev).to(eng.x_dtype)
-            sd = torch.from_numpy(sf[:1]).to(dev)
-            eng.predict(xd, sd, disp=th)
-            out["dispersion"] = th.cpu().numpy()
-        return out
+        return (eng, data.n, bs) + data._predictor(eng, bs)
 
-    def _run_predict_device(self, adata, dd, want_mean, want_disp, want_pi, want_latent):
-        """_run_predict with X and the size factors read from a DeviceDataset (device_data.py) of adata's cells.  Each
-        batch's outputs go to one of two device buffer sets and are copied to pinned host memory on a side stream, so
-        the copy of one batch overlaps the next batch."""
-        eng, N, bs, run, theta, session = self._device_source(adata, dd)
-        with session():
-            return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
-
-    def _run_predict_stream(self, adata, sd, want_mean, want_disp, want_pi, want_latent):
-        """_run_predict with the input batches streamed from a stream_data.StreamedDataset of adata's cells: each batch
-        is copied from the packed host counts and expanded with the exact transform while the previous one runs
-        (dca_stream_predict); the outputs travel to the host as in _run_predict_device."""
-        eng, N, bs, run, theta, session = self._stream_source(adata, sd)
-        with session():
-            return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
-
-    def _run_predict_packed(self, adata, pd, want_mean, want_disp, want_pi, want_latent):
-        """_run_predict with every batch expanded by row index from a packed_data.PackedDeviceDataset of adata's cells
-        (dca_packed_predict); the outputs travel to the host as in _run_predict_device."""
-        eng, N, bs, run, theta, session = self._packed_source(adata, pd)
-        with session():
-            return self._predict_batches(eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta)
-
-    # -- input sources of the batched inference: (engine, cells, batch rows, run, theta, session).  run(i, s, e, buffers)
-    # is the inference of batch i, rows [s, e), into the device buffers {"mean", "disp", "pi", "latent"} (any subset);
-    # theta(th) writes the per-gene dispersion of the const-disp types; a pass of run over the batches, and theta, go
-    # inside `with session():`.
     def _host_source(self, adata):
         X = np.ascontiguousarray(np.asarray(adata.X), dtype=np.float32)
         eng = self.ensure_engine(max_batch=max(getattr(self, "_max_batch", 32), min(PREDICT_BATCH, X.shape[0])))
@@ -259,72 +206,6 @@ class Autoencoder:
             sd = torch.from_numpy(sf[:1]).to(dev)
             eng.predict(xd, sd, disp=th)
         return eng, X.shape[0], min(PREDICT_BATCH, eng.max_batch), run, theta, contextlib.nullcontext
-
-    def _device_source(self, adata, dd):
-        N = dd.n
-        if adata is not None and adata.n_obs != N:
-            raise ValueError("device_data covers %d cells, adata has %d" % (N, adata.n_obs))
-        eng = self.ensure_engine(max_batch=max(getattr(self, "_max_batch", 32), min(PREDICT_BATCH, N)))
-        dev = eng.device
-        if dd.X.device != dev or dd.x_dtype != eng.x_dtype:
-            raise ValueError("device_data X is %s on %s, the network expects %s on %s"
-                             % (dd.x_dtype, dd.X.device, eng.x_dtype, dev))
-        bs = min(PREDICT_BATCH, eng.max_batch)
-
-        def run(i, s, e, b):
-            eng.predict(dd.X, dd.sf, rows=dd.rows[s:e], mean=b.get("mean"), disp=b.get("disp"), pi=b.get("pi"),
-                        latent=b.get("latent"))
-
-        def theta(th):
-            eng.predict(dd.X, dd.sf, rows=dd.rows[:1], disp=th)
-        return eng, N, bs, run, theta, contextlib.nullcontext
-
-    def _stream_source(self, adata, sd):
-        N = sd.n
-        if adata is not None and adata.n_obs != N:
-            raise ValueError("stream_data covers %d cells, adata has %d" % (N, adata.n_obs))
-        eng = self.ensure_engine(max_batch=max(getattr(self, "_max_batch", 32), min(PREDICT_BATCH, N)))
-        dev = eng.device
-        if sd.device != dev or sd.x_dtype != eng.x_dtype:
-            raise ValueError("stream_data X is %s for %s, the network expects %s on %s" % (sd.x_dtype, sd.device, eng.x_dtype, dev))
-        if eng.n_in != sd.n_genes:
-            raise ValueError("stream_data has %d genes, the network %d inputs" % (sd.n_genes, eng.n_in))
-        bs = min(PREDICT_BATCH, eng.max_batch)
-        nb = (N + bs - 1) // bs
-
-        def run(i, s, e, b):
-            eng.stream_predict(i, i + 1 if i + 1 < nb else -1, mean=b.get("mean"), disp=b.get("disp"),
-                               pi=b.get("pi"), latent=b.get("latent"))
-
-        def theta(th):
-            eng.stream_predict(0, -1, disp=th)
-
-        @contextlib.contextmanager
-        def session():
-            sd.stream_batches(eng, bs)
-            try:
-                yield
-            finally:
-                eng.stream_end()
-        return eng, N, bs, run, theta, session
-
-    def _packed_source(self, adata, pd):
-        N = pd.n
-        if adata is not None and adata.n_obs != N:
-            raise ValueError("packed_data covers %d cells, adata has %d" % (N, adata.n_obs))
-        eng = self.ensure_engine(max_batch=max(getattr(self, "_max_batch", 32), min(PREDICT_BATCH, N)))
-        if eng.n_in != pd.n_genes:
-            raise ValueError("packed_data has %d genes, the network %d inputs" % (pd.n_genes, eng.n_in))
-        bs = min(PREDICT_BATCH, eng.max_batch)
-        eng.set_input_transform_exact(pd.mean, pd.std, pd.median, pd.flags)
-
-        def run(i, s, e, b):
-            eng.packed_predict(pd, pd.rows[s:e], mean=b.get("mean"), disp=b.get("disp"), pi=b.get("pi"),
-                               latent=b.get("latent"))
-
-        def theta(th):
-            eng.packed_predict(pd, pd.rows[:1], disp=th)
-        return eng, N, bs, run, theta, contextlib.nullcontext
 
     def _predict_batches(self, eng, N, bs, want_mean, want_disp, want_pi, want_latent, run, theta):
         """The outputs of run(i, s, e, buffers) -- the inference of batch i, rows [s, e), into one of two device buffer
@@ -444,20 +325,7 @@ class Autoencoder:
                          packed_data=packed_data)
             self.write(adata, file_path, mode=mode, colnames=colnames)
             return
-        if packed_data is not None:
-            if device_data is not None or stream_data is not None:
-                raise ValueError("give one of device_data, stream_data and packed_data")
-            eng, N, bs, run, theta, session = self._packed_source(adata, packed_data)
-        elif stream_data is not None:
-            if device_data is not None:
-                raise ValueError("give device_data or stream_data, not both")
-            eng, N, bs, run, theta, session = self._stream_source(adata, stream_data)
-        elif device_data is not None:
-            eng, N, bs, run, theta, session = self._device_source(adata, device_data)
-        elif adata is not None:
-            eng, N, bs, run, theta, session = self._host_source(adata)
-        else:
-            raise ValueError("give adata, device_data, stream_data or packed_data")
+        eng, N, bs, run, theta, session = self._source(adata, _one_dataset(device_data, stream_data, packed_data))
         rownames, colnames = list(rownames), list(colnames)
         G = self.output_size
         if len(rownames) != N or len(colnames) != G:

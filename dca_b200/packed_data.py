@@ -15,6 +15,7 @@ filtering) a multiple of 8 (the packed format).
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 from types import SimpleNamespace
 
@@ -24,10 +25,10 @@ import torch
 from . import _lib
 from . import io as dio
 from ._lib import check
-from .device_data import _is_csr, preprocess_flags
-from .stream_data import _chunk_rows, _moments, _stream, _totals
+from .device_data import (_counts_matrix, _Dataset, _device, _is_csr, _resident_fit, _size_factors, _stream, _X_DTYPES,
+                          preprocess_flags)
+from .stream_data import _chunk_rows, _moments, _totals
 
-_XDT = {"float32": torch.float32, "bfloat16": torch.bfloat16, torch.float32: torch.float32, torch.bfloat16: torch.bfloat16}
 _ESC_ROW = {1: 1, 4: 1, 8: 2, 16: 3}           # row of the count-pass statistics holding a width's overflow entries
 
 
@@ -81,21 +82,17 @@ class _HostChunks:
                                                   self.G, _stream(self.dev)), "dca_counts_csr_to_dense")
 
 
-class PackedDeviceDataset:
+class PackedDeviceDataset(_Dataset):
     """Raw counts packed in device memory (``packed``, ``ovf_indptr``, ``entries`` and, in the sparse format (bits 1),
     ``nib_indptr`` and ``nibbles``: the arrays of io.PackedCounts with absolute offsets), their fp64 row totals
     ``n_counts`` and ``rows``, the int32 storage rows of the cells this dataset covers, in order (``take`` composes it,
     as DeviceDataset.take does).  The statistics and masks are those of StreamedDataset (``n_counts_host``,
     ``size_factors_host``, ``mean``, ``std``, ``median``, ``flags``, ``gene_mask``, ``cell_mask``, ``sf_mask``,
     ``gene_totals_host``, ``input_gene_totals``, ``n_bad``), so io.apply_device_normalize(adata, pd, ..., set_x=False)
-    mutates an AnnData the same way."""
-
-    # the arrays are never written after from_counts: copies of an AnnData share them instead of duplicating HBM
-    def __copy__(self):
-        return self
-
-    def __deepcopy__(self, memo):
-        return self
+    mutates an AnnData the same way.  Training, validation and prediction expand every batch from the packed arrays by
+    row index with the exact transform (the interface of device_data._Dataset, keyword ``packed_data``); training
+    reshuffles the rows every epoch as DeviceDataset does."""
+    kind = "packed_data"
 
     @property
     def n(self) -> int:
@@ -115,17 +112,9 @@ class PackedDeviceDataset:
         lib = _lib.load()
         if not torch.cuda.is_available():
             raise _lib.DcaError("PackedDeviceDataset needs a CUDA device (H100); there is no CPU fallback")
-        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        if dev.index is None:
-            dev = torch.device("cuda", torch.cuda.current_device())
-        xdt = _XDT[x_dtype]
-        if not _is_csr(counts):
-            counts = np.asarray(counts.toarray() if hasattr(counts, "toarray") else counts)
-        if counts.ndim != 2 or counts.shape[0] < 1 or counts.shape[1] < 1:
-            raise ValueError("counts must be a non-empty cells x genes matrix")
+        dev, xdt = _device(device), _X_DTYPES[x_dtype]
+        counts = _counts_matrix(counts)
         N0, G0 = (int(s) for s in counts.shape)
-        if N0 >= 2 ** 31:
-            raise ValueError("at most 2**31 - 1 cells")
         if G0 % 8 != 0:
             raise ValueError("the packed format needs a gene count that is a multiple of 8 (got %d)" % G0)
         choose_format(0, np.zeros((3, 0), np.int64), 0, G0, bits)          # reject a bad `bits` before any work
@@ -169,12 +158,7 @@ class PackedDeviceDataset:
             filtered = N != N0 or G != G0
             if filtered:
                 nc, gene_tot, _ = _totals(SimpleNamespace(n_rows=N, n_genes=G), dev, chunk_rows, pd._chunks)
-            if size_factors:
-                med = float(np.median(nc))
-                sf_h = (nc / med).astype(np.float32)
-            else:
-                med = 1.0
-                sf_h = np.ones(N, np.float32)
+            med, sf_h = _size_factors(nc, size_factors)
             flags = preprocess_flags(size_factors, logtrans_input, normalize_input)
             pd.n_counts = torch.from_numpy(np.ascontiguousarray(nc, dtype=np.float64)).to(dev)
             pd.desc.n_counts = pd.n_counts.data_ptr()
@@ -256,15 +240,7 @@ class PackedDeviceDataset:
     def take(self, mask_or_index):
         """The cells ``mask_or_index`` (a boolean mask over this dataset's cells or integer positions) selects, in
         that order: only ``rows`` (and the host per-cell arrays) are composed, no packed byte is copied."""
-        idx = np.asarray(mask_or_index)
-        if idx.dtype == bool:
-            if idx.shape != (self.n,):
-                raise ValueError("a mask must have one entry per cell (%d), got shape %s" % (self.n, idx.shape))
-            idx = np.flatnonzero(idx)
-        idx = idx.astype(np.int64).reshape(-1)
-        if idx.size and (idx.min() < -self.n or idx.max() >= self.n):
-            raise IndexError("cell index out of range for %d cells" % self.n)
-        idx = idx % max(self.n, 1)
+        idx = self._positions(mask_or_index)
         pd = PackedDeviceDataset.__new__(PackedDeviceDataset)
         pd.__dict__.update(self.__dict__)
         pd.rows = self.rows[torch.from_numpy(idx).to(self.device)].contiguous()
@@ -306,5 +282,21 @@ class PackedDeviceDataset:
               self._mean_d, self._std_d]
         return sum(t.numel() * t.element_size() for t in ts if t is not None)
 
-    def host_size_factors(self) -> np.ndarray:
-        return self.size_factors_host
+    # ------------------------------------------------------------------ training and prediction
+    def _bind(self, eng):
+        self._check_genes(eng)
+        super()._bind(eng)
+        eng.set_input_transform_exact(self.mean, self.std, self.median, self.flags)
+
+    def _fit(self, eng, n_tr, batch, shuffle):
+        return _resident_fit(eng, n_tr, self.n, batch, shuffle, lambda rows: eng.packed_train_step(self, rows),
+                             lambda s, e: eng.packed_eval_step(self, self.rows[s:e]), self.rows)
+
+    def _predictor(self, eng, bs):
+        def run(i, s, e, b):
+            eng.packed_predict(self, self.rows[s:e], mean=b.get("mean"), disp=b.get("disp"), pi=b.get("pi"),
+                               latent=b.get("latent"))
+
+        def theta(th):
+            eng.packed_predict(self, self.rows[:1], disp=th)
+        return run, theta, contextlib.nullcontext

@@ -13,6 +13,7 @@ non-negative integers and the gene count a multiple of 8 (the packed format).
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 
 import numpy as np
@@ -21,13 +22,10 @@ import torch
 from . import _lib
 from . import io as dio
 from ._lib import check
-from .device_data import PRE_SIZE_FACTORS, preprocess_flags
+from .device_data import (PRE_SIZE_FACTORS, _counts_matrix, _Dataset, _device, _size_factors, _stream, _X_DTYPES,
+                          preprocess_flags)
 
 _CHUNK_BYTES = 256 << 20          # fp32 counts of one chunk of rows on the device
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def pin_packed(pc, device_index=0):
@@ -172,23 +170,36 @@ def expand_exact(pc, n_counts, median, flags, mean, std, x_dtype, dev):
     return Y, X, sf
 
 
-class StreamedDataset:
+def stream_epoch(eng, n, batch, shuffle, begin):
+    """epoch(update) over the n rows of a host stream that begin() starts, in batches of ``batch`` rows: the batches
+    in a new random order every epoch (global NumPy RNG; in order with shuffle=False), update() after each step."""
+    nb = (n + batch - 1) // batch
+
+    def epoch(update):
+        border = np.random.permutation(nb) if shuffle else np.arange(nb)
+        begin()
+        for k in range(nb):
+            eng.stream_step(int(border[k]), int(border[k + 1]) if k + 1 < nb else -1)
+            update()
+        eng.stream_end()
+    return epoch
+
+
+class StreamedDataset(_Dataset):
     """Packed raw counts ``pc`` (io.PackedCounts, cells in order) with the statistics of the device preprocessing:
     ``n_counts_host`` (fp64), ``size_factors_host`` (fp32), ``mean`` / ``std`` (fp64 per gene), ``median``, ``flags``.
     The masks of the filtering steps (``gene_mask``, ``cell_mask``, ``sf_mask``), ``gene_totals_host``,
     ``input_gene_totals`` and ``n_bad`` are those of DeviceDataset, so io.apply_device_normalize(adata, sd, ...,
-    set_x=False) mutates an AnnData the same way."""
+    set_x=False) mutates an AnnData the same way.  Training, validation and prediction stream their batches from the
+    packed counts (the interface of device_data._Dataset, keyword ``stream_data``); training shuffles the rows once
+    and permutes whole batches every epoch."""
+    kind = "stream_data"
+    _on = "is for"
 
     def __init__(self, pc, n_counts_host, size_factors_host, mean, std, median, flags, x_dtype, device):
         self.pc, self.n_counts_host, self.size_factors_host = pc, n_counts_host, size_factors_host
         self.mean, self.std, self.median, self.flags = mean, std, median, flags
         self.x_dtype, self.device = x_dtype, device
-
-    def __copy__(self):
-        return self
-
-    def __deepcopy__(self, memo):
-        return self
 
     @property
     def n(self) -> int:
@@ -209,21 +220,9 @@ class StreamedDataset:
         (default: 256 MB of fp32 counts)."""
         if not torch.cuda.is_available():
             raise _lib.DcaError("StreamedDataset needs a CUDA device (H100); there is no CPU fallback")
-        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        if dev.index is None:
-            dev = torch.device("cuda", torch.cuda.current_device())
-        xdt = {"float32": torch.float32, "bfloat16": torch.bfloat16, torch.float32: torch.float32,
-               torch.bfloat16: torch.bfloat16}[x_dtype]
-        csr = hasattr(counts, "tocsr") and getattr(counts, "format", None) == "csr"
-        if not csr and hasattr(counts, "toarray"):
-            counts = counts.toarray()
-        if not csr:
-            counts = np.asarray(counts)
-        if counts.ndim != 2 or counts.shape[0] < 1 or counts.shape[1] < 1:
-            raise ValueError("counts must be a non-empty cells x genes matrix")
+        dev, xdt = _device(device), _X_DTYPES[x_dtype]
+        counts = _counts_matrix(counts)
         N0, G0 = (int(s) for s in counts.shape)
-        if N0 >= 2 ** 31:
-            raise ValueError("at most 2**31 - 1 cells")
         if G0 % 8 != 0:
             raise ValueError("streaming from packed counts needs a gene count that is a multiple of 8 (got %d)" % G0)
         with torch.cuda.device(dev):
@@ -251,11 +250,7 @@ class StreamedDataset:
                 if not sf_mask.all():
                     pc = pc.take_rows(np.flatnonzero(sf_mask))
                     nc, gene_tot, _ = _totals(pc, dev, chunk_rows)
-                med = float(np.median(nc))
-                sf_h = (nc / med).astype(np.float32)
-            else:
-                med = 1.0
-                sf_h = np.ones(nc.shape[0], np.float32)
+            med, sf_h = _size_factors(nc, size_factors)
             flags = preprocess_flags(size_factors, logtrans_input, normalize_input)
             mean, std = _moments(pc, nc, med, flags, dev, chunk_rows)
         sd = cls(pc, nc, sf_h, mean, std, med, flags, xdt, dev)
@@ -266,15 +261,7 @@ class StreamedDataset:
     def take(self, mask_or_index):
         """The cells ``mask_or_index`` (a boolean mask over this dataset's cells or integer positions) selects, in that
         order; the packed rows are copied (io.PackedCounts.take_rows) unless the selection is every cell in order."""
-        idx = np.asarray(mask_or_index)
-        if idx.dtype == bool:
-            if idx.shape != (self.n,):
-                raise ValueError("a mask must have one entry per cell (%d), got shape %s" % (self.n, idx.shape))
-            idx = np.flatnonzero(idx)
-        idx = idx.astype(np.int64).reshape(-1)
-        if idx.size and (idx.min() < -self.n or idx.max() >= self.n):
-            raise IndexError("cell index out of range for %d cells" % self.n)
-        idx = idx % max(self.n, 1)
+        idx = self._positions(mask_or_index)
         if idx.size == self.n and np.array_equal(idx, np.arange(self.n)):
             return self
         sd = StreamedDataset.__new__(StreamedDataset)
@@ -313,8 +300,48 @@ class StreamedDataset:
         return expand_exact(self.pc, self.n_counts_host, self.median, self.flags, self.mean, self.std, self.x_dtype,
                             self.device)
 
-    def host_size_factors(self) -> np.ndarray:
-        return self.size_factors_host
+    # ------------------------------------------------------------------ training and prediction
+    def _bind(self, eng):
+        self._check_genes(eng)
+        super()._bind(eng)
+
+    def _fit(self, eng, n_tr, batch, shuffle):
+        """The training rows shuffled ONCE (a packed copy in that order), every epoch permuting whole batches; the
+        validation rows streamed as well (dca_stream_eval), so device memory does not grow with the dataset."""
+        order0 = np.arange(n_tr)
+        if shuffle:
+            np.random.shuffle(order0)
+        tr = self.take(order0)
+        va = self.rows(n_tr, self.n) if n_tr < self.n else None
+        nb_va = (self.n - n_tr + batch - 1) // batch
+
+        def validate():
+            if va is None:
+                return
+            va.stream_batches(eng, batch)
+            for k in range(nb_va):
+                eng.stream_eval(k, k + 1 if k + 1 < nb_va else -1)
+            eng.stream_end()
+        return stream_epoch(eng, n_tr, batch, shuffle, lambda: tr.stream_batches(eng, batch)), validate
+
+    def _predictor(self, eng, bs):
+        nb = (self.n + bs - 1) // bs
+
+        def run(i, s, e, b):
+            eng.stream_predict(i, i + 1 if i + 1 < nb else -1, mean=b.get("mean"), disp=b.get("disp"),
+                               pi=b.get("pi"), latent=b.get("latent"))
+
+        def theta(th):
+            eng.stream_predict(0, -1, disp=th)
+
+        @contextlib.contextmanager
+        def session():
+            self.stream_batches(eng, bs)
+            try:
+                yield
+            finally:
+                eng.stream_end()
+        return run, theta, session
 
 
 def _chunk_rows(G):

@@ -84,16 +84,14 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
     shuffled ONCE and every epoch visits the batches in a new random order (documented deviation from Keras' per-epoch
     row shuffle).  Other keywords of the reference's model.fit (e.g. shuffle=False) are honoured or rejected loudly.
 
-    ``device_data``: a device_data.DeviceDataset of the cells of ``adata`` (in order), preprocessed in HBM.  X, the
-    raw-count target and the size factors are then read there (steps gather their rows through the dataset's
-    ``rows``) and adata's matrices are not used; the updates are those of the host arrays holding the same values.
-    Single process only, use_raw_as_output only, and with ``output_subset`` the dataset's Y must already hold those
-    genes (DeviceDataset.with_output_genes).  adata is then only read for ``raw.var_names`` (output_subset) and may be
-    None otherwise.
-
-    ``packed_data``: a packed_data.PackedDeviceDataset of the cells of ``adata`` (in order): raw counts packed in HBM,
-    every batch expanded on the device by row index.  The resident loop as with device_data (rows reshuffled every
-    epoch exactly like Keras) and the same updates; single process only, use_raw_as_output only, no output_subset."""
+    ``device_data`` / ``stream_data`` / ``packed_data``: a dataset of the cells of ``adata`` (in order) preprocessed on
+    the device -- device_data.DeviceDataset (resident in HBM), stream_data.StreamedDataset (packed counts in pinned
+    host memory, streamed as above) or packed_data.PackedDeviceDataset (packed counts in HBM, every batch expanded on
+    the device by row index).  X, the raw-count target and the size factors then come from the dataset and adata's
+    matrices are not used; the updates are those of the host arrays holding the same values.  Single process only,
+    use_raw_as_output only, and ``output_subset`` only with a DeviceDataset whose Y already holds those genes
+    (DeviceDataset.with_output_genes).  adata is then only read for ``raw.var_names`` (output_subset) and may be None
+    otherwise."""
     stream = kwds.pop('stream', False)
     shuffle = kwds.pop('shuffle', True)
     device_data = kwds.pop('device_data', None)
@@ -102,6 +100,7 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
     if kwds:
         raise TypeError("train() got keyword arguments the accelerated fit loop does not implement: %s" % sorted(kwds))
     from . import _lib as _L
+    from .device_data import _one_dataset
     if optimizer not in _L.OPTIMIZERS:
         raise NotImplementedError("optimizer %r is not on the accelerated path (supported: %s)"
                                   % (optimizer, sorted(k for k in _L.OPTIMIZERS if not k.islower())))
@@ -109,23 +108,17 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
         raise NotImplementedError("tensorboard logging is not part of the accelerated path")
     if output_dir is not None:
         os.makedirs(output_dir, exist_ok=True)
-    if packed_data is not None:
-        if device_data is not None or stream_data is not None or stream:
-            raise ValueError("packed_data is resident in HBM: it cannot be combined with stream, device_data or "
-                             "stream_data")
-        return _train_packed_data(adata, network, packed_data, output_subset, use_raw_as_output, optimizer,
-                                  learning_rate, batch_size, validation_split, epochs, reduce_lr, early_stop, clip_grad,
-                                  verbose, save_weights, output_dir, shuffle)
-    if stream_data is not None:
-        if device_data is not None:
-            raise ValueError("give device_data or stream_data, not both")
-        return _train_stream_data(adata, network, stream_data, output_subset, use_raw_as_output, optimizer, learning_rate,
-                                  batch_size, validation_split, epochs, reduce_lr, early_stop, clip_grad, verbose,
-                                  save_weights, output_dir, shuffle)
-    if device_data is not None:
-        return _train_device_data(adata, network, device_data, stream, output_subset, use_raw_as_output, optimizer,
-                                  learning_rate, batch_size, validation_split, epochs, reduce_lr, early_stop, clip_grad,
-                                  verbose, save_weights, output_dir, shuffle)
+    fit = dict(optimizer=optimizer, learning_rate=learning_rate, epochs=epochs, reduce_lr=reduce_lr,
+               early_stop=early_stop, clip_grad=clip_grad, verbose=verbose, save_weights=save_weights,
+               output_dir=output_dir)
+    data = _one_dataset(device_data, stream_data, packed_data, stream)
+    if data is not None:
+        _check_target(data, adata, output_subset, use_raw_as_output)
+        eng = network.ensure_engine(max_batch=batch_size)
+        data._bind(eng)
+        n_tr = _split(data.n, validation_split)
+        epoch, validate = data._fit(eng, n_tr, batch_size, shuffle)
+        return _fit(eng, network, epoch, validate, data.n - n_tr, **fit)
 
     X = np.asarray(adata.X, dtype=np.float32)
     sf = np.asarray(adata.obs['size_factors'], dtype=np.float32).reshape(-1)
@@ -138,103 +131,83 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
     Yh = np.asarray(Yh.toarray() if hasattr(Yh, "toarray") else Yh, dtype=np.float32)
 
     N = X.shape[0]
-    split_at = int(N * (1. - validation_split)) if validation_split and 0. < validation_split < 1. else N
+    split_at = _split(N, validation_split)
     rank, world = D.rank_world()
 
     # cells shard across ranks (SURVEY.md 8e): contiguous row ranges, equal count per rank
     tr_lo, tr_hi = D.shard_bounds(split_at, rank, world, equal=True)
     va_lo, va_hi = D.shard_bounds(N - split_at, rank, world, equal=False)
-    va_lo += split_at; va_hi += split_at
+    tr, va = (tr_lo, tr_hi), (va_lo + split_at, va_hi + split_at)
 
     if world > 1 and rank == 0 and (split_at % world) and verbose:
         print("dca: %d training cells do not divide over %d ranks; the last %d are left out of every epoch"
               % (split_at, world, split_at % world))
     eng = network.ensure_engine(max_batch=batch_size)
-    dev = eng.device
     if stream == 'auto':
-        free = torch.cuda.mem_get_info(dev)[0]
+        free = torch.cuda.mem_get_info(eng.device)[0]
         stream = (tr_hi - tr_lo + va_hi - va_lo) * X.shape[1] * (4 + eng.params.element_size()) > 0.6 * free
-    # opt.__dict__[optimizer](clipvalue=clip_grad[, lr=learning_rate])                   (dca/train.py:54-57)
-    default_lr = eng.set_optimizer(optimizer)
-    if learning_rate is None:
-        learning_rate = default_lr
-    if stream:
-        return _fit_stream(eng, network, X, Yh, sf, (tr_lo, tr_hi), (va_lo, va_hi), batch_size, epochs, learning_rate, reduce_lr,
-                           early_stop, clip_grad, world, rank, verbose, save_weights, output_dir, shuffle)
-    Xd = _to_device(np.concatenate([X[tr_lo:tr_hi], X[va_lo:va_hi]]), eng.x_dtype, dev)
-    Yd = _to_device(np.concatenate([Yh[tr_lo:tr_hi], Yh[va_lo:va_hi]]), torch.float32, dev)
-    sfd = _to_device(np.concatenate([sf[tr_lo:tr_hi], sf[va_lo:va_hi]]), torch.float32, dev)
-    n_tr = tr_hi - tr_lo
-    n_va = va_hi - va_lo
-
+    feed = _host_stream if stream else _host_resident
+    epoch, validate = feed(eng, X, Yh, sf, tr, va, batch_size, shuffle, world)
     if world > 1:
         D.broadcast_(eng.params, src=0); D.broadcast_(eng.bn_state, src=0)
         eng.params_changed()
         if torch.distributed.get_backend() == "nccl":
             eng.comm_init()          # gradient exchange inside the library: one CUDA graph per step (dca_train_step_dp)
-    eng.reset_optimizer()
-
-    lr = float(learning_rate)
-    ctl = PlateauAndStop(lr, reduce_lr, early_stop, verbose)
-    hist = History()
-    if verbose:
-        print(network.summary())
-
-    steps = (n_tr + batch_size - 1) // batch_size
-    gscale = 1.0 / world
-    # run on a non-default stream (CUDA-graph replay of the step needs a capturable stream)
-    torch.cuda.synchronize(dev)
-    prev_stream = torch.cuda.current_stream(dev)
-    torch.cuda.set_stream(torch.cuda.Stream(dev))
-    try:
-        hist = _fit_loop(eng, network, Xd, Yd, sfd, n_tr, n_va, steps, batch_size, epochs, ctl, clip_grad, gscale, world, rank,
-                         dev, hist, verbose, save_weights, output_dir, shuffle)
-    finally:
-        torch.cuda.synchronize(dev)
-        torch.cuda.set_stream(prev_stream)
-    if not hist.history["val_loss"]:
-        del hist.history["val_loss"]
-    return hist
+    return _fit(eng, network, epoch, validate, va[1] - va[0], gscale=1.0 / world, world=world, rank=rank, **fit)
 
 
-def _epoch_end(eng, network, hist, ctl, epoch, epochs, n_va, world, rank, dev, verbose, save_weights, output_dir, best_val):
-    """Epoch bookkeeping shared by the resident and the streaming loop: reduce the accumulators over ranks, history,
-    ModelCheckpoint, ReduceLROnPlateau / EarlyStopping.  Returns (stop, best_val)."""
-    acc = np.asarray(eng.read_epoch_acc(reset=True), dtype=np.float64)
-    if world > 1:
-        acc = D.all_reduce_sum_host(acc, dev)
-        if eng.bn_state.numel():
-            D.all_reduce_sum_(eng.bn_state); eng.bn_state.mul_(1.0 / world)
-    loss = acc[0] / acc[1] if acc[1] > 0 else float("nan")
-    if not np.isfinite(loss):
-        loss = float("inf")                       # _nan2inf convention, dca/loss.py:148
-    val = None
-    if n_va > 0 or (world > 1 and acc[3] > 0):
-        val = acc[2] / acc[3] + network.penalty_value()
-        if not np.isfinite(val):
-            val = float("inf")
-    hist.epoch.append(epoch)
-    hist.history["loss"].append(float(loss))
-    hist.history["lr"].append(float(ctl.lr))
-    if val is not None:
-        hist.history["val_loss"].append(float(val))
-    if verbose and rank == 0:
-        print("Epoch %d/%d - loss: %.4f%s - lr: %g" % (epoch + 1, epochs, loss,
-                                                    "" if val is None else " - val_loss: %.4f" % val, ctl.lr))
-    if save_weights and output_dir is not None and rank == 0:
-        mon = val if val is not None else loss
-        if mon < best_val:                       # ModelCheckpoint(save_best_only=True), dca/train.py:64-69
-            best_val = mon
-            network.save_weights(os.path.join(output_dir, "weights.npz"))
-    return ctl.on_epoch_end(epoch, val), best_val
+def _split(n, validation_split):
+    """Training rows of n: the tail ``validation_split`` validates (taken before shuffling, as Keras does)."""
+    return int(n * (1. - validation_split)) if validation_split and 0. < validation_split < 1. else n
 
 
-def _fit_stream(eng, network, X, Yh, sf, tr, va, batch_size, epochs, learning_rate, reduce_lr, early_stop, clip_grad, world, rank,
-                verbose, save_weights, output_dir, shuffle):
+def _check_target(data, adata, output_subset, use_raw_as_output):
+    """The rules every dataset kind trains under: one process, the raw counts of its cells as the target, and an
+    output_subset only through a DeviceDataset whose Y holds those genes (y_cols)."""
+    if D.rank_world()[1] > 1:
+        raise NotImplementedError("%s trains on one GPU; a torch.distributed world larger than 1 is not supported"
+                                  % data.kind)
+    if not use_raw_as_output:
+        raise ValueError("%s holds the raw counts as the target: use_raw_as_output=False is not supported" % data.kind)
+    if not hasattr(data, "y_cols"):
+        if output_subset:
+            raise NotImplementedError("%s needs the raw counts of the input genes as the target (no output_subset)"
+                                      % data.kind)
+    elif output_subset:
+        if adata is None:
+            raise ValueError("output_subset names genes of adata.raw: pass the AnnData with device_data")
+        raw_names = np.asarray(adata.raw.var_names)
+        gene_idx = [int(np.where(raw_names == x)[0][0]) for x in output_subset]
+        if data.y_cols is None or list(data.y_cols) != gene_idx:
+            raise ValueError("output_subset needs a dataset whose Y holds those genes: "
+                             "device_data.with_output_genes(<their positions in adata.raw.var_names>)")
+    elif data.y_cols is not None:
+        raise ValueError("the dataset's Y holds a subset of the genes, but no output_subset was given")
+    data._cover(adata)
+
+
+def _host_resident(eng, X, Yh, sf, tr, va, batch_size, shuffle, world):
+    """(epoch, validate) of the rows tr + va of the host arrays, copied to the device once: the training rows
+    reshuffled every epoch as Keras does, the gradients all-reduced over the ranks in the step when world > 1."""
+    from .device_data import _resident_fit
+    (tr_lo, tr_hi), (va_lo, va_hi) = tr, va
+    dev = eng.device
+    Xd = _to_device(np.concatenate([X[tr_lo:tr_hi], X[va_lo:va_hi]]), eng.x_dtype, dev)
+    Yd = _to_device(np.concatenate([Yh[tr_lo:tr_hi], Yh[va_lo:va_hi]]), torch.float32, dev)
+    sfd = _to_device(np.concatenate([sf[tr_lo:tr_hi], sf[va_lo:va_hi]]), torch.float32, dev)
+    n_tr = tr_hi - tr_lo
+    step = eng.train_step_allreduce if world > 1 else eng.train_step     # NCCL all-reduce overlapped with the backward
+    return _resident_fit(eng, n_tr, n_tr + va_hi - va_lo, batch_size, shuffle,
+                         lambda rows: step(Xd, Yd, sfd, rows=rows),
+                         lambda s, e: eng.eval_step(Xd[s:e], Yd[s:e], sfd[s:e]))
+
+
+def _host_stream(eng, X, Yh, sf, tr, va, batch_size, shuffle, world):
     """Training from host memory (dca_stream_*): see train().  X is only used for the (small, resident) validation rows;
     the training rows travel as bit-packed raw counts and are normalised on the device."""
     from . import io as dio
     from .hostmem import pin_near_gpu
+    from .stream_data import stream_epoch
     dev = eng.device
     (tr_lo, tr_hi), (va_lo, va_hi) = tr, va
     if eng.n_in != eng.n_out or Yh.shape[1] != X.shape[1]:
@@ -267,255 +240,89 @@ def _fit_stream(eng, network, X, Yh, sf, tr, va, batch_size, epochs, learning_ra
     Xv = _to_device(X[va_lo:va_hi], eng.x_dtype, dev) if n_va else None
     Yv = _to_device(Yh[va_lo:va_hi], torch.float32, dev) if n_va else None
     sfv = _to_device(sf[va_lo:va_hi], torch.float32, dev) if n_va else None
+    steps = stream_epoch(eng, n_tr, batch_size, shuffle, lambda: eng.stream_begin(packed, sf_h, batch_size))
+
+    def epoch(update):
+        if world == 1:
+            return steps(update)
+
+        def reduced():                            # the gradients summed over the ranks before every update
+            eng.allreduce_grads() if getattr(eng, "_comm", False) else D.all_reduce_sum_(eng.grads)
+            update()
+        steps(reduced)
+
+    def validate():
+        for s0 in range(0, n_va, batch_size):
+            e = min(s0 + batch_size, n_va)
+            eng.eval_step(Xv[s0:e], Yv[s0:e], sfv[s0:e])
+    return epoch, validate
+
+
+def _fit(eng, network, epoch, validate, n_va, optimizer, learning_rate, epochs, reduce_lr, early_stop, clip_grad, verbose,
+         save_weights, output_dir, gscale=1.0, world=1, rank=0):
+    """The fit loop of every input: optimizer, ReduceLROnPlateau / EarlyStopping, history and ModelCheckpoint around
+    epoch(update) -- one epoch's training steps, update() after each -- and validate(), the pass over the n_va
+    validation rows."""
+    # opt.__dict__[optimizer](clipvalue=clip_grad[, lr=learning_rate])                   (dca/train.py:54-57)
+    default_lr = eng.set_optimizer(optimizer)
+    eng.reset_optimizer()
+    ctl = PlateauAndStop(float(default_lr if learning_rate is None else learning_rate), reduce_lr, early_stop, verbose)
+    hist = History()
+    if verbose:
+        print(network.summary())
+    dev = eng.device
+    # run on a non-default stream (CUDA-graph replay of the step needs a capturable stream)
+    torch.cuda.synchronize(dev)
+    prev_stream = torch.cuda.current_stream(dev)
+    torch.cuda.set_stream(torch.cuda.Stream(dev))
+    best_val = np.inf
+    try:
+        for e in range(epochs):
+            eng.read_epoch_acc(reset=True)
+            epoch(lambda: eng.apply_update(ctl.lr, clip_grad, gscale))
+            validate()
+            stop, best_val = _epoch_end(eng, network, hist, ctl, e, epochs, n_va, world, rank, dev, verbose, save_weights,
+                                        output_dir, best_val)
+            if stop:
+                break
+    finally:
+        torch.cuda.synchronize(dev)
+        torch.cuda.set_stream(prev_stream)
+    if not hist.history["val_loss"]:
+        del hist.history["val_loss"]
+    return hist
+
+
+def _epoch_end(eng, network, hist, ctl, epoch, epochs, n_va, world, rank, dev, verbose, save_weights, output_dir, best_val):
+    """Epoch bookkeeping: reduce the accumulators over ranks, history, ModelCheckpoint, ReduceLROnPlateau /
+    EarlyStopping.  Returns (stop, best_val)."""
+    acc = np.asarray(eng.read_epoch_acc(reset=True), dtype=np.float64)
     if world > 1:
-        D.broadcast_(eng.params, src=0); D.broadcast_(eng.bn_state, src=0)
-        eng.params_changed()
-        if torch.distributed.get_backend() == "nccl":
-            eng.comm_init()
-    eng.reset_optimizer()
-    lr = float(learning_rate)
-    ctl = PlateauAndStop(lr, reduce_lr, early_stop, verbose)
-    hist = History()
-    nb = (n_tr + batch_size - 1) // batch_size
-    gscale = 1.0 / world
-    torch.cuda.synchronize(dev)
-    prev_stream = torch.cuda.current_stream(dev)
-    torch.cuda.set_stream(torch.cuda.Stream(dev))
-    best_val = np.inf
-    try:
-        for epoch in range(epochs):
-            border = np.random.permutation(nb) if shuffle else np.arange(nb)
-            eng.read_epoch_acc(reset=True)
-            eng.stream_begin(packed, sf_h, batch_size)
-            for k in range(nb):
-                eng.stream_step(int(border[k]), int(border[k + 1]) if k + 1 < nb else -1)
-                if world > 1:
-                    eng.allreduce_grads() if getattr(eng, "_comm", False) else D.all_reduce_sum_(eng.grads)
-                eng.apply_update(ctl.lr, clip_grad, gscale)
-            eng.stream_end()
-            for s0 in range(0, n_va, batch_size):
-                e = min(s0 + batch_size, n_va)
-                eng.eval_step(Xv[s0:e], Yv[s0:e], sfv[s0:e])
-            stop, best_val = _epoch_end(eng, network, hist, ctl, epoch, epochs, n_va, world, rank, dev, verbose, save_weights,
-                                        output_dir, best_val)
-            if stop:
-                break
-    finally:
-        torch.cuda.synchronize(dev)
-        torch.cuda.set_stream(prev_stream)
-    if not hist.history["val_loss"]:
-        del hist.history["val_loss"]
-    return hist
-
-
-def _train_stream_data(adata, network, sd, output_subset, use_raw_as_output, optimizer, learning_rate, batch_size,
-                       validation_split, epochs, reduce_lr, early_stop, clip_grad, verbose, save_weights, output_dir, shuffle):
-    """train() on a stream_data.StreamedDataset: the split and stream semantics of _fit_stream (the training rows shuffled
-    once, every epoch permuting whole batches; in order with shuffle=False), with batches normalised by the exact transform
-    of the device preprocessing.  The validation rows are streamed as well (dca_stream_eval), so device memory does not
-    grow with the dataset."""
-    if D.rank_world()[1] > 1:
-        raise NotImplementedError("stream_data trains on one GPU; a torch.distributed world larger than 1 is not supported")
-    if not use_raw_as_output:
-        raise ValueError("stream_data holds the raw counts as the target: use_raw_as_output=False is not supported")
-    if output_subset:
-        raise NotImplementedError("stream_data needs the raw counts of the input genes as the target (no output_subset)")
-    if adata is not None and adata.n_obs != sd.n:
-        raise ValueError("stream_data covers %d cells, adata has %d" % (sd.n, adata.n_obs))
-    eng = network.ensure_engine(max_batch=batch_size)
-    if eng.n_in != sd.n_genes or eng.n_out != sd.n_genes:
-        raise ValueError("stream_data has %d genes, the network %d inputs and %d outputs" % (sd.n_genes, eng.n_in, eng.n_out))
-    if sd.device != eng.device:
-        raise ValueError("stream_data is for %s, the network on %s" % (sd.device, eng.device))
-    if sd.x_dtype != eng.x_dtype:
-        raise ValueError("stream_data X is %s, the network expects %s (network_kwds x_dtype)" % (sd.x_dtype, eng.x_dtype))
-    dev = eng.device
-    N = sd.n
-    n_tr = int(N * (1. - validation_split)) if validation_split and 0. < validation_split < 1. else N
-    n_va = N - n_tr
-    order0 = np.arange(n_tr)
-    if shuffle:
-        np.random.shuffle(order0)                 # ONE row shuffle; the epochs permute whole batches (as _fit_stream)
-    tr = sd.take(order0)
-    va = sd.rows(n_tr, N) if n_va else None
-    nb_va = (n_va + batch_size - 1) // batch_size
-    default_lr = eng.set_optimizer(optimizer)
-    if learning_rate is None:
-        learning_rate = default_lr
-    eng.reset_optimizer()
-    ctl = PlateauAndStop(float(learning_rate), reduce_lr, early_stop, verbose)
-    hist = History()
-    if verbose:
-        print(network.summary())
-    nb = (n_tr + batch_size - 1) // batch_size
-    torch.cuda.synchronize(dev)
-    prev_stream = torch.cuda.current_stream(dev)
-    torch.cuda.set_stream(torch.cuda.Stream(dev))
-    best_val = np.inf
-    try:
-        for epoch in range(epochs):
-            border = np.random.permutation(nb) if shuffle else np.arange(nb)
-            eng.read_epoch_acc(reset=True)
-            tr.stream_batches(eng, batch_size)
-            for k in range(nb):
-                eng.stream_step(int(border[k]), int(border[k + 1]) if k + 1 < nb else -1)
-                eng.apply_update(ctl.lr, clip_grad, 1.0)
-            eng.stream_end()
-            if n_va:
-                va.stream_batches(eng, batch_size)
-                for k in range(nb_va):
-                    eng.stream_eval(k, k + 1 if k + 1 < nb_va else -1)
-                eng.stream_end()
-            stop, best_val = _epoch_end(eng, network, hist, ctl, epoch, epochs, n_va, 1, 0, dev, verbose, save_weights,
-                                        output_dir, best_val)
-            if stop:
-                break
-    finally:
-        torch.cuda.synchronize(dev)
-        torch.cuda.set_stream(prev_stream)
-    if not hist.history["val_loss"]:
-        del hist.history["val_loss"]
-    return hist
-
-
-def _train_device_data(adata, network, dd, stream, output_subset, use_raw_as_output, optimizer, learning_rate, batch_size,
-                       validation_split, epochs, reduce_lr, early_stop, clip_grad, verbose, save_weights, output_dir, shuffle):
-    """train() on a DeviceDataset: the resident loop of train() with positions mapped through dd.rows."""
-    if stream:
-        raise ValueError("device_data is resident in HBM: it cannot be combined with stream=True")
-    if D.rank_world()[1] > 1:
-        raise NotImplementedError("device_data trains on one GPU; a torch.distributed world larger than 1 is not supported")
-    if not use_raw_as_output:
-        raise ValueError("device_data holds the raw counts as the target: use_raw_as_output=False is not supported")
-    if output_subset:
-        if adata is None:
-            raise ValueError("output_subset names genes of adata.raw: pass the AnnData with device_data")
-        raw_names = np.asarray(adata.raw.var_names)
-        gene_idx = [int(np.where(raw_names == x)[0][0]) for x in output_subset]
-        if dd.y_cols is None or list(dd.y_cols) != gene_idx:
-            raise ValueError("output_subset needs a dataset whose Y holds those genes: "
-                             "device_data.with_output_genes(<their positions in adata.raw.var_names>)")
-    elif dd.y_cols is not None:
-        raise ValueError("the dataset's Y holds a subset of the genes, but no output_subset was given")
-    if adata is not None and adata.n_obs != dd.n:
-        raise ValueError("device_data covers %d cells, adata has %d" % (dd.n, adata.n_obs))
-    eng = network.ensure_engine(max_batch=batch_size)
-    if dd.X.device != eng.device:
-        raise ValueError("device_data lives on %s, the network on %s" % (dd.X.device, eng.device))
-    if dd.x_dtype != eng.x_dtype:
-        raise ValueError("device_data X is %s, the network expects %s (network_kwds x_dtype)" % (dd.x_dtype, eng.x_dtype))
-    N = dd.n
-    n_tr = int(N * (1. - validation_split)) if validation_split and 0. < validation_split < 1. else N
-    n_va = N - n_tr
-    default_lr = eng.set_optimizer(optimizer)
-    if learning_rate is None:
-        learning_rate = default_lr
-    eng.reset_optimizer()
-    ctl = PlateauAndStop(float(learning_rate), reduce_lr, early_stop, verbose)
-    hist = History()
-    if verbose:
-        print(network.summary())
-    steps = (n_tr + batch_size - 1) // batch_size
-    dev = eng.device
-    torch.cuda.synchronize(dev)
-    prev_stream = torch.cuda.current_stream(dev)
-    torch.cuda.set_stream(torch.cuda.Stream(dev))
-    try:
-        hist = _fit_loop(eng, network, dd.X, dd.Y, dd.sf, n_tr, n_va, steps, batch_size, epochs, ctl, clip_grad, 1.0, 1, 0,
-                         dev, hist, verbose, save_weights, output_dir, shuffle, rows_map=dd.rows)
-    finally:
-        torch.cuda.synchronize(dev)
-        torch.cuda.set_stream(prev_stream)
-    if not hist.history["val_loss"]:
-        del hist.history["val_loss"]
-    return hist
-
-
-def _train_packed_data(adata, network, pd, output_subset, use_raw_as_output, optimizer, learning_rate, batch_size,
-                       validation_split, epochs, reduce_lr, early_stop, clip_grad, verbose, save_weights, output_dir, shuffle):
-    """train() on a PackedDeviceDataset: the resident loop of train() with every batch expanded from the packed counts
-    by row index (dca_packed_train_step / dca_packed_eval_step) with the exact transform of the device preprocessing."""
-    if D.rank_world()[1] > 1:
-        raise NotImplementedError("packed_data trains on one GPU; a torch.distributed world larger than 1 is not supported")
-    if not use_raw_as_output:
-        raise ValueError("packed_data holds the raw counts as the target: use_raw_as_output=False is not supported")
-    if output_subset:
-        raise NotImplementedError("packed_data needs the raw counts of the input genes as the target (no output_subset)")
-    if adata is not None and adata.n_obs != pd.n:
-        raise ValueError("packed_data covers %d cells, adata has %d" % (pd.n, adata.n_obs))
-    eng = network.ensure_engine(max_batch=batch_size)
-    if eng.n_in != pd.n_genes or eng.n_out != pd.n_genes:
-        raise ValueError("packed_data has %d genes, the network %d inputs and %d outputs" % (pd.n_genes, eng.n_in, eng.n_out))
-    if pd.device != eng.device:
-        raise ValueError("packed_data lives on %s, the network on %s" % (pd.device, eng.device))
-    if pd.x_dtype != eng.x_dtype:
-        raise ValueError("packed_data X is %s, the network expects %s (network_kwds x_dtype)" % (pd.x_dtype, eng.x_dtype))
-    N = pd.n
-    n_tr = int(N * (1. - validation_split)) if validation_split and 0. < validation_split < 1. else N
-    n_va = N - n_tr
-    default_lr = eng.set_optimizer(optimizer)
-    if learning_rate is None:
-        learning_rate = default_lr
-    eng.reset_optimizer()
-    eng.set_input_transform_exact(pd.mean, pd.std, pd.median, pd.flags)
-    ctl = PlateauAndStop(float(learning_rate), reduce_lr, early_stop, verbose)
-    hist = History()
-    if verbose:
-        print(network.summary())
-    steps = (n_tr + batch_size - 1) // batch_size
-    dev = eng.device
-    torch.cuda.synchronize(dev)
-    prev_stream = torch.cuda.current_stream(dev)
-    torch.cuda.set_stream(torch.cuda.Stream(dev))
-    try:
-        hist = _fit_loop(eng, network, None, None, None, n_tr, n_va, steps, batch_size, epochs, ctl, clip_grad, 1.0, 1, 0,
-                         dev, hist, verbose, save_weights, output_dir, shuffle, rows_map=pd.rows, packed=pd)
-    finally:
-        torch.cuda.synchronize(dev)
-        torch.cuda.set_stream(prev_stream)
-    if not hist.history["val_loss"]:
-        del hist.history["val_loss"]
-    return hist
-
-
-def _fit_loop(eng, network, Xd, Yd, sfd, n_tr, n_va, steps, batch_size, epochs, ctl, clip_grad, gscale, world, rank, dev, hist,
-              verbose, save_weights, output_dir, shuffle=True, rows_map=None, packed=None):
-    """rows_map (int32 device tensor, n_tr + n_va entries): the storage row of each position in Xd / Yd / sfd; None:
-    position = row.  packed: a PackedDeviceDataset whose storage rows rows_map names (Xd, Yd, sfd unused): every batch
-    is expanded from its packed counts."""
-    best_val = np.inf
-    for epoch in range(epochs):
-        # Keras: np.random.shuffle(index_array) with the global NumPy RNG (seeded in api.dca / CLI)
-        order = np.arange(n_tr)
-        if shuffle:
-            np.random.shuffle(order)
-        order_d = torch.from_numpy(order.astype(np.int32)).to(dev)
-        if rows_map is not None:
-            order_d = rows_map[order_d.long()]
-        eng.read_epoch_acc(reset=True)
-        for s in range(steps):
-            rows = order_d[s * batch_size: min((s + 1) * batch_size, n_tr)]
-            if packed is not None:
-                eng.packed_train_step(packed, rows)
-            elif world > 1:
-                eng.train_step_allreduce(Xd, Yd, sfd, rows=rows)     # NCCL all-reduce overlapped with the backward tail
-            else:
-                eng.train_step(Xd, Yd, sfd, rows=rows)
-            eng.apply_update(ctl.lr, clip_grad, gscale)
-        # validation pass: inference-mode BN over the held-out tail
-        for s in range(n_tr, n_tr + n_va, batch_size):
-            e = min(s + batch_size, n_tr + n_va)
-            if packed is not None:
-                eng.packed_eval_step(packed, rows_map[s:e])
-            elif rows_map is not None:
-                eng.eval_step(Xd, Yd, sfd, rows=rows_map[s:e])
-            else:
-                eng.eval_step(Xd[s:e], Yd[s:e], sfd[s:e])
-        stop, best_val = _epoch_end(eng, network, hist, ctl, epoch, epochs, n_va, world, rank, dev, verbose, save_weights,
-                                    output_dir, best_val)
-        if stop:
-            break
-    return hist
+        acc = D.all_reduce_sum_host(acc, dev)
+        if eng.bn_state.numel():
+            D.all_reduce_sum_(eng.bn_state); eng.bn_state.mul_(1.0 / world)
+    loss = acc[0] / acc[1] if acc[1] > 0 else float("nan")
+    if not np.isfinite(loss):
+        loss = float("inf")                       # _nan2inf convention, dca/loss.py:148
+    val = None
+    if n_va > 0 or (world > 1 and acc[3] > 0):
+        val = acc[2] / acc[3] + network.penalty_value()
+        if not np.isfinite(val):
+            val = float("inf")
+    hist.epoch.append(epoch)
+    hist.history["loss"].append(float(loss))
+    hist.history["lr"].append(float(ctl.lr))
+    if val is not None:
+        hist.history["val_loss"].append(float(val))
+    if verbose and rank == 0:
+        print("Epoch %d/%d - loss: %.4f%s - lr: %g" % (epoch + 1, epochs, loss,
+                                                    "" if val is None else " - val_loss: %.4f" % val, ctl.lr))
+    if save_weights and output_dir is not None and rank == 0:
+        mon = val if val is not None else loss
+        if mon < best_val:                       # ModelCheckpoint(save_best_only=True), dca/train.py:64-69
+            best_val = mon
+            network.save_weights(os.path.join(output_dir, "weights.npz"))
+    return ctl.on_epoch_end(epoch, val), best_val
 
 
 def train_with_args(args):
@@ -560,9 +367,8 @@ def train_with_args(args):
                          normalize_input=args.norminput,
                          device=torch.device('cuda', torch.cuda.current_device()) if preprocess == 'device' else None,
                          stream=stream, packed=packed)
-    dd = adata.uns.pop('dca_device_data', None)
-    sd = adata.uns.pop('dca_stream_data', None)
-    pdd = adata.uns.pop('dca_packed_data', None)
+    ds = next((adata.uns.pop(k) for k in ('dca_device_data', 'dca_stream_data', 'dca_packed_data') if k in adata.uns),
+              None)
 
     if args.denoisesubset:
         genelist = list(set(io.read_genelist(args.denoisesubset)))
@@ -601,16 +407,12 @@ def train_with_args(args):
 
     train_mask = np.asarray(adata.obs.dca_split == 'train')
     extra = {}
-    if dd is not None:
-        dd_train = dd.take(train_mask)
-        if genelist:
+    if ds is not None:
+        ds_train = ds.take(train_mask)
+        if genelist:                              # a DeviceDataset: --stream and --packed reject --denoisesubset
             raw_names = np.asarray(adata.raw.var_names)
-            dd_train = dd_train.with_output_genes([int(np.where(raw_names == x)[0][0]) for x in genelist])
-        extra['device_data'] = dd_train
-    if sd is not None:
-        extra['stream_data'] = sd.take(train_mask)
-    if pdd is not None:
-        extra['packed_data'] = pdd.take(train_mask)
+            ds_train = ds_train.with_output_genes([int(np.where(raw_names == x)[0][0]) for x in genelist])
+        extra[ds.kind] = ds_train
     losses = train(adata[adata.obs.dca_split == 'train'], net,
                    output_dir=args.outputdir,
                    learning_rate=args.learningrate,
@@ -632,5 +434,5 @@ def train_with_args(args):
     # the files of net.predict(adata, mode='full', return_info=True, ...) + net.write(...), written in gene blocks
     # from the device: host memory holds the labels and the text buffers, never a cells x genes output
     net.write_predictions(args.outputdir, adata.obs_names.values, predict_columns, mode='full', return_info=True,
-                          device_data=dd, stream_data=sd, packed_data=pdd, adata=adata)
+                          adata=adata, **({ds.kind: ds} if ds is not None else {}))
     return losses

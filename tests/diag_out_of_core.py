@@ -7,7 +7,7 @@ after a warm-up at 1/8 of the rows) of io.pack_rows, of each statistics pass ove
 StreamedDataset.from_counts end to end, against DeviceDataset.from_counts and host io.normalize; streamed-step
 cells/s with the exact transform (dca_set_input_transform_exact) against the float transform
 (dca_set_input_transform) on the same packed bytes, the two alternated three times; streamed predict against
-_run_predict_device; dca(epochs) with training_kwds preprocess 'host', 'device' and 'device' + stream.  The card's
+predict from the DeviceDataset; dca(epochs) with training_kwds preprocess 'host', 'device' and 'device' + stream.  The card's
 name and power limit are read in the same run.  Needs a GPU.
 """
 import argparse

@@ -100,7 +100,10 @@ def child(path, n, g, out):
     if path == "new":
         stats["writer"] = writer
         # one predict pass over all cells, device time (what each gene block repeats)
-        eng, N, bs, run, theta, session = net._packed_source(None, pdd)
+        eng, N = net.engine, pdd.n                # sized for predict by write_predictions above
+        pdd._bind(eng)
+        bs = min(network.PREDICT_BATCH, eng.max_batch)
+        run, theta, session = pdd._predictor(eng, bs)
         bufs = {k: torch.empty((bs, g), device=dev) for k in ("mean", "disp", "pi")}
         bufs["latent"] = torch.empty((bs, eng.latent_dim), device=dev)
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
