@@ -141,13 +141,14 @@ class TorchExtraNet:
     """float64 autograd statement of one training step of the extra types (the role TF autodiff plays in the reference);
     same parameter names as the engine.  TEST INFRASTRUCTURE ONLY."""
 
-    def __init__(self, params, hidden, ae_type, batchnorm=True, ridge=0.0, dtype=torch.float64, activation="relu"):
+    def __init__(self, params, hidden, ae_type, batchnorm=True, ridge=0.0, dtype=torch.float64, activation="relu",
+                 device="cpu"):
         assert ae_type in EXTRA_TYPES
         self.hidden = tuple(hidden); self.ae_type = ae_type; self.batchnorm = batchnorm; self.ridge = ridge; self.dtype = dtype
-        self.activation = activation
+        self.activation = activation; self.device = torch.device(device)
         self.masks = {}; self.rates = {}      # dropout: layer id (-1 input, i hidden, 8 + b fork branch) -> keep mask / rate
         self.names = layer_names(len(self.hidden)); self.center = len(self.hidden) // 2
-        self.p = {k: torch.as_tensor(v).to(dtype).clone() for k, v in params.items()}
+        self.p = {k: torch.as_tensor(v).to(self.device, dtype).clone() for k, v in params.items()}
         self.train_keys = [k for k in self.p if k.endswith(("/kernel", "/bias", "/bn_beta", "_act/alpha"))]
         for k in self.train_keys:
             self.p[k].requires_grad_(True)
@@ -169,7 +170,8 @@ class TorchExtraNet:
             out = apply_dropout(out, self.masks[lid], self.rates[lid])
         return a, out
 
-    def forward(self, X, sf, training=True):
+    def hidden_stack(self, X, training=True):
+        """(head inputs {branch: activation}, latent, BatchNorm batch statistics): everything in front of the heads."""
         stats = []
         h = X; latent = None
         if training and -1 in self.masks:
@@ -184,10 +186,21 @@ class TorchExtraNet:
             a, h = self._layer(h, nm, training, stats, i)
             if nm == "center":
                 latent = a
-        hin = lambda br: branch.get(br, h)
+        return {br: branch.get(br, h) for br in ("mean", "disp", "pi")}, latent, stats
+
+    def forward(self, X, sf, training=True):
+        ins, latent, stats = self.hidden_stack(X, training)
+        out = self.heads(ins, sf)
+        out.update(latent=latent, stats=stats)
+        return out
+
+    def heads(self, ins, sf):
+        """mean / dispersion / pi of the rows of ``ins`` (one activation per branch; all three are the trunk's
+        last activation except for the fork types)."""
+        h = ins["mean"]
         dense = lambda nm, x: x @ self.p[nm + "/kernel"] + self.p[nm + "/bias"]
         sfc = sf.reshape(-1, 1)
-        out = {"latent": latent, "stats": stats}
+        out = {}
         t = self.ae_type
         if t == "normal":
             out["mean"] = dense("mean", h) * sfc
@@ -197,33 +210,69 @@ class TorchExtraNet:
             out["mean"] = torch.clamp(torch.exp(tt), 1e-5, 1e6) * sfc
             out["dispersion"] = torch.clamp(torch.nn.functional.softplus(dense("dispersion", h)), 1e-4, 1e4)
         else:
-            out["mean"] = torch.clamp(torch.exp(dense("mean", hin("mean"))), 1e-5, 1e6) * sfc
+            out["mean"] = torch.clamp(torch.exp(dense("mean", ins["mean"])), 1e-5, 1e6) * sfc
             if t != "poisson":
-                out["dispersion"] = torch.clamp(torch.nn.functional.softplus(dense("dispersion", hin("disp"))), 1e-4, 1e4)
+                out["dispersion"] = torch.clamp(torch.nn.functional.softplus(dense("dispersion", ins["disp"])), 1e-4, 1e4)
             if t in ("zinb-shared", "zinb-fork"):
-                out["pi"] = torch.sigmoid(dense("pi", hin("pi")))
+                out["pi"] = torch.sigmoid(dense("pi", ins["pi"]))
         return out
+
+    def _loss_sum(self, o, Y):
+        """Sum of the element losses of the rows in ``o`` (not divided by the element count)."""
+        mu = o["mean"]
+        if self.ae_type == "normal":
+            return ((mu - Y) ** 2).sum()                                 # keras mean_squared_error
+        if self.ae_type == "poisson":
+            return poisson_elem_sum_and_count(Y, mu)[0]
+        if "pi" in o:
+            return zinb_elem(Y, mu, o["dispersion"].expand_as(mu), o["pi"].expand_as(mu), self.ridge).sum()
+        return nb_elem(Y, mu, o["dispersion"].expand_as(mu)).sum()
+
+    def _n_elem(self, Y):
+        """The loss is a mean over this many elements (poisson: the non-NaN targets, at least one)."""
+        if self.ae_type == "poisson":
+            return poisson_elem_sum_and_count(Y, torch.ones_like(Y))[1]
+        return Y.numel()
 
     def loss(self, X, Y, sf, training=True):
         o = self.forward(X, sf, training)
-        mu = o["mean"]
-        if self.ae_type == "normal":
-            l = ((mu - Y) ** 2).mean()                                   # keras mean_squared_error + batch mean
-        elif self.ae_type == "poisson":
-            s, n = poisson_elem_sum_and_count(Y, mu); l = s / n
-        elif "pi" in o:
-            l = zinb_elem(Y, mu, o["dispersion"].expand_as(mu), o["pi"].expand_as(mu), self.ridge).mean()
-        else:
-            l = nb_elem(Y, mu, o["dispersion"].expand_as(mu)).mean()
-        return l, o["stats"]
+        return self._loss_sum(o, Y) / self._n_elem(Y), o["stats"]
+
+    def _grads(self):
+        return {k: (self.p[k].grad.detach().clone() if self.p[k].grad is not None else torch.zeros_like(self.p[k]))
+                for k in self.train_keys}
 
     def loss_and_grads(self, X, Y, sf):
         for k in self.train_keys:
             self.p[k].grad = None
         loss, stats = self.loss(X, Y, sf, True)
         loss.backward()
-        return float(loss.detach()), {k: (self.p[k].grad.detach().clone() if self.p[k].grad is not None else torch.zeros_like(self.p[k]))
-                                      for k in self.train_keys}, stats
+        return float(loss.detach()), self._grads(), stats
+
+    def loss_and_grads_chunked(self, X, Y, sf, chunk=256):
+        """loss_and_grads with the heads and the loss evaluated ``chunk`` rows at a time, so that the autograd graph of
+        the B x G head and loss tensors exists for one chunk only.  The hidden stack runs on the whole batch (BatchNorm
+        needs the batch statistics); its outputs become leaves whose gradient the chunks accumulate, and that gradient
+        is then backpropagated through the stack once.  Same mean loss and gradients as loss_and_grads."""
+        for k in self.train_keys:
+            self.p[k].grad = None
+        ins, _, stats = self.hidden_stack(X, True)
+        leaves = {}                                       # one leaf per distinct tensor (branches may share the trunk)
+        for v in ins.values():
+            if id(v) not in leaves:
+                leaves[id(v)] = (v, v.detach().requires_grad_(True))
+        lins = {br: leaves[id(v)][1] for br, v in ins.items()}
+        n = self._n_elem(Y)
+        total = 0.0
+        for s in range(0, X.shape[0], chunk):
+            o = self.heads({br: v[s:s + chunk] for br, v in lins.items()}, sf[s:s + chunk])
+            part = self._loss_sum(o, Y[s:s + chunk])
+            (part / n).backward()
+            total += float(part.detach())
+        outs = [(v, leaf.grad) for v, leaf in leaves.values() if v.requires_grad and leaf.grad is not None]
+        if outs:
+            torch.autograd.backward([v for v, _ in outs], [g for _, g in outs])
+        return total / float(n), self._grads(), stats
 
     _apply = None
 
@@ -235,19 +284,19 @@ class TorchExtraNet:
     @torch.no_grad()
     def predict(self, X, sf):
         o = self.forward(X, sf, False)
-        return {k: v.detach().numpy() for k, v in o.items() if k != "stats" and v is not None}
+        return {k: v.detach().cpu().numpy() for k, v in o.items() if k != "stats" and v is not None}
 
 
 class TorchRefNet:
     """Same parameter names / layouts as oracle.dca_oracle.OracleNet."""
 
     def __init__(self, params: Dict[str, "torch.Tensor"], hidden: Sequence[int], ae_type: str,
-                 batchnorm=True, ridge=0.0, dtype=torch.float32, activation="relu"):
+                 batchnorm=True, ridge=0.0, dtype=torch.float32, activation="relu", device="cpu"):
         self.hidden = tuple(hidden); self.ae_type = ae_type; self.batchnorm = batchnorm
-        self.ridge = ridge; self.dtype = dtype; self.activation = activation
+        self.ridge = ridge; self.dtype = dtype; self.activation = activation; self.device = torch.device(device)
         self.masks = {}; self.rates = {}      # dropout: layer id (-1 input, i hidden) -> keep mask / rate
         self.names = layer_names(len(self.hidden)); self.heads = head_names(ae_type)
-        self.p = {k: torch.as_tensor(v).to(dtype).clone() for k, v in params.items()}
+        self.p = {k: torch.as_tensor(v).to(self.device, dtype).clone() for k, v in params.items()}
         self.train_keys = [k for k in self.p if k.endswith(("/kernel", "/bias", "/bn_beta", "/theta", "_act/alpha"))]
         for k in self.train_keys:
             self.p[k].requires_grad_(True)
@@ -255,12 +304,19 @@ class TorchRefNet:
         self.mom = KERAS_DEFAULTS["bn_momentum"]; self.bn_eps = KERAS_DEFAULTS["bn_eps"]
 
     def forward(self, X, sf, training=True):
-        h = X
+        h, stats, _ = self.hidden_stack(X, training)
+        return self.head_outputs(h, sf) + (stats,)
+
+    def hidden_stack(self, X, training=True):
+        """(last hidden activation, BatchNorm batch statistics, latent: the pre-BatchNorm output of 'center')."""
+        h = X; latent = None
         if training and -1 in self.masks:
             h = apply_dropout(h, self.masks[-1], self.rates[-1])
         stats = []
         for i, nm in enumerate(self.names):
             a = h @ self.p[nm + "/kernel"] + self.p[nm + "/bias"]
+            if nm == "center":
+                latent = a
             if self.batchnorm:
                 if training:
                     mean = a.mean(0); var = a.var(0, unbiased=False)
@@ -271,6 +327,10 @@ class TorchRefNet:
             h = hidden_activation(self.activation, a, self.p.get(nm + "_act/alpha"))
             if training and i in self.masks:
                 h = apply_dropout(h, self.masks[i], self.rates[i])
+        return h, stats, latent
+
+    def head_outputs(self, h, sf):
+        """(mu, theta, pi) of the rows of h; theta is [1 x G] for the per-gene dispersion types, pi None for NB."""
         z = {nm: h @ self.p[nm + "/kernel"] + self.p[nm + "/bias"] for nm in self.heads}
         m = torch.clamp(torch.exp(z["mean"]), 1e-5, 1e6)
         mu = m * sf.reshape(-1, 1)
@@ -279,16 +339,15 @@ class TorchRefNet:
         else:
             theta = torch.clamp(torch.exp(self.p["dispersion/theta"]), 1e-3, 1e4).reshape(1, -1)
         pi = torch.sigmoid(z["pi"]) if "pi" in z else None
-        return mu, theta, pi, stats
+        return mu, theta, pi
+
+    def _elem(self, Y, mu, theta, pi):
+        theta = theta.expand_as(mu)
+        return zinb_elem(Y, mu, theta, pi, self.ridge) if pi is not None else nb_elem(Y, mu, theta)
 
     def loss(self, X, Y, sf, training=True):
         mu, theta, pi, stats = self.forward(X, sf, training)
-        theta = theta.expand_as(mu)
-        if pi is not None:
-            el = zinb_elem(Y, mu, theta, pi, self.ridge)
-        else:
-            el = nb_elem(Y, mu, theta)
-        return el.mean(), stats
+        return self._elem(Y, mu, theta, pi).mean(), stats
 
     def loss_and_grads(self, X, Y, sf):
         for k in self.train_keys:
@@ -296,6 +355,29 @@ class TorchRefNet:
         loss, stats = self.loss(X, Y, sf, True)
         loss.backward()
         return float(loss.detach()), {k: self.p[k].grad.detach().clone() for k in self.train_keys}, stats
+
+    def loss_and_grads_chunked(self, X, Y, sf, chunk=256):
+        """loss_and_grads with the heads and the loss evaluated ``chunk`` rows at a time, so that the autograd graph of
+        the B x G head and loss tensors exists for one chunk only (a 4096 x 20000 float64 ZINB graph in one piece
+        holds tens of GB).  The hidden stack runs on the whole batch (BatchNorm needs the batch statistics); its last
+        activation becomes a leaf whose gradient the chunks accumulate, and that gradient is then backpropagated
+        through the stack once.  Same mean loss and gradients as loss_and_grads."""
+        for k in self.train_keys:
+            self.p[k].grad = None
+        h, stats, _ = self.hidden_stack(X, True)
+        leaf = h.detach().requires_grad_(True)
+        n = Y.numel()
+        total = 0.0
+        for s in range(0, X.shape[0], chunk):
+            mu, theta, pi = self.head_outputs(leaf[s:s + chunk], sf[s:s + chunk])
+            part = self._elem(Y[s:s + chunk], mu, theta, pi).sum()
+            (part / n).backward()
+            total += float(part.detach())
+        if h.requires_grad:
+            h.backward(leaf.grad)
+        grads = {k: (self.p[k].grad.detach().clone() if self.p[k].grad is not None else torch.zeros_like(self.p[k]))
+                 for k in self.train_keys}
+        return total / n, grads, stats
 
     @torch.no_grad()
     def _apply(self, grads, stats, lr, clip):
