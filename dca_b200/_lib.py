@@ -114,6 +114,7 @@ PROTOTYPES = {
     "dca_zinb_elem_host": (C.c_int, [_i32, _f, _f, _f, _f, _f, _f, C.POINTER(_f * 4)]),
     "dca_dropout_mask_host": (C.c_int, [C.c_uint64, C.c_uint64, _i32, _i64, _f, _vp]),
     "dca_activation_host": (C.c_int, [_i32, _f, _f, C.POINTER(_f * 2)]),
+    "dca_activation_bwd_host": (C.c_int, [_i32, _f, _f, _f, _i32, _f, C.POINTER(_f * 2)]),
     "dca_dense_heads_fwd": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                       _vp, _vp, _vp, _i64, _vp]),
     "dca_tc_heads_fwd": (C.c_int, [_vp, _i32, _vp, _vp, _i32, _i32, C.POINTER(_i32 * 3), _vp, _vp, _vp, _vp, _i64, _vp]),

@@ -49,22 +49,23 @@ __global__ void act_bwd_kernel(float* __restrict__ dh, const float* __restrict__
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)M * N) return;
   const int r = (int)(i / N), c = (int)(i % N);
-  float g = dh[i];
+  const float g = dh[i];
+  const float rate = stage == 0 ? sp.rate : 0.f;
   bool kept = true;
-  if (sp.rate > 0.f && stage == 0) {
-    const uint64_t key = act::drop_key(sp.seed, *sp.step, sp.layer);
-    kept = act::drop_keep(key, (uint64_t)i, sp.thr);
-    g = kept ? g * sp.inv_keep : 0.f;
-  }
+  if (rate > 0.f) kept = act::drop_keep(act::drop_key(sp.seed, *sp.step, sp.layer), (uint64_t)i, sp.thr);
   if (sp.kind == DCA_ACT_PRELU) {
     const float x = xhat ? xhat[i] + beta[c] : a[(int64_t)r * ld + c];
-    if (stage == 0) { dh[i] = g; scr[i] = fminf(x, 0.f); return; }
-    dh[i] = g * act::deriv(DCA_ACT_PRELU, 0.f, x, sp.alpha[c]);
+    if (stage == 0) {                                        // dropout only: the slope gradient reads this dh
+      dh[i] = act::bwd_elem(DCA_ACT_LINEAR, g, 0.f, 0.f, 0.f, rate, sp.keep, sp.inv_keep, kept);
+      scr[i] = fminf(x, 0.f);
+      return;
+    }
+    dh[i] = act::bwd_elem(DCA_ACT_PRELU, g, 0.f, x, sp.alpha[c], 0.f, 1.f, 1.f, true);
     return;
   }
-  // the stored h is the dropped, rescaled activation: undo the scale where the element was kept
-  const float hv = sp.rate > 0.f ? h[i] * sp.keep : h[i];
-  dh[i] = kept ? g * act::deriv(sp.kind, hv, 0.f, 0.f) : 0.f;
+  // hard_sigmoid takes its derivative from the pre-activation, not from the rescaled stored h (act::bwd_elem)
+  const float x = sp.kind != DCA_ACT_HARD_SIGMOID ? 0.f : xhat ? xhat[i] + beta[c] : a[(int64_t)r * ld + c];
+  dh[i] = act::bwd_elem(sp.kind, g, h[i], x, 0.f, rate, sp.keep, sp.inv_keep, kept);
 }
 
 __device__ __forceinline__ float elem_to_f(float v) { return v; }
@@ -179,5 +180,14 @@ extern "C" int dca_activation_host(int32_t act, float x, float alpha, float out[
   if (!out || act < DCA_ACT_RELU || act > DCA_ACT_PRELU) return DCA_ERR_BAD_ARG;
   out[0] = dca::act::value(act, x, alpha);
   out[1] = dca::act::deriv(act, out[0], x, alpha);
+  return DCA_OK;
+}
+
+extern "C" int dca_activation_bwd_host(int32_t act, float x, float alpha, float rate, int32_t kept, float g, float out[2]) {
+  if (!out || act < DCA_ACT_RELU || act > DCA_ACT_PRELU || !(rate >= 0.f && rate < 1.f)) return DCA_ERR_BAD_ARG;
+  const float keep = 1.f - rate, inv_keep = 1.f / keep;
+  const float v = dca::act::value(act, x, alpha);
+  out[0] = rate > 0.f ? (kept ? v * inv_keep : 0.f) : v;                    // the stored output, as act_fwd_kernel writes it
+  out[1] = dca::act::bwd_elem(act, g, out[0], x, alpha, rate, keep, inv_keep, rate <= 0.f || kept != 0);
   return DCA_OK;
 }

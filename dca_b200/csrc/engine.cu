@@ -1067,7 +1067,7 @@ int Engine::stream_prefetch(int64_t i, int b, int e) {
   // expansion on its own low-priority stream: the next copy does not queue behind it, the step's kernels go first
   DCA_CUDA_OK(cudaStreamWaitEvent(hs.expand, hs.h2d_done[b], 0));
   DCA_CUDA_OK(cudaStreamWaitEvent(hs.expand, hs.step_done[e], 0));       // the step that read the expanded buffers b has finished
-  const int x_bf16 = tc_enc ? 1 : (cfg.x_dtype == DCA_BF16);
+  const int x_bf16 = expand_bf16();
   int max_nib = 0;                       // longest nibble run of a row of this batch (host CSR): sizes the expansion's smem
   if (sparse) for (int64_t r = r0; r < r0 + nb; ++r) { const int len = (int)(hs.nib_indptr[r + 1] - hs.nib_indptr[r]); if (len > max_nib) max_nib = len; }
   const ExactXform ex{reinterpret_cast<const double*>(base + o_ncst[b]), tf_median, tf_flags,
@@ -1269,7 +1269,7 @@ int stream_run(dca_handle* h, const char* who, int64_t i, int64_t next, void* st
   static const int diag = [] { const char* v = getenv("DCA_STREAM_DIAG"); return v ? atoi(v) : 0; }();
   int st = DCA_OK;
   if (diag != 1) {                                  // (1 = diagnosis: copies + expansion only)
-    e.x_override_bf16 = e.tc_enc ? 1 : 0;           // the tensor-core encoder reads the expanded bf16 batch in place
+    e.x_override_bf16 = e.expand_bf16();           // the element type stream_prefetch expanded the batch in
     st = body(e, xb, nb, s);
     e.x_override_bf16 = 0;
   }
@@ -1456,9 +1456,9 @@ int packed_run(dca_handle* h, const char* who, const dca_packed_counts* src, con
   cudaStream_t s = (cudaStream_t)stream;
   const ExactXform ex{src->n_counts, e.tf_median, e.tf_flags, reinterpret_cast<const double*>(e.base + e.o_gmean64),
                       reinterpret_cast<const double*>(e.base + e.o_gstd64), e.f(e.o_gx0)};
-  const int x_bf16 = e.tc_enc ? 1 : (e.cfg.x_dtype == DCA_BF16);
+  const int x_bf16 = e.expand_bf16();
   DCA_TRY(expand_packed_rows(src, rows, batch, ex, e.f(e.o_sy[0]), e.base + e.o_sx[0], x_bf16, e.f(e.o_ssf[0]), s));
-  e.x_override_bf16 = e.tc_enc ? 1 : 0;             // the tensor-core encoder reads the expanded bf16 batch in place
+  e.x_override_bf16 = x_bf16;
   const int st = body(e, batch, s);
   e.x_override_bf16 = 0;
   return st;

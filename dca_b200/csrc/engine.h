@@ -77,6 +77,10 @@ struct Engine {
     void tl_mark(cudaStream_t st) { cudaEvent_t e; if (cudaEventCreate(&e) == cudaSuccess) { cudaEventRecord(e, st); tl.push_back(e); } }
   } hs;
   int stream_prefetch(int64_t i, int raw_buf, int exp_buf);
+  // element type of an expanded batch (host stream, packed counts): bf16 when X is stored in bf16, or when the
+  // tensor-core encoder can read it in place.  fp32 X with input dropout stays fp32, so that the mask scales the fp32 value
+  // and the encoder's gather rounds it once, bf16(x * inv_keep), as on a resident fp32 X
+  int expand_bf16() const { return cfg.x_dtype == DCA_BF16 || (tc_enc && !(cfg.input_dropout > 0.f)); }
   // optional phase timing
   struct Prof {
     bool on = false;

@@ -403,9 +403,13 @@ int dca_zinb_elem_host(int32_t ae_type, float y, float m, float sf, float d, flo
  * dca_dropout_mask_host writes the keep mask (1 = kept) the device applies at training step `step` (1 for the first
  * dca_train_step after dca_create) to elements [0, n) of `layer` (hidden layer index; -1 = the input; fork branches
  * use DCA_MAX_HIDDEN + branch); kept values are scaled by 1 / (1 - rate) as keras.layers.Dropout does.
- * dca_activation_host evaluates activation `act` (value and derivative; PReLU with slope `alpha`). */
+ * dca_activation_host evaluates activation `act` (value and derivative; PReLU with slope `alpha`).
+ * dca_activation_bwd_host runs one element of a training step through activation + dropout at `rate` (0: none) with
+ * keep flag `kept`: out[0] = the stored layer output, out[1] = the gradient w.r.t. the activation's input x given the
+ * gradient g w.r.t. the layer's output. */
 int dca_dropout_mask_host(uint64_t seed, uint64_t step, int32_t layer, int64_t n, float rate, uint8_t* keep);
 int dca_activation_host(int32_t act, float x, float alpha, float out[2]);
+int dca_activation_bwd_host(int32_t act, float x, float alpha, float rate, int32_t kept, float g, float out[2]);
 
 /* Head Dense layers with fused output activations (dca/network.py:369-381, :38-39,
  * dca/layers.py:85): H (B x K float32, ld ldh) times the Keras-layout kernels (K x G) plus bias,

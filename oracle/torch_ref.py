@@ -43,6 +43,37 @@ def hidden_activation(name, x, alpha=None):
     raise ValueError(name)
 
 
+def bf16_round(t):
+    """Round-to-nearest-even to bfloat16 of t's float32 value, returned in t's dtype (dca_oracle.bf16_round)."""
+    return t.to(torch.float32).to(torch.bfloat16).to(t.dtype)
+
+
+class RoundOperand(torch.autograd.Function):
+    """A tensor-core GEMM operand: rounded to bf16 going forward; the gradient passes straight through to the fp32
+    tensor it was rounded from (the engine keeps fp32 masters and activations)."""
+
+    @staticmethod
+    def forward(ctx, x):
+        return bf16_round(x)
+
+    @staticmethod
+    def backward(ctx, g):
+        return g
+
+
+class RoundGrad(torch.autograd.Function):
+    """Identity going forward; the gradient arriving here is rounded to bf16, as the engine rounds dZ and dA of the
+    first layer before the tensor-core GEMMs read them."""
+
+    @staticmethod
+    def forward(ctx, x):
+        return x.view_as(x)
+
+    @staticmethod
+    def backward(ctx, g):
+        return bf16_round(g)
+
+
 def apply_dropout(x, mask, rate):
     """keras.layers.Dropout in training mode with the mask handed in: x * mask / (1 - rate)  (dca/network.py:98-99,137-138)."""
     return x * mask.to(x.dtype).reshape(x.shape) / (1.0 - rate)
@@ -288,10 +319,18 @@ class TorchExtraNet:
 
 
 class TorchRefNet:
-    """Same parameter names / layouts as oracle.dca_oracle.OracleNet."""
+    """Same parameter names / layouts as oracle.dca_oracle.OracleNet.
+
+    emulate_bf16 ("both" | "encoder" | "heads" | "none", True / False = "both" / "none") has OracleNet's meaning: the
+    same-rounding statement of the tensor-core path (DESIGN section 3).  "encoder" rounds X (after input dropout) and the
+    first kernel going forward and dA of the first layer going backward; "heads" rounds the last hidden activation
+    (after dropout) and the head kernels going forward and dZ going backward.  Everything else stays in ``dtype``."""
 
     def __init__(self, params: Dict[str, "torch.Tensor"], hidden: Sequence[int], ae_type: str,
-                 batchnorm=True, ridge=0.0, dtype=torch.float32, activation="relu", device="cpu"):
+                 batchnorm=True, ridge=0.0, dtype=torch.float32, activation="relu", device="cpu", emulate_bf16=False):
+        side = {True: "both", False: "none"}.get(emulate_bf16, emulate_bf16)
+        assert side in ("both", "none", "encoder", "heads"), emulate_bf16
+        self.rnd_enc = side in ("both", "encoder"); self.rnd_heads = side in ("both", "heads")
         self.hidden = tuple(hidden); self.ae_type = ae_type; self.batchnorm = batchnorm
         self.ridge = ridge; self.dtype = dtype; self.activation = activation; self.device = torch.device(device)
         self.masks = {}; self.rates = {}      # dropout: layer id (-1 input, i hidden) -> keep mask / rate
@@ -311,10 +350,21 @@ class TorchRefNet:
         """(last hidden activation, BatchNorm batch statistics, latent: the pre-BatchNorm output of 'center')."""
         h = X; latent = None
         if training and -1 in self.masks:
-            h = apply_dropout(h, self.masks[-1], self.rates[-1])
+            if self.rnd_enc:
+                # the device scales fp32 X by fp32(1 / keep) and rounds that product to bf16: a 1-ulp difference in the
+                # scale would move ~2^-16 of the elements across a bf16 rounding boundary, by 2^-8 of their value.  The
+                # product of two fp32 values is exact in float64; its float32 rounding is the device's product.
+                one = torch.tensor(1.0, dtype=torch.float32)
+                inv_keep = float(one / (one - torch.tensor(self.rates[-1], dtype=torch.float32)))
+                h = (h * self.masks[-1].to(h.dtype).reshape(h.shape) * inv_keep).to(torch.float32).to(h.dtype)
+            else:
+                h = apply_dropout(h, self.masks[-1], self.rates[-1])
         stats = []
         for i, nm in enumerate(self.names):
-            a = h @ self.p[nm + "/kernel"] + self.p[nm + "/bias"]
+            if i == 0 and self.rnd_enc:
+                a = RoundGrad.apply(RoundOperand.apply(h) @ RoundOperand.apply(self.p[nm + "/kernel"])) + self.p[nm + "/bias"]
+            else:
+                a = h @ self.p[nm + "/kernel"] + self.p[nm + "/bias"]
             if nm == "center":
                 latent = a
             if self.batchnorm:
@@ -331,7 +381,11 @@ class TorchRefNet:
 
     def head_outputs(self, h, sf):
         """(mu, theta, pi) of the rows of h; theta is [1 x G] for the per-gene dispersion types, pi None for NB."""
-        z = {nm: h @ self.p[nm + "/kernel"] + self.p[nm + "/bias"] for nm in self.heads}
+        if self.rnd_heads:
+            hr = RoundOperand.apply(h)
+            z = {nm: RoundGrad.apply(hr @ RoundOperand.apply(self.p[nm + "/kernel"]) + self.p[nm + "/bias"]) for nm in self.heads}
+        else:
+            z = {nm: h @ self.p[nm + "/kernel"] + self.p[nm + "/bias"] for nm in self.heads}
         m = torch.clamp(torch.exp(z["mean"]), 1e-5, 1e6)
         mu = m * sf.reshape(-1, 1)
         if "dispersion" in z:

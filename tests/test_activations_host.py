@@ -94,3 +94,44 @@ def test_dropout_mask_known_answers():
         m = _mask(lib, seed, step, layer, 64, rate)
         got = sum(int(b) << i for i, b in enumerate(m))
         assert got == want, (seed, step, layer, rate, hex(got))
+
+
+def _bwd(lib, name, x, rate, kept, g=1.0, alpha=0.0):
+    out = (C.c_float * 2)()
+    assert lib.dca_activation_bwd_host(_lib.ACTIVATION_IDS[name], C.c_float(x), C.c_float(alpha), C.c_float(rate), kept,
+                                       C.c_float(g), C.byref(out)) == 0
+    return out[0], out[1]
+
+
+@pytest.mark.parametrize("rate", [0.01, 0.11, 0.15, 0.23, 0.77])
+def test_saturated_hard_sigmoid_has_no_gradient_under_dropout(rate):
+    """hard_sigmoid is flat outside (-2.5, 2.5).  At these rates the stored output of a saturated, kept unit times keep
+    is 1 - 2^-24 in fp32, not 1: the backward element must take the slope from the input, not from that value."""
+    lib = _lib.load()
+    keep = np.float32(1) - np.float32(rate)
+    assert (np.float32(1) / keep) * keep != np.float32(1)              # the rounding this case is about
+    for x in (2.6, 3.0, 7.5, -2.6, -9.0):
+        h, dx = _bwd(lib, "hard_sigmoid", x, rate, 1, g=0.75)
+        assert h == np.float32(1) / keep if x > 0 else h == 0.0, (x, h)
+        assert dx == 0.0, (rate, x, dx)
+    for x in (-2.4, -0.3, 0.0, 1.1, 2.4):                              # the linear part: 0.2 g / keep
+        h, dx = _bwd(lib, "hard_sigmoid", x, rate, 1, g=0.75)
+        assert dx == pytest.approx(0.2 * 0.75 / (1 - rate), rel=1e-6), (rate, x, dx)
+        assert _bwd(lib, "hard_sigmoid", x, rate, 0, g=0.75) == (0.0, 0.0)      # dropped
+
+
+@pytest.mark.parametrize("name", sorted(_lib.ACTIVATION_IDS))
+def test_backward_element_matches_autograd_through_dropout(name):
+    """dca_activation_bwd_host (the element act_bwd_kernel computes) against autograd of dropout(act(x)) in float64."""
+    lib = _lib.load()
+    xs = np.array([-4.0, -2.6, -1.3, -0.2, 0.3, 1.7, 2.6, 4.5], np.float32)
+    alpha = 0.17
+    for rate in (0.0, 0.11, 0.77):
+        for kept in (1, 0) if rate > 0 else (1,):
+            for x in xs:
+                t = torch.tensor(float(x), dtype=torch.float64, requires_grad=True)
+                y = hidden_activation(name, t, torch.tensor(alpha, dtype=torch.float64)) * kept / (1.0 - rate)
+                (gref,) = torch.autograd.grad(y * 0.6, t)
+                h, dx = _bwd(lib, name, float(x), rate, kept, g=0.6, alpha=alpha)
+                assert abs(h - float(y)) <= 2e-6 * max(1.0, abs(float(y))), (name, rate, kept, x, h, float(y))
+                assert abs(dx - float(gref)) <= 3e-6 * max(1.0, abs(float(gref))), (name, rate, kept, x, dx, float(gref))

@@ -75,3 +75,33 @@ def test_chunked_extra_reference_equals_unchunked(ae_type, B):
     l2, g2, _ = TorchExtraNet(p0, HIDDEN, ae_type, True, ridge=0.02).loss_and_grads_chunked(T(X), T(Y), T(sf), chunk=16)
     assert np.isfinite(l1) and abs(l2 - l1) <= 1e-12 * abs(l1)
     _assert_grads_close({k: v.numpy() for k, v in g2.items()}, {k: v.numpy() for k, v in g1.items()}, 1e-12, ae_type)
+
+
+@pytest.mark.parametrize("side", ["both", "encoder", "heads", "none"])
+@pytest.mark.parametrize("batchnorm", [True, False])
+@pytest.mark.parametrize("ae_type", ["zinb-conddisp", "nb"])
+def test_same_rounding_reference_equals_oracle(ae_type, batchnorm, side):
+    """TorchRefNet(emulate_bf16=side), the same-rounding reference of the tensor-core path for every activation and
+    dropout, rounds exactly where OracleNet(emulate_bf16=side)'s closed form does for relu models: the same loss and
+    gradients, in one piece and in row chunks.  The rounding is visible: "both" is far from the exact statement."""
+    G, B = 48, 70
+    X, Y, sf = _problem(B, G, 9)
+    p0 = _nontrivial(O.init_params(G, G, HIDDEN, ae_type, batchnorm, seed=3, dtype=np.float64), 4)
+    net = O.OracleNet(G, G, HIDDEN, ae_type, batchnorm, dtype=np.float64, params=p0, emulate_bf16=side)
+    oloss, og = net.loss_and_grads(X, Y, sf, update_bn=False)
+    T = lambda a: torch.tensor(a, dtype=torch.float64)
+    ref = TorchRefNet(p0, HIDDEN, ae_type, batchnorm, dtype=torch.float64, emulate_bf16=side)
+    for tag, (loss, g, _) in (("one piece", ref.loss_and_grads(T(X), T(Y), T(sf))),
+                              ("chunked", ref.loss_and_grads_chunked(T(X), T(Y), T(sf), chunk=16))):
+        assert abs(loss - oloss) <= 1e-10 * abs(oloss), (side, tag, loss, oloss)
+        # hidden biases in front of a BatchNorm are zero in exact arithmetic: the two float64 evaluations leave ~1e-17
+        floor = 1e-4 * max(float(np.max(np.abs(v))) for v in og.values())
+        assert set(g) == set(og), tag
+        for k, w in og.items():
+            err = float(np.max(np.abs(g[k].numpy().reshape(w.shape) - w)))
+            assert err <= 1e-10 * max(float(np.max(np.abs(w))), floor), (side, tag, k, err)
+    if side == "both":
+        exact = TorchRefNet(p0, HIDDEN, ae_type, batchnorm, dtype=torch.float64)
+        _, ge, _ = exact.loss_and_grads(T(X), T(Y), T(sf))
+        diff = max(float((ge[k] - g[k]).abs().max() / ge[k].abs().max()) for k in ("enc0/kernel", "mean/kernel"))
+        assert diff > 1e-4, diff
