@@ -138,6 +138,11 @@ PROTOTYPES = {
     "dca_format_fixed6_host": (C.c_int, [_vp, _i64, _vp, _vp]),
     "dca_read_text_counts": (C.c_int, [C.c_char_p, _i32, _i32, _i64, _i32, _vp, _vp, _i64, _vp, _vp, _i64, _vp]),
     "dca_read_mtx_counts": (C.c_int, [C.c_char_p, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "dca_read_text_counts_gz": (C.c_int, [C.c_char_p, _i32, _i32, _i64, _i32, _vp, _vp, _i64, _vp, _vp, _i64, _vp]),
+    "dca_read_mtx_counts_gz": (C.c_int, [C.c_char_p, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "dca_gunzip": (C.c_int, [C.c_char_p, _i32, _vp, _vp, _i64, _vp]),
+    "dca_inflate_span_host": (C.c_int, [_vp, _i64, _i32, _i64, _i64, _vp, _i64, _vp]),
+    "dca_inflate_find_host": (C.c_int, [_vp, _i64, _i64, _i64, _vp]),
     "dca_count_escapes": (C.c_int, [_vp, _i32, _i64, _i64, _i64, _vp, _i32]),
     "dca_pack_counts": (C.c_int, [_vp, _i32, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _i32]),
     "dca_sparse_counts": (C.c_int, [_vp, _i32, _i64, _i64, _i64, _vp, _vp, _i32]),

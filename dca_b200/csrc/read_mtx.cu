@@ -130,12 +130,12 @@ struct Buffers : ChunkBuffers {
 };
 
 struct Reader {
-  int fd = -1;
+  std::unique_ptr<ByteSource> src;
   int prev_device = -1;                // the caller's current device, restored on return
   MtxState* d_state = nullptr;
   Buffers b[2];
   ~Reader() {
-    if (fd >= 0) close(fd);
+    src.reset();
     for (Buffers& x : b) { x.release(); cudaFree(x.keys); cudaFreeHost(x.h_err); }
     cudaFree(d_state);
     if (prev_device >= 0) cudaSetDevice(prev_device);
@@ -158,12 +158,13 @@ bool header_number(const std::string& h, size_t* p, long long* v) {
 }
 
 // The banner, the '%' comment lines and the size line "M N NNZ", read on the host.
-int read_header(int fd, Header* hd) {
+int read_header(const char* who, ByteSource& src, Header* hd) {
   static const char* kBanner[2] = {"%%MatrixMarket matrix coordinate integer general",
                                    "%%MatrixMarket matrix coordinate real general"};
   std::string h;
   unsigned char tmp[65536];
   bool eof = false;
+  int status = DCA_OK;                 // of a failed read
   size_t pos = 0;                      // start of the current line
   // the line starting at pos without its line end; false at the end of the file without one
   auto line = [&](size_t* end, size_t* next) -> int {
@@ -171,19 +172,19 @@ int read_header(int fd, Header* hd) {
       const size_t nl = h.find('\n', pos);
       if (nl != std::string::npos) { *next = nl + 1; *end = nl > pos && h[nl - 1] == '\r' ? nl - 1 : nl; return 1; }
       if (eof) { *end = *next = h.size(); return 0; }
-      const long long r = read_full(fd, tmp, sizeof(tmp));
-      if (r < 0) { set_error("dca_read_mtx_counts: read failed"); return -1; }
+      const long long r = src.read(tmp, sizeof(tmp));
+      if (r < 0) { status = (int)r; return -1; }
       eof = r < (long long)sizeof(tmp);
       h.append((const char*)tmp, (size_t)r);
     }
   };
-  auto unsupported = [](const char* what) {
-    set_error("dca_read_mtx_counts: unsupported file: %s", what);
+  auto unsupported = [who](const char* what) {
+    set_error("%s: unsupported file: %s", who, what);
     return DCA_ERR_UNSUPPORTED;
   };
   size_t end = 0, next = 0;
   int st = line(&end, &next);
-  if (st < 0) return DCA_ERR_BAD_ARG;
+  if (st < 0) return status;
   const std::string banner = h.substr(0, end);
   if (banner == kBanner[0]) hd->max_digits = kMaxIntDigits;
   else if (banner == kBanner[1]) hd->max_digits = kMaxRealDigits;
@@ -192,7 +193,7 @@ int read_header(int fd, Header* hd) {
     if (!st) return unsupported("no size line");
     pos = next;
     st = line(&end, &next);
-    if (st < 0) return DCA_ERR_BAD_ARG;
+    if (st < 0) return status;
     if (pos < h.size() && h[pos] == '%') continue;
     break;
   }
@@ -214,44 +215,46 @@ int read_header(int fd, Header* hd) {
 
 using namespace dca;
 
-extern "C" int dca_read_mtx_counts(const char* path, int32_t transpose, int64_t chunk_bytes, int32_t device, void* stream,
-                                   int64_t* indptr, int32_t* indices, float* data, int64_t* info) {
+namespace {
+// both entry points: the file's bytes, or (gz) the inflated bytes of a gzip file
+int read_mtx_counts(const char* who, bool gz, const char* path, int32_t transpose, int64_t chunk_bytes, int32_t device,
+                    void* stream, int64_t* indptr, int32_t* indices, float* data, int64_t* info) {
   const bool fill = indptr != nullptr;
   if (!path || !info || chunk_bytes < 0 || (fill && info[2] > 0 && (!indices || !data))) {
-    set_error("dca_read_mtx_counts: bad argument"); return DCA_ERR_BAD_ARG;
+    set_error("%s: bad argument", who); return DCA_ERR_BAD_ARG;
   }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     (void)cudaGetLastError();
-    set_error("dca_read_mtx_counts: no CUDA device available (this library has no CPU fallback)");
+    set_error("%s: no CUDA device available (this library has no CPU fallback)", who);
     return DCA_ERR_NO_DEVICE;
   }
-  if (device < 0 || device >= ndev) { set_error("dca_read_mtx_counts: no CUDA device %d", device); return DCA_ERR_BAD_ARG; }
+  if (device < 0 || device >= ndev) { set_error("%s: no CUDA device %d", who, device); return DCA_ERR_BAD_ARG; }
   Reader rd;
   DCA_CUDA_OK(cudaGetDevice(&rd.prev_device));
   DCA_CUDA_OK(cudaSetDevice(device));
   cudaStream_t s = (cudaStream_t)stream;
 
-  rd.fd = open(path, O_RDONLY);
-  if (rd.fd < 0) { set_error("dca_read_mtx_counts: cannot open %s", path); return DCA_ERR_BAD_ARG; }
+  DCA_TRY(gz ? open_gzip_source(who, path, &rd.src) : open_file_source(who, path, &rd.src));
   Header hd;
-  DCA_TRY(read_header(rd.fd, &hd));
+  DCA_TRY(read_header(who, *rd.src, &hd));
   const long long rows = transpose ? hd.n : hd.m, cols = transpose ? hd.m : hd.n;
   const ChunkGeometry geo = chunk_geometry(chunk_bytes, 3);      // "i j v": 3 fields
-  if (geo.cap > (1ll << 30)) { set_error("dca_read_mtx_counts: chunk_bytes above 1 GB"); return DCA_ERR_BAD_ARG; }
+  if (geo.cap > (1ll << 30)) { set_error("%s: chunk_bytes above 1 GB", who); return DCA_ERR_BAD_ARG; }
   if (!fill) {
     info[0] = rows;
     info[1] = cols;
     info[2] = hd.nnz;
     // device bytes of the two chunk buffers
-    info[3] = 2 * (geo.padded + 2ll * geo.tiles_cap * 4 + 2ll * geo.max_lines * 4 + 8ll * geo.max_lines);
+    info[3] = 2 * (geo.padded + 2ll * geo.tiles_cap * 4 + 2ll * geo.max_lines * 4 + 8ll * geo.max_lines) +
+              (gz ? gzip_source_device_bytes() : 0);
     return DCA_OK;
   }
   if (info[0] != rows || info[1] != cols || info[2] != hd.nnz) {
-    set_error("dca_read_mtx_counts: unsupported file: its size line changed since the first call");
+    set_error("%s: unsupported file: its size line changed since the first call", who);
     return DCA_ERR_UNSUPPORTED;
   }
-  if (lseek(rd.fd, hd.bytes, SEEK_SET) != hd.bytes) { set_error("dca_read_mtx_counts: seek failed"); return DCA_ERR_BAD_ARG; }
+  DCA_TRY(rd.src->seek(hd.bytes));
 
   DCA_CUDA_OK(cudaMalloc(&rd.d_state, sizeof(MtxState)));
   for (Buffers& x : rd.b) {
@@ -280,7 +283,7 @@ extern "C" int dca_read_mtx_counts(const char* path, int32_t transpose, int64_t 
   };
   // a problem ends the read: the first one in file order is in the chunks read so far
   auto collect = [&](ChunkBuffers& cb) -> int { return *static_cast<Buffers&>(cb).h_err != ~0ull ? 1 : DCA_OK; };
-  DCA_TRY(for_each_chunk("dca_read_mtx_counts", rd.fd, hd.bytes, geo, rd.b[0], rd.b[1], ' ', rd.d_state, s, launch,
+  DCA_TRY(for_each_chunk(who, *rd.src, hd.bytes, geo, rd.b[0], rd.b[1], ' ', rd.d_state, s, launch,
                          collect));
   fill_tail_kernel<<<std::max(1, std::min(1024, cdiv(rows + 1, kThreads))), kThreads, 0, s>>>(
       indptr, rows, hd.nnz, cols, (int)(chunks & 1), rd.d_state);
@@ -290,10 +293,23 @@ extern "C" int dca_read_mtx_counts(const char* path, int32_t transpose, int64_t 
   DCA_CUDA_OK(cudaStreamSynchronize(s));
   int reason = fin.err == ~0ull ? R_NONE : (int)(fin.err & 0xff);
   long long where = fin.err == ~0ull ? 0 : (long long)(fin.err >> 8);
-  if (!reason && fin.lines_done != hd.nnz) { reason = R_FEWER; where = lseek(rd.fd, 0, SEEK_CUR); }
+  if (!reason && fin.lines_done != hd.nnz) { reason = R_FEWER; where = rd.src->tell(); }
   if (reason) {
-    set_error("dca_read_mtx_counts: unsupported file: %s (byte %lld)", reason_text(reason), where);
+    set_error("%s: unsupported file: %s (byte %lld)%s", who, reason_text(reason), where, gz ? " of the inflated stream" : "");
     return DCA_ERR_UNSUPPORTED;
   }
   return DCA_OK;
+}
+}  // namespace
+
+extern "C" int dca_read_mtx_counts(const char* path, int32_t transpose, int64_t chunk_bytes, int32_t device, void* stream,
+                                   int64_t* indptr, int32_t* indices, float* data, int64_t* info) {
+  return read_mtx_counts("dca_read_mtx_counts", false, path, transpose, chunk_bytes, device, stream, indptr, indices, data,
+                         info);
+}
+
+extern "C" int dca_read_mtx_counts_gz(const char* path, int32_t transpose, int64_t chunk_bytes, int32_t device,
+                                      void* stream, int64_t* indptr, int32_t* indices, float* data, int64_t* info) {
+  return read_mtx_counts("dca_read_mtx_counts_gz", true, path, transpose, chunk_bytes, device, stream, indptr, indices,
+                         data, info);
 }

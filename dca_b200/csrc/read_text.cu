@@ -157,7 +157,7 @@ struct Buffers : ChunkBuffers {
 };
 
 struct Reader {
-  int fd = -1;
+  std::unique_ptr<ByteSource> src;
   int prev_device = -1;                // the caller's current device, restored on return
   ReadState* d_state = nullptr;
   Buffers b[2];
@@ -166,7 +166,7 @@ struct Reader {
     if (prev_device >= 0) cudaSetDevice(prev_device);
   }
   void release() {
-    if (fd >= 0) close(fd);
+    src.reset();
     for (Buffers& x : b) {
       x.release();
       cudaFreeHost(x.h_lab); cudaFree(x.label_end); cudaFree(x.stage);
@@ -177,18 +177,18 @@ struct Reader {
 
 // The header line: its byte length (with the line end) and field count; DCA_ERR_UNSUPPORTED for a header pandas would
 // read differently from a plain split (quotes, NUL, a lone '\r') or a file without data lines.
-int read_header(int fd, unsigned char sep, long long* header_bytes, int* fields) {
+int read_header(const char* who, ByteSource& src, unsigned char sep, long long* header_bytes, int* fields) {
   std::string h;
   unsigned char tmp[65536];
   long long nl = -1;
   while (nl < 0) {
-    const long long r = read_full(fd, tmp, sizeof(tmp));
-    if (r < 0) { set_error("dca_read_text_counts: read failed"); return DCA_ERR_BAD_ARG; }
+    const long long r = src.read(tmp, sizeof(tmp));
+    if (r < 0) return (int)r;
     const size_t old = h.size();
     h.append((const char*)tmp, (size_t)r);
     const void* q = memchr(h.data() + old, '\n', (size_t)r);
     if (q) nl = (const char*)q - h.data();
-    else if (r == 0) { set_error("dca_read_text_counts: unsupported file: no data lines"); return DCA_ERR_UNSUPPORTED; }
+    else if (r == 0) { set_error("%s: unsupported file: no data lines", who); return DCA_ERR_UNSUPPORTED; }
   }
   long long end = nl;
   if (end > 0 && h[(size_t)end - 1] == '\r') --end;
@@ -196,7 +196,7 @@ int read_header(int fd, unsigned char sep, long long* header_bytes, int* fields)
   for (long long i = 0; i < end; ++i) {
     const unsigned char c = (unsigned char)h[(size_t)i];
     if (c == '"' || c == 0 || c == '\r') {
-      set_error("dca_read_text_counts: unsupported file: a quote, NUL or carriage return in the header line");
+      set_error("%s: unsupported file: a quote, NUL or carriage return in the header line", who);
       return DCA_ERR_UNSUPPORTED;
     }
     f += c == sep;
@@ -211,42 +211,43 @@ int read_header(int fd, unsigned char sep, long long* header_bytes, int* fields)
 
 using namespace dca;
 
-extern "C" int dca_read_text_counts(const char* path, int32_t sep, int32_t transpose, int64_t chunk_bytes, int32_t device,
-                                    void* stream, float* out, int64_t out_elems, int64_t* label_offsets, char* label_bytes,
-                                    int64_t label_cap, int64_t* info) {
+namespace {
+// both entry points: the file's bytes, or (gz) the inflated bytes of a gzip file
+int read_text_counts(const char* who, bool gz, const char* path, int32_t sep, int32_t transpose, int64_t chunk_bytes,
+                     int32_t device, void* stream, float* out, int64_t out_elems, int64_t* label_offsets,
+                     char* label_bytes, int64_t label_cap, int64_t* info) {
   if (!path || !info || sep <= 0 || sep > 127 || sep == '\n' || sep == '\r' || sep == '"' || chunk_bytes < 0 ||
       (out && (!label_offsets || (label_cap > 0 && !label_bytes)))) {
-    set_error("dca_read_text_counts: bad argument"); return DCA_ERR_BAD_ARG;
+    set_error("%s: bad argument", who); return DCA_ERR_BAD_ARG;
   }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     (void)cudaGetLastError();
-    set_error("dca_read_text_counts: no CUDA device available (this library has no CPU fallback)");
+    set_error("%s: no CUDA device available (this library has no CPU fallback)", who);
     return DCA_ERR_NO_DEVICE;
   }
-  if (device < 0 || device >= ndev) { set_error("dca_read_text_counts: no CUDA device %d", device); return DCA_ERR_BAD_ARG; }
+  if (device < 0 || device >= ndev) { set_error("%s: no CUDA device %d", who, device); return DCA_ERR_BAD_ARG; }
   Reader rd;
   DCA_CUDA_OK(cudaGetDevice(&rd.prev_device));
   DCA_CUDA_OK(cudaSetDevice(device));
   const bool fill = out != nullptr;
   const long long rows_expect = fill ? info[0] : -1;
   if (fill && (info[0] <= 0 || info[1] <= 0 || out_elems < info[0] * info[1] || label_cap < info[2])) {
-    set_error("dca_read_text_counts: the outputs do not match the sizes of the first call"); return DCA_ERR_BAD_ARG;
+    set_error("%s: the outputs do not match the sizes of the first call", who); return DCA_ERR_BAD_ARG;
   }
   cudaStream_t s = (cudaStream_t)stream;
   const unsigned char sp = (unsigned char)sep;
 
-  rd.fd = open(path, O_RDONLY);
-  if (rd.fd < 0) { set_error("dca_read_text_counts: cannot open %s", path); return DCA_ERR_BAD_ARG; }
+  DCA_TRY(gz ? open_gzip_source(who, path, &rd.src) : open_file_source(who, path, &rd.src));
   long long header_bytes = 0; int fields = 0;
-  DCA_TRY(read_header(rd.fd, sp, &header_bytes, &fields));
-  if (fields < 2) { set_error("dca_read_text_counts: unsupported file: no value columns"); return DCA_ERR_UNSUPPORTED; }
+  DCA_TRY(read_header(who, *rd.src, sp, &header_bytes, &fields));
+  if (fields < 2) { set_error("%s: unsupported file: no value columns", who); return DCA_ERR_UNSUPPORTED; }
   const int cols = fields - 1;
-  if (lseek(rd.fd, header_bytes, SEEK_SET) != header_bytes) { set_error("dca_read_text_counts: seek failed"); return DCA_ERR_BAD_ARG; }
+  DCA_TRY(rd.src->seek(header_bytes));
 
   const ChunkGeometry geo = chunk_geometry(chunk_bytes, fields);
   const long long cap = geo.cap, padded = geo.padded;
-  if (cap > (1ll << 30)) { set_error("dca_read_text_counts: chunk_bytes above 1 GB"); return DCA_ERR_BAD_ARG; }
+  if (cap > (1ll << 30)) { set_error("%s: chunk_bytes above 1 GB", who); return DCA_ERR_BAD_ARG; }
   const int tiles_cap = geo.tiles_cap, max_lines = geo.max_lines;
   const bool staged = fill && transpose;
 
@@ -297,9 +298,9 @@ extern "C" int dca_read_text_counts(const char* path, int32_t sep, int32_t trans
     }
     return DCA_OK;
   };
-  DCA_TRY(for_each_chunk("dca_read_text_counts", rd.fd, header_bytes, geo, rd.b[0], rd.b[1], sp, rd.d_state, s, launch,
+  DCA_TRY(for_each_chunk(who, *rd.src, header_bytes, geo, rd.b[0], rd.b[1], sp, rd.d_state, s, launch,
                          collect));
-  const long long file_off = lseek(rd.fd, 0, SEEK_CUR);
+  const long long file_off = rd.src->tell();
 
   ReadState fin;
   DCA_CUDA_OK(cudaMemcpyAsync(&fin, rd.d_state, sizeof(fin), cudaMemcpyDeviceToHost, s));
@@ -307,10 +308,10 @@ extern "C" int dca_read_text_counts(const char* path, int32_t sep, int32_t trans
   int reason = fin.err == ~0ull ? R_NONE : (int)(fin.err & 0xff);
   long long where = fin.err == ~0ull ? 0 : (long long)(fin.err >> 8);
   if (!reason && fin.any_dot && fin.max_val > (1ull << 53)) reason = R_BIG_DOT;
-  if (!reason && rows == 0) { set_error("dca_read_text_counts: unsupported file: no data lines"); return DCA_ERR_UNSUPPORTED; }
+  if (!reason && rows == 0) { set_error("%s: unsupported file: no data lines", who); return DCA_ERR_UNSUPPORTED; }
   if (!reason && fill && rows != rows_expect) { reason = R_ROWS; where = file_off; }
   if (reason) {
-    set_error("dca_read_text_counts: unsupported file: %s (byte %lld)", reason_text(reason), where);
+    set_error("%s: unsupported file: %s (byte %lld)%s", who, reason_text(reason), where, gz ? " of the inflated stream" : "");
     return DCA_ERR_UNSUPPORTED;
   }
   if (fill) label_offsets[rows] = labels;
@@ -318,6 +319,22 @@ extern "C" int dca_read_text_counts(const char* path, int32_t sep, int32_t trans
   info[1] = cols;
   info[2] = labels;
   // device bytes of the two chunk buffers (with the transpose stage of the second call)
-  info[3] = 2 * (padded + 2ll * tiles_cap * 4 + 3ll * max_lines * 4 + (transpose ? (long long)max_lines * cols * 4 : 0));
+  info[3] = 2 * (padded + 2ll * tiles_cap * 4 + 3ll * max_lines * 4 + (transpose ? (long long)max_lines * cols * 4 : 0)) +
+            (gz ? gzip_source_device_bytes() : 0);
   return DCA_OK;
+}
+}  // namespace
+
+extern "C" int dca_read_text_counts(const char* path, int32_t sep, int32_t transpose, int64_t chunk_bytes, int32_t device,
+                                    void* stream, float* out, int64_t out_elems, int64_t* label_offsets, char* label_bytes,
+                                    int64_t label_cap, int64_t* info) {
+  return read_text_counts("dca_read_text_counts", false, path, sep, transpose, chunk_bytes, device, stream, out, out_elems,
+                          label_offsets, label_bytes, label_cap, info);
+}
+
+extern "C" int dca_read_text_counts_gz(const char* path, int32_t sep, int32_t transpose, int64_t chunk_bytes,
+                                       int32_t device, void* stream, float* out, int64_t out_elems,
+                                       int64_t* label_offsets, char* label_bytes, int64_t label_cap, int64_t* info) {
+  return read_text_counts("dca_read_text_counts_gz", true, path, sep, transpose, chunk_bytes, device, stream, out,
+                          out_elems, label_offsets, label_bytes, label_cap, info);
 }

@@ -106,6 +106,35 @@ long long read_full(int fd, unsigned char* dst, long long want) {
   return got;
 }
 
+namespace {
+class FileSource : public ByteSource {
+ public:
+  FileSource(const char* who, int fd) : who_(who), fd_(fd) {}
+  ~FileSource() override { close(fd_); }
+  long long read(unsigned char* dst, long long want) override {
+    const long long got = read_full(fd_, dst, want);
+    if (got < 0) { set_error("%s: read failed", who_); return DCA_ERR_BAD_ARG; }
+    return got;
+  }
+  int seek(long long off) override {
+    if (lseek(fd_, off, SEEK_SET) != off) { set_error("%s: seek failed", who_); return DCA_ERR_BAD_ARG; }
+    return DCA_OK;
+  }
+  long long tell() override { return lseek(fd_, 0, SEEK_CUR); }
+
+ private:
+  const char* who_;
+  int fd_;
+};
+}  // namespace
+
+int open_file_source(const char* who, const char* path, std::unique_ptr<ByteSource>* out) {
+  const int fd = open(path, O_RDONLY);
+  if (fd < 0) { set_error("%s: cannot open %s", who, path); return DCA_ERR_BAD_ARG; }
+  out->reset(new FileSource(who, fd));
+  return DCA_OK;
+}
+
 ChunkGeometry chunk_geometry(long long chunk_bytes, int fields) {
   ChunkGeometry g;
   g.cap = chunk_bytes ? chunk_bytes : kDefaultChunk;
@@ -135,7 +164,7 @@ void ChunkBuffers::release() {
   h_buf = nullptr; h_count = nullptr; d_buf = nullptr; tile_nl = tile_sep = nl_pos = nl_seprank = nullptr;
 }
 
-int for_each_chunk(const char* who, int fd, long long file_off, const ChunkGeometry& g, ChunkBuffers& b0,
+int for_each_chunk(const char* who, ByteSource& src, long long file_off, const ChunkGeometry& g, ChunkBuffers& b0,
                    ChunkBuffers& b1, unsigned char sep, ChunkState* st, cudaStream_t s,
                    const std::function<int(ChunkBuffers&, long long, long long, long long, int)>& launch,
                    const std::function<int(ChunkBuffers&)>& collect) {
@@ -152,8 +181,8 @@ int for_each_chunk(const char* who, int fd, long long file_off, const ChunkGeome
   int cur = 0;
   for (;;) {
     ChunkBuffers& x = *b[cur];
-    const long long got = read_full(fd, x.h_buf + carry, cap - carry);
-    if (got < 0) { set_error("%s: read failed", who); return DCA_ERR_BAD_ARG; }
+    const long long got = src.read(x.h_buf + carry, cap - carry);
+    if (got < 0) return (int)got;
     const long long len = carry + got;
     if (len == 0) break;
     const bool eof = got < cap - carry;

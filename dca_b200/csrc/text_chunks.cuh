@@ -1,7 +1,8 @@
 // Chunked reading of a text file on the device, shared by the GPU readers of count tables (read_text.cu) and of
 // Matrix Market files (read_mtx.cu).
 //
-// The host reads the file in chunks into two pinned staging buffers; a chunk ends at its last '\n' and the partial
+// The host reads the bytes (of the file, or of a gzip file's inflated stream: ByteSource) in chunks into two pinned
+// staging buffers; a chunk ends at its last '\n' and the partial
 // line carries over to the next one, so the disk read of one chunk overlaps the copy and the kernels of the other.
 // Per chunk, on the caller's stream (text_chunks.cu):
 //   tile_count    per 4 KB tile: '\n' and separator counts; flags quotes, NUL bytes and a '\r' without '\n'
@@ -13,6 +14,7 @@
 #include "dca_internal.cuh"
 
 #include <functional>
+#include <memory>
 
 namespace dca {
 namespace chunked {
@@ -83,6 +85,19 @@ __device__ __forceinline__ int count16(const uint4& q, long long p, long long n,
 // read() until `want` bytes or the end of the file: the bytes read, -1 on an error
 long long read_full(int fd, unsigned char* dst, long long want);
 
+// Where a reader's bytes come from: the file (open_file_source), or the inflated stream of a gzip file
+// (open_gzip_source, inflate.cu), whose bytes are inflated on the device segment by segment as they are read.
+struct ByteSource {
+  virtual ~ByteSource() = default;
+  // up to `want` bytes into dst (fewer only at the end); a negative status (message set) on an error or a decline
+  virtual long long read(unsigned char* dst, long long want) = 0;
+  virtual int seek(long long off) = 0;       // to byte `off` of the stream
+  virtual long long tell() = 0;
+};
+int open_file_source(const char* who, const char* path, std::unique_ptr<ByteSource>* out);
+int open_gzip_source(const char* who, const char* path, std::unique_ptr<ByteSource>* out);
+long long gzip_source_device_bytes();        // device memory of a gzip source at most
+
 // chunk sizes of one read: chunk bytes, the padded device buffer, its tiles, and the most lines a chunk may hold when
 // every line has `fields` non-empty fields (at least 2 * fields - 1 bytes besides its '\n'; more is flagged R_LINES)
 struct ChunkGeometry {
@@ -104,12 +119,12 @@ struct ChunkBuffers {
   void release();                      // waits for the chunk in flight, then frees
 };
 
-// Reads the file from its current offset (file_off bytes into it) to the end, chunk by chunk through b0 / b1, and per
+// Reads the source from its current offset (file_off bytes into it) to the end, chunk by chunk through b0 / b1, and per
 // chunk enqueues the copy, the three shared kernels (separator `sep`, state st) and launch(buffer, chunk index, chunk
 // bytes, file offset, tiles), then an event.  collect(buffer) runs on the host once a buffer's chunk is done, before
 // the buffer is reused and for both buffers at the end; a positive return stops the read (no further chunk is
 // started), a negative one is returned as the status.  `who` prefixes the error messages.
-int for_each_chunk(const char* who, int fd, long long file_off, const ChunkGeometry& g, ChunkBuffers& b0,
+int for_each_chunk(const char* who, ByteSource& src, long long file_off, const ChunkGeometry& g, ChunkBuffers& b0,
                    ChunkBuffers& b1, unsigned char sep, ChunkState* st, cudaStream_t s,
                    const std::function<int(ChunkBuffers&, long long chunk, long long end, long long file_off, int tiles)>& launch,
                    const std::function<int(ChunkBuffers&)>& collect);

@@ -22,7 +22,7 @@ def _dense(X):
 def read_text_or_h5ad(path: str):
     """sc.read(path, first_column_names=True) -- dca/io.py:59.  Text tables go through the GPU reader when it can take
     them (read_counts_text), otherwise through pandas; Matrix Market files through read_counts_mtx, otherwise through
-    scipy; both give the same AnnData."""
+    scipy; gzip files of either through read_counts_gzip first; all give the same AnnData."""
     return _read_path(path, False)[0]
 
 
@@ -40,6 +40,10 @@ def _read_path(path, transpose):
         except ImportError as e:
             raise ImportError("reading .h5ad needs the anndata package, which is not installed") from e
         return anndata.read_h5ad(path), False
+    if ext == ".gz" and _cuda_available() and _is_gzip(path):
+        ad = read_counts_gzip(path, transpose)
+        if ad is not None:
+            return ad, transpose
     if path.lower().endswith(".mtx.gz"):         # Cell Ranger >= 3 writes its matrix gzipped: scipy decompresses it
         return _read_mtx_scipy(path), False
     if ext == ".mtx":
@@ -63,6 +67,11 @@ def _read_text_pandas(path, sep):
                    var=pd.DataFrame(index=tab.columns.astype(str)))
 
 
+def _is_gzip(path):
+    with open(path, "rb") as f:
+        return f.read(2) == b"\x1f\x8b"
+
+
 def _cuda_available():
     try:
         import torch
@@ -80,27 +89,33 @@ def read_counts_text(path, sep, transpose=False, chunk_bytes=0, device=None):
     labels come from pandas reading the header alone; row labels from pandas reading a two-column table made of the
     header's first field and every line's first field, in the row chunks pandas' own reader infers types in, so they
     are the same strings (numeric-looking labels, NA tokens, booleans, duplicates, the index name, a BOM)."""
-    import ctypes as C
-    import torch
-    from . import _lib
     with open(path, "rb") as f:
         if any(f.read(6).startswith(m) for m in _COMPRESSED_MAGIC):
             return None
+    return _read_text_gpu(path, sep, transpose, chunk_bytes, device, "dca_read_text_counts")
+
+
+def _read_text_gpu(path, sep, transpose, chunk_bytes, device, entry):
+    """read_counts_text through the native reader `entry` (the file's bytes, or those of its inflated stream)."""
+    import ctypes as C
+    import torch
+    from . import _lib
     dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     if dev.type != "cuda":
         raise ValueError("read_counts_text parses on a CUDA device (got %s)" % dev)
     lib = _lib.load()
+    read = getattr(lib, entry)
     sep_b = sep.encode()
     if len(sep_b) != 1:
         return None
     info = np.zeros(4, dtype=np.int64)
     stream = torch.cuda.current_stream(dev)
     with torch.cuda.device(dev):
-        st = lib.dca_read_text_counts(os.fsencode(path), sep_b[0], int(bool(transpose)), int(chunk_bytes), dev.index,
-                                      C.c_void_p(stream.cuda_stream), None, 0, None, None, 0, info.ctypes.data)
+        st = read(os.fsencode(path), sep_b[0], int(bool(transpose)), int(chunk_bytes), dev.index,
+                  C.c_void_p(stream.cuda_stream), None, 0, None, None, 0, info.ctypes.data)
         if st == -3:
             return None
-        _lib.check(st, "dca_read_text_counts")
+        _lib.check(st, entry)
         rows, cols, nlab, work = (int(v) for v in info)
         if rows * cols * 4 + work > torch.cuda.mem_get_info(dev)[0]:
             return None
@@ -110,12 +125,12 @@ def read_counts_text(path, sep, transpose=False, chunk_bytes=0, device=None):
         out = torch.empty((cols, rows) if transpose else (rows, cols), dtype=torch.float32, device=dev)
         offsets = np.zeros(rows + 1, dtype=np.int64)
         labels = np.zeros(max(nlab, 1), dtype=np.uint8)
-        st = lib.dca_read_text_counts(os.fsencode(path), sep_b[0], int(bool(transpose)), int(chunk_bytes), dev.index,
-                                      C.c_void_p(stream.cuda_stream), C.c_void_p(out.data_ptr()), out.numel(),
-                                      offsets.ctypes.data, labels.ctypes.data, nlab, info.ctypes.data)
+        st = read(os.fsencode(path), sep_b[0], int(bool(transpose)), int(chunk_bytes), dev.index,
+                  C.c_void_p(stream.cuda_stream), C.c_void_p(out.data_ptr()), out.numel(),
+                  offsets.ctypes.data, labels.ctypes.data, nlab, info.ctypes.data)
         if st == -3:                 # the file changed between the two passes
             return None
-        _lib.check(st, "dca_read_text_counts")
+        _lib.check(st, entry)
         X = out.cpu().numpy()
     del out
     index = _row_labels(path, sep_b, labels[:nlab].tobytes(), offsets, cols + 1)
@@ -147,38 +162,43 @@ def read_counts_mtx(path, transpose=False, chunk_bytes=0, device=None):
 
     The file's bytes go to the device in chunks of chunk_bytes (0: 64 MB) in one pass, and the CSR arrays come back.
     The index arrays are int32 unless NNZ or a dimension reaches 2^31, as scipy chooses."""
+    with open(path, "rb") as f:
+        if any(f.read(6).startswith(m) for m in _COMPRESSED_MAGIC):
+            return None
+    return _read_mtx_gpu(path, transpose, chunk_bytes, device, "dca_read_mtx_counts")
+
+
+def _read_mtx_gpu(path, transpose, chunk_bytes, device, entry):
+    """read_counts_mtx through the native reader `entry` (the file's bytes, or those of its inflated stream)."""
     import ctypes as C
     import torch
     import scipy.sparse as sp
     from . import _lib
-    with open(path, "rb") as f:
-        if any(f.read(6).startswith(m) for m in _COMPRESSED_MAGIC):
-            return None
     dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     if dev.type != "cuda":
         raise ValueError("read_counts_mtx parses on a CUDA device (got %s)" % dev)
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
-    lib = _lib.load()
+    read = getattr(_lib.load(), entry)
     info = np.zeros(4, dtype=np.int64)
     stream = torch.cuda.current_stream(dev)
     with torch.cuda.device(dev):
         args = (os.fsencode(path), int(bool(transpose)), int(chunk_bytes), dev.index, C.c_void_p(stream.cuda_stream))
-        st = lib.dca_read_mtx_counts(*args, None, None, None, info.ctypes.data)
+        st = read(*args, None, None, None, info.ctypes.data)
         if st == -3:
             return None
-        _lib.check(st, "dca_read_mtx_counts")
+        _lib.check(st, entry)
         rows, cols, nnz, work = (int(v) for v in info)
         if 8 * (rows + 1) + 8 * nnz + work > torch.cuda.mem_get_info(dev)[0]:
             return None
         indptr = torch.empty(rows + 1, dtype=torch.int64, device=dev)
         indices = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
         data = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
-        st = lib.dca_read_mtx_counts(*args, C.c_void_p(indptr.data_ptr()), C.c_void_p(indices.data_ptr()),
-                                     C.c_void_p(data.data_ptr()), info.ctypes.data)
+        st = read(*args, C.c_void_p(indptr.data_ptr()), C.c_void_p(indices.data_ptr()), C.c_void_p(data.data_ptr()),
+                  info.ctypes.data)
         if st == -3:
             return None
-        _lib.check(st, "dca_read_mtx_counts")
+        _lib.check(st, entry)
         indptr, indices, data = indptr.cpu().numpy(), indices[:nnz].cpu().numpy(), data[:nnz].cpu().numpy()
     if max(rows, cols, nnz) < 2 ** 31:
         indptr = indptr.astype(np.int32)
@@ -186,6 +206,19 @@ def read_counts_mtx(path, transpose=False, chunk_bytes=0, device=None):
         indices = indices.astype(np.int64)
     X = sp.csr_matrix((data, indices, indptr), shape=(rows, cols), copy=False)
     return AnnData(X, keep_sparse=True)
+
+
+def read_counts_gzip(path, transpose=False, chunk_bytes=0, device=None):
+    """The AnnData today's route gives for a gzip file (scipy's reader for a .mtx.gz path, else pandas' with the tab
+    separator _read_path uses for a '.gz' extension), inflated and parsed on a CUDA device: dca_read_mtx_counts_gz or
+    dca_read_text_counts_gz (csrc/inflate.cu) with the outputs, labels and orientation of read_counts_mtx and
+    read_counts_text.  None when the file is not gzip, the inflate declines it (include/dca_b200.h, dca_gunzip), the
+    parser does not take its inflated bytes, or the outputs do not fit in free device memory."""
+    if not _is_gzip(path):
+        return None
+    if path.lower().endswith(".mtx.gz"):
+        return _read_mtx_gpu(path, transpose, chunk_bytes, device, "dca_read_mtx_counts_gz")
+    return _read_text_gpu(path, "\t", transpose, chunk_bytes, device, "dca_read_text_counts_gz")
 
 
 def _pandas_chunk_rows(width):
@@ -203,8 +236,9 @@ def _row_labels(path, sep, labels, offsets, width):
     every data line: pandas reads them as a two-column table (a second column keeps an empty label from being a blank
     line), chunk by chunk in the chunks its reader of the `width`-field file infers types in.  None when the chunks
     infer different types (pandas then mixes them into one object column, which this does not restate)."""
+    import gzip
     import io as _io
-    with open(path, "rb") as f:
+    with (gzip.open if _is_gzip(path) else open)(path, "rb") as f:
         header = f.readline()
     head = header.split(sep, 1)[0]
     n = len(offsets) - 1

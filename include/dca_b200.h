@@ -634,6 +634,43 @@ int dca_read_text_counts(const char* path, int32_t sep, int32_t transpose, int64
 int dca_read_mtx_counts(const char* path, int32_t transpose, int64_t chunk_bytes, int32_t device, void* stream,
                         int64_t* indptr, int32_t* indices, float* data, int64_t* info);
 
+/* The same readers over the inflated bytes of a gzip file (dca_b200/io.py:read_counts_gzip): the parameters, outputs,
+ * accepted files and two calls of dca_read_text_counts and dca_read_mtx_counts, with the file inflated on `device` as
+ * dca_gunzip does (each call inflates it again; info[3] includes the inflate's device memory).  A file dca_gunzip
+ * declines returns DCA_ERR_UNSUPPORTED.  The entry points above keep reading compressed files as bytes. */
+int dca_read_text_counts_gz(const char* path, int32_t sep, int32_t transpose, int64_t chunk_bytes, int32_t device,
+                            void* stream, float* out, int64_t out_elems, int64_t* label_offsets, char* label_bytes,
+                            int64_t label_cap, int64_t* info);
+int dca_read_mtx_counts_gz(const char* path, int32_t transpose, int64_t chunk_bytes, int32_t device, void* stream,
+                           int64_t* indptr, int32_t* indices, float* data, int64_t* info);
+
+/* GPU inflate of a gzip file (RFC 1952: one or more members of DEFLATE data, RFC 1951) into DEVICE memory, with no
+ * zlib: the host reads the compressed file in 64 MB segments and the device decodes each segment in spans of about
+ * 32 KB in parallel, speculatively from block starts it finds, then checks the chain of spans, the CRC-32 and the
+ * ISIZE of every member.  Headers may have FTEXT, FEXTRA, FNAME, FCOMMENT and FHCRC (checked).  It declines
+ * (DCA_ERR_UNSUPPORTED, the reason in dca_last_error()) a file that is not one or more such members back to back:
+ * CM != 8, reserved flag bits, a bad FHCRC, invalid DEFLATE data, a distance before the member's start, a CRC-32 or
+ * ISIZE mismatch, truncation or trailing bytes; and a file whose chain of spans needs more than 16 rounds in a segment
+ * or a block longer than a segment.  Device memory does not depend on the file's size (at most about 1 GB besides
+ * `out`).  Two calls with the same arguments:
+ *   1. out == NULL: inflates and checks the file; info[0..3] = output bytes, device bytes this call took (the
+ *      second call takes 256 MB less: it has no scratch output window), the most rounds of span decoding any segment
+ *      needed (1: every speculative span was right), members.
+ *   2. out: device bytes [out_bytes], out_bytes = info[0] of the first call: the same, into out.
+ * Work runs on `stream` (of `device`); it returns when it is done.  Without a CUDA device: DCA_ERR_NO_DEVICE. */
+int dca_gunzip(const char* path, int32_t device, void* stream, void* out, int64_t out_bytes, int64_t* info);
+/* The span decoder of dca_gunzip run on the CPU, for tests: decodes in[0, n) (eof != 0: n is the end of the file) from
+ * bit `start` to the first block boundary at or beyond bit `stop`, or to the end of the file's last member.  out: NULL
+ * to count, else 16-bit symbols: a byte (< 0x8000), or 0x8000 | k for the byte k + 1 positions before the span's first
+ * output byte.  info[0..5] = status (0 stopped at a boundary, 1 end of the file, 2 input ran out, 3 invalid), the bit
+ * where it stopped, output bytes, the lowest output position a back-reference reached in the span's first member
+ * (< 0 before the span), the output position of the last member starting in the span (-1: none), member trailers. */
+int dca_inflate_span_host(const uint8_t* in, int64_t n, int32_t eof, int64_t start, int64_t stop, uint16_t* out,
+                          int64_t out_cap, int64_t* info);
+/* The block-start test of dca_gunzip on the CPU: *found = the first bit in [first_bit, end_bit) of in[0, n) where a
+ * dynamic block with a fully valid header or a stored block with LEN = ~NLEN and zero padding could start, or -1. */
+int dca_inflate_find_host(const uint8_t* in, int64_t n, int64_t first_bit, int64_t end_bit, int64_t* found);
+
 /* Host-side packer for dca_stream_begin_packed (multi-threaded counterpart of dca_b200/io.py:pack_counts; no
  * reference counterpart).  counts: HOST matrix rows x cols (ld elements per row) of dtype 0 float32, 1 float64,
  * 2 uint16, 3 int32, 4 int64 holding non-negative integers.  dca_count_escapes fills per_row[w*rows + r] with the
