@@ -200,21 +200,24 @@ int Engine::plan(const dca_config& c) {
     // converted into this buffer
     if (c.x_dtype != DCA_BF16) o_xb = take(2 * B * (size_t)c.n_in);
   }
-  // double-buffered staging of raw uint16 counts streamed from the host + the input transform
-  for (int k = 0; k < 2; ++k) { o_cnt[k] = take(sizeof(uint16_t) * B * (size_t)c.n_in); o_sfst[k] = take(sizeof(float) * B); }
-  ovf_cap = (int64_t)(B * (size_t)c.n_in / 32); if (ovf_cap < 4096) ovf_cap = 4096;
+  // double-buffered staging of raw uint16 counts streamed from the host + the input transform, at the stored width g_store
+  g_store = (c.n_in + 7) / 8 * 8;
+  for (int k = 0; k < 2; ++k) { o_cnt[k] = take(sizeof(uint16_t) * B * (size_t)g_store); o_sfst[k] = take(sizeof(float) * B); }
+  ovf_cap = (int64_t)(B * (size_t)g_store / 32); if (ovf_cap < 4096) ovf_cap = 4096;
   for (int k = 0; k < 2; ++k) { o_ovp[k] = take(sizeof(int64_t) * (B + 1)); o_ove[k] = take(8 * (size_t)ovf_cap); }
-  nib_cap = (int64_t)(B * (size_t)c.n_in / 4) + 64;       // sparse format: up to 50 % non-zero entries per batch
+  nib_cap = (int64_t)(B * (size_t)g_store / 4) + 64;           // sparse format: up to 50 % non-zero entries per batch
   for (int k = 0; k < 2; ++k) { o_nibp[k] = take(sizeof(int64_t) * (B + 1)); o_nib[k] = take((size_t)nib_cap); }
   o_gmean = take(sizeof(float) * (size_t)c.n_in); o_ginv = take(sizeof(float) * (size_t)c.n_in);
-  o_gmean64 = take(sizeof(double) * (size_t)c.n_in); o_gstd64 = take(sizeof(double) * (size_t)c.n_in);
-  o_gx0 = take(sizeof(float) * (size_t)c.n_in);
+  o_gmean64 = take(sizeof(double) * (size_t)g_store); o_gstd64 = take(sizeof(double) * (size_t)g_store);
+  o_gx0 = take(sizeof(float) * (size_t)g_store);
   for (int k = 0; k < 2; ++k) o_ncst[k] = take(sizeof(double) * B);
-  // staging for the host-buffer entry point
+  // staging for the host-buffer entry point and the expanded batches (rows of g_store entries: the streamed and packed paths
+  // need n_in == n_out)
   const size_t xb = (c.x_dtype == DCA_BF16) ? 2 : 4;
+  const size_t gy = (size_t)((G + 7) / 8 * 8);
   for (int k = 0; k < kExpBufs; ++k) {
-    o_sx[k] = take(xb * B * (size_t)c.n_in);
-    o_sy[k] = take(sizeof(float) * B * (size_t)G);
+    o_sx[k] = take(xb * B * (size_t)g_store);
+    o_sy[k] = take(sizeof(float) * B * gy);
     o_ssf[k] = take(sizeof(float) * B);
   }
   o_stage_x = o_sx[0]; o_stage_y = o_sy[0]; o_stage_sf = o_ssf[0];
@@ -1037,7 +1040,7 @@ int Engine::stream_prefetch(int64_t i, int b, int e) {
   const int64_t r0 = i * hs.batch;
   const int64_t nb = (hs.n_rows - r0 < hs.batch) ? (hs.n_rows - r0) : hs.batch;
   const bool sparse = hs.bits == 1;
-  const size_t tight = (size_t)cfg.n_in * (size_t)hs.bits / 8;             // bytes of one packed row (sparse: its bitmap)
+  const size_t tight = (size_t)g_store * (size_t)hs.bits / 8;                   // bytes of one packed row (sparse: its bitmap)
   DCA_CUDA_OK(cudaStreamWaitEvent(hs.copy, hs.cnt_free[b], 0));          // the expansion two batches ago has consumed staging b
   if (hs.tl_base && hs.tl.size() < 400) hs.tl_mark(hs.copy);
   if ((size_t)hs.row_bytes == tight)  // contiguous rows: one linear copy (faster than the pitched path)
@@ -1076,12 +1079,12 @@ int Engine::stream_prefetch(int64_t i, int b, int e) {
   const ExactXform* exact = tf_exact ? &ex : nullptr;
   if (sparse)
     DCA_TRY(expand_sparse(base + o_cnt[b], reinterpret_cast<const int64_t*>(base + o_nibp[b]), base + o_nib[b],
-                          hs.sf ? f(o_sfst[b]) : nullptr, (int)nb, cfg.n_in, tf_set == 2 ? f(o_gmean) : nullptr,
+                          hs.sf ? f(o_sfst[b]) : nullptr, (int)nb, g_store, tf_set == 2 ? f(o_gmean) : nullptr,
                           tf_set == 2 ? f(o_ginv) : nullptr, tf_use_sf && hs.sf, tf_use_log1p, f(o_sy[e]), base + o_sx[e], x_bf16,
                           f(o_ssf[e]), has_ovf ? reinterpret_cast<const int64_t*>(base + o_ovp[b]) : nullptr,
                           has_ovf ? (const void*)(base + o_ove[b]) : nullptr, max_nib, hs.expand, exact));
   else
-  DCA_TRY(expand_counts(base + o_cnt[b], hs.bits, hs.sf ? f(o_sfst[b]) : nullptr, (int)nb, cfg.n_in,
+  DCA_TRY(expand_counts(base + o_cnt[b], hs.bits, hs.sf ? f(o_sfst[b]) : nullptr, (int)nb, g_store,
                         tf_set == 2 ? f(o_gmean) : nullptr, tf_set == 2 ? f(o_ginv) : nullptr, tf_use_sf && hs.sf,
                         tf_use_log1p, f(o_sy[e]), base + o_sx[e], x_bf16, f(o_ssf[e]),
                         has_ovf ? reinterpret_cast<const int64_t*>(base + o_ovp[b]) : nullptr,
@@ -1134,11 +1137,16 @@ extern "C" int dca_set_input_transform_exact(dca_handle* h, const double* gene_m
   }
   if (e.hs.active) { set_error("dca_set_input_transform_exact: a host stream is active (call dca_stream_end first)"); return DCA_ERR_BAD_ARG; }
   cudaStream_t s = (cudaStream_t)stream;
-  const size_t n = (size_t)e.cfg.n_in;
+  const size_t n = (size_t)e.cfg.n_in, pad = (size_t)e.g_store - n;
+  static const double neutral[2][8] = {{0, 0, 0, 0, 0, 0, 0, 0}, {1, 1, 1, 1, 1, 1, 1, 1}};   // pad genes: mean 0, std 1
   DCA_CUDA_OK(cudaMemcpyAsync(e.base + e.o_gmean64, gene_mean_host, sizeof(double) * n, cudaMemcpyHostToDevice, s));
   DCA_CUDA_OK(cudaMemcpyAsync(e.base + e.o_gstd64, gene_std_host, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+  if (pad) {
+    DCA_CUDA_OK(cudaMemcpyAsync(e.base + e.o_gmean64 + sizeof(double) * n, neutral[0], sizeof(double) * pad, cudaMemcpyHostToDevice, s));
+    DCA_CUDA_OK(cudaMemcpyAsync(e.base + e.o_gstd64 + sizeof(double) * n, neutral[1], sizeof(double) * pad, cudaMemcpyHostToDevice, s));
+  }
   DCA_TRY(exact_zero_inputs(reinterpret_cast<const double*>(e.base + e.o_gmean64),
-                            reinterpret_cast<const double*>(e.base + e.o_gstd64), (int)n, e.f(e.o_gx0), s));
+                            reinterpret_cast<const double*>(e.base + e.o_gstd64), e.g_store, e.f(e.o_gx0), s));
   DCA_CUDA_OK(cudaStreamSynchronize(s));
   e.tf_set = 3; e.tf_exact = true; e.tf_flags = flags; e.tf_median = (flags & DCA_PRE_SIZE_FACTORS) ? median : 1.0;
   return DCA_OK;
@@ -1162,12 +1170,16 @@ extern "C" int dca_stream_begin_packed(dca_handle* h, const void* packed_host, i
   Engine& e = h->e;
   if (!packed_host || n_rows <= 0 || batch <= 0 || batch > e.cfg.max_batch) { set_error("dca_stream_begin: bad argument"); return DCA_ERR_BAD_ARG; }
   if (bits != 1 && bits != 4 && bits != 8 && bits != 16) { set_error("dca_stream_begin: bits must be 4, 8 or 16 (got %d)", bits); return DCA_ERR_BAD_ARG; }
-  if (row_bytes < (int64_t)e.cfg.n_in * bits / 8) { set_error("dca_stream_begin: row stride smaller than a packed row"); return DCA_ERR_BAD_ARG; }
+  if (row_bytes < (int64_t)e.g_store * bits / 8) { set_error("dca_stream_begin: row stride smaller than a packed row"); return DCA_ERR_BAD_ARG; }
   if (bits == 1 && !e.hs.nib_indptr) { set_error("dca_stream_begin: the sparse format starts with dca_stream_begin_sparse"); return DCA_ERR_BAD_ARG; }
   if ((ovf_indptr_host == nullptr) != (ovf_entries_host == nullptr)) { set_error("dca_stream_begin: give both overflow arrays or neither"); return DCA_ERR_BAD_ARG; }
   if (e.cfg.n_in != e.cfg.n_out) { set_error("dca_stream_begin: needs n_in == n_out"); return DCA_ERR_UNSUPPORTED; }
-  if (e.cfg.n_in % 8 != 0) { set_error("dca_stream_begin: n_in must be a multiple of 8"); return DCA_ERR_UNSUPPORTED; }
   if (!e.tf_set) { set_error("dca_stream_begin: call dca_set_input_transform first"); return DCA_ERR_BAD_ARG; }
+  if (e.cfg.n_in != e.g_store && !e.tf_exact) {
+    set_error("dca_stream_begin: n_in = %d is not a multiple of 8: its rows are stored %d wide, which only the exact transform "
+              "(dca_set_input_transform_exact) expands", e.cfg.n_in, e.g_store);
+    return DCA_ERR_UNSUPPORTED;
+  }
   if (ovf_indptr_host) {
     for (int64_t r0 = 0; r0 < n_rows; r0 += batch) {
       const int64_t r1 = (r0 + batch < n_rows) ? r0 + batch : n_rows;
@@ -1228,7 +1240,7 @@ extern "C" int dca_stream_begin_sparse(dca_handle* h, const void* bitmap_host, c
     }
   }
   e.hs.nib_indptr = nib_indptr_host; e.hs.nibbles = reinterpret_cast<const unsigned char*>(nibbles_host);
-  return dca_stream_begin_packed(h, bitmap_host, 1, (int64_t)e.cfg.n_in / 8, ovf_indptr_host, ovf_entries_host, sf_host, n_rows,
+  return dca_stream_begin_packed(h, bitmap_host, 1, (int64_t)e.g_store / 8, ovf_indptr_host, ovf_entries_host, sf_host, n_rows,
                                  batch, stream);
 }
 
@@ -1281,13 +1293,13 @@ int stream_run(dca_handle* h, const char* who, int64_t i, int64_t next, void* st
 
 extern "C" int dca_stream_step(dca_handle* h, int64_t i, int64_t next, void* stream) {
   return stream_run(h, "dca_stream_step", i, next, stream, [](Engine& e, int xb, int nb, cudaStream_t s) {
-    return e.train_step(e.base + e.o_sx[xb], e.cfg.n_in, e.f(e.o_sy[xb]), e.cfg.n_out, e.f(e.o_ssf[xb]), nullptr, nb, s, 0);
+    return e.train_step(e.base + e.o_sx[xb], e.g_store, e.f(e.o_sy[xb]), e.g_store, e.f(e.o_ssf[xb]), nullptr, nb, s, 0);
   });
 }
 
 extern "C" int dca_stream_eval(dca_handle* h, int64_t i, int64_t next, void* stream) {
   return stream_run(h, "dca_stream_eval", i, next, stream, [](Engine& e, int xb, int nb, cudaStream_t s) {
-    return e.eval_step(e.base + e.o_sx[xb], e.cfg.n_in, e.f(e.o_sy[xb]), e.cfg.n_out, e.f(e.o_ssf[xb]), nullptr, nb, s);
+    return e.eval_step(e.base + e.o_sx[xb], e.g_store, e.f(e.o_sy[xb]), e.g_store, e.f(e.o_ssf[xb]), nullptr, nb, s);
   });
 }
 
@@ -1301,7 +1313,7 @@ extern "C" int dca_stream_capacity(const dca_handle* h, int64_t* ovf_entries, in
 extern "C" int dca_stream_predict(dca_handle* h, int64_t i, int64_t next, float* mean_out, float* disp_out, float* pi_out,
                                   int64_t ld_out, float* latent_out, void* stream) {
   return stream_run(h, "dca_stream_predict", i, next, stream, [&](Engine& e, int xb, int nb, cudaStream_t s) {
-    return e.predict(e.base + e.o_sx[xb], e.cfg.n_in, e.f(e.o_ssf[xb]), nullptr, nb, mean_out, disp_out, pi_out, ld_out,
+    return e.predict(e.base + e.o_sx[xb], e.g_store, e.f(e.o_ssf[xb]), nullptr, nb, mean_out, disp_out, pi_out, ld_out,
                      latent_out, s);
   });
 }
@@ -1447,9 +1459,11 @@ int packed_run(dca_handle* h, const char* who, const dca_packed_counts* src, con
   Engine& e = h->e;
   if (e.hs.active) { set_error("%s: a host stream is active (call dca_stream_end first)", who); return DCA_ERR_BAD_ARG; }
   if (e.cfg.n_in != e.cfg.n_out) { set_error("%s: needs n_in == n_out", who); return DCA_ERR_UNSUPPORTED; }
-  if (e.cfg.n_in % 8 != 0) { set_error("%s: n_in must be a multiple of 8", who); return DCA_ERR_UNSUPPORTED; }
   DCA_TRY(check_packed_counts(who, src));
-  if (src->genes != e.cfg.n_in) { set_error("%s: the packed counts have %d genes, the engine %d", who, src->genes, e.cfg.n_in); return DCA_ERR_BAD_ARG; }
+  if (src->genes != e.g_store) {
+    set_error("%s: the packed counts have %d genes, the engine %d (stored %d wide)", who, src->genes, e.cfg.n_in, e.g_store);
+    return DCA_ERR_BAD_ARG;
+  }
   if (batch <= 0 || batch > e.cfg.max_batch) { set_error("%s: batch %d outside (0, max_batch=%d]", who, batch, e.cfg.max_batch); return DCA_ERR_BAD_ARG; }
   if (!e.tf_exact) { set_error("%s: call dca_set_input_transform_exact first", who); return DCA_ERR_BAD_ARG; }
   if ((e.tf_flags & DCA_PRE_SIZE_FACTORS) && !src->n_counts) { set_error("%s: size factors need the row totals (n_counts)", who); return DCA_ERR_BAD_ARG; }
@@ -1479,14 +1493,14 @@ extern "C" int dca_expand_rows_exact(const dca_packed_counts* src, const int32_t
 extern "C" int dca_packed_train_step(dca_handle* h, const dca_packed_counts* src, const int32_t* rows, int32_t batch,
                                      void* stream) {
   return packed_run(h, "dca_packed_train_step", src, rows, batch, stream, [](Engine& e, int nb, cudaStream_t s) {
-    return e.train_step(e.base + e.o_sx[0], e.cfg.n_in, e.f(e.o_sy[0]), e.cfg.n_out, e.f(e.o_ssf[0]), nullptr, nb, s, 0);
+    return e.train_step(e.base + e.o_sx[0], e.g_store, e.f(e.o_sy[0]), e.g_store, e.f(e.o_ssf[0]), nullptr, nb, s, 0);
   });
 }
 
 extern "C" int dca_packed_eval_step(dca_handle* h, const dca_packed_counts* src, const int32_t* rows, int32_t batch,
                                     void* stream) {
   return packed_run(h, "dca_packed_eval_step", src, rows, batch, stream, [](Engine& e, int nb, cudaStream_t s) {
-    return e.eval_step(e.base + e.o_sx[0], e.cfg.n_in, e.f(e.o_sy[0]), e.cfg.n_out, e.f(e.o_ssf[0]), nullptr, nb, s);
+    return e.eval_step(e.base + e.o_sx[0], e.g_store, e.f(e.o_sy[0]), e.g_store, e.f(e.o_ssf[0]), nullptr, nb, s);
   });
 }
 
@@ -1494,7 +1508,7 @@ extern "C" int dca_packed_predict(dca_handle* h, const dca_packed_counts* src, c
                                   float* mean_out, float* disp_out, float* pi_out, int64_t ld_out, float* latent_out,
                                   void* stream) {
   return packed_run(h, "dca_packed_predict", src, rows, batch, stream, [&](Engine& e, int nb, cudaStream_t s) {
-    return e.predict(e.base + e.o_sx[0], e.cfg.n_in, e.f(e.o_ssf[0]), nullptr, nb, mean_out, disp_out, pi_out, ld_out,
+    return e.predict(e.base + e.o_sx[0], e.g_store, e.f(e.o_ssf[0]), nullptr, nb, mean_out, disp_out, pi_out, ld_out,
                      latent_out, s);
   });
 }

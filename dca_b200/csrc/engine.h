@@ -81,6 +81,10 @@ struct Engine {
   // tensor-core encoder can read it in place.  fp32 X with input dropout stays fp32, so that the mask scales the fp32 value
   // and the encoder's gather rounds it once, bf16(x * inv_keep), as on a resident fp32 X
   int expand_bf16() const { return cfg.x_dtype == DCA_BF16 || (tc_enc && !(cfg.input_dropout > 0.f)); }
+  // stored width of packed rows and of the expanded batches: n_in rounded up to a multiple of 8.  The step reads the
+  // first n_in columns of an expanded batch at leading dimension g_store; the g_store - n_in pad genes are zero counts
+  // that never reach the model (their mean / std entries of the exact transform are 0 / 1)
+  int g_store = 0;
   // optional phase timing
   struct Prof {
     bool on = false;

@@ -93,13 +93,15 @@ def _size_factors(nc, size_factors):
 def build_dataset(counts, device=None, x_dtype="float32", stream=False, packed=False, batch=32, **flags):
     """The dataset of the device preprocessing of ``counts`` with the flags of io.normalize (``flags``): resident
     (DeviceDataset), out of core from packed host counts (stream: stream_data.StreamedDataset, packed for a training
-    batch of ``batch`` rows) or packed in device memory (packed: packed_data.PackedDeviceDataset)."""
+    batch of ``batch`` rows) or packed in device memory (packed: packed_data.PackedDeviceDataset).  The packed kinds
+    take any gene count, before and after the gene filter: their rows are stored zero-padded to a multiple of 8
+    (pad_genes=True)."""
     if packed:
         from .packed_data import PackedDeviceDataset
-        return PackedDeviceDataset.from_counts(counts, device, x_dtype, **flags)
+        return PackedDeviceDataset.from_counts(counts, device, x_dtype, pad_genes=True, **flags)
     if stream:
         from .stream_data import StreamedDataset
-        return StreamedDataset.from_counts(counts, device, x_dtype, batch=batch, **flags)
+        return StreamedDataset.from_counts(counts, device, x_dtype, batch=batch, pad_genes=True, **flags)
     return DeviceDataset.from_counts(counts, device, x_dtype, **flags)
 
 

@@ -362,7 +362,8 @@ class DeviceEngine:
     def stream_begin(self, counts, sf: Optional[torch.Tensor], batch: int):
         """Train from HOST memory.  counts: a HOST uint16 tensor [n_rows x n_in] (pin it, hostmem.pin_near_gpu), or an
         io.PackedCounts (4/8/16 bits per entry + overflow list, see io.pack_counts) whose arrays are pinned
-        here; sf: HOST float32 [n_rows] or None."""
+        here (with n_in off a multiple of 8: packed with pad_genes=True, and the exact transform set); sf: HOST
+        float32 [n_rows] or None."""
         if sf is not None and sf.is_cuda:
             raise ValueError("stream_begin takes HOST tensors")
         if isinstance(counts, torch.Tensor):
@@ -376,8 +377,9 @@ class DeviceEngine:
                   "dca_stream_begin")
             return
         pc = counts
-        if pc.n_genes != self.n_in:
-            raise ValueError("packed counts have %d genes, the engine %d" % (pc.n_genes, self.n_in))
+        if pc.genes != self.n_in or pc.n_genes != (self.n_in + 7) // 8 * 8:
+            raise ValueError("packed counts have %d genes (stored %d wide), the engine %d"
+                             % (pc.genes, pc.n_genes, self.n_in))
 
         from .stream_data import pin_packed
         packed, indptr, entries = pin_packed(pc, self.device.index or 0)[:3]

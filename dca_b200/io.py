@@ -539,11 +539,14 @@ def read_pickle(inputfile):
 class PackedCounts:
     """bits-per-entry matrix + CSR overflow list; see pack_counts().  bits == 1 is the SPARSE format: ``packed`` is the
     non-zero bitmap (n_genes/8 bytes per row), ``nibbles`` the 4-bit codes of the non-zero counts in gene order (each row
-    starts on a byte boundary at ``nib_indptr[row]``), codes of 15 escape into the overflow list."""
+    starts on a byte boundary at ``nib_indptr[row]``), codes of 15 escape into the overflow list.  ``n_genes`` is the
+    stored width (a multiple of 8), ``genes`` the matrix's gene count: smaller when a ragged matrix was packed as its
+    zero-padded form (pack_counts(..., pad_genes=True)), whose last n_genes - genes columns are all zero."""
 
-    def __init__(self, packed, bits, n_genes, indptr, entries, nib_indptr=None, nibbles=None):
+    def __init__(self, packed, bits, n_genes, indptr, entries, nib_indptr=None, nibbles=None, genes=None):
         self.packed, self.bits, self.n_genes, self.indptr, self.entries = packed, bits, n_genes, indptr, entries
         self.nib_indptr, self.nibbles = nib_indptr, nibbles
+        self.genes = n_genes if genes is None else int(genes)
         self._pinned = None            # pinned host copies, made by DeviceEngine.stream_begin on first use
 
     @property
@@ -577,11 +580,13 @@ class PackedCounts:
     def _take_block(self, idx):
         indptr, entries = _gather_segments(self.indptr, self.entries, idx)
         if self.bits != 1:
-            return PackedCounts(np.ascontiguousarray(self.packed[idx]), self.bits, self.n_genes, indptr, entries)
+            return PackedCounts(np.ascontiguousarray(self.packed[idx]), self.bits, self.n_genes, indptr, entries,
+                                genes=self.genes)
         nib_indptr, nib = _gather_segments(self.nib_indptr, self.nibbles, idx)
         nibbles = np.zeros(nib.size + 16, dtype=np.uint8)            # + slack: the device reads whole bytes
         nibbles[:nib.size] = nib
-        return PackedCounts(np.ascontiguousarray(self.packed[idx]), 1, self.n_genes, indptr, entries, nib_indptr, nibbles)
+        return PackedCounts(np.ascontiguousarray(self.packed[idx]), 1, self.n_genes, indptr, entries, nib_indptr, nibbles,
+                            genes=self.genes)
 
 
 def _gather_segments(indptr, data, idx):
@@ -600,8 +605,8 @@ def concat_packed(parts):
     parts = list(parts)
     if not parts:
         raise ValueError("nothing to concatenate")
-    bits, g = parts[0].bits, parts[0].n_genes
-    if any(p.bits != bits or p.n_genes != g for p in parts):
+    bits, g, genes = parts[0].bits, parts[0].n_genes, parts[0].genes
+    if any(p.bits != bits or p.n_genes != g or p.genes != genes for p in parts):
         raise ValueError("packed parts differ in width or gene count")
 
     def cat_ptr(ptrs):
@@ -615,39 +620,57 @@ def concat_packed(parts):
     indptr = cat_ptr([p.indptr for p in parts])
     entries = np.concatenate([p.entries for p in parts]) if parts else np.empty(0, OVERFLOW_ENTRY)
     if bits != 1:
-        return PackedCounts(packed, bits, g, indptr, entries)
+        return PackedCounts(packed, bits, g, indptr, entries, genes=genes)
     nib_indptr = cat_ptr([p.nib_indptr for p in parts])
     nibbles = np.zeros(int(nib_indptr[-1]) + 16, dtype=np.uint8)
     for p, o in zip(parts, nib_indptr[np.cumsum([0] + [p.n_rows for p in parts[:-1]])]):
         n = int(p.nib_indptr[-1] - p.nib_indptr[0])
         nibbles[o:o + n] = p.nibbles[:n]
-    return PackedCounts(packed, 1, g, indptr, entries, nib_indptr, nibbles)
+    return PackedCounts(packed, 1, g, indptr, entries, nib_indptr, nibbles, genes=genes)
 
 
-def pack_rows(counts, bits="auto", batch=None, chunk_rows=16384, threads=0):
+def pack_rows(counts, bits="auto", batch=None, chunk_rows=16384, threads=0, pad_genes=False):
     """pack_counts of a dense matrix or a scipy.sparse CSR matrix, ``chunk_rows`` rows at a time (a CSR matrix is
     never dense on the host as a whole), concatenated with concat_packed: the bytes pack_counts writes for the whole
-    matrix.  bits='auto' / 'sparse' / 'dense' decide the format once, from the whole matrix as pack_counts does."""
+    matrix.  bits='auto' / 'sparse' / 'dense' decide the format once, from the whole matrix as pack_counts does.
+    pad_genes: as for pack_counts (each chunk is padded as it is densified)."""
     csr = hasattr(counts, "tocsr") and getattr(counts, "format", None) == "csr"
     n, g = (int(s) for s in counts.shape)
-    if g % 8 != 0:
-        raise ValueError("the number of genes must be a multiple of 8 for the packed format (got %d)" % g)
+    gp = _packed_width(g, pad_genes)
     if n <= chunk_rows and not csr:
-        return pack_counts(counts, bits, batch=batch, threads=threads)
+        return pack_counts(counts, bits, batch=batch, threads=threads, pad_genes=pad_genes)
     if bits in ("auto", "sparse", "dense"):
-        bits = _choose_format(counts, csr, bits, batch, chunk_rows)
+        bits = _choose_format(counts, csr, bits, batch, chunk_rows, gp)
 
     def rows(r0, r1):
         m = counts[r0:r1]
         return m.toarray() if csr else np.asarray(m)
-    return concat_packed([pack_counts(rows(r0, min(n, r0 + chunk_rows)), bits, threads=threads)
+    return concat_packed([pack_counts(rows(r0, min(n, r0 + chunk_rows)), bits, threads=threads, pad_genes=pad_genes)
                           for r0 in range(0, n, chunk_rows)])
 
 
-def _choose_format(counts, csr, bits, batch, chunk_rows):
+def _packed_width(g, pad_genes):
+    """The stored width of g genes: g itself when it is a multiple of 8, else g rounded up with pad_genes."""
+    if g % 8 == 0:
+        return g
+    if not pad_genes:
+        raise ValueError("the number of genes must be a multiple of 8 for the packed format (got %d)" % g)
+    return (g + 7) // 8 * 8
+
+
+def _zero_padded(C, gp):
+    """C (n x g) with gp - g all-zero columns appended."""
+    if C.shape[1] == gp:
+        return C
+    out = np.zeros((C.shape[0], gp), dtype=C.dtype)
+    out[:, :C.shape[1]] = C
+    return out
+
+
+def _choose_format(counts, csr, bits, batch, chunk_rows, g):
     """The width pack_counts(counts, bits, batch) would choose (1 = sparse), from per-row statistics gathered chunk by
     chunk (the native escape counter; non-integer or negative counts raise)."""
-    n, g = counts.shape
+    n = counts.shape[0]                                  # g: the stored width (pad genes hold no count)
     nnz = np.zeros(n, dtype=np.int64)
     per_row = np.zeros((3, n), dtype=np.int64)
     for r0 in range(0, n, chunk_rows):
@@ -721,8 +744,10 @@ def fit_batches(pc, batch, ovf_cap, nib_cap, chunk_rows=16384):
         ptr = np.zeros(n + 1, dtype=np.int64)
         np.cumsum(per_row[w], out=ptr[1:])
         if _worst_batch(ptr, batch) <= ovf_cap:
-            return concat_packed([pack_counts(unpack_counts(pc.take_rows(np.arange(r0, min(n, r0 + chunk_rows)))), b)
-                                  for r0 in range(0, n, chunk_rows)])
+            out = concat_packed([pack_counts(unpack_counts(pc.take_rows(np.arange(r0, min(n, r0 + chunk_rows)))), b)
+                                 for r0 in range(0, n, chunk_rows)])
+            out.genes = pc.genes
+            return out
     raise ValueError("a batch of %d rows holds more than %d counts >= 65535 (the overflow capacity of one streamed batch)"
                      % (batch, ovf_cap))
 
@@ -812,20 +837,29 @@ def _pack_sparse(C, batch):
     return PackedCounts(np.ascontiguousarray(bitmap), 1, g, indptr, entries, nib_indptr, nibbles)
 
 
-def pack_counts(counts, bits="auto", batch=None, native=True, threads=0):
+def pack_counts(counts, bits="auto", batch=None, native=True, threads=0, pad_genes=False):
     """Pack an integer-valued count matrix (cells x genes, any numeric dtype) into `bits` bits per entry.
 
     Counts >= 2**bits - 1 are stored as the escape value 2**bits - 1 and listed (row-sorted) in the overflow
     CSR: indptr int64[n_rows+1], entries {int32 gene, float32 count}.  bits='auto' picks the width in
     (4, 8, 16) with the fewest total bytes whose per-batch overflow (when `batch` is given) stays under
     batch*genes/32 entries (the device staging capacity).  native=True runs the multi-threaded packer of the
-    library (dca_count_escapes / dca_pack_counts); native=False is the NumPy statement of the same format."""
+    library (dca_count_escapes / dca_pack_counts); native=False is the NumPy statement of the same format.
+    The gene count must be a multiple of 8; with pad_genes=True any gene count packs as its zero-padded form: the
+    bytes of the matrix with all-zero columns appended up to the next multiple of 8 (PackedCounts.genes records the
+    gene count, n_genes the stored width)."""
     C = np.asarray(counts)
     if C.ndim != 2:
         raise ValueError("counts must be a 2-d matrix")
+    genes = C.shape[1]
+    C = _zero_padded(C, _packed_width(genes, pad_genes))
+    pc = _pack_padded(C, bits, batch, native, threads)
+    pc.genes = genes
+    return pc
+
+
+def _pack_padded(C, bits, batch, native, threads):
     n, g = C.shape
-    if g % 8 != 0:
-        raise ValueError("the number of genes must be a multiple of 8 for the packed format (got %d)" % g)
     if bits not in ("auto", "sparse", "dense") and bits not in (4, 8, 16):
         raise ValueError("bits must be 4, 8, 16, 'sparse', 'dense' (best dense width) or 'auto' (smallest of all)")
     if bits in ("sparse", "auto") and n > 0:

@@ -10,8 +10,11 @@ index on the device (``dca_packed_train_step`` ... in include/dca_b200.h): nothi
 reshuffled every epoch as Keras does.
 
 On the same counts every result is bit-identical to ``DeviceDataset``: size factors, n_counts, gene totals, mean, std
-and every X the training step and predict read.  The counts must be non-negative integers and the gene count (after
-filtering) a multiple of 8 (the packed format).
+and every X the training step and predict read.  The counts must be non-negative integers.  With ``pad_genes=True``
+any gene count is accepted, before and after filtering: the rows are packed at the gene count rounded up to a multiple
+of 8, the pad genes all zero (the bytes of io.pack_rows(..., pad_genes=True)), and the statistics, the expansion and
+the model see the real genes only.  With the default ``pad_genes=False`` the gene count after filtering must be a
+multiple of 8.
 """
 from __future__ import annotations
 
@@ -27,7 +30,7 @@ from . import io as dio
 from ._lib import check
 from .device_data import (_counts_matrix, _Dataset, _device, _is_csr, _resident_fit, _size_factors, _stream, _X_DTYPES,
                           preprocess_flags)
-from .stream_data import _chunk_rows, _moments, _totals
+from .stream_data import _chunk_rows, _moments, _pad_stats, _totals
 
 _ESC_ROW = {1: 1, 4: 1, 8: 2, 16: 3}           # row of the count-pass statistics holding a width's overflow entries
 
@@ -50,14 +53,17 @@ def choose_format(nnz, per_row, n, g, bits="auto"):
 
 class _HostChunks:
     """fn(r0, n, Y) for consecutive row chunks of a host matrix (dense, or scipy CSR densified on the device by
-    dca_counts_csr_to_dense: a CSR matrix is never dense on the host as a whole); Y = the chunk's fp32 counts."""
+    dca_counts_csr_to_dense: a CSR matrix is never dense on the host as a whole); Y = the chunk's fp32 counts, ``ld``
+    wide: the gene count rounded up to a multiple of 8, whose pad columns stay zero (the packer's count pass reads whole
+    16-byte groups)."""
 
     def __init__(self, counts, dev):
         self.counts, self.dev, self.csr = counts, dev, _is_csr(counts)
         self.N, self.G = (int(s) for s in counts.shape)
+        self.ld = (self.G + 7) // 8 * 8
 
     def __call__(self, chunk, fn):
-        Y = torch.empty((chunk, self.G), dtype=torch.float32, device=self.dev)
+        Y = torch.zeros((chunk, self.ld), dtype=torch.float32, device=self.dev)
         for r0 in range(0, self.N, chunk):
             r1 = min(self.N, r0 + chunk)
             self._upload(r0, r1, Y)
@@ -65,7 +71,7 @@ class _HostChunks:
 
     def _upload(self, r0, r1, Y):
         if not self.csr:
-            Y[: r1 - r0].copy_(torch.from_numpy(np.ascontiguousarray(self.counts[r0:r1], dtype=np.float32)))
+            Y[: r1 - r0, : self.G].copy_(torch.from_numpy(np.ascontiguousarray(self.counts[r0:r1], dtype=np.float32)))
             return
         m = self.counts[r0:r1]
         if not m.has_canonical_format:
@@ -79,7 +85,7 @@ class _HostChunks:
         data = torch.from_numpy(np.ascontiguousarray(m.data, dtype=np.float32)).to(self.dev)
         check(_lib.load().dca_counts_csr_to_dense(indptr.data_ptr(), indices.data_ptr() if m.nnz else None,
                                                   data.data_ptr() if m.nnz else None, r1 - r0, self.G, Y.data_ptr(),
-                                                  self.G, _stream(self.dev)), "dca_counts_csr_to_dense")
+                                                  self.ld, _stream(self.dev)), "dca_counts_csr_to_dense")
 
 
 class PackedDeviceDataset(_Dataset):
@@ -100,34 +106,36 @@ class PackedDeviceDataset(_Dataset):
 
     @property
     def n_genes(self) -> int:
-        return int(self.desc.genes)
+        return int(getattr(self, "genes", self.desc.genes))        # the real genes; desc.genes is the stored width
 
     @classmethod
     def from_counts(cls, counts, device=None, x_dtype="float32", size_factors=True, logtrans_input=True,
-                    normalize_input=True, filter_min_counts=False, bits="auto", chunk_rows=None):
+                    normalize_input=True, filter_min_counts=False, bits="auto", chunk_rows=None, pad_genes=False):
         """counts: cells x genes, a dense ndarray or a scipy.sparse CSR matrix of raw counts.  The filtering and
         normalisation steps of io.normalize with the same flags; x_dtype 'float32' | 'bfloat16' (the X the training
         step reads); bits: the packing as io.pack_rows(counts, bits) chooses it ('auto', 'sparse', 'dense', 4, 8, 16);
-        chunk_rows: rows per uploaded / expanded chunk (default: 256 MB of fp32 counts)."""
+        chunk_rows: rows per uploaded / expanded chunk (default: 256 MB of fp32 counts); pad_genes: accept a gene count
+        off a multiple of 8, before and after the gene filter (stored zero-padded to the next multiple of 8,
+        ``desc.genes``; ``genes`` and every result cover the real genes)."""
         lib = _lib.load()
         if not torch.cuda.is_available():
             raise _lib.DcaError("PackedDeviceDataset needs a CUDA device (H100); there is no CPU fallback")
         dev, xdt = _device(device), _X_DTYPES[x_dtype]
         counts = _counts_matrix(counts)
         N0, G0 = (int(s) for s in counts.shape)
-        if G0 % 8 != 0:
+        if G0 % 8 != 0 and not pad_genes:
             raise ValueError("the packed format needs a gene count that is a multiple of 8 (got %d)" % G0)
-        choose_format(0, np.zeros((3, 0), np.int64), 0, G0, bits)          # reject a bad `bits` before any work
+        choose_format(0, np.zeros((3, 0), np.int64), 0, dio._packed_width(G0, pad_genes), bits)          # reject a bad `bits` before any work
         host = _HostChunks(counts, dev)
         with torch.cuda.device(dev):
             # pass 1 over the host counts: totals (the chunked column pass) and the per-row statistics of the packer
             stats = torch.empty((5, N0), dtype=torch.int64, device=dev)
 
             def upload_and_count(chunk, fn):
-                def both(r0, n, Y):
-                    check(lib.dca_pack_count_rows(Y.data_ptr(), G0, n, G0, stats.data_ptr() + 8 * r0, N0, _stream(dev)),
-                          "dca_pack_count_rows")
-                    fn(r0, n, Y)
+                def both(r0, n, Y):                          # (the pad columns of a ragged chunk hold no count)
+                    check(lib.dca_pack_count_rows(Y.data_ptr(), host.ld, n, host.ld, stats.data_ptr() + 8 * r0, N0,
+                                                  _stream(dev)), "dca_pack_count_rows")
+                    fn(r0, n, Y[:, :G0])
                 host(chunk, both)
             nc, gene_tot, n_bad = _totals(SimpleNamespace(n_rows=N0, n_genes=G0), dev, chunk_rows, upload_and_count)
             st = stats.cpu().numpy()
@@ -140,7 +148,7 @@ class PackedDeviceDataset(_Dataset):
             cell_mask = np.ones(N0, bool)
             if filter_min_counts:
                 gene_mask = gene_tot >= 1
-                if not gene_mask.all() and gene_mask.sum() % 8 != 0:
+                if not gene_mask.all() and gene_mask.sum() % 8 != 0 and not pad_genes:
                     raise ValueError("filtering leaves %d genes; the packed format needs a multiple of 8 "
                                      "(filter the genes before, or use the resident device path)" % gene_mask.sum())
                 cell_mask = nc >= 1
@@ -164,22 +172,26 @@ class PackedDeviceDataset(_Dataset):
             pd.desc.n_counts = pd.n_counts.data_ptr()
             mean, std = _moments(SimpleNamespace(n_rows=N, n_genes=G), nc, med, flags, dev, chunk_rows, pd._chunks)
         pd.n_counts_host, pd.size_factors_host, pd.mean, pd.std, pd.median, pd.flags = nc, sf_h, mean, std, med, flags
-        pd._mean_d = torch.from_numpy(mean).to(dev)
-        pd._std_d = torch.from_numpy(std).to(dev)
+        Gp = int(pd.desc.genes)                          # the expansion reads per-gene statistics at the stored width
+        pd._mean_d = torch.from_numpy(_pad_stats(mean, Gp, 0.0)).to(dev)
+        pd._std_d = torch.from_numpy(_pad_stats(std, Gp, 1.0)).to(dev)
         pd.gene_totals_host, pd.input_gene_totals, pd.n_bad = gene_tot, input_gene_totals, input_n_bad
         pd.gene_mask, pd.cell_mask, pd.sf_mask = gene_mask, cell_mask, sf_mask
         return pd
 
     @classmethod
     def _pack(cls, lib, host, st, keep, cols, all_genes, bits, dev, chunk_rows):
-        """Pass 2 over the host counts: the kept rows ``keep`` and genes ``cols`` packed into new device arrays."""
+        """Pass 2 over the host counts: the kept rows ``keep`` and genes ``cols`` packed into new device arrays, at the
+        stored width Gp (the gene count rounded up to a multiple of 8; the pad genes hold no count, so the per-row
+        statistics ``st`` stand for the padded rows)."""
         N0, G0 = host.N, host.G
         N, G = int(keep.size), int(cols.size)
-        w = choose_format(int(st[0, keep].sum()), st[1:4, keep], N, G, bits)
+        Gp = (G + 7) // 8 * 8
+        w = choose_format(int(st[0, keep].sum()), st[1:4, keep], N, Gp, bits)
         keep_d = torch.from_numpy(keep).to(dev)
         pd = cls.__new__(cls)
-        pd.bits = w
-        row_bytes = G // 8 if w == 1 else G * w // 8
+        pd.bits, pd.genes = w, G
+        row_bytes = Gp // 8 if w == 1 else Gp * w // 8
         pd.packed = torch.empty(N * row_bytes, dtype=torch.uint8, device=dev)
         pd.ovf_indptr = torch.zeros(N + 1, dtype=torch.int64, device=dev)
         pd.ovf_indptr[1:] = torch.cumsum(torch.from_numpy(st[_ESC_ROW[w]]).to(dev)[keep_d], 0)
@@ -196,12 +208,14 @@ class PackedDeviceDataset(_Dataset):
             pd.nib_indptr = pd.nibbles = None
         pd.rows = torch.arange(N, dtype=torch.int32, device=dev)
         pd.desc = _lib.PackedCountsDesc(
-            C.sizeof(_lib.PackedCountsDesc), w, N, G, max_nib, pd.packed.data_ptr(),
+            C.sizeof(_lib.PackedCountsDesc), w, N, Gp, max_nib, pd.packed.data_ptr(),
             pd.ovf_indptr.data_ptr() if n_ovf else None, pd.entries.data_ptr() if n_ovf else None,
             pd.nib_indptr.data_ptr() if w == 1 else None, pd.nibbles.data_ptr() if w == 1 else None, None)
         cols_d = None if all_genes else torch.from_numpy(cols.astype(np.int32)).to(dev)
         chunk = min(N0, chunk_rows or _chunk_rows(G0))
-        sel = torch.empty((chunk, G), dtype=torch.float32, device=dev) if (cols_d is not None or N != N0) else None
+        # the kept rows and genes of a chunk, Gp wide: the pad columns are zeroed once and never written
+        sel = (torch.zeros((chunk, Gp), dtype=torch.float32, device=dev)
+               if (cols_d is not None or N != N0 or Gp != G) else None)
 
         def pack(r0, n, Y):
             a, b = np.searchsorted(keep, [r0, r0 + n])
@@ -210,20 +224,22 @@ class PackedDeviceDataset(_Dataset):
             src = Y
             if sel is not None:                          # the kept rows and genes of the chunk (dca_gather_counts)
                 local = torch.from_numpy((keep[a:b] - r0).astype(np.int32)).to(dev)
-                check(lib.dca_gather_counts(Y.data_ptr(), G0, local.data_ptr(), int(b - a),
-                                            None if cols_d is None else cols_d.data_ptr(), G, sel.data_ptr(), G,
+                check(lib.dca_gather_counts(Y.data_ptr(), host.ld, local.data_ptr(), int(b - a),
+                                            None if cols_d is None else cols_d.data_ptr(), G, sel.data_ptr(), Gp,
                                             _stream(dev)), "dca_gather_counts")
                 src = sel
-            check(lib.dca_pack_rows_device(src.data_ptr(), G, int(b - a), int(a), C.byref(pd.desc), _stream(dev)),
+            check(lib.dca_pack_rows_device(src.data_ptr(), src.stride(0), int(b - a), int(a), C.byref(pd.desc),
+                                           _stream(dev)),
                   "dca_pack_rows_device")
         host(chunk, pack)
         return pd
 
     def _chunks(self, chunk, fn):
         """fn(r0, n, Y) for consecutive row chunks of every storage row, Y expanded from the packed arrays (the
-        statistics passes read the counts from here: no second host upload)."""
+        statistics passes read the counts from here: no second host upload); Y holds the real genes, a view with row
+        stride desc.genes that drops the pad genes."""
         lib = _lib.load()
-        dev, G, N = self.device, self.n_genes, int(self.desc.n_rows)
+        dev, G, N = self.device, int(self.desc.genes), int(self.desc.n_rows)
         Y = torch.empty((chunk, G), dtype=torch.float32, device=dev)
         X = torch.empty((chunk, G), dtype=torch.bfloat16, device=dev)
         sf = torch.empty(chunk, dtype=torch.float32, device=dev)
@@ -234,7 +250,7 @@ class PackedDeviceDataset(_Dataset):
             check(lib.dca_expand_rows_exact(C.byref(self.desc), r.data_ptr(), n, 1.0, 0, zero.data_ptr(), one.data_ptr(),
                                             Y.data_ptr(), X.data_ptr(), _lib.BF16, sf.data_ptr(), _stream(dev)),
                   "dca_expand_rows_exact")
-            fn(r0, n, Y)
+            fn(r0, n, Y[:, :self.n_genes])
 
     # ------------------------------------------------------------------ views
     def take(self, mask_or_index):
@@ -250,8 +266,8 @@ class PackedDeviceDataset(_Dataset):
 
     def expand(self):
         """(Y, X, sf) of this dataset's cells on the device, expanded by row index (dca_expand_rows_exact): the rows of
-        a DeviceDataset's Y, X and sf for the same cells."""
-        n, G = self.n, self.n_genes
+        a DeviceDataset's Y, X and sf for the same cells (expanded at the stored width, returned over the real genes)."""
+        n, G = self.n, int(self.desc.genes)
         Y = torch.empty((n, G), dtype=torch.float32, device=self.device)
         X = torch.empty((n, G), dtype=self.x_dtype, device=self.device)
         sf = torch.empty(n, dtype=torch.float32, device=self.device)
@@ -259,13 +275,15 @@ class PackedDeviceDataset(_Dataset):
                                                 self._mean_d.data_ptr(), self._std_d.data_ptr(), Y.data_ptr(),
                                                 X.data_ptr(), _lib.BF16 if self.x_dtype == torch.bfloat16 else _lib.F32,
                                                 sf.data_ptr(), _stream(self.device)), "dca_expand_rows_exact")
+        if G != self.n_genes:
+            Y, X = Y[:, :self.n_genes].contiguous(), X[:, :self.n_genes].contiguous()
         torch.cuda.synchronize(self.device)
         return Y, X, sf
 
     def host_packed(self):
         """Host copy of the packed arrays as an io.PackedCounts over every storage row (the bytes io.pack_rows writes
-        for the same counts)."""
-        N, G = int(self.desc.n_rows), self.n_genes
+        for the same counts, pad genes included)."""
+        N, G = int(self.desc.n_rows), int(self.desc.genes)
         packed = self.packed.cpu().numpy()
         if self.bits == 16:
             packed = packed.view(np.uint16)
@@ -273,8 +291,9 @@ class PackedDeviceDataset(_Dataset):
         indptr = self.ovf_indptr.cpu().numpy()
         entries = self.entries.cpu().numpy()[: 8 * int(indptr[-1])].view(dio.OVERFLOW_ENTRY)
         if self.bits != 1:
-            return dio.PackedCounts(packed, self.bits, G, indptr, entries)
-        return dio.PackedCounts(packed, 1, G, indptr, entries, self.nib_indptr.cpu().numpy(), self.nibbles.cpu().numpy())
+            return dio.PackedCounts(packed, self.bits, G, indptr, entries, genes=self.n_genes)
+        return dio.PackedCounts(packed, 1, G, indptr, entries, self.nib_indptr.cpu().numpy(), self.nibbles.cpu().numpy(),
+                                genes=self.n_genes)
 
     def device_bytes(self) -> int:
         """Device memory the dataset holds: packed arrays, row totals and the row map."""

@@ -9,7 +9,10 @@ matrix ever exists in device memory, and no normalised matrix exists on the host
 
 On the same counts every result is bit-identical to ``device_data.DeviceDataset`` (dca/io.py:88-111 computed in HBM):
 size factors, n_counts, gene totals, mean, std and every X the training step and predict read.  The counts must be
-non-negative integers and the gene count a multiple of 8 (the packed format).
+non-negative integers.  With ``pad_genes=True`` any gene count is accepted, before and after filtering: the rows are
+packed at the gene count rounded up to a multiple of 8, the pad genes all zero (io.pack_rows(..., pad_genes=True)),
+and the statistics, the expansion and the model see the real genes only.  With the default ``pad_genes=False`` the
+gene count must be a multiple of 8.
 """
 from __future__ import annotations
 
@@ -111,7 +114,8 @@ def _chunk_bounds(pc, chunk_rows):
 
 
 def for_each_chunk(pc, dev, chunk_rows, fn):
-    """fn(r0, n, Y) for consecutive row chunks of pc in order, Y = the chunk's fp32 counts on the device.  The packed bytes
+    """fn(r0, n, Y) for consecutive row chunks of pc in order, Y = the chunk's fp32 counts of the pc.genes real genes
+    on the device (a view with row stride pc.n_genes: the pad genes are dropped).  The packed bytes
     of the next chunk are copied host->device on a side stream while the current one is expanded and processed
     (two staging buffers); everything else runs on the current stream."""
     lib = _lib.load()
@@ -146,13 +150,14 @@ def for_each_chunk(pc, dev, chunk_rows, fn):
         stage[k % 2].expand(lib, pc, n, has_ovf, mnib, Y, X, torch.bfloat16, dev)
         freed[k % 2] = torch.cuda.Event()
         freed[k % 2].record(comp)
-        fn(bounds[k], n, Y)
+        fn(bounds[k], n, Y[:, :pc.genes])
     torch.cuda.synchronize(dev)
 
 
 def expand_exact(pc, n_counts, median, flags, mean, std, x_dtype, dev):
     """Y (fp32), X (x_dtype) and sf (fp32) of every row of pc on the device through the exact expansion: the rows of a
-    DeviceDataset's Y, X and sf for the same cells.  n_counts: host fp64 [pc.n_rows]; mean / std: host fp64."""
+    DeviceDataset's Y, X and sf for the same cells (pc.genes columns).  n_counts: host fp64 [pc.n_rows]; mean / std:
+    host fp64 [pc.genes].  The rows are expanded at the stored width, the pad genes with mean 0 and std 1."""
     lib = _lib.load()
     n, G = pc.n_rows, pc.n_genes
     _, max_e, max_nib = _chunk_bounds(pc, max(n, 1))
@@ -163,11 +168,20 @@ def expand_exact(pc, n_counts, median, flags, mean, std, x_dtype, dev):
     X = torch.empty((n, G), dtype=x_dtype, device=dev)
     sf = torch.empty(n, dtype=torch.float32, device=dev)
     nc = torch.from_numpy(np.ascontiguousarray(n_counts, dtype=np.float64)).to(dev)
-    md = torch.from_numpy(np.ascontiguousarray(mean, dtype=np.float64)).to(dev)
-    sd = torch.from_numpy(np.ascontiguousarray(std, dtype=np.float64)).to(dev)
+    md = torch.from_numpy(_pad_stats(mean, G, 0.0)).to(dev)
+    sd = torch.from_numpy(_pad_stats(std, G, 1.0)).to(dev)
     pk.expand(lib, pc, n, has_ovf, mnib, Y, X, x_dtype, dev, exact=(nc, median, flags, md, sd, sf))
+    if pc.genes != G:
+        Y, X = Y[:, :pc.genes].contiguous(), X[:, :pc.genes].contiguous()
     torch.cuda.synchronize(dev)
     return Y, X, sf
+
+
+def _pad_stats(v, width, fill):
+    """fp64 per-gene vector v extended to ``width`` entries with ``fill`` (the pad genes' neutral mean 0 / std 1)."""
+    out = np.full(width, fill, dtype=np.float64)
+    out[:len(v)] = v
+    return out
 
 
 def stream_epoch(eng, n, batch, shuffle, begin):
@@ -207,26 +221,28 @@ class StreamedDataset(_Dataset):
 
     @property
     def n_genes(self) -> int:
-        return self.pc.n_genes
+        return self.pc.genes
 
     @classmethod
     def from_counts(cls, counts, device=None, x_dtype="float32", size_factors=True, logtrans_input=True,
-                    normalize_input=True, filter_min_counts=False, batch=32, bits="auto", chunk_rows=None):
+                    normalize_input=True, filter_min_counts=False, batch=32, bits="auto", chunk_rows=None,
+                    pad_genes=False):
         """counts: cells x genes, a dense ndarray or a scipy.sparse CSR matrix of raw counts (a CSR matrix is packed in
         row chunks and never densified whole).  The filtering and normalisation steps of io.normalize with the same
         flags; x_dtype 'float32' | 'bfloat16' (the X the training step reads); batch: the training batch the packing
         the format is chosen for (overflow entries per batch; the streaming calls check and, where needed, widen the
         packing for the batch they stream in: stream_batches); chunk_rows: rows per chunk of the statistics passes
-        (default: 256 MB of fp32 counts)."""
+        (default: 256 MB of fp32 counts); pad_genes: accept a gene count off a multiple of 8, before and after the
+        gene filter (the rows are packed zero-padded to the next multiple of 8; every result covers the real genes)."""
         if not torch.cuda.is_available():
             raise _lib.DcaError("StreamedDataset needs a CUDA device (H100); there is no CPU fallback")
         dev, xdt = _device(device), _X_DTYPES[x_dtype]
         counts = _counts_matrix(counts)
         N0, G0 = (int(s) for s in counts.shape)
-        if G0 % 8 != 0:
+        if G0 % 8 != 0 and not pad_genes:
             raise ValueError("streaming from packed counts needs a gene count that is a multiple of 8 (got %d)" % G0)
         with torch.cuda.device(dev):
-            pc = dio.pack_rows(counts, bits, batch=batch)
+            pc = dio.pack_rows(counts, bits, batch=batch, pad_genes=pad_genes)
             nc, gene_tot, n_bad = _totals(pc, dev, chunk_rows)
             input_gene_totals, input_n_bad = gene_tot, n_bad
             gene_mask = np.ones(G0, bool)
@@ -234,11 +250,11 @@ class StreamedDataset(_Dataset):
             if filter_min_counts:                                            # dca/io.py:90-92
                 gene_mask = gene_tot >= 1
                 if not gene_mask.all():
-                    if gene_mask.sum() % 8 != 0:
+                    if gene_mask.sum() % 8 != 0 and not pad_genes:
                         raise ValueError("filtering leaves %d genes; streaming from packed counts needs a multiple of 8 "
                                          "(filter the genes before, or use the resident device path)" % gene_mask.sum())
                     counts = counts[:, np.flatnonzero(gene_mask)]
-                    pc = dio.pack_rows(counts, bits, batch=batch)
+                    pc = dio.pack_rows(counts, bits, batch=batch, pad_genes=pad_genes)
                     nc, gene_tot, _ = _totals(pc, dev, chunk_rows)
                 cell_mask = nc >= 1
                 if not cell_mask.all():
@@ -344,6 +360,10 @@ class StreamedDataset(_Dataset):
         return run, theta, session
 
 
+def _genes(pc):
+    return getattr(pc, "genes", pc.n_genes)
+
+
 def _chunk_rows(G):
     return max(1, _CHUNK_BYTES // (4 * G))
 
@@ -357,9 +377,10 @@ def _workspace(lib, N, G, chunk, dev):
 def _totals(pc, dev, chunk_rows=None, chunks=None):
     """(n_counts fp64 [N], gene totals fp64 [G], number of bad entries) on the host.  chunks(chunk, fn) feeds the row
     chunks of the matrix to fn(r0, n, Y) (default: for_each_chunk over the packed host counts pc); pc then only needs
-    n_rows and n_genes."""
+    n_rows and n_genes.  G: pc.genes when pc has it (the real genes of padded rows), else pc.n_genes; Y may have a row
+    stride above G."""
     lib = _lib.load()
-    N, G = pc.n_rows, pc.n_genes
+    N, G = pc.n_rows, _genes(pc)
     chunk = min(N, chunk_rows or _chunk_rows(G))
     ws = _workspace(lib, N, G, chunk, dev)
     n_counts = torch.empty(N, dtype=torch.float64, device=dev)
@@ -368,7 +389,7 @@ def _totals(pc, dev, chunk_rows=None, chunks=None):
     check(lib.dca_stats_begin(N, G, ws.data_ptr(), ws.numel(), _stream(dev)), "dca_stats_begin")
 
     def rows(r0, n, Y):
-        check(lib.dca_count_totals_rows(Y.data_ptr(), G, r0, n, N, G, n_counts.data_ptr(), ws.data_ptr(), ws.numel(),
+        check(lib.dca_count_totals_rows(Y.data_ptr(), Y.stride(0), r0, n, N, G, n_counts.data_ptr(), ws.data_ptr(), ws.numel(),
                                         _stream(dev)), "dca_count_totals_rows")
     (chunks or (lambda c, fn: for_each_chunk(pc, dev, c, fn)))(chunk, rows)
     check(lib.dca_count_totals_finish(N, G, gene_tot.data_ptr(), n_bad.data_ptr(), ws.data_ptr(), ws.numel(),
@@ -380,7 +401,7 @@ def _moments(pc, nc_host, median, flags, dev, chunk_rows=None, chunks=None):
     """Gene mean and std (fp64, host) of l over the rows of pc: passes 1 and 2 of dca_log_moments (chunks: as for
     _totals)."""
     lib = _lib.load()
-    N, G = pc.n_rows, pc.n_genes
+    N, G = pc.n_rows, _genes(pc)
     chunk = min(N, chunk_rows or _chunk_rows(G))
     ws = _workspace(lib, N, G, chunk, dev)
     nc = torch.from_numpy(np.ascontiguousarray(nc_host, dtype=np.float64)).to(dev) if flags & PRE_SIZE_FACTORS else None
@@ -390,7 +411,7 @@ def _moments(pc, nc_host, median, flags, dev, chunk_rows=None, chunks=None):
         check(lib.dca_stats_begin(N, G, ws.data_ptr(), ws.numel(), _stream(dev)), "dca_stats_begin")
         if flags & 4:                           # DCA_PRE_SCALE: otherwise mean = 0, std = 1 without reading the counts
             def rows(r0, n, Y, p=p):
-                check(lib.dca_log_moments_rows(p, Y.data_ptr(), G, r0, n, N, G, ncp, median, flags, out[0].data_ptr(),
+                check(lib.dca_log_moments_rows(p, Y.data_ptr(), Y.stride(0), r0, n, N, G, ncp, median, flags, out[0].data_ptr(),
                                                ws.data_ptr(), ws.numel(), _stream(dev)), "dca_log_moments_rows")
             (chunks or (lambda c, fn: for_each_chunk(pc, dev, c, fn)))(chunk, rows)
         check(lib.dca_log_moments_finish(p, N, G, flags, out[p - 1].data_ptr(), ws.data_ptr(), ws.numel(), _stream(dev)),

@@ -256,12 +256,16 @@ int dca_stream_begin(dca_handle* h, const uint16_t* counts_host, int64_t ld_coun
  * int64[n_rows+1], ovf_entries_host {int32 gene; float count}[ovf_indptr[n_rows]] sorted by row; each step
  * copies its batch's segment with the tile and patches the escapes on the device.  Both NULL: no escapes
  * (2^bits-1 is a literal count).  A batch may carry at most max_batch*n_in/32 (>= 4096) overflow entries.
- * dca_b200/io.py:pack_counts builds the format; dca_stream_begin(...) == bits 16 without an overflow list. */
+ * dca_b200/io.py:pack_counts builds the format; dca_stream_begin(...) == bits 16 without an overflow list.
+ * Ragged gene counts: the rows are Gp = n_in rounded up to a multiple of 8 entries wide, the Gp - n_in pad genes
+ * zero counts (io.pack_rows(..., pad_genes=True)).  Batches are expanded Gp wide and the step reads their first n_in
+ * columns; the pad genes never reach the model, its loss or its outputs.  Such an engine streams only with the exact
+ * transform (dca_set_input_transform_exact), which gives the pad genes mean 0 and std 1. */
 int dca_stream_begin_packed(dca_handle* h, const void* packed_host, int32_t bits, int64_t row_bytes,
                             const int64_t* ovf_indptr_host, const void* ovf_entries_host, const float* sf_host,
                             int64_t n_rows, int32_t batch, void* stream);
 /* Sparse host format for matrices with <= 50 % non-zero entries (scRNA-seq: ~10-20 %): bitmap_host = one bit per entry
- * (row-major, n_in/8 bytes per row, bit g%8 of byte g/8 set when the count is non-zero), nibbles_host = the non-zero counts
+ * (row-major, Gp/8 bytes per row, bit g%8 of byte g/8 set when the count is non-zero), nibbles_host = the non-zero counts
  * of every row as consecutive 4-bit codes in gene order (low nibble first; 1..14 literal, 15 = escape into the overflow
  * list above), each row starting on a byte boundary at nib_indptr_host[row] (int64[n_rows+1], byte offsets).  ~0.2 bytes
  * per entry cross PCIe per step instead of 0.5 (4-bit dense) or the reference's 8 (float32 X + Y, dca/train.py:78-98).
@@ -332,7 +336,7 @@ typedef struct dca_packed_counts {
   int32_t struct_bytes;           /* sizeof(dca_packed_counts), ABI guard */
   int32_t bits;                   /* 1 (sparse: bitmap + 4-bit codes of the non-zeros), 4, 8 or 16 bits per entry */
   int64_t n_rows;
-  int32_t genes;                  /* a multiple of 8 */
+  int32_t genes;                  /* the stored width, a multiple of 8: an engine's n_in rounded up (pad genes are zero) */
   int32_t max_row_nibble_bytes;   /* sparse: the longest row's code bytes (sizes the expansion's shared memory) */
   const void* packed;             /* [n_rows x genes*bits/8] bytes, 16-byte aligned (sparse: the bitmap) */
   const int64_t* ovf_indptr;      /* int64 [n_rows + 1], absolute offsets into ovf_entries; NULL: no overflow entries */
@@ -363,7 +367,8 @@ int dca_expand_rows_exact(const dca_packed_counts* src, const int32_t* rows, int
  * transform of dca_set_input_transform_exact (which must come first) into the engine's expanded-batch staging (bf16 X
  * for the tensor-core encoder) on `stream`, then the step runs on that contiguous batch.  The same bits as the step on
  * a resident dataset of the same cells.  DCA_ERR_BAD_ARG while a host stream is active (dca_stream_begin*);
- * DCA_ERR_UNSUPPORTED when n_in != n_out or n_in % 8 != 0. */
+ * DCA_ERR_UNSUPPORTED when n_in != n_out; DCA_ERR_BAD_ARG when src->genes is not n_in rounded up to a multiple of 8
+ * (the pad genes of a ragged n_in are expanded with the batch and never reach the model). */
 int dca_packed_train_step(dca_handle* h, const dca_packed_counts* src, const int32_t* rows, int32_t batch, void* stream);
 int dca_packed_eval_step(dca_handle* h, const dca_packed_counts* src, const int32_t* rows, int32_t batch, void* stream);
 int dca_packed_predict(dca_handle* h, const dca_packed_counts* src, const int32_t* rows, int32_t batch, float* mean_out,
