@@ -127,6 +127,7 @@ PROTOTYPES = {
     "dca_tc_gene_gemm_rows": (C.c_int, [_i32, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _i64, _i32, _vp, _vp, _vp, _vp, _i32]),
     "dca_head_bwd_schedule": (C.c_int, [_i32, _i32, _i32, _i32, _i32, _vp, _i64, C.POINTER(_i64), _vp]),
+    "dca_enc_bwd_schedule": (C.c_int, [_i32, _i32, _vp, _i64, _vp]),
     "dca_tc_probe": (C.c_int, [_vp, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32,
                                _vp, _vp]),
     "dca_profile_enable": (C.c_int, [_vp, _i32]),

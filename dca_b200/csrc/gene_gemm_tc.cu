@@ -4,7 +4,9 @@
 //   encoder forward  (K1)  A1[B x 64]  += X[B x G] . W1[G x 64]                      (b), W MN-major
 //   head backward    (K4)  dH3[B x 64] += sum_h dZ_h . Wh^T                          (b), W K-major
 //                          dWh[64 x G] += H3^T . dZ_h,  db_h += colsum(dZ_h)         (a) + column sums
-//   encoder backward (K5)  dW1[G x 64] += X^T . dA1                                   (a)
+//   encoder backward (K5)  dW1[G x 64] += X^T . dA1                                   (a), 64-gene blocks
+//
+// K5 has a kernel of its own (gene_gemm_enc_bwd_kernel, below) that spreads 64-gene blocks evenly over the SMs.
 //
 // "Z" is the cells x genes bf16 operand (X or dZ), brought into shared memory by TMA as 128-cell x 128-gene tiles
 // (two SWIZZLE_128B boxes of 64 genes).  K1 and K5 may instead name the batch's cells by row index into a larger X
@@ -150,7 +152,7 @@ gene_gemm_kernel(const __grid_constant__ CUtensorMap map_z0, const __grid_consta
   // CTA consumed in earlier items, so that stage and mbarrier phase continue across items (every issued tile is consumed
   // before the next item starts).
   uint32_t T0 = 0;
-  // Gathered rows (Params::rows; K1 / K5): the Z half of a stage is filled by all 256 threads with 16-byte cp.async
+  // Gathered rows (Params::rows; K1): the Z half of a stage is filled by all 256 threads with 16-byte cp.async
   // copies instead of TMA boxes (a TMA box per 128-byte row half issues too slowly).  Thread (rh = tid / 8, c = tid % 8)
   // copies chunk c (genes 8c .. 8c+7) of half rh % 2 of tile rows rh / 2 + 16 i, i < 8: each warp instruction reads
   // four whole 128-byte row halves.  A chunk goes where SWIZZLE_128B puts it -- chunk c of row r at byte
@@ -403,6 +405,158 @@ void plan_banded(Params& p, int n_heads, int sm_count, int* grid) {
   *grid = min(p.total_items, sm_count >= band ? sm_count / band * band : sm_count);
 }
 
+// ------------------------------------------------------------------------------------ encoder backward (K5)
+// dW1[G x 64] += X^T . dA1 in 64-gene blocks: one warpgroup owns a block over all cells, which is the (a) product of
+// the gene_gemm_kernel warpgroup for those genes -- the same m64n64k16 chain over cell tiles 0, 1, ... and k16 steps in
+// order, from zero, added to dW once by a staging-tile reduce-add -- so dW1 has the same bits whatever the schedule.
+// CTA c of `ctas` owns the contiguous blocks [eb_first(c), eb_first(c + 1)), within one of each other in count, and
+// walks them in passes of up to kEbMaxW blocks, one consumer warpgroup each, sharing each stage's dA1 tile.  At
+// G = 20000 (313 blocks) on 132 SMs that is 3 blocks on 49 CTAs and 2 on 83, one pass each: 3 x 64 genes in the
+// longest lane, where 128-gene items take 4 x 64 (two rounds of one item or one round of two).
+constexpr int kEbMaxW = 3;                                 // 64-gene blocks per pass = consumer warpgroups
+constexpr int kEbThreads = 128 * kEbMaxW;
+constexpr uint32_t kEbSub = 128 * 128;                     // [128 cells x 64 genes] bf16: one SWIZZLE_128B box
+constexpr uint32_t kEbStage = kEbMaxW * kEbSub + kHBytes;  // X sub-tiles of the pass's blocks | dA1 tile
+constexpr int kEbStages = 3;
+constexpr uint32_t kEbSmem = kEbStages * kEbStage + 1024;
+static_assert(kEbMaxW * 64 * 64 * 4 <= kEbStage, "the flush staging tiles fit in the first stage");
+
+struct EncBwdParams {
+  int B, G, n_cb, n_blk;          // cell blocks (128), gene blocks (64)
+  const int32_t* rows; const __nv_bfloat16* zsrc; int64_t ldz;   // gathered rows as in Params; rows == null: map_z
+};
+
+// first 64-gene block of CTA c (c = ctas: n_blk); the first n_blk % ctas CTAs own one block more than the others
+__host__ __device__ inline int eb_first(int c, int n_blk, int ctas) { return c * (n_blk / ctas) + min(c, n_blk % ctas); }
+inline int eb_ctas(int n_blk, int sm_count) { return max(1, min(sm_count, n_blk)); }
+
+__global__ void __launch_bounds__(kEbThreads, 1)
+gene_gemm_enc_bwd_kernel(const __grid_constant__ CUtensorMap map_z, const __grid_constant__ CUtensorMap map_h,
+                         const __grid_constant__ CUtensorMap map_dw, const int dw_transposed, const EncBwdParams p) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* s_st = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // [kEbStages][X x kEbMaxW | dA1]
+  __shared__ uint64_t full[kEbStages];
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < kEbStages; ++i) mbar_init(&full[i], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  const int wg = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+  const int frow = 16 * w + (l >> 2), fcol = 2 * (l & 3);
+  // Gathered rows: warpgroup wg copies its own block's sub-tile, thread (r0 = tid / 8, c = tid % 8) chunk c of tile rows
+  // r0 + 16 i, i < 8, at its SWIZZLE_128B place (as in gene_gemm_kernel, one 64-gene half per warpgroup)
+  const bool gather = p.rows != nullptr;
+  const int g_r0 = (threadIdx.x & 127) >> 3, g_c = threadIdx.x & 7;
+  const uint32_t g_dst = wg * kEbSub + g_r0 * 128 + ((g_c ^ (g_r0 & 7)) << 4);
+  int src_row[8];
+
+  const int last = eb_first(blockIdx.x + 1, p.n_blk, gridDim.x);
+  uint32_t T0 = 0;                                 // tiles consumed in earlier passes: stage and phase continue
+  for (int blk0 = eb_first(blockIdx.x, p.n_blk, gridDim.x); blk0 < last; blk0 += kEbMaxW) {
+    const int nw = min(kEbMaxW, last - blk0);
+    const bool mine = wg < nw;                     // this warpgroup owns block blk0 + wg in this pass
+    // the previous pass's flush has read its staging tiles (stage memory) before this pass loads into it
+    if (threadIdx.x == 0) bulk_wait_read<0>();
+    __syncthreads();
+
+    auto issue = [&](int t) {                      // thread 0: dA1 tile t (and the X sub-tiles when not gathered)
+      const int st = (T0 + t) % kEbStages;
+      uint8_t* dst = s_st + st * kEbStage;
+      mbar_expect_tx(&full[st], kHBytes + (gather ? 0u : nw * kEbSub));
+      if (!gather)
+        for (int j = 0; j < nw; ++j) tma_load_2d(dst + j * kEbSub, &map_z, (blk0 + j) * 64, t * 128, &full[st]);
+      tma_load_2d(dst + kEbMaxW * kEbSub, &map_h, 0, t * 128, &full[st]);
+    };
+    auto load_rows = [&](int t) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int r = t * 128 + g_r0 + 16 * i;
+        src_row[i] = r < p.B ? __ldg(p.rows + r) : -1;
+      }
+    };
+    auto copy_rows = [&](int t) {                  // this thread's 8 chunks of its warpgroup's sub-tile of tile t
+      if (mine) {
+        const int g0 = (blk0 + wg) * 64 + g_c * 8;
+        const uint32_t gbytes = g0 < p.G ? (uint32_t)min(16, 2 * (p.G - g0)) : 0u;
+        const uint32_t dst = smem_u32(s_st + ((T0 + t) % kEbStages) * kEbStage) + g_dst;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const bool ok = src_row[i] >= 0 && gbytes != 0;
+          cp_async_16(dst + i * 2048, ok ? p.zsrc + (int64_t)src_row[i] * p.ldz + g0 : p.zsrc, ok ? gbytes : 0u);
+        }
+        if (t + 1 < p.n_cb) load_rows(t + 1);
+      }
+    };
+    if (gather && mine) load_rows(0);
+    for (int t = 0; t < kEbStages - 1; ++t) {      // (gathered rows: one cp.async group per tile slot, empty or not)
+      if (t < p.n_cb) {
+        if (threadIdx.x == 0) issue(t);
+        if (gather) copy_rows(t);
+      }
+      if (gather) cp_async_commit();
+    }
+
+    float acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+    for (int t = 0; t < p.n_cb; ++t) {
+      if (t + kEbStages - 1 < p.n_cb) {            // its stage was released at tile t-1
+        if (threadIdx.x == 0) issue(t + kEbStages - 1);
+        if (gather) copy_rows(t + kEbStages - 1);
+      }
+      if (gather) {
+        cp_async_commit();
+        cp_async_wait<kEbStages - 1>();
+        fence_proxy_async_smem();
+        __syncthreads();
+      }
+      const int st = (T0 + t) % kEbStages;
+      mbar_wait(&full[st], ((T0 + t) / kEbStages) & 1);
+      if (mine) {
+        const uint32_t zb = smem_u32(s_st + st * kEbStage) + wg * kEbSub, hb = smem_u32(s_st + st * kEbStage) + kEbMaxW * kEbSub;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+          wgmma_m64n64k16<1, 1>(acc, make_smem_desc(zb + k * 2048, 0, 1024), make_smem_desc(hb + k * 2048, 0, 1024), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        acc_fence(acc);
+      }
+      __syncthreads();                             // every warpgroup is done with stage st
+    }
+    T0 += p.n_cb;
+
+    // flush: every tile is consumed, so block j's [64 x 64] fp32 staging tile goes at byte j * kEbSub of the stages
+    float* s_o = reinterpret_cast<float*>(s_st + wg * kEbSub);
+    if (mine) {
+      if (dw_transposed) {                         // Keras [64 x G]: staging [64 feats][64 genes]
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int g = frow + 8 * ((i >> 1) & 1), f = 8 * (i >> 2) + fcol + (i & 1);
+          s_o[f * 64 + g] = acc[i];
+        }
+      } else {                                     // [G x 64]: staging [64 genes][64 feats]
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+          const int g = frow + 8 * ((i >> 1) & 1), f = 8 * (i >> 2) + fcol;
+          *reinterpret_cast<float2*>(s_o + g * 64 + f) = make_float2(acc[i], acc[i + 1]);
+        }
+      }
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int j = 0; j < nw; ++j) {
+        const int g = (blk0 + j) * 64;
+        tma_reduce_add_2d(&map_dw, dw_transposed ? g : 0, dw_transposed ? 0 : g, s_st + j * kEbSub);
+      }
+      bulk_commit();
+    }
+  }
+  if (threadIdx.x == 0) bulk_wait<0>();
+}
+
 }  // namespace gg
 
 size_t gene_gemm_workspace_bytes(int B) { return sizeof(float) * (size_t)gg::kMaxSlots * cdiv(B, 128) * 128 * 64; }
@@ -474,12 +628,21 @@ int gene_gemm_tc(int mode, const __nv_bfloat16* const Z[3], int64_t ldz, const i
     DCA_LAUNCH_CHECK();
     return DCA_OK;
   }
-  if (do_a) {
+  if (mode == 2) {        // 64-gene blocks, the staging tile one block: [64 x 64] boxes of dW
+    EncBwdParams p{B, G, base.n_cb, cdiv(G, 64), rows, Z[0], ldz};
+    CUtensorMap mdw64;
+    if (dW_transposed) DCA_TRY(make_tensor_map_2d(&mdw64, dW[0], 4, 0, 64, (uint64_t)G, (uint64_t)dW_ld, 64, 64, 0));
+    else DCA_TRY(make_tensor_map_2d(&mdw64, dW[0], 4, 0, (uint64_t)G, 64, 64, 64, 64, 0));
+    static bool attr = false;
+    if (!attr) { DCA_CUDA_OK(cudaFuncSetAttribute(gene_gemm_enc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEbSmem)); attr = true; }
+    gene_gemm_enc_bwd_kernel<<<eb_ctas(p.n_blk, sm_count), kEbThreads, kEbSmem, s>>>(mz[0], mh, mdw64, dW_transposed, p);
+    DCA_LAUNCH_CHECK();
+    return DCA_OK;
+  }
+  if (do_a) {             // head backward, dW / db pass
     Params p = base;
     plan_a(p, n_heads, sm_count);
-    const int grid = min(p.total_items, sm_count);
-    if (mode == 3) DCA_GG_LAUNCH(p, grid, true, false, true, false, kMaxGb, false);
-    else DCA_GG_LAUNCH(p, grid, true, false, false, false, kMaxGb, false);
+    DCA_GG_LAUNCH(p, min(p.total_items, sm_count), true, false, true, false, kMaxGb, false);
   }
   if (do_b) {
     Params p = base;
@@ -576,5 +739,12 @@ extern "C" int dca_head_bwd_schedule(int32_t batch, int32_t genes, int32_t n_hea
     }
   }
   *n_items = k;
+  return DCA_OK;
+}
+extern "C" int dca_enc_bwd_schedule(int32_t genes, int32_t sm_count, int32_t* first, int64_t cap, int32_t* ctas) {
+  if (genes <= 0 || sm_count < 1 || !ctas) { set_error("dca_enc_bwd_schedule: bad argument"); return DCA_ERR_BAD_ARG; }
+  const int n_blk = cdiv(genes, 64);
+  *ctas = tc::gg::eb_ctas(n_blk, sm_count);
+  for (int64_t c = 0; first && c < cap && c <= *ctas; ++c) first[c] = tc::gg::eb_first((int)c, n_blk, *ctas);
   return DCA_OK;
 }

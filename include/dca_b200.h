@@ -479,6 +479,12 @@ int dca_tc_gene_gemm_rows(int32_t mode, const void* Z0, const void* Z1, const vo
  * launch's items c, c + grid, c + 2 grid, ... */
 int dca_head_bwd_schedule(int32_t batch, int32_t genes, int32_t n_heads, int32_t sm_count, int32_t banded,
                           int32_t* items, int64_t cap, int64_t* n_items, int32_t* grid);
+/* The schedule of mode 2 (host only, no device needed) for `genes` genes and a grid of at most sm_count CTAs.  The
+ * genes are cut into blocks of 64 (the last may be shorter); CTA c owns blocks first[c] .. first[c + 1] - 1, a
+ * contiguous run, and the runs differ in length by at most one.  Writes *ctas and min(*ctas + 1, cap) entries of first
+ * (may be NULL).  Each block's dW rows are summed over all cells by one warpgroup, in cell order, so the schedule does
+ * not change the bits of dW. */
+int dca_enc_bwd_schedule(int32_t genes, int32_t sm_count, int32_t* first, int64_t cap, int32_t* ctas);
 
 /* ---- preprocessing of raw counts in HBM (csrc/preprocess.cu) ------------------------------------------------------
  * dca/io.py:88-111 -- scanpy's pp.filter_genes / pp.filter_cells(min_counts=1), pp.normalize_per_cell, pp.log1p and
