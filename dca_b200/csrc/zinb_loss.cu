@@ -12,7 +12,6 @@
 #include "zinb_math.cuh"
 #include "tc_common.cuh"
 #include "head_act.cuh"
-#include <cstdlib>
 
 namespace dca {
 namespace tc { extern int g_gg_profile; extern int g_head_bwd_banded; extern int g_head_bwd_stagger; }
@@ -24,10 +23,8 @@ constexpr int kVec = 4;
 constexpr int kColsPerBlock = kThreads * kVec;   // 1024 genes per block
 constexpr int kMaxBlocks = 65536;                // bound of the per-block loss-partial buffer
 
-// Launch tunables (dca_set_tunable; defaults from a launch-parameter sweep, tests/diag_loss_sweep.py)
-struct LossTune { int target_blocks; unsigned producer_sleep_ns, consumer_sleep_ns; int branch_free; int ring; };
-LossTune g_tune = {0 /* auto */, 0u, 0u, 1 /* branch-free zero branch (the faster variant in the sweep) */,
-                   1 /* per-warp rings + f32x2 arithmetic (zinb_loss_bwd_ring_kernel); 0 = block-wide ring (staged kernel) */};
+// Launch-plan override (dca_set_tunable "loss_target_blocks"): blocks per launch, 0 = auto (make_plan)
+int g_target_blocks = 0;
 
 int sm_count_cached() {
   static int n = 0;
@@ -42,7 +39,7 @@ inline Plan make_plan(int B, int G, int cols_per_block, int max_rpb = 1 << 30) {
   p.col_blocks = cdiv(G, cols_per_block);
   // auto: small batches (C2: 4096 x 2000) run as ONE wave of 3 resident blocks per SM (block start-up and the
   // partial last wave cost 15 % there), large ones as ~5 waves for dynamic balance
-  const int target = g_tune.target_blocks > 0 ? g_tune.target_blocks
+  const int target = g_target_blocks > 0 ? g_target_blocks
                      : ((long long)B * G <= (32ll << 20) ? 3 * sm_count_cached() : 16 * sm_count_cached());
   int chunks = target / p.col_blocks;
   if (chunks < 1) chunks = 1;
@@ -187,326 +184,20 @@ zinb_loss_kernel(const float* __restrict__ Y, int64_t ldy, const int32_t* __rest
   if (threadIdx.x == 0) loss_partial[blockIdx.y * gridDim.x + blockIdx.x] = tot;
 }
 
-// ZINB models, 128-bit path, backward: the expensive NB branch (y > 0, ~10-20 % of a scRNA-seq
-// matrix) is warp-compacted through shared memory.  Every lane evaluates the cheap zero branch
-// for its own zero counts; the non-zero elements of the warp's 128-gene strip are queued in
-// shared memory (16 B items), evaluated densely (item i by lane i mod 32) and handed back.
-// Without this the NB branch runs once per vector slot with ~17 % of the lanes active.
-template <bool COND_DISP, typename GT>
-__global__ void __launch_bounds__(kThreads, 4)
-zinb_loss_bwd_compact_kernel(const float* __restrict__ Y, int64_t ldy, const int32_t* __restrict__ rows,
-                             const float* __restrict__ sf, const float* m, const float* d, const float* pi,
-                             int64_t ld, int B, int G, float ridge, float inv_n, int rows_per_block,
-                             GT* dzm, GT* dzd, GT* dzp, float* __restrict__ dth_acc,
-                             double* __restrict__ loss_partial, const float* __restrict__ lf_global) {
-  __shared__ double red[8];
-  __shared__ float lf[zmath::kLogFactN];
-  __shared__ float4 items[kThreads / 32][32 * kVec];                 // 16 KB
-  if (threadIdx.x < zmath::kLogFactN) lf[threadIdx.x] = lf_global[threadIdx.x];
-  __syncthreads();
-  using Ops = zmath::FastOps;
-  constexpr unsigned kFull = 0xffffffffu;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float4* q = items[warp];
-  const int col0 = (blockIdx.x * kThreads + threadIdx.x) * kVec;
-  const bool active = col0 < G;                                       // G % 4 == 0 on this path
-  const int r0 = blockIdx.y * rows_per_block;
-  const int r1 = min(B, r0 + rows_per_block);
-  float lsum = 0.f;
-  float tacc[kVec] = {0.f, 0.f, 0.f, 0.f};
-  float thg[kVec] = {1.f, 1.f, 1.f, 1.f};
-  if (!COND_DISP && active) {
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) thg[j] = d[col0 + j];
-  }
-  RowVals<kVec> cur, nxt;
-  if (active) load_row<true, COND_DISP, kVec>(cur, Y, ldy, rows, sf, m, d, pi, ld, r0, col0);
-  for (int r = r0; r < r1; ++r) {
-    if (active && r + 1 < r1) load_row<true, COND_DISP, kVec>(nxt, Y, ldy, rows, sf, m, d, pi, ld, r + 1, col0);
-    // ---- queue the non-zero counts of this warp's strip (ballot compaction: items ordered by j, then lane)
-    unsigned bal[kVec];
-    int nz = 0;
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) {
-      const bool is_nz = active && !(cur.y[j] < 1e-8f);                                  // loss.py:138
-      bal[j] = __ballot_sync(kFull, is_nz);
-      nz |= is_nz ? (1 << j) : 0;
-    }
-    const unsigned lt = (1u << lane) - 1u;
-    int pos[kVec];
-    int base = 0;
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) { pos[j] = base + __popc(bal[j] & lt); base += __popc(bal[j]); }
-    const int total = base;
-    const float row_sf = __shfl_sync(kFull, active ? cur.sf : 1.0f, 0);                  // lane 0 of an active warp is active
-#pragma unroll
-    for (int j = 0; j < kVec; ++j)
-      if (nz & (1 << j)) q[pos[j]] = make_float4(cur.y[j], cur.m[j], COND_DISP ? cur.d[j] : thg[j], cur.p[j]);
-    __syncwarp();
-    // ---- zero branch for my own zero counts (branch-free per element)
-    float gm[kVec], gd[kVec], gp[kVec];
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) {
-      gm[j] = gd[j] = gp[j] = 0.f;
-      if (active && !(nz & (1 << j))) {
-        const zmath::Elem e = zmath::zinb_elem_zero<Ops, COND_DISP>(cur.m[j], cur.sf, COND_DISP ? cur.d[j] : thg[j], cur.p[j], ridge);
-        lsum += e.loss; gm[j] = e.gm; gd[j] = e.gd; gp[j] = e.gp;
-      }
-    }
-    // ---- dense NB pass over the queue
-    for (int i = lane; i < total; i += 32) {
-      const float4 it = q[i];
-      const zmath::Elem e = zmath::zinb_elem_nb<Ops, true, COND_DISP>(it.x, it.y, row_sf, it.z, it.w, ridge, lf);
-      q[i] = make_float4(e.loss, e.gm, e.gd, e.gp);
-    }
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < kVec; ++j)
-      if (nz & (1 << j)) { const float4 e = q[pos[j]]; lsum += e.x; gm[j] = e.y; gd[j] = e.z; gp[j] = e.w; }
-    __syncwarp();
-    if (active) {
-      const int64_t off = (int64_t)r * ld + col0;
-      if (!COND_DISP) {
-#pragma unroll
-        for (int j = 0; j < kVec; ++j) tacc[j] += gd[j];
-      }
-      st4(dzm + off, gm[0] * inv_n, gm[1] * inv_n, gm[2] * inv_n, gm[3] * inv_n);
-      if (COND_DISP) st4(dzd + off, gd[0] * inv_n, gd[1] * inv_n, gd[2] * inv_n, gd[3] * inv_n);
-      st4(dzp + off, gp[0] * inv_n, gp[1] * inv_n, gp[2] * inv_n, gp[3] * inv_n);
-    }
-    cur = nxt;
-  }
-  if (!COND_DISP && active) {
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) atomicAdd(dth_acc + col0 + j, tacc[j]);
-  }
-  const double tot = block_reduce_sum(lsum, red);
-  if (threadIdx.x == 0) loss_partial[blockIdx.y * gridDim.x + blockIdx.x] = tot;
-}
-
-// Same arithmetic, operands STAGED THROUGH SHARED MEMORY: one producer warp streams the block's rows with bulk
-// async copies (cp.async.bulk global->shared, one 16-byte-aligned row segment per tensor, completion on an
-// mbarrier) into a 3-deep ring, eight consumer warps read their 128-bit vectors from the ring.  The gather of
-// the count rows (rows[]) is free -- the producer simply points the copy at row rows[r] -- and the consumers
-// carry no address arithmetic or load latency, only the math, the warp compaction and the coalesced stores.
-struct FoldArgs {
-  unsigned* counter; double* loss_sum; const double* penalty; float* loss_slot; double* epoch_acc; int batch;
-};
-
-constexpr int kStageRows = 3;
-constexpr int kMaxRowsPerBlock = 256;
-constexpr int kStagedThreads = kThreads + 32;      // 8 consumer warps + 1 producer warp
-
-template <bool COND_DISP, typename GT, bool BF>
-__global__ void __launch_bounds__(kStagedThreads, 3)
-zinb_loss_bwd_staged_kernel(const float* __restrict__ Y, int64_t ldy, const int32_t* __restrict__ rows,
-                            const float* __restrict__ sf, const float* m, const float* d, const float* pi,
-                            int64_t ld, int B, int G, float ridge, float inv_n, int rows_per_block,
-                            GT* dzm, GT* dzd, GT* dzp, float* __restrict__ dth_acc,
-                            double* __restrict__ loss_partial, const float* __restrict__ lf_global, const FoldArgs fa,
-                            const unsigned producer_sleep_ns, const unsigned consumer_sleep_ns) {
-  extern __shared__ __align__(128) unsigned char smem_loss[];
-  constexpr int kArrays = COND_DISP ? 4 : 3;                           // y, m, [d], pi
-  constexpr uint32_t kArrBytes = kColsPerBlock * 4;                    // one row segment of one tensor
-  constexpr uint32_t kStageBytes = kArrays * kArrBytes;
-  float4* items = reinterpret_cast<float4*>(smem_loss + kStageRows * kStageBytes);   // [8 warps][128]
-  __shared__ double red[8];
-  __shared__ float lf[zmath::kLogFactN];
-  __shared__ float s_sf[kMaxRowsPerBlock];
-  __shared__ int s_row[kMaxRowsPerBlock];
-  __shared__ uint64_t full_bar[kStageRows], empty_bar[kStageRows];
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int c0 = blockIdx.x * kColsPerBlock;
-  const int ncols = min(kColsPerBlock, G - c0);                        // multiple of 4 on this path
-  const int r0 = blockIdx.y * rows_per_block;
-  const int nrows = min(rows_per_block, B - r0);
-  if (threadIdx.x < zmath::kLogFactN) lf[threadIdx.x] = lf_global[threadIdx.x];
-  for (int t = threadIdx.x; t < nrows; t += kStagedThreads) {
-    const int yr = rows ? rows[r0 + t] : (r0 + t);
-    s_row[t] = yr;
-    s_sf[t] = sf ? sf[yr] : 1.0f;
-  }
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kStageRows; ++i) { tc::mbar_init(&full_bar[i], 1); tc::mbar_init(&empty_bar[i], kThreads / 32); }
-    tc::fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp == kThreads / 32) {
-    // ===================================================== producer
-    if (lane == 0) {
-      const uint32_t bytes = (uint32_t)ncols * 4u;
-      for (int i = 0; i < nrows; ++i) {
-        const int st = i % kStageRows; const uint32_t ph = (i / kStageRows) & 1;
-        tc::mbar_wait_backoff(&empty_bar[st], ph ^ 1, producer_sleep_ns);
-        unsigned char* dst = smem_loss + (size_t)st * kStageBytes;
-        tc::mbar_expect_tx(&full_bar[st], bytes * kArrays);
-        const int64_t off = (int64_t)(r0 + i) * ld + c0;
-        auto bulk = [&](unsigned char* to, const float* from) {
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                       ::"r"(tc::smem_u32(to)), "l"(reinterpret_cast<uint64_t>(from)), "r"(bytes), "r"(tc::smem_u32(&full_bar[st])) : "memory");
-        };
-        bulk(dst, Y + (int64_t)s_row[i] * ldy + c0);
-        bulk(dst + kArrBytes, m + off);
-        if (COND_DISP) bulk(dst + 2 * kArrBytes, d + off);
-        bulk(dst + (kArrays - 1) * kArrBytes, pi + off);
-      }
-    }
-    return;
-  }
-
-  // ======================================================= consumers
-  using Ops = zmath::FastOps;
-  constexpr unsigned kFull = 0xffffffffu;
-  float4* q = items + warp * (32 * kVec);
-  const int col = threadIdx.x * kVec;                                  // column inside the block tile
-  const bool active = col < ncols;
-  float lsum = 0.f;
-  float tacc[kVec] = {0.f, 0.f, 0.f, 0.f};
-  float thg[kVec] = {1.f, 1.f, 1.f, 1.f};
-  if (!COND_DISP && active) {
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) thg[j] = d[c0 + col + j];
-  }
-  const unsigned lt = (1u << lane) - 1u;
-  GT* om = dzm + (int64_t)r0 * ld + c0 + col;
-  GT* od = COND_DISP ? dzd + (int64_t)r0 * ld + c0 + col : nullptr;
-  GT* op = dzp + (int64_t)r0 * ld + c0 + col;
-  for (int i = 0; i < nrows; ++i) {
-    const int st = i % kStageRows; const uint32_t ph = (i / kStageRows) & 1;
-    const unsigned char* src = smem_loss + (size_t)st * kStageBytes + (size_t)threadIdx.x * 16;
-    tc::mbar_wait_backoff(&full_bar[st], ph, consumer_sleep_ns);
-    float4 vy = make_float4(0.f, 0.f, 0.f, 0.f), vm = vy, vd = vy, vp = vy;
-    if (active) {
-      vy = *reinterpret_cast<const float4*>(src);
-      vm = *reinterpret_cast<const float4*>(src + kArrBytes);
-      if (COND_DISP) vd = *reinterpret_cast<const float4*>(src + 2 * kArrBytes);
-      vp = *reinterpret_cast<const float4*>(src + (kArrays - 1) * kArrBytes);
-    }
-    __syncwarp();
-    if (lane == 0) tc::mbar_arrive(&empty_bar[st]);                    // operands are in registers: free the slot
-    const float y[kVec] = {vy.x, vy.y, vy.z, vy.w}, mm[kVec] = {vm.x, vm.y, vm.z, vm.w};
-    const float dd[kVec] = {COND_DISP ? vd.x : thg[0], COND_DISP ? vd.y : thg[1], COND_DISP ? vd.z : thg[2], COND_DISP ? vd.w : thg[3]};
-    const float pp[kVec] = {vp.x, vp.y, vp.z, vp.w};
-    const float row_sf = s_sf[i];
-    // ---- queue the non-zero counts of this warp's strip (ballot compaction: items ordered by j, then lane)
-    unsigned bal[kVec];
-    int nz = 0, pos[kVec], base = 0;
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) {
-      const bool is_nz = active && !(y[j] < 1e-8f);                    // loss.py:138
-      bal[j] = __ballot_sync(kFull, is_nz);
-      nz |= is_nz ? (1 << j) : 0;
-    }
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) { pos[j] = base + __popc(bal[j] & lt); base += __popc(bal[j]); }
-    const int total = base;
-#pragma unroll
-    for (int j = 0; j < kVec; ++j)
-      if (nz & (1 << j)) q[pos[j]] = make_float4(y[j], mm[j], dd[j], pp[j]);
-    __syncwarp();
-    // ---- zero branch for my own zero counts
-    float gm[kVec], gd[kVec], gp[kVec];
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) {
-      gm[j] = gd[j] = gp[j] = 0.f;
-      if (BF) {   // branch-free: the four independent chains of a thread interleave (zinb_math.cuh)
-        const zmath::Elem e = zmath::zinb_elem_zero_bf<Ops, COND_DISP>(mm[j], row_sf, dd[j], pp[j], ridge);
-        const bool use = active && !(nz & (1 << j));
-        lsum += use ? e.loss : 0.f; gm[j] = use ? e.gm : 0.f; gd[j] = use ? e.gd : 0.f; gp[j] = use ? e.gp : 0.f;
-      } else if (active && !(nz & (1 << j))) {
-        const zmath::Elem e = zmath::zinb_elem_zero<Ops, COND_DISP>(mm[j], row_sf, dd[j], pp[j], ridge);
-        lsum += e.loss; gm[j] = e.gm; gd[j] = e.gd; gp[j] = e.gp;
-      }
-    }
-    // ---- dense NB pass over the queue
-    for (int k = lane; k < total; k += 32) {
-      const float4 it = q[k];
-      const zmath::Elem e = zmath::zinb_elem_nb<Ops, true, COND_DISP>(it.x, it.y, row_sf, it.z, it.w, ridge, lf);
-      q[k] = make_float4(e.loss, e.gm, e.gd, e.gp);
-    }
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < kVec; ++j)
-      if (nz & (1 << j)) { const float4 e = q[pos[j]]; lsum += e.x; gm[j] = e.y; gd[j] = e.z; gp[j] = e.w; }
-    __syncwarp();
-    if (active) {
-      if (!COND_DISP) {
-#pragma unroll
-        for (int j = 0; j < kVec; ++j) tacc[j] += gd[j];
-      }
-      st4(om, gm[0] * inv_n, gm[1] * inv_n, gm[2] * inv_n, gm[3] * inv_n);
-      if (COND_DISP) st4(od, gd[0] * inv_n, gd[1] * inv_n, gd[2] * inv_n, gd[3] * inv_n);
-      st4(op, gp[0] * inv_n, gp[1] * inv_n, gp[2] * inv_n, gp[3] * inv_n);
-    }
-    om += ld; op += ld;
-    if (COND_DISP) od += ld;
-  }
-  if (!COND_DISP && active) {
-#pragma unroll
-    for (int j = 0; j < kVec; ++j) atomicAdd(dth_acc + c0 + col + j, tacc[j]);
-  }
-  // block reduction over the 8 consumer warps (the producer warp has returned: named barrier on 256 threads)
-  double dsum = (double)lsum;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) dsum += __shfl_xor_sync(kFull, dsum, o);
-  if (lane == 0) red[warp] = dsum;
-  tc::named_barrier_sync(1, kThreads);
-  __shared__ int s_last;
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-#pragma unroll
-    for (int w = 0; w < kThreads / 32; ++w) t += red[w];
-    loss_partial[blockIdx.y * gridDim.x + blockIdx.x] = t;
-    __threadfence();
-    const unsigned nblk = gridDim.x * gridDim.y;
-    const unsigned done = atomicAdd(fa.counter, 1u);
-    s_last = (done == nblk - 1);
-    if (s_last) *fa.counter = 0;                                       // self-resetting
-  }
-  tc::named_barrier_sync(1, kThreads);
-  if (!s_last) return;
-  // ---- the last block to finish folds the per-block partials in a FIXED order (deterministic) and finalises
-  __threadfence();
-  const int n = gridDim.x * gridDim.y;
-  double a = 0.0;
-  for (int i = threadIdx.x; i < n; i += kThreads) a += __ldcg(loss_partial + i);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(kFull, a, o);
-  if (lane == 0) red[warp] = a;
-  tc::named_barrier_sync(1, kThreads);
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-#pragma unroll
-    for (int w = 0; w < kThreads / 32; ++w) t += red[w];
-    *fa.loss_sum = t;
-    if (fa.loss_slot) {
-      double l = t * (double)inv_n;
-      if (l != l) l = INFINITY;                                        // _nan2inf, dca/loss.py:148
-      if (fa.penalty) l += *fa.penalty;
-      const float lf32 = (float)l;
-      fa.loss_slot[0] = lf32;
-      fa.loss_slot[1] = (isfinite(lf32)) ? 0.f : 1.f;
-      if (fa.epoch_acc) { fa.epoch_acc[0] += l * (double)fa.batch; fa.epoch_acc[1] += (double)fa.batch; }
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
-// "Ring" kernel (default for ZINB backward on aligned shapes): operands are staged through shared memory by the
-// threads themselves -- every thread streams the 16 bytes it owns of each tensor row (4 consecutive genes of y, m,
-// [d], pi) with cp.async (LDGSTS, L2-only) into a kRing-deep ring of its own, kRing rows ahead of the arithmetic,
-// and reads them back with one 128-bit LDS per tensor.  A thread only ever reads what it copied itself, so the
-// pipeline needs no barrier of any kind (cp.async.wait_group orders a thread's own copies), no producer warp and
-// no single-lane issue path: in the block-wide bulk-copy ring of zinb_loss_bwd_staged_kernel a warp could run at
-// most three rows ahead of the slowest warp of its block (the one that met a large count and took the Stirling
-// path), and a fifth of all issued instructions were mbarrier polls of warps waiting for a slot their neighbour
-// had not released (3-instruction loops executed 9-13x per row).  The gather of the count
-// rows costs one address computation (rows[] cached in shared memory).  The arithmetic runs on f32x2 pairs
-// (zinb_math.cuh: zinb_zero_pair / finish_factors_pair), the queued non-zero counts return raw derivatives only
-// (zinb_nb_raw) and the activation chain / clip masks / 1/N are applied once per element by its owner.
+// "Ring" kernel (ZINB backward on aligned shapes): operands are staged through shared memory by the threads
+// themselves -- every thread streams the 16 bytes it owns of each tensor row (4 consecutive genes of y, m, [d], pi)
+// with cp.async (LDGSTS, L2-only) into a kRing-deep ring of its own, kRing rows ahead of the arithmetic, and reads
+// them back with one 128-bit LDS per tensor.  A thread only ever reads what it copied itself, so the pipeline needs
+// no barrier of any kind (cp.async.wait_group orders a thread's own copies), no producer warp and no single-lane
+// issue path.  A ring shared by the block would tie every warp to the slowest warp of its block (the one that met a
+// large count and took the Stirling path): no warp could run more than the ring's depth ahead of it, and warps would
+// spend their issue slots polling for a slot their neighbour had not released.  The gather of the count rows costs
+// one address computation (rows[] cached in shared memory).  The arithmetic runs on f32x2 pairs (zinb_math.cuh:
+// zinb_zero_pair / finish_factors_pair), the queued non-zero counts return raw derivatives only (zinb_nb_raw) and
+// the activation chain / clip masks / 1/N are applied once per element by its owner.
 constexpr int kRing = 3;                                  // rows in flight per thread
+constexpr int kMaxRowsPerBlock = 256;                     // rows of one block (row indices / size factors in shared memory)
 
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
@@ -593,6 +284,12 @@ __device__ __forceinline__ RowGrads zinb_row_ring(const float4 vy, const float4 
   return g;
 }
 
+// Where the last block of a launch folds the loss partials: its arrival counter, the loss sum and the optional loss slot
+// (loss * inv_n + penalty, its finite flag) and epoch accumulator (loss * batch, batch).
+struct FoldArgs {
+  unsigned* counter; double* loss_sum; const double* penalty; float* loss_slot; double* epoch_acc; int batch;
+};
+
 // Block sum of the per-thread loss terms into loss_partial[block]; the last block to finish folds the per-block partials
 // in a FIXED order (deterministic) and finalises the loss slot.  Called by all NT threads of the block.
 template <int NT>
@@ -644,10 +341,7 @@ __device__ __forceinline__ void block_loss_fold(double dsum, double* red, int* s
   }
 }
 
-// IDXQ (tunable loss_ring = 2): the queue of non-zero counts holds one-byte ELEMENT INDICES instead of 16-byte operand
-// copies -- the evaluating lane reads y / m / d / pi of the element from the staging slot itself and writes the three raw
-// derivatives back in place, the owner re-reads its vector -- which frees 15 KB of shared memory for a fourth ring slot.
-template <bool COND_DISP, typename GT, bool IDXQ>
+template <bool COND_DISP, typename GT>
 __global__ void __launch_bounds__(kThreads, 3)
 zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_t* __restrict__ rows,
                           const float* __restrict__ sf, const float* m, const float* d, const float* pi,
@@ -659,18 +353,15 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
   constexpr int kArrays = COND_DISP ? 4 : 3;                           // y, m, [d], pi
   constexpr uint32_t kSegBytes = kThreads * 16;                        // one block-row segment of one tensor (4 KB)
   constexpr uint32_t kSlotBytes = kArrays * kSegBytes;
-  constexpr int RING = IDXQ ? kRing + 1 : kRing;
-  float4* items = reinterpret_cast<float4*>(smem_ring + RING * kSlotBytes);            // [8 warps][128] operand copies | indices
+  float4* items = reinterpret_cast<float4*>(smem_ring + kRing * kSlotBytes);           // [8 warps][128] operand copies
   __shared__ double red[kWarps];
   __shared__ float lf[zmath::kLogFactN];
   __shared__ float s_sf[kMaxRowsPerBlock];
   __shared__ int s_row[kMaxRowsPerBlock];
   __shared__ int s_last;
 
-  using Ops = zmath::FastOps;
   using namespace zmath;
-  constexpr unsigned kFull = 0xffffffffu;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const int c0 = blockIdx.x * kColsPerBlock;
   const bool active = c0 + (int)threadIdx.x * kVec < G;                // G % 4 == 0 on this path
   // threads past the last gene (only in the last column block) work on a DUPLICATE of the last valid vector: they copy,
@@ -687,7 +378,7 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
   __syncthreads();
 
   const uint32_t my = tc::smem_u32(smem_ring) + threadIdx.x * 16;      // my 16 bytes inside every segment
-  const uint32_t ring_end = my + RING * kSlotBytes;
+  const uint32_t ring_end = my + kRing * kSlotBytes;
   const float* ysrc = Y + c0 + col;
   const float* msrc = m + (int64_t)r0 * ld + c0 + col;
   const float* dsrc = COND_DISP ? d + (int64_t)r0 * ld + c0 + col : nullptr;
@@ -714,20 +405,16 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
   float tacc[kVec] = {0.f, 0.f, 0.f, 0.f};
   {
 #pragma unroll
-    for (int i = 0; i < RING; ++i) {                                   // one group per row, empty groups keep the count fixed
+    for (int i = 0; i < kRing; ++i) {                                  // one group per row, empty groups keep the count fixed
       if (i < nrows) issue_next();
       cp_async_commit();
     }
     float4* q = items + warp * (32 * kVec);
-    unsigned char* qb = reinterpret_cast<unsigned char*>(items) + warp * (32 * kVec);
-    auto lds32 = [](uint32_t addr) { float v; asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory"); return v; };
-    auto sts32 = [](uint32_t addr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); };
     float thg[kVec] = {1.f, 1.f, 1.f, 1.f};
     if (!COND_DISP) {
 #pragma unroll
       for (int j = 0; j < kVec; ++j) thg[j] = d[c0 + col + j];
     }
-    const unsigned lt = (1u << lane) - 1u;
     GT* om = dzm + (int64_t)r0 * ld + c0 + col;
     GT* od = COND_DISP ? dzd + (int64_t)r0 * ld + c0 + col : nullptr;
     GT* op = dzp + (int64_t)r0 * ld + c0 + col;
@@ -738,93 +425,20 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
       return v;
     };
     for (int i = 0; i < nrows; ++i) {
-      cp_async_wait<RING - 1>();                                       // my copies of row i have landed
-      const uint32_t cslot = rslot, wstrip = rslot - (uint32_t)lane * 16u;       // my vector / my warp's strip in this slot
+      cp_async_wait<kRing - 1>();                                      // my copies of row i have landed
       const float4 vy = lds128(rslot), vm = lds128(rslot + kSegBytes);
       const float4 vd = COND_DISP ? lds128(rslot + 2 * kSegBytes) : make_float4(thg[0], thg[1], thg[2], thg[3]);
       const float4 vp = lds128(rslot + (kArrays - 1) * kSegBytes);
       rslot += kSlotBytes;
       if (rslot == ring_end) rslot = my;
       const float row_sf = s_sf[i];
-      if constexpr (!IDXQ) {
-        // refill: the operands of row i have been consumed (they fed the ballots / the queue): stream row i + kRing
-        const RowGrads g = zinb_row_ring<COND_DISP>(vy, vm, vd, vp, row_sf, active, ridge, inv_n, q, lf, lsum_lg, lsum_nb,
-                                                    lsum_r, tacc, [&] { if (nxt < nrows) issue_next(); cp_async_commit(); });
-        if (active) {
-          st4(om, g.gmA.x, g.gmA.y, g.gmB.x, g.gmB.y);
-          if (COND_DISP) st4(od, g.gdA.x, g.gdA.y, g.gdB.x, g.gdB.y);
-          st4(op, g.gpA.x, g.gpA.y, g.gpB.x, g.gpB.y);
-        }
-      } else {
-      const float y[kVec] = {vy.x, vy.y, vy.z, vy.w};
-      const float2 mA = make_float2(vm.x, vm.y), mB = make_float2(vm.z, vm.w);
-      const float2 dA = make_float2(vd.x, vd.y), dB = make_float2(vd.z, vd.w);
-      const float2 pA = make_float2(vp.x, vp.y), pB = make_float2(vp.z, vp.w);
-      const float2 muA = mul2(mA, splat(row_sf)), muB = mul2(mB, splat(row_sf));        // dca/layers.py:85
-      const float dd[kVec] = {dA.x, dA.y, dB.x, dB.y};
-      // ---- queue the non-zero counts of this warp's strip (ballot compaction: items ordered by j, then lane)
-      bool isnz[kVec];
-      int pos[kVec], base = 0;
-#pragma unroll
-      for (int j = 0; j < kVec; ++j) {
-        isnz[j] = active && !(y[j] < 1e-8f);                           // loss.py:138
-        const unsigned bal = __ballot_sync(kFull, isnz[j]);
-        pos[j] = base + __popc(bal & lt); base += __popc(bal);
-      }
-      const int total = base;
-#pragma unroll
-      for (int j = 0; j < kVec; ++j)
-        if (isnz[j]) qb[pos[j]] = (unsigned char)(lane * kVec + j);
-      __syncwarp();
-      // ---- zero branch of my four elements (as in zinb_row_ring)
-      const float m_lo = fminf(fminf(vm.x, vm.y), fminf(vm.z, vm.w)), m_hi = fmaxf(fmaxf(vm.x, vm.y), fmaxf(vm.z, vm.w));
-      const float d_lo = fminf(fminf(dd[0], dd[1]), fminf(dd[2], dd[3])), d_hi = fmaxf(fmaxf(dd[0], dd[1]), fmaxf(dd[2], dd[3]));
-      const bool plain = (m_lo > 1e-5f) && (m_hi < 1e6f) &&
-                         (COND_DISP ? (d_lo > 0.03125f) && (d_hi < 1e4f) : (d_hi <= 1e6f));   // const-disp: theta is not an activation
-      Raw2 zA, zB; Fin2 fA, fB;
-      if (__all_sync(kFull, plain)) {
-        zA = zinb_zero_pair<Ops, true>(muA, dA, pA); zB = zinb_zero_pair<Ops, true>(muB, dB, pB);
-        fA = finish_factors_pair_plain<Ops, COND_DISP>(dA, pA, inv_n); fB = finish_factors_pair_plain<Ops, COND_DISP>(dB, pB, inv_n);
-      } else {
-        zA = zinb_zero_pair<Ops>(muA, dA, pA); zB = zinb_zero_pair<Ops>(muB, dB, pB);
-        fA = finish_factors_pair<Ops, COND_DISP>(mA, dA, pA, inv_n); fB = finish_factors_pair<Ops, COND_DISP>(mB, dB, pB, inv_n);
-      }
-      lsum_lg += ((active && !isnz[0]) ? zA.lgD.x : 0.f) + ((active && !isnz[1]) ? zA.lgD.y : 0.f)
-               + ((active && !isnz[2]) ? zB.lgD.x : 0.f) + ((active && !isnz[3]) ? zB.lgD.y : 0.f);
-      // ---- dense NB pass over the queue (item k by lane k mod 32): raw derivatives back into the staging slot
-      for (int k = lane; k < total; k += 32) {
-        const int idx = qb[k];
-        const uint32_t e4 = wstrip + (uint32_t)idx * 4u;
-        const float th = COND_DISP ? lds32(e4 + 2 * kSegBytes) : __ldg(d + c0 + warp * (32 * kVec) + idx);
-        const Raw1 e = zinb_nb_raw<Ops>(lds32(e4), lds32(e4 + kSegBytes) * row_sf, th, lds32(e4 + (kArrays - 1) * kSegBytes), lf);
-        lsum_nb += e.loss;
-        sts32(e4, e.gmu); sts32(e4 + kSegBytes, e.dth); sts32(e4 + (kArrays - 1) * kSegBytes, e.dpi);   // in place of y, m, pi
-      }
-      __syncwarp();
-      const float4 r0v = lds128(cslot), r1v = lds128(cslot + kSegBytes), r2v = lds128(cslot + (kArrays - 1) * kSegBytes);
-      zA.gmu.x = isnz[0] ? r0v.x : zA.gmu.x; zA.dth.x = isnz[0] ? r1v.x : zA.dth.x; zA.dpi.x = isnz[0] ? r2v.x : zA.dpi.x;
-      zA.gmu.y = isnz[1] ? r0v.y : zA.gmu.y; zA.dth.y = isnz[1] ? r1v.y : zA.dth.y; zA.dpi.y = isnz[1] ? r2v.y : zA.dpi.y;
-      zB.gmu.x = isnz[2] ? r0v.z : zB.gmu.x; zB.dth.x = isnz[2] ? r1v.z : zB.dth.x; zB.dpi.x = isnz[2] ? r2v.z : zB.dpi.x;
-      zB.gmu.y = isnz[3] ? r0v.w : zB.gmu.y; zB.dth.y = isnz[3] ? r1v.w : zB.dth.y; zB.dpi.y = isnz[3] ? r2v.w : zB.dpi.y;
-      __syncwarp();
-      // the slot has been read back by its owners: refill it with row i + RING
-      if (nxt < nrows) issue_next();
-      cp_async_commit();
-      if (ridge != 0.f) {                                              // loss.py:139-140 (uniform; ridge defaults to 0)
-        if (active) lsum_r += ridge * (pA.x * pA.x + pA.y * pA.y + pB.x * pB.x + pB.y * pB.y);
-        zA.dpi = fma2(splat(2.0f * ridge), pA, zA.dpi); zB.dpi = fma2(splat(2.0f * ridge), pB, zB.dpi);
-      }
+      // refill: the operands of row i have been consumed (they fed the ballots / the queue): stream row i + kRing
+      const RowGrads g = zinb_row_ring<COND_DISP>(vy, vm, vd, vp, row_sf, active, ridge, inv_n, q, lf, lsum_lg, lsum_nb,
+                                                  lsum_r, tacc, [&] { if (nxt < nrows) issue_next(); cp_async_commit(); });
       if (active) {
-        if (!COND_DISP) { tacc[0] += zA.dth.x; tacc[1] += zA.dth.y; tacc[2] += zB.dth.x; tacc[3] += zB.dth.y; }
-        const float2 gmA = mul2(zA.gmu, fA.fm), gmB = mul2(zB.gmu, fB.fm);
-        const float2 gpA = mul2(zA.dpi, fA.fp), gpB = mul2(zB.dpi, fB.fp);
-        st4(om, gmA.x, gmA.y, gmB.x, gmB.y);
-        if (COND_DISP) {
-          const float2 gdA = mul2(zA.dth, fA.fd), gdB = mul2(zB.dth, fB.fd);
-          st4(od, gdA.x, gdA.y, gdB.x, gdB.y);
-        }
-        st4(op, gpA.x, gpA.y, gpB.x, gpB.y);
-      }
+        st4(om, g.gmA.x, g.gmA.y, g.gmB.x, g.gmB.y);
+        if (COND_DISP) st4(od, g.gdA.x, g.gdA.y, g.gdB.x, g.gdB.y);
+        st4(op, g.gpA.x, g.gpA.y, g.gpB.x, g.gpB.y);
       }
       om += ld; op += ld;
       if (COND_DISP) od += ld;
@@ -1117,58 +731,28 @@ int launch(const LossArgs& a, cudaStream_t s) {
   float* tpart = a.dtheta;                                            // const-disp: accumulated with atomics
   if (BWD && !cond) DCA_CUDA_OK(cudaMemsetAsync(a.dtheta, 0, sizeof(float) * (size_t)a.G, s));
 
-  static const bool use_compact = [] { const char* e = getenv("DCA_LOSS_KERNEL"); return e && e[0] == 'c'; }();
+  // ZINB backward on aligned shapes: the ring kernel, unless its plan (at most kMaxRowsPerBlock rows per block) needs
+  // more blocks than the partial buffer holds or more row chunks than a grid's y dimension
   const Plan ps = make_plan(a.B, a.G, kColsPerBlock, kMaxRowsPerBlock);
-  const bool staged_ok = BWD && vec && has_pi && !use_compact && (long long)ps.row_chunks * ps.col_blocks <= kMaxBlocks &&
-                         ps.row_chunks <= 65535;
-  if (staged_ok) {
+  if (BWD && vec && has_pi && (long long)ps.row_chunks * ps.col_blocks <= kMaxBlocks && ps.row_chunks <= 65535) {
     grid = dim3(ps.col_blocks, ps.row_chunks);
     FoldArgs fa{reinterpret_cast<unsigned*>(reinterpret_cast<char*>(a.ws) + sizeof(double) * (size_t)kMaxBlocks), a.loss_sum,
                 a.fin_penalty, a.fin_loss_slot, a.fin_epoch_acc, a.fin_batch};
     if (!a.counter_ready) DCA_CUDA_OK(cudaMemsetAsync(fa.counter, 0, sizeof(unsigned), s));
-#define DCA_RING2(CD, GT, IQ)                                                                                     \
+#define DCA_RING(CD, GT)                                                                                          \
   do {                                                                                                             \
-    constexpr size_t sm = IQ ? (size_t)(kRing + 1) * (CD ? 4 : 3) * kColsPerBlock * 4 + (size_t)(kThreads / 32) * 32 * kVec     \
-                             : (size_t)kRing * (CD ? 4 : 3) * kColsPerBlock * 4 + (size_t)(kThreads / 32) * 32 * kVec * 16; \
+    constexpr size_t sm = (size_t)kRing * (CD ? 4 : 3) * kColsPerBlock * 4 + (size_t)(kThreads / 32) * 32 * kVec * 16; \
     static bool attr = false;                                                                                      \
-    if (!attr) { DCA_CUDA_OK(cudaFuncSetAttribute(zinb_loss_bwd_ring_kernel<CD, GT, IQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); attr = true; } \
-    zinb_loss_bwd_ring_kernel<CD, GT, IQ><<<grid, kThreads, sm, s>>>(a.Y, a.ldy, a.rows, a.sf, a.m, a.d, a.pi, a.ld, a.B, a.G, a.ridge, \
+    if (!attr) { DCA_CUDA_OK(cudaFuncSetAttribute(zinb_loss_bwd_ring_kernel<CD, GT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); attr = true; } \
+    zinb_loss_bwd_ring_kernel<CD, GT><<<grid, kThreads, sm, s>>>(a.Y, a.ldy, a.rows, a.sf, a.m, a.d, a.pi, a.ld, a.B, a.G, a.ridge, \
         a.inv_n, ps.rows_per_block, (GT*)a.dzm, (GT*)a.dzd, (GT*)a.dzp, tpart, lpart, lf_dev, fa);                  \
   } while (0)
-#define DCA_RING(CD, GT) do { if (g_tune.ring == 2) DCA_RING2(CD, GT, true); else DCA_RING2(CD, GT, false); } while (0)
-    if (g_tune.ring) {
-      if (a.grad_bf16) { if (cond) DCA_RING(true, __nv_bfloat16); else DCA_RING(false, __nv_bfloat16); }
-      else             { if (cond) DCA_RING(true, float); else DCA_RING(false, float); }
-      DCA_LAUNCH_CHECK();
-      return DCA_OK;                                                    // the fold is done by the last block
-    }
+    if (a.grad_bf16) { if (cond) DCA_RING(true, __nv_bfloat16); else DCA_RING(false, __nv_bfloat16); }
+    else             { if (cond) DCA_RING(true, float); else DCA_RING(false, float); }
 #undef DCA_RING
-#undef DCA_RING2
-#define DCA_STAGED2(CD, GT, BFV)                                                                                   \
-  do {                                                                                                             \
-    constexpr size_t sm = (size_t)kStageRows * (CD ? 4 : 3) * kColsPerBlock * 4 + (size_t)(kThreads / 32) * 32 * kVec * 16; \
-    static bool attr = false;                                                                                      \
-    if (!attr) { DCA_CUDA_OK(cudaFuncSetAttribute(zinb_loss_bwd_staged_kernel<CD, GT, BFV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); attr = true; } \
-    zinb_loss_bwd_staged_kernel<CD, GT, BFV><<<grid, kStagedThreads, sm, s>>>(a.Y, a.ldy, a.rows, a.sf, a.m, a.d, a.pi, a.ld, a.B, \
-        a.G, a.ridge, a.inv_n, ps.rows_per_block, (GT*)a.dzm, (GT*)a.dzd, (GT*)a.dzp, tpart, lpart, lf_dev, fa,     \
-        g_tune.producer_sleep_ns, g_tune.consumer_sleep_ns);                                                       \
-  } while (0)
-#define DCA_STAGED(CD, GT) do { if (g_tune.branch_free) DCA_STAGED2(CD, GT, true); else DCA_STAGED2(CD, GT, false); } while (0)
-    if (a.grad_bf16) { if (cond) DCA_STAGED(true, __nv_bfloat16); else DCA_STAGED(false, __nv_bfloat16); }
-    else             { if (cond) DCA_STAGED(true, float); else DCA_STAGED(false, float); }
-#undef DCA_STAGED2
-#undef DCA_STAGED
     DCA_LAUNCH_CHECK();
     return DCA_OK;                                                      // the fold is done by the last block
-  } else if (BWD && vec && has_pi) {
-#define DCA_COMPACT(CD, GT)                                                                                   \
-  zinb_loss_bwd_compact_kernel<CD, GT><<<grid, block, 0, s>>>(a.Y, a.ldy, a.rows, a.sf, a.m, a.d, a.pi, a.ld, a.B, a.G, \
-                                                              a.ridge, a.inv_n, p.rows_per_block, (GT*)a.dzm,  \
-                                                              (GT*)a.dzd, (GT*)a.dzp, tpart, lpart, lf_dev)
-    if (a.grad_bf16) { if (cond) DCA_COMPACT(true, __nv_bfloat16); else DCA_COMPACT(false, __nv_bfloat16); }
-    else             { if (cond) DCA_COMPACT(true, float); else DCA_COMPACT(false, float); }
-#undef DCA_COMPACT
-  } else {
+  }
 #define DCA_LOSS_LAUNCH(HP, CD, GT, V)                                                                 \
   zinb_loss_kernel<HP, CD, GT, V, BWD><<<grid, block, 0, s>>>(                                          \
       a.Y, a.ldy, a.rows, a.sf, a.m, a.d, a.pi, a.ld, a.B, a.G, a.ridge, a.inv_n, p.rows_per_block,      \
@@ -1180,14 +764,13 @@ int launch(const LossArgs& a, cudaStream_t s) {
     else if (!has_pi && cond) DCA_LOSS_LAUNCH(false, true, GT, V); \
     else DCA_LOSS_LAUNCH(false, false, GT, V);                     \
   } while (0)
-    if (BWD && a.grad_bf16) {
-      if (vec) DCA_LOSS_DISPATCH(__nv_bfloat16, 4); else DCA_LOSS_DISPATCH(__nv_bfloat16, 1);
-    } else {
-      if (vec) DCA_LOSS_DISPATCH(float, 4); else DCA_LOSS_DISPATCH(float, 1);
-    }
+  if (BWD && a.grad_bf16) {
+    if (vec) DCA_LOSS_DISPATCH(__nv_bfloat16, 4); else DCA_LOSS_DISPATCH(__nv_bfloat16, 1);
+  } else {
+    if (vec) DCA_LOSS_DISPATCH(float, 4); else DCA_LOSS_DISPATCH(float, 1);
+  }
 #undef DCA_LOSS_DISPATCH
 #undef DCA_LOSS_LAUNCH
-  }
   DCA_LAUNCH_CHECK();
   fold_partials_kernel<<<1, 256, 0, s>>>(lpart, (int)(grid.x * grid.y), a.loss_sum, BWD ? 0 : 1, a.fin_penalty, a.inv_n,
                                          a.fin_batch, BWD ? a.fin_loss_slot : nullptr, a.fin_epoch_acc);
@@ -1253,12 +836,8 @@ using namespace dca;
 extern "C" int dca_set_tunable(const char* name, int64_t value) {
   if (!name) { set_error("dca_set_tunable: null name"); return DCA_ERR_BAD_ARG; }
   const std::string n(name);
-  if (n == "loss_target_blocks" && value >= 0 && value <= kMaxBlocks) g_tune.target_blocks = (int)value;
-  else if (n == "loss_producer_sleep_ns" && value >= 0 && value <= 100000) g_tune.producer_sleep_ns = (unsigned)value;
-  else if (n == "loss_consumer_sleep_ns" && value >= 0 && value <= 100000) g_tune.consumer_sleep_ns = (unsigned)value;
+  if (n == "loss_target_blocks" && value >= 0 && value <= kMaxBlocks) g_target_blocks = (int)value;
   else if (n == "fused_heads" && (value == 0 || value == 1)) g_fused_heads_default = (int)value;
-  else if (n == "loss_branch_free" && (value == 0 || value == 1)) g_tune.branch_free = (int)value;
-  else if (n == "loss_ring" && value >= 0 && value <= 2) g_tune.ring = (int)value;
   else if (n == "gg_profile" && (value == 0 || value == 1)) tc::g_gg_profile = (int)value;
   else if (n == "head_bwd_banded" && (value == 0 || value == 1)) tc::g_head_bwd_banded = (int)value;
   else if (n == "head_bwd_stagger" && value >= 0 && value <= 100000) tc::g_head_bwd_stagger = (int)value;
@@ -1335,23 +914,6 @@ extern "C" int dca_zinb_elem_host(int32_t ae_type, float y, float m, float sf, f
     }
     if (ridge != 0.f) { loss += ridge * pi * pi; dpi = fmaf(2.0f * ridge, pi, dpi); }
     out[0] = loss; out[1] = gmu * f.fm.y; out[2] = dth * f.fd.y; out[3] = dpi * f.fp.y;
-    return DCA_OK;
-  }
-  if (ae_type & 0x100) {
-    // the formulations the staged / fused kernels run: branch-free zero branch, NB branch evaluated from mu by a
-    // different lane than the element's owner (which then applies the MeanAct clip mask)
-    const int base = ae_type & 0xff;
-    if (base != DCA_AE_ZINB_CONDDISP && base != DCA_AE_ZINB) { set_error("dca_zinb_elem_host: kernel variant needs a ZINB type"); return DCA_ERR_BAD_ARG; }
-    if (y < 1e-8f) {
-      e = base == DCA_AE_ZINB_CONDDISP ? zmath::zinb_elem_zero_bf<P, true>(m, sf, d, pi, ridge)
-                                       : zmath::zinb_elem_zero_bf<P, false>(m, sf, d, pi, ridge);
-    } else if (base == DCA_AE_ZINB_CONDDISP) {
-      e = zmath::zinb_elem_nb_mu<P>(y, m * sf, d, pi, ridge, lf);
-      if (!(m > 1e-5f && m < 1e6f)) e.gm = 0.f;
-    } else {
-      e = zmath::zinb_elem<P, true, false>(y, m, sf, d, pi, ridge, lf);
-    }
-    out[0] = e.loss; out[1] = e.gm; out[2] = e.gd; out[3] = e.gp;
     return DCA_OK;
   }
   switch (ae_type) {

@@ -166,12 +166,10 @@ DCA_HD float one_minus_exp_neg(float d) {
 }
 
 // Chain rule through the output activations + ridge, shared by both branches.
-template <class Ops, bool HAS_PI, bool COND_DISP, bool MASK_M = true>
+template <class Ops, bool HAS_PI, bool COND_DISP>
 DCA_HD void finish_elem(Elem& o, float dth, float dpi, float m, float th, float pi, float ridge) {
-  if (MASK_M) {
-    const bool m_pass = (m > 1e-5f) && (m < 1e6f);         // clip_by_value gradient mask (network.py:38)
-    o.gm = m_pass ? o.gm : 0.f;
-  }
+  const bool m_pass = (m > 1e-5f) && (m < 1e6f);           // clip_by_value gradient mask (network.py:38)
+  o.gm = m_pass ? o.gm : 0.f;
   if (COND_DISP) {
     const bool d_pass = (th > 1e-4f) && (th < 1e4f);       // DispAct clip mask (network.py:39)
     o.gd = d_pass ? dth * one_minus_exp_neg<Ops>(th) : 0.f;
@@ -205,49 +203,6 @@ DCA_HD Elem zinb_elem_zero(float m, float sf, float th, float pi, float ridge) {
   return o;
 }
 
-// The same zero-branch arithmetic without control flow (both sides of the two series/MUFU choices are evaluated
-// and selected): a thread can then interleave the independent chains of several elements, which matters where few
-// warps are resident (the fused head/loss/backward kernel).  Results equal zinb_elem_zero's.
-template <class Ops, bool COND_DISP>
-DCA_HD Elem zinb_elem_zero_bf(float m, float sf, float th_in, float pi, float ridge) {
-  const float mu = m * sf;
-  const float th = fminf(th_in, 1e6f);
-  const float te = th + kEps;
-  const float rden = Ops::rcp(te + mu);
-  const float q = mu * rden;
-  float p = fmaf(q, 0.125f, 0.142857143f);
-  p = fmaf(q, p, 0.166666667f); p = fmaf(q, p, 0.2f); p = fmaf(q, p, 0.25f);
-  p = fmaf(q, p, 0.333333333f); p = fmaf(q, p, 0.5f);
-  const float f_ser = q * q * p, L1_ser = q + f_ser;
-  const float L1_log = -kLn2 * Ops::lg2(te * rden), f_log = L1_log - q;
-  const bool small_q = q < 0.0625f;
-  const float L1 = small_q ? L1_ser : L1_log, f = small_q ? f_ser : f_log;
-  const float z = Ops::ex2(-th * L1 * kLog2e);
-  const float omp = 1.0f - pi;
-  const float D = pi + omp * z + kEps;
-  const float rD = Ops::rcp(D);
-  Elem o;
-  o.loss = -kLn2 * Ops::lg2(D);
-  const float w = omp * z * rD;
-  o.gm = w * th * q;
-  o.gm = ((m > 1e-5f) && (m < 1e6f)) ? o.gm : 0.f;
-  const float dth = w * f;
-  if (COND_DISP) {
-    float pp = fmaf(th_in, 0.0416666667f, -0.166666667f);
-    pp = fmaf(th_in, pp, 0.5f);
-    const float ome_ser = th_in - th_in * th_in * pp;
-    const float ome_exp = 1.0f - Ops::ex2(-th_in * kLog2e);
-    const float ome = th_in < 0.03125f ? ome_ser : ome_exp;
-    o.gd = ((th_in > 1e-4f) && (th_in < 1e4f)) ? dth * ome : 0.f;
-  } else {
-    o.gd = dth;
-  }
-  o.loss = fmaf(ridge * pi, pi, o.loss);                    // ridge defaults to 0: adds an exact 0
-  const float dpi = fmaf(2.0f * ridge, pi, (z - 1.0f) * rD);
-  o.gp = dpi * (pi * (1.0f - pi));
-  return o;
-}
-
 // NB branch of loss.py:87-88,130 (all elements of NB models; y >= 1e-8 for ZINB models)
 template <class Ops, bool HAS_PI, bool COND_DISP>
 DCA_HD Elem zinb_elem_nb(float y, float m, float sf, float th, float pi, float ridge, const float* lf_table) {
@@ -268,24 +223,6 @@ DCA_HD Elem zinb_elem_nb(float y, float m, float sf, float th, float pi, float r
   return o;
 }
 
-// NB branch of a ZINB conditional-dispersion element given mu = m * sf directly; the MeanAct clip mask on gm is
-// left to the caller (used where another thread than the element's owner evaluates the queued NB elements).
-template <class Ops>
-DCA_HD Elem zinb_elem_nb_mu(float y, float mu, float th, float pi, float ridge, const float* lf_table) {
-  const Shared s = shared_terms<Ops>(mu, 1.0f, th);
-  Elem o;
-  float lg, dg;
-  lgam_digam_diff<Ops>(s.te, y, lg, dg);
-  float nb = lgamma_1p<Ops>(y, lf_table) - lg + s.th * s.L1 - y * (kLn2 * Ops::lg2((s.mu + kEps) * s.rden));
-  if (nb != nb) nb = INFINITY;                             // _nan2inf  loss.py:105
-  o.gm = s.th * (s.mu + kEps - y) * s.rden * (s.mu * Ops::rcp(s.mu + kEps));
-  const float qq = 1.0f - pi + kEps;
-  nb -= kLn2 * Ops::lg2(qq);                               // loss.py:130
-  o.loss = nb;
-  finish_elem<Ops, true, true, false>(o, s.f + y * s.rden - dg, Ops::rcp(qq), 1.0f, th, pi, ridge);
-  return o;
-}
-
 // ------------------------------------------------------------------------------------ packed (f32x2) formulation
 // The element-wise chains below are written over float2 (two genes of a thread): the two chains are independent, so
 // they interleave in the FMA pipe; MUFU, min/max and selects stay scalar.  sm_90 has no paired fp32 FMA, so device
@@ -302,7 +239,9 @@ DCA_HD float2 neg2(float2 a) { return make_float2(-a.x, -a.y); }
 struct Raw2 { float2 lgD, gmu, dth, dpi; };
 
 // zero branch (y < 1e-8) of two ZINB elements: loss = -ln2 * lgD,  gmu = dL/dmu * mu,  dth = dL/dtheta,  dpi = dL/dpi
-// (branch-free; same arithmetic as zinb_elem_zero_bf).  mu = m * sf is computed by the caller (the NB items need it too).
+// (the formulas of zinb_elem_zero without control flow: both sides of the series / MUFU choice are evaluated and
+// selected, so the independent chains of a thread's elements interleave).  mu = m * sf is computed by the caller (the
+// NB items need it too).
 // TH_BOUNDED: the caller knows theta <= 1e6 (the kernels check the row's theta range once per thread), so the
 // min(theta, 1e6) of loss.py:85,134 is the identity and is skipped.
 template <class Ops, bool TH_BOUNDED = false>

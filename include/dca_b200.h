@@ -399,8 +399,8 @@ int dca_zinb_loss_fwd(const float* Y, int64_t ldy, const int32_t* rows, const fl
 /* HOST mirror of the per-element device arithmetic of the loss kernel (same source compiled for
  * the CPU); a testing aid so the formulas can be checked against the oracle without a GPU.
  * out = {element loss, dL/dzm, dL/dzd (or raw dL/dtheta for const-disp types), dL/dzp}, not / N.
- * ae_type | 0x100 (ZINB types) evaluates the formulations the staged / fused kernels execute instead: the
- * branch-free zero branch and the NB branch computed from mu = m * sf with the MeanAct mask applied afterwards. */
+ * ae_type | 0x200 (ZINB types) evaluates the formulation the ring and heads + loss kernels execute instead: the
+ * f32x2 zero branch and the raw NB derivatives, chained through the activations by shared finishing factors. */
 int dca_zinb_elem_host(int32_t ae_type, float y, float m, float sf, float d, float pi, float ridge,
                        float out[4]);
 
@@ -703,8 +703,8 @@ int dca_pack_sparse(const void* counts, int32_t dtype, int64_t rows, int64_t col
 
 int64_t dca_launch_count(void);
 /* Launch tunables of the loss kernel (process-wide; set them BEFORE the first training step of an engine,
- * a captured step graph keeps the values it was recorded with): "loss_target_blocks",
- * "loss_producer_sleep_ns", "loss_consumer_sleep_ns", "loss_branch_free" (0 | 1, default 1); "fused_heads" (0 | 1, default 0): engines created afterwards
+ * a captured step graph keeps the values it was recorded with): "loss_target_blocks" (blocks per launch of the
+ * loss kernel, default 0 = auto); "fused_heads" (0 | 1, default 0): engines created afterwards
  * run head forward + loss + head backward of a zinb-conddisp training step as one fused kernel (flash_zinb.cu)
  * instead of three (environment override DCA_FUSED_HEADS); "head_bwd_banded" (0 | 1, default 1): the head backward
  * as one band-ordered launch instead of two (same bits); "head_bwd_stagger" (SM cycles, default 1300): the start delay

@@ -58,92 +58,82 @@ def _oracle_rows(y, m, sf, d, pi, ridge=0.0):
     return el, gm, gd, gp
 
 
-@pytest.mark.parametrize("ring", [1, 2, 0])
-def test_loss_kernel_at_benchmark_size_vs_oracle(ring):
+def test_loss_kernel_at_benchmark_size_vs_oracle():
     """4096 x 20000, zinb-conddisp, row gather, bf16 and fp32 gradients: sampled rows element-wise against the float64
     oracle (3e-4 of the tensor scale for fp32 gradients, 2^-8 relative for bf16 storage), the loss of those rows to
     2e-5, and the whole-batch loss as a checksum of checksums (sum over 8 row slabs computed by separate launches)."""
     L = _L(); lib = L.load()
-    L.check(lib.dca_set_tunable(b"loss_ring", ring))
-    try:
-        B, G, N = 4096, 20000, 5000
-        g = torch.Generator(device=DEV); g.manual_seed(5)
-        logm = torch.randn(G, device=DEV, generator=g) * 1.5 - 2.0
-        depth = torch.exp(torch.randn(N, 1, device=DEV, generator=g) * 0.35)
-        Y = torch.poisson(torch._standard_gamma(torch.full((N, G), 2.0, device=DEV), generator=g) * depth * torch.exp(logm)[None, :] / 2.0,
-                          generator=g)
-        Y[torch.rand(N, G, device=DEV, generator=g) < 0.2] = 0
-        Y[0, :6] = torch.tensor([0., 17., 40., 1000., 30000., 5.], device=DEV)
-        rows = torch.randperm(N, device=DEV, generator=g)[:B].int().contiguous()
-        rows[0] = 0
-        sf = depth.flatten().contiguous()
-        m = torch.exp(logm[None, :] + torch.randn(B, G, device=DEV, generator=g) * 0.7).clamp(1e-5, 1e6)
-        d = torch.nn.functional.softplus(torch.randn(B, G, device=DEV, generator=g) * 2.0).clamp(1e-4, 1e4)
-        p = torch.sigmoid(torch.randn(B, G, device=DEV, generator=g) * 2.0)
-        inv_n = 1.0 / (B * G)
-        samp = torch.cat([torch.tensor([0], device=DEV), torch.randperm(B, device=DEV, generator=g)[:23]]).sort().values
-        ys = Y[rows[samp].long()].cpu().numpy(); ms, ds, ps = m[samp].cpu().numpy(), d[samp].cpu().numpy(), p[samp].cpu().numpy()
-        sfs = sf[rows[samp].long()].cpu().numpy()
-        el, rgm, rgd, rgp = _oracle_rows(ys, ms, sfs, ds, ps)
-        for gdt, tol in ((L.F32, 3e-4), (L.BF16, 6e-3)):
-            total, gm, gd, gp, _ = _loss_call(lib, L, Y, G, rows, sf, m, d, p, B, G, 0, 0.0, inv_n, gdt)
-            for got, ref, nm in ((gm, rgm, "dzm"), (gd, rgd, "dzd"), (gp, rgp, "dzp")):
-                e = rel_err(got[samp].float().cpu().numpy(), ref * inv_n)
-                assert e < tol, (ring, nm, gdt, e)
-            # loss of the sampled rows alone (a 24-row launch on contiguous copies of their operands)
-            sub_rows = rows[samp].contiguous()
-            l_s, *_ = _loss_call(lib, L, Y, G, sub_rows, sf, m[samp].contiguous(), d[samp].contiguous(), p[samp].contiguous(),
-                                 len(samp), G, 0, 0.0, 1.0, gdt)
-            assert abs(l_s - el.sum()) <= 2e-5 * abs(el.sum()), (ring, l_s, el.sum())
-            # checksum of checksums: the batch loss equals the sum over 8 slabs of 512 rows
-            parts = 0.0
-            for k in range(8):
-                sl = slice(512 * k, 512 * (k + 1))
-                l_k, *_ = _loss_call(lib, L, Y, G, rows[sl].contiguous(), sf, m[sl], d[sl], p[sl], 512, G, 0, 0.0, 1.0, gdt)
-                parts += l_k
-            assert abs(total - parts) <= 1e-6 * abs(parts), (ring, total, parts)
-    finally:
-        L.check(lib.dca_set_tunable(b"loss_ring", 1))
+    B, G, N = 4096, 20000, 5000
+    g = torch.Generator(device=DEV); g.manual_seed(5)
+    logm = torch.randn(G, device=DEV, generator=g) * 1.5 - 2.0
+    depth = torch.exp(torch.randn(N, 1, device=DEV, generator=g) * 0.35)
+    Y = torch.poisson(torch._standard_gamma(torch.full((N, G), 2.0, device=DEV), generator=g) * depth * torch.exp(logm)[None, :] / 2.0,
+                      generator=g)
+    Y[torch.rand(N, G, device=DEV, generator=g) < 0.2] = 0
+    Y[0, :6] = torch.tensor([0., 17., 40., 1000., 30000., 5.], device=DEV)
+    rows = torch.randperm(N, device=DEV, generator=g)[:B].int().contiguous()
+    rows[0] = 0
+    sf = depth.flatten().contiguous()
+    m = torch.exp(logm[None, :] + torch.randn(B, G, device=DEV, generator=g) * 0.7).clamp(1e-5, 1e6)
+    d = torch.nn.functional.softplus(torch.randn(B, G, device=DEV, generator=g) * 2.0).clamp(1e-4, 1e4)
+    p = torch.sigmoid(torch.randn(B, G, device=DEV, generator=g) * 2.0)
+    inv_n = 1.0 / (B * G)
+    samp = torch.cat([torch.tensor([0], device=DEV), torch.randperm(B, device=DEV, generator=g)[:23]]).sort().values
+    ys = Y[rows[samp].long()].cpu().numpy(); ms, ds, ps = m[samp].cpu().numpy(), d[samp].cpu().numpy(), p[samp].cpu().numpy()
+    sfs = sf[rows[samp].long()].cpu().numpy()
+    el, rgm, rgd, rgp = _oracle_rows(ys, ms, sfs, ds, ps)
+    for gdt, tol in ((L.F32, 3e-4), (L.BF16, 6e-3)):
+        total, gm, gd, gp, _ = _loss_call(lib, L, Y, G, rows, sf, m, d, p, B, G, 0, 0.0, inv_n, gdt)
+        for got, ref, nm in ((gm, rgm, "dzm"), (gd, rgd, "dzd"), (gp, rgp, "dzp")):
+            e = rel_err(got[samp].float().cpu().numpy(), ref * inv_n)
+            assert e < tol, (nm, gdt, e)
+        # loss of the sampled rows alone (a 24-row launch on contiguous copies of their operands)
+        sub_rows = rows[samp].contiguous()
+        l_s, *_ = _loss_call(lib, L, Y, G, sub_rows, sf, m[samp].contiguous(), d[samp].contiguous(), p[samp].contiguous(),
+                             len(samp), G, 0, 0.0, 1.0, gdt)
+        assert abs(l_s - el.sum()) <= 2e-5 * abs(el.sum()), (l_s, el.sum())
+        # checksum of checksums: the batch loss equals the sum over 8 slabs of 512 rows
+        parts = 0.0
+        for k in range(8):
+            sl = slice(512 * k, 512 * (k + 1))
+            l_k, *_ = _loss_call(lib, L, Y, G, rows[sl].contiguous(), sf, m[sl], d[sl], p[sl], 512, G, 0, 0.0, 1.0, gdt)
+            parts += l_k
+        assert abs(total - parts) <= 1e-6 * abs(parts), (total, parts)
 
 
-@pytest.mark.parametrize("ring", [1, 2, 0])
 @pytest.mark.parametrize("gdt_name", ["f32", "bf16"])
-def test_loss_kernel_edge_cases_on_device(ring, gdt_name):
+def test_loss_kernel_edge_cases_on_device(gdt_name):
     """Activations AT their clip bounds (network.py:38-39: gradient through the clipped activation is zero), pi -> 0 / 1,
     counts 0 / 1 / 16 / 17 / 1e3 / 3e4, extreme size factors -- on the DEVICE, through the vectorised kernels (shape
-    aligned so that the staged / ring kernels run): everything finite, equal to the float64 oracle."""
+    aligned so that the ring kernel runs): everything finite, equal to the float64 oracle."""
     L = _L(); lib = L.load()
-    L.check(lib.dca_set_tunable(b"loss_ring", ring))
-    try:
-        gdt = L.F32 if gdt_name == "f32" else L.BF16
-        B, G = 64, 1024
-        rng = np.random.default_rng(3)
-        ms = np.array([1e-5, 1e6, 2e-5, 5e5, 1.0, 30.0, 1e-3, 1e3], np.float32)
-        dsv = np.array([1e-4, 1e4, 2e-4, 9e3, 0.03125, 0.031, 1.0, 50.0], np.float32)
-        pis = np.array([0.0, 1.0, 1e-7, 1 - 1e-7, 0.5, 0.01, 0.99, 0.3], np.float32)
-        ysv = np.array([0, 1, 2, 4, 5, 16, 17, 1000, 30000, 0, 0, 3], np.float32)
-        m = rng.choice(ms, (B, G)).astype(np.float32); d = rng.choice(dsv, (B, G)).astype(np.float32)
-        pi = rng.choice(pis, (B, G)).astype(np.float32); Y = rng.choice(ysv, (B, G)).astype(np.float32)
-        sf = np.exp(rng.normal(0, 1.0, B)).astype(np.float32); sf[:3] = [1e-2, 1e2, 1.0]
-        el, rgm, rgd, rgp = _oracle_rows(Y, m, sf, d, pi)
-        assert np.all(np.isfinite(el)) and np.all(np.isfinite(rgm)) and np.all(np.isfinite(rgd)) and np.all(np.isfinite(rgp))
-        total, gm, gd, gp, _ = _loss_call(lib, L, _t(Y), G, None, _t(sf), _t(m), _t(d), _t(pi), B, G, 0, 0.0, 1.0, gdt)
-        assert np.isfinite(total) and abs(total - el.sum()) <= 5e-5 * abs(el.sum()), (total, el.sum())
-        gmn, gdn, gpn = [x.float().cpu().numpy() for x in (gm, gd, gp)]
-        assert np.all(np.isfinite(gmn)) and np.all(np.isfinite(gdn)) and np.all(np.isfinite(gpn))
-        # exactly zero through a clipped activation
-        assert np.all(gmn[(m <= 1e-5) | (m >= 1e6)] == 0) and np.all(gdn[(d <= 1e-4) | (d >= 1e4)] == 0)
-        # element-wise, relative to max(|ref|, 1e-3 * tensor scale)
-        tol = 3e-4 if gdt == L.F32 else 6e-3
-        for got, ref, nm in ((gmn, rgm, "dzm"), (gdn, rgd, "dzd"), (gpn, rgp, "dzp")):
-            scale = np.maximum(np.abs(ref), 1e-3 * np.max(np.abs(ref)) + 1e-30)
-            err = np.abs(got - ref) / scale
-            k = np.unravel_index(int(np.argmax(err)), err.shape)
-            print("\n[edge ring=%d %s %s] worst %.2e at y=%g m=%g sf=%g d=%g pi=%g: got %g ref %g"
-                  % (ring, gdt_name, nm, err[k], Y[k], m[k], sf[k[0]], d[k], pi[k], got[k], ref[k]))
-            assert err[k] < tol, (nm, err[k])
-    finally:
-        L.check(lib.dca_set_tunable(b"loss_ring", 1))
+    gdt = L.F32 if gdt_name == "f32" else L.BF16
+    B, G = 64, 1024
+    rng = np.random.default_rng(3)
+    ms = np.array([1e-5, 1e6, 2e-5, 5e5, 1.0, 30.0, 1e-3, 1e3], np.float32)
+    dsv = np.array([1e-4, 1e4, 2e-4, 9e3, 0.03125, 0.031, 1.0, 50.0], np.float32)
+    pis = np.array([0.0, 1.0, 1e-7, 1 - 1e-7, 0.5, 0.01, 0.99, 0.3], np.float32)
+    ysv = np.array([0, 1, 2, 4, 5, 16, 17, 1000, 30000, 0, 0, 3], np.float32)
+    m = rng.choice(ms, (B, G)).astype(np.float32); d = rng.choice(dsv, (B, G)).astype(np.float32)
+    pi = rng.choice(pis, (B, G)).astype(np.float32); Y = rng.choice(ysv, (B, G)).astype(np.float32)
+    sf = np.exp(rng.normal(0, 1.0, B)).astype(np.float32); sf[:3] = [1e-2, 1e2, 1.0]
+    el, rgm, rgd, rgp = _oracle_rows(Y, m, sf, d, pi)
+    assert np.all(np.isfinite(el)) and np.all(np.isfinite(rgm)) and np.all(np.isfinite(rgd)) and np.all(np.isfinite(rgp))
+    total, gm, gd, gp, _ = _loss_call(lib, L, _t(Y), G, None, _t(sf), _t(m), _t(d), _t(pi), B, G, 0, 0.0, 1.0, gdt)
+    assert np.isfinite(total) and abs(total - el.sum()) <= 5e-5 * abs(el.sum()), (total, el.sum())
+    gmn, gdn, gpn = [x.float().cpu().numpy() for x in (gm, gd, gp)]
+    assert np.all(np.isfinite(gmn)) and np.all(np.isfinite(gdn)) and np.all(np.isfinite(gpn))
+    # exactly zero through a clipped activation
+    assert np.all(gmn[(m <= 1e-5) | (m >= 1e6)] == 0) and np.all(gdn[(d <= 1e-4) | (d >= 1e4)] == 0)
+    # element-wise, relative to max(|ref|, 1e-3 * tensor scale)
+    tol = 3e-4 if gdt == L.F32 else 6e-3
+    for got, ref, nm in ((gmn, rgm, "dzm"), (gdn, rgd, "dzd"), (gpn, rgp, "dzp")):
+        scale = np.maximum(np.abs(ref), 1e-3 * np.max(np.abs(ref)) + 1e-30)
+        err = np.abs(got - ref) / scale
+        k = np.unravel_index(int(np.argmax(err)), err.shape)
+        print("\n[edge %s %s] worst %.2e at y=%g m=%g sf=%g d=%g pi=%g: got %g ref %g"
+              % (gdt_name, nm, err[k], Y[k], m[k], sf[k[0]], d[k], pi[k], got[k], ref[k]))
+        assert err[k] < tol, (nm, err[k])
 
 
 @pytest.mark.parametrize("gemm_path", ["generic", "tcgen05"])
@@ -392,34 +382,28 @@ def test_train_streaming_from_host_equals_resident_training():
     assert np.all(np.isfinite(h["loss"])) and len(h["val_loss"]) == 2
 
 
-@pytest.mark.parametrize("ring", [0, 1, 2])
 @pytest.mark.parametrize("ae_type", ["zinb", "zinb-conddisp"])
-def test_loss_kernel_variants_vs_oracle(ring, ae_type):
-    """All three ZINB backward kernels (dca_set_tunable loss_ring: 0 block-wide bulk-copy ring, 1 per-thread cp.async
-    ring, 2 the same with the index queue) on an aligned shape with row gather, ridge and a partial last column block,
-    against the float64 oracle -- including the per-gene theta gradient of the constant-dispersion model."""
+def test_loss_kernel_variants_vs_oracle(ae_type):
+    """The ZINB backward kernel (per-thread cp.async rings) on an aligned shape with row gather, ridge and a partial last
+    column block, against the float64 oracle -- including the per-gene theta gradient of the constant-dispersion model."""
     from tests.test_gpu_parity import _oracle_loss, _post_act
     L = _L(); lib = L.load()
-    L.check(lib.dca_set_tunable(b"loss_ring", ring))
-    try:
-        B, G = 200, 1028 + 1024                       # three column blocks, the last one 4 genes wide
-        N = B + 13
-        Y = synth_counts(N, G, 1); Y[0, :4] = [0, 17, 40, 3000]
-        sf = np.exp(np.random.default_rng(2).normal(0, 0.3, N)).astype(np.float32)
-        rows = np.random.default_rng(3).permutation(N)[:B].astype(np.int32)
-        m, d, pi = _post_act(B, G, 4)
-        cond = ae_type.endswith("conddisp")
-        ref = _oracle_loss(ae_type, Y, sf, m, d, pi, 0.01, rows)
-        dd = _t(d) if cond else _t(d[0])
-        for gdt, tol in ((L.F32, 3e-4), (L.BF16, 6e-3)):
-            total, gm, gd, gp, dth = _loss_call(lib, L, _t(Y), G, torch.as_tensor(rows).to(DEV), _t(sf), _t(m), dd, _t(pi), B, G,
-                                                L.AE_TYPE_IDS[ae_type], 0.01, 1.0 / (B * G), gdt, cond=cond)
-            assert abs(total - ref["sum"]) <= 2e-5 * abs(ref["sum"]), (ring, ae_type, total, ref["sum"])
-            assert rel_err(gm.float().cpu().numpy(), ref["dzm"]) < tol
-            assert rel_err(gp.float().cpu().numpy(), ref["dzp"]) < tol
-            if cond:
-                assert rel_err(gd.float().cpu().numpy(), ref["dzd"]) < tol
-            else:
-                assert rel_err(dth.cpu().numpy(), ref["dtheta"]) < 3e-4
-    finally:
-        L.check(lib.dca_set_tunable(b"loss_ring", 1))
+    B, G = 200, 1028 + 1024                       # three column blocks, the last one 4 genes wide
+    N = B + 13
+    Y = synth_counts(N, G, 1); Y[0, :4] = [0, 17, 40, 3000]
+    sf = np.exp(np.random.default_rng(2).normal(0, 0.3, N)).astype(np.float32)
+    rows = np.random.default_rng(3).permutation(N)[:B].astype(np.int32)
+    m, d, pi = _post_act(B, G, 4)
+    cond = ae_type.endswith("conddisp")
+    ref = _oracle_loss(ae_type, Y, sf, m, d, pi, 0.01, rows)
+    dd = _t(d) if cond else _t(d[0])
+    for gdt, tol in ((L.F32, 3e-4), (L.BF16, 6e-3)):
+        total, gm, gd, gp, dth = _loss_call(lib, L, _t(Y), G, torch.as_tensor(rows).to(DEV), _t(sf), _t(m), dd, _t(pi), B, G,
+                                            L.AE_TYPE_IDS[ae_type], 0.01, 1.0 / (B * G), gdt, cond=cond)
+        assert abs(total - ref["sum"]) <= 2e-5 * abs(ref["sum"]), (ae_type, total, ref["sum"])
+        assert rel_err(gm.float().cpu().numpy(), ref["dzm"]) < tol
+        assert rel_err(gp.float().cpu().numpy(), ref["dzp"]) < tol
+        if cond:
+            assert rel_err(gd.float().cpu().numpy(), ref["dzd"]) < tol
+        else:
+            assert rel_err(dth.cpu().numpy(), ref["dtheta"]) < 3e-4

@@ -12,7 +12,7 @@ def _host_elem(ae_type, y, m, sf, d, pi, ridge, kernel_variant=False):
     lib = _lib.load()
     out = (C.c_float * 4)()
     res = np.zeros((len(y), 4), np.float32)
-    t = _lib.AE_TYPE_IDS[ae_type] | ({False: 0, True: 0x100, "ring": 0x200}[kernel_variant])
+    t = _lib.AE_TYPE_IDS[ae_type] | ({False: 0, "ring": 0x200}[kernel_variant])
     for i in range(len(y)):
         assert lib.dca_zinb_elem_host(t, float(y[i]), float(m[i]), float(sf[i]), float(d[i]), float(pi[i]),
                                       float(ridge), C.byref(out)) == 0
@@ -83,10 +83,10 @@ def test_host_math_clip_bounds():
 
 @pytest.mark.parametrize("ae_type", ["zinb-conddisp", "zinb"])
 @pytest.mark.parametrize("ridge", [0.0, 0.05])
-def test_kernel_formulations_equal_the_reference_formulation(ae_type, ridge):
-    """The branch-free zero branch (staged + fused kernels) and the NB branch evaluated from mu = m*sf with the
-    clip mask applied by the owner (fused kernel) return what the plain per-element function returns -- including
-    the series / MUFU switch points (q = 1/16, d = 1/32), the clip bounds and rows with extreme size factors."""
+def test_ring_formulation_equals_the_reference_formulation(ae_type, ridge):
+    """The formulation of the ring and heads + loss kernels (zinb_zero_pair, zinb_nb_raw, finish_factors_pair) returns
+    what the plain per-element function returns -- including the series / MUFU switch points (q = 1/16, d = 1/32), the
+    clip bounds and rows with extreme size factors."""
     y, m, sf, d, pi = _cases(4000, 11)
     m[:6] = [1e-5, 1e6, 2e-5, 5e5, 1.0, 1.0]; d[:6] = [1e-4, 1e4, 0.03125, 0.031, 0.0313, 9e3]
     sf[6:10] = [1e-3, 1e3, 1.0, 1.0]
@@ -94,16 +94,15 @@ def test_kernel_formulations_equal_the_reference_formulation(ae_type, ridge):
     m[10:14] = [1.0 / 15.0, 0.0666, 0.0667, 0.07]; sf[10:14] = 1.0; d[10:14] = 1.0; y[10:14] = 0
     y, m, sf, d, pi = [a.astype(np.float32).astype(np.float64) for a in (y, m, sf, d, pi)]
     a = _host_elem(ae_type, y, m, sf, d, pi, ridge).astype(np.float64)
-    # True: branch-free zero branch / NB from mu (staged + fused kernels); "ring": the f32x2 pair functions, the masked
-    # rising-product groups and the shared finishing factors of zinb_loss_bwd_ring_kernel (the default loss kernel)
-    for variant, tol in ((True, 2e-6), ("ring", 2e-5)):
-        b = _host_elem(ae_type, y, m, sf, d, pi, ridge, kernel_variant=variant).astype(np.float64)
-        assert np.all(np.isfinite(a) == np.isfinite(b))
-        fin = np.isfinite(a)
-        scale = np.maximum(np.abs(a), 1e-3 * np.max(np.abs(np.where(fin, a, 0.0)), axis=0, keepdims=True) + 1e-30)
-        err = np.where(fin, np.abs(a - b) / scale, 0.0)
-        k = np.unravel_index(int(np.argmax(err)), err.shape)
-        assert err[k] <= tol, (ae_type, ridge, variant, k, a[k], b[k], y[k[0]], m[k[0]], sf[k[0]], d[k[0]], pi[k[0]])
+    # "ring": the f32x2 pair functions, the masked rising-product groups and the shared finishing factors of
+    # zinb_loss_bwd_ring_kernel and heads_loss_kernel
+    b = _host_elem(ae_type, y, m, sf, d, pi, ridge, kernel_variant="ring").astype(np.float64)
+    assert np.all(np.isfinite(a) == np.isfinite(b))
+    fin = np.isfinite(a)
+    scale = np.maximum(np.abs(a), 1e-3 * np.max(np.abs(np.where(fin, a, 0.0)), axis=0, keepdims=True) + 1e-30)
+    err = np.where(fin, np.abs(a - b) / scale, 0.0)
+    k = np.unravel_index(int(np.argmax(err)), err.shape)
+    assert err[k] <= 2e-5, (ae_type, ridge, k, a[k], b[k], y[k[0]], m[k[0]], sf[k[0]], d[k[0]], pi[k[0]])
 
 
 @pytest.mark.parametrize("ae_type", ["zinb-conddisp", "zinb"])
