@@ -58,11 +58,13 @@ _OPTIONS = [
     (('--packed',), dict(dest='packed', action='store_true',
                          help='With --preprocess device: keep the raw counts packed in GPU memory (several times more '
                               'cells than the normalised matrix; every batch is expanded on the GPU; same results)')),
+    (('--gzip',), dict(dest='gzip', action='store_true',
+                       help='Write the output matrices gzip-compressed (mean.tsv.gz, ...; compressed on the GPU)')),
 ]
 
 _DEFAULTS = dict(transpose=False, testsplit=False, saveweights=False, sizefactors=True, batchnorm=True,
                  checkcounts=True, norminput=True, hyper=False, debug=False, tensorboard=False, loginput=True,
-                 stream=False, packed=False)
+                 stream=False, packed=False, gzip=False)
 
 
 def build_parser():

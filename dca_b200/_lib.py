@@ -136,6 +136,8 @@ PROTOTYPES = {
     "dca_write_text_matrix": (C.c_int, [C.c_char_p, _vp, _i32, _i64, _i64, _i64, _vp, _vp, _i32, _i32]),
     "dca_write_text_device": (C.c_int, [C.c_char_p, _i32, _vp, _i64, _i64, _i64, _i32, _vp, _i64, _vp, _vp, _i64, _i32, _vp,
                                         _vp]),
+    "dca_write_text_device_gz": (C.c_int, [C.c_char_p, _i32, _vp, _i64, _i64, _i64, _i32, _vp, _i64, _vp, _vp, _i64, _i32,
+                                           _vp, _vp]),
     "dca_format_fixed6_host": (C.c_int, [_vp, _i64, _vp, _vp]),
     "dca_read_text_counts": (C.c_int, [C.c_char_p, _i32, _i32, _i64, _i32, _vp, _vp, _i64, _vp, _vp, _i64, _vp]),
     "dca_read_mtx_counts": (C.c_int, [C.c_char_p, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
@@ -144,6 +146,8 @@ PROTOTYPES = {
     "dca_gunzip": (C.c_int, [C.c_char_p, _i32, _vp, _vp, _i64, _vp]),
     "dca_inflate_span_host": (C.c_int, [_vp, _i64, _i32, _i64, _i64, _vp, _i64, _vp]),
     "dca_inflate_find_host": (C.c_int, [_vp, _i64, _i64, _i64, _vp]),
+    "dca_gzip_device": (C.c_int, [_vp, _i64, _vp, _i64, _i32, _vp, _vp]),
+    "dca_gzip_host": (C.c_int, [_vp, _i64, _vp, _i64, C.POINTER(_i64)]),
     "dca_count_escapes": (C.c_int, [_vp, _i32, _i64, _i64, _i64, _vp, _i32]),
     "dca_pack_counts": (C.c_int, [_vp, _i32, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _i32]),
     "dca_sparse_counts": (C.c_int, [_vp, _i32, _i64, _i64, _i64, _vp, _vp, _i32]),

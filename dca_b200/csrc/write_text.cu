@@ -6,12 +6,14 @@
 //   label_write / field_write   fill the bytes at those offsets (a tile is formatted in shared memory, then copied)
 // The offsets depend on the values only, so the text is a function of the input.  The group's text goes to the host in
 // pieces through two pinned buffers; a writer thread appends one piece to the file while the next is formatted and
-// copied.
+// copied.  dca_write_text_device_gz takes the same path with one more step per group: the header and each group's
+// text are compressed on the device (deflate.cu, one gzip member per call), and the pieces carry the compressed bytes.
 //
 // Number format: '%.6f' of the float32 value (exact in double), correctly rounded, ties to even, on integers only.
 // v = +-m * 2^e with m < 2^24: for e < 0, m * 10^6 < 2^44 is shifted right by -e with round-half-even on the bits
 // shifted out; for e >= 0, v is an integer below 2^128, written in base-10^9 groups, then ".000000".
 #include "dca_internal.cuh"
+#include "deflate.cuh"
 #include "text_chunks.cuh"
 
 #include <algorithm>
@@ -214,6 +216,8 @@ struct DeviceTextWriter {
   long long *d_seg = nullptr, *d_pos = nullptr;
   char* d_text = nullptr;
   long long text_cap = 0;
+  uint8_t* d_gz = nullptr;                             // gzip: the compressed header or group
+  long long gz_cap = 0;
   char* h_buf[2] = {nullptr, nullptr};
   long long* h_total = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -264,12 +268,35 @@ struct DeviceTextWriter {
       th.join();
     }
     if (s) (void)cudaStreamSynchronize(s);
-    cudaFree(d_labels); cudaFree(d_lab_off); cudaFree(d_seg); cudaFree(d_pos); cudaFree(d_text);
+    cudaFree(d_labels); cudaFree(d_lab_off); cudaFree(d_seg); cudaFree(d_pos); cudaFree(d_text); cudaFree(d_gz);
     cudaFreeHost(h_buf[0]); cudaFreeHost(h_buf[1]); cudaFreeHost(h_total);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (f) fclose(f);
     if (prev_device >= 0) (void)cudaSetDevice(prev_device);
+  }
+  // src[0, total) (device) to the file, piece by piece, alternating the pinned buffers
+  int send(const char* src, long long total, long long piece, int* slot) {
+    for (long long off = 0; off < total; off += piece, *slot ^= 1) {
+      const long long n = std::min(piece, total - off);
+      const auto t0 = std::chrono::steady_clock::now();
+      wait_free(*slot);
+      wait_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+      DCA_CUDA_OK(cudaMemcpyAsync(h_buf[*slot], src + off, (size_t)n, cudaMemcpyDeviceToHost, s));
+      DCA_CUDA_OK(cudaStreamSynchronize(s));
+      submit(*slot, n);
+    }
+    return DCA_OK;
+  }
+  // gzip: room for the compressed form of `n` bytes
+  int gz_room(long long n) {
+    const long long want = deflate::gzip_bound(n);
+    if (want <= gz_cap) return DCA_OK;
+    DCA_CUDA_OK(cudaFree(d_gz));
+    d_gz = nullptr;
+    gz_cap = want + want / 4;
+    DCA_CUDA_OK(cudaMalloc(&d_gz, (size_t)gz_cap));
+    return DCA_OK;
   }
 };
 
@@ -278,28 +305,31 @@ struct DeviceTextWriter {
 
 using namespace dca;
 
-extern "C" int dca_write_text_device(const char* path, int32_t append, const float* matrix, int64_t rows, int64_t cols,
-                                     int64_t ld, int32_t transpose, const char* header, int64_t header_len,
-                                     const char* labels, const int64_t* label_offsets, int64_t chunk_bytes,
-                                     int32_t device, void* stream, int64_t* info) {
+namespace {
+
+// dca_write_text_device (who = its name, gz = false) and dca_write_text_device_gz
+int write_text_device(const char* who, bool gz, const char* path, int32_t append, const float* matrix, int64_t rows,
+                      int64_t cols, int64_t ld, int32_t transpose, const char* header, int64_t header_len,
+                      const char* labels, const int64_t* label_offsets, int64_t chunk_bytes, int32_t device,
+                      void* stream, int64_t* info) {
   if (!path || !matrix || rows < 1 || cols < 1 || ld < cols || header_len < 0 ||
       (header_len > 0 && !header) || chunk_bytes < 0 || (label_offsets && !labels)) {
-    set_error("dca_write_text_device: bad argument");
+    set_error("%s: bad argument", who);
     return DCA_ERR_BAD_ARG;
   }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     (void)cudaGetLastError();
-    set_error("dca_write_text_device: no CUDA device available (this library has no CPU fallback)");
+    set_error("%s: no CUDA device available (this library has no CPU fallback)", who);
     return DCA_ERR_NO_DEVICE;
   }
-  if (device < 0 || device >= ndev) { set_error("dca_write_text_device: no CUDA device %d", device); return DCA_ERR_BAD_ARG; }
+  if (device < 0 || device >= ndev) { set_error("%s: no CUDA device %d", who, device); return DCA_ERR_BAD_ARG; }
   const long long out_rows = transpose ? cols : rows, out_cols = transpose ? rows : cols;
   const long long piece = chunk_bytes ? chunk_bytes : kDefaultPiece;
   const int tiles = cdiv(out_cols, kFmtThreads);
   // whole lines per group: about piece / 8 fields (a field takes 9 to 11 bytes at typical magnitudes)
   const long long group = std::max(1ll, std::min(out_rows, std::max(1ll, piece / 8) / out_cols));
-  if (group * (tiles + 1) >= (1ll << 31)) { set_error("dca_write_text_device: too many tiles in a line group"); return DCA_ERR_BAD_ARG; }
+  if (group * (tiles + 1) >= (1ll << 31)) { set_error("%s: too many tiles in a line group", who); return DCA_ERR_BAD_ARG; }
 
   DeviceTextWriter w;
   DCA_CUDA_OK(cudaGetDevice(&w.prev_device));
@@ -324,18 +354,38 @@ extern "C" int dca_write_text_device(const char* path, int32_t append, const flo
   DCA_CUDA_OK(cudaHostAlloc(&w.h_total, sizeof(long long), cudaHostAllocDefault));
   DCA_CUDA_OK(cudaEventCreate(&w.ev0));
   DCA_CUDA_OK(cudaEventCreate(&w.ev1));
+  deflate::GzipMember member;
+  if (gz) {
+    DCA_TRY(member.init(s));
+    DCA_TRY(w.gz_room(std::max(w.text_cap, (long long)header_len)));
+  }
 
   w.f = fopen(path, append ? "ab" : "wb");
-  if (!w.f) { set_error("dca_write_text_device: cannot open %s", path); return DCA_ERR_BAD_ARG; }
-  if (header_len && fwrite(header, 1, (size_t)header_len, w.f) != (size_t)header_len) {
-    set_error("dca_write_text_device: write to %s failed", path);
-    return DCA_ERR_CUDA;
-  }
-  w.start();
-
-  long long bytes = header_len, groups = 0;
+  if (!w.f) { set_error("%s: cannot open %s", who, path); return DCA_ERR_BAD_ARG; }
+  long long bytes = 0, groups = 0;
   double kernel_ms = 0.0;
   int slot = 0;
+  if (header_len && !gz) {
+    if (fwrite(header, 1, (size_t)header_len, w.f) != (size_t)header_len) {
+      set_error("%s: write to %s failed", who, path);
+      return DCA_ERR_CUDA;
+    }
+    bytes = header_len;
+  }
+  w.start();
+  if (header_len && gz) {                              // the header line opens the member
+    if (header_len > w.text_cap) {
+      DCA_CUDA_OK(cudaFree(w.d_text));
+      w.d_text = nullptr;
+      w.text_cap = header_len;
+      DCA_CUDA_OK(cudaMalloc(&w.d_text, (size_t)w.text_cap));
+    }
+    DCA_CUDA_OK(cudaMemcpyAsync(w.d_text, header, (size_t)header_len, cudaMemcpyHostToDevice, s));
+    long long zn = 0;
+    DCA_TRY(member.feed((const uint8_t*)w.d_text, header_len, true, false, w.d_gz, &zn));
+    DCA_TRY(w.send((const char*)w.d_gz, zn, piece, &slot));
+    bytes += zn;
+  }
   for (long long line0 = 0; line0 < out_rows; line0 += group, ++groups) {
     const long long lines = std::min(group, out_rows - line0);
     const long long n = lines * (tiles + 1);
@@ -367,21 +417,20 @@ extern "C" int dca_write_text_device(const char* path, int32_t append, const flo
     field_write_kernel<<<(unsigned)(lines * tiles), kFmtThreads, 0, s>>>(matrix, ld, transpose, line0, out_cols, tiles,
                                                                          w.d_pos, w.d_text);
     DCA_LAUNCH_CHECK();
+    const char* src = w.d_text;
+    long long len = total;
+    if (gz) {
+      DCA_TRY(w.gz_room(total));
+      DCA_TRY(member.feed((const uint8_t*)w.d_text, total, groups == 0 && !header_len, line0 + lines == out_rows,
+                          w.d_gz, &len));
+      src = (const char*)w.d_gz;
+    }
     DCA_CUDA_OK(cudaEventRecord(w.ev1, s));
     DCA_CUDA_OK(cudaEventSynchronize(w.ev1));
     DCA_CUDA_OK(cudaEventElapsedTime(&ms, w.ev0, w.ev1));
     kernel_ms += ms;
-    // the group's text to the file, piece by piece, alternating the pinned buffers
-    for (long long off = 0; off < total; off += piece, slot ^= 1) {
-      const long long len = std::min(piece, total - off);
-      const auto t0 = std::chrono::steady_clock::now();
-      w.wait_free(slot);
-      w.wait_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-      DCA_CUDA_OK(cudaMemcpyAsync(w.h_buf[slot], w.d_text + off, (size_t)len, cudaMemcpyDeviceToHost, s));
-      DCA_CUDA_OK(cudaStreamSynchronize(s));
-      w.submit(slot, len);
-    }
-    bytes += total;
+    DCA_TRY(w.send(src, len, piece, &slot));
+    bytes += len;
   }
   const auto t0 = std::chrono::steady_clock::now();
   w.wait_free(-1);
@@ -389,7 +438,7 @@ extern "C" int dca_write_text_device(const char* path, int32_t append, const flo
   const bool failed = w.failed;
   const int cl = fclose(w.f);
   w.f = nullptr;
-  if (failed || cl != 0) { set_error("dca_write_text_device: write to %s failed", path); return DCA_ERR_CUDA; }
+  if (failed || cl != 0) { set_error("%s: write to %s failed", who, path); return DCA_ERR_CUDA; }
   if (info) {
     info[0] = bytes;
     info[1] = groups;
@@ -397,6 +446,24 @@ extern "C" int dca_write_text_device(const char* path, int32_t append, const flo
     info[3] = (int64_t)(w.wait_ms * 1e3);
   }
   return DCA_OK;
+}
+
+}  // namespace
+
+extern "C" int dca_write_text_device(const char* path, int32_t append, const float* matrix, int64_t rows, int64_t cols,
+                                     int64_t ld, int32_t transpose, const char* header, int64_t header_len,
+                                     const char* labels, const int64_t* label_offsets, int64_t chunk_bytes,
+                                     int32_t device, void* stream, int64_t* info) {
+  return write_text_device("dca_write_text_device", false, path, append, matrix, rows, cols, ld, transpose, header,
+                           header_len, labels, label_offsets, chunk_bytes, device, stream, info);
+}
+
+extern "C" int dca_write_text_device_gz(const char* path, int32_t append, const float* matrix, int64_t rows,
+                                        int64_t cols, int64_t ld, int32_t transpose, const char* header,
+                                        int64_t header_len, const char* labels, const int64_t* label_offsets,
+                                        int64_t chunk_bytes, int32_t device, void* stream, int64_t* info) {
+  return write_text_device("dca_write_text_device_gz", true, path, append, matrix, rows, cols, ld, transpose, header,
+                           header_len, labels, label_offsets, chunk_bytes, device, stream, info);
 }
 
 // The formatter of the kernels above, run on the CPU: out gets the '%.6f' text of the float32 bit patterns bits[0..n)

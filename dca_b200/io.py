@@ -419,9 +419,22 @@ def read_genelist(filename):
     return genelist
 
 
-def write_text_matrix(matrix, filename, rownames=None, colnames=None, transpose=False, threads=0):
+def write_text_matrix(matrix, filename, rownames=None, colnames=None, transpose=False, threads=0, gzip=False,
+                      device=None):
     """TSV with '%.6f' values, the files of dca/io.py:120-129 byte for byte.  float32 / float64 matrices go through
-    the multi-threaded native writer (dca_write_text_matrix); anything else through pandas like the reference."""
+    the multi-threaded native writer (dca_write_text_matrix); anything else through pandas like the reference.
+
+    gzip=True writes the same text gzip-compressed on the CUDA device `device` (default: the current one): the text
+    goes to a temporary file beside `filename`, which gzip_file_device compresses in pieces and then removes."""
+    if gzip:
+        tmp = "%s.%d.tmp" % (filename, os.getpid())
+        try:
+            write_text_matrix(matrix, tmp, rownames, colnames, transpose, threads)
+            gzip_file_device(tmp, filename, device=device)
+        finally:
+            if os.path.exists(tmp):
+                os.remove(tmp)
+        return
     import ctypes as C
     m = np.asarray(matrix)
     native = m.ndim == 2 and m.dtype in (np.float32, np.float64) and m.size > 0
@@ -478,8 +491,49 @@ def header_bytes(colnames, has_rownames):
     return (b"\t" if has_rownames else b"") + b"\t".join(quote_label(v) for v in list(colnames)) + b"\n"
 
 
+def gzip_device(data, device=None, info=None):
+    """One gzip member of `data` (bytes, or a 1-d uint8 CUDA tensor) compressed on a CUDA device by dca_gzip_device
+    (csrc/deflate.cu), as a uint8 CUDA tensor.  Bytes go to `device` (default: the current one) first.  info: an int64
+    array of 3, filled with the member's bytes, blocks and stored blocks."""
+    import ctypes as C
+    import torch
+    from . import _lib
+    if isinstance(data, torch.Tensor):
+        if not data.is_cuda or data.dtype != torch.uint8 or data.dim() != 1:
+            raise ValueError("gzip_device takes bytes or a 1-d uint8 CUDA tensor")
+        src = data.contiguous()
+    else:
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        src = torch.frombuffer(bytearray(data), dtype=torch.uint8).to(dev) if len(data) else \
+            torch.empty(0, dtype=torch.uint8, device=dev)
+    lib = _lib.load()
+    n = src.numel()
+    info_arr = np.zeros(3, dtype=np.int64)
+    _lib.check(lib.dca_gzip_device(None, n, None, 0, 0, None, info_arr.ctypes.data), "dca_gzip_device")
+    out = torch.empty(int(info_arr[0]), dtype=torch.uint8, device=src.device)
+    stream = torch.cuda.current_stream(src.device)
+    with torch.cuda.device(src.device):
+        _lib.check(lib.dca_gzip_device(C.c_void_p(src.data_ptr() if n else 0), n, C.c_void_p(out.data_ptr()), out.numel(),
+                                       src.device.index, C.c_void_p(stream.cuda_stream), info_arr.ctypes.data),
+                   "dca_gzip_device")
+    if info is not None:
+        info[:] = info_arr
+    return out[:int(info_arr[0])]
+
+
+def gzip_file_device(src, dst, device=None, piece_bytes=64 << 20):
+    """dst = src gzip-compressed on a CUDA device: one gzip member per piece of piece_bytes, so host memory holds one
+    piece whatever the file's size."""
+    with open(src, "rb") as f, open(dst, "wb") as g:
+        while True:
+            data = f.read(piece_bytes)
+            g.write(gzip_device(data, device).cpu().numpy().tobytes())
+            if len(data) < piece_bytes:
+                break
+
+
 def write_text_matrix_device(tensor, filename, rownames=None, colnames=None, transpose=False, append=False,
-                             header=True, chunk_bytes=0, info=None):
+                             header=True, chunk_bytes=0, info=None, gzip=False):
     """write_text_matrix(tensor.cpu().numpy(), filename, rownames, colnames, transpose) byte for byte, formatted on the
     tensor's CUDA device (dca_write_text_device, csrc/write_text.cu): a float32 matrix in device memory becomes text
     without a host copy of it.  The text reaches the file in pinned pieces of chunk_bytes (0: 16 MB), the write of one
@@ -488,7 +542,11 @@ def write_text_matrix_device(tensor, filename, rownames=None, colnames=None, tra
     append=True appends to the file instead of creating it, and header=False leaves out the header line, so that a
     matrix can be written in blocks of output lines.  info: an int64 array of 4, filled with the bytes written, line
     groups, microseconds of formatting kernels and microseconds waiting for the file writes.  An empty matrix goes
-    through write_text_matrix."""
+    through write_text_matrix.
+
+    gzip=True writes the text as one gzip member instead (appended as one more member with append=True), compressed
+    on the device before it leaves it (dca_write_text_device_gz): the file decompresses to the bytes gzip=False writes,
+    and info[0] counts compressed bytes."""
     import ctypes as C
     import torch
     from . import _lib
@@ -498,7 +556,7 @@ def write_text_matrix_device(tensor, filename, rownames=None, colnames=None, tra
     if t.numel() == 0:
         if append or not header:
             raise ValueError("an empty matrix is written whole")
-        write_text_matrix(t.cpu().numpy(), filename, rownames, colnames, transpose)
+        write_text_matrix(t.cpu().numpy(), filename, rownames, colnames, transpose, gzip=gzip, device=t.device)
         return
     if t.stride(1) != 1 or t.stride(0) < t.shape[1]:
         t = t.contiguous()
@@ -518,11 +576,12 @@ def write_text_matrix_device(tensor, filename, rownames=None, colnames=None, tra
     info_arr = np.zeros(4, dtype=np.int64)
     stream = torch.cuda.current_stream(dev)
     with torch.cuda.device(dev):
-        _lib.check(lib.dca_write_text_device(os.fsencode(filename), int(bool(append)), C.c_void_p(t.data_ptr()), rows, cols,
-                                             t.stride(0), int(bool(transpose)), head, len(head), labels,
-                                             None if offsets is None else offsets.ctypes.data, int(chunk_bytes), dev.index,
-                                             C.c_void_p(stream.cuda_stream), info_arr.ctypes.data),
-                   "dca_write_text_device")
+        entry = "dca_write_text_device_gz" if gzip else "dca_write_text_device"
+        _lib.check(getattr(lib, entry)(os.fsencode(filename), int(bool(append)), C.c_void_p(t.data_ptr()), rows, cols,
+                                       t.stride(0), int(bool(transpose)), head, len(head), labels,
+                                       None if offsets is None else offsets.ctypes.data, int(chunk_bytes), dev.index,
+                                       C.c_void_p(stream.cuda_stream), info_arr.ctypes.data),
+                   entry)
     if info is not None:
         info[:] = info_arr
 

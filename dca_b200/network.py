@@ -25,6 +25,11 @@ from .io import write_text_matrix, write_text_matrix_device
 PREDICT_BATCH = 4096      # rows per dca_predict call (Keras predict uses 32; result is identical)
 
 
+def _out_name(name, gzip):
+    """The file name of one output matrix: <name>.tsv, or <name>.tsv.gz with gzip."""
+    return name + (".tsv.gz" if gzip else ".tsv")
+
+
 def gene_block(n_cells, n_genes, n_heads, free_bytes, max_block_bytes=None):
     """Genes per block of write_predictions: the device holds n_cells x block float32 per gene-major head, within half
     of free_bytes (the rest is left to the batch buffers and the text writer) and within max_block_bytes (all heads
@@ -284,23 +289,29 @@ class Autoencoder:
             adata.X = adata.raw.X.copy()  # as the reference does (dca/network.py:208-209)
         return adata if copy else None
 
+    def _device(self):
+        """The engine's CUDA device (the current one before the engine exists): where write(gzip=True) compresses."""
+        return self.engine.device if self.engine is not None else None
+
     # -- dca/network.py:213-231
-    def write(self, adata, file_path, mode='denoise', colnames=None):
+    def write(self, adata, file_path, mode='denoise', colnames=None, gzip=False):
+        """gzip=True writes each <name>.tsv as <name>.tsv.gz, compressed on the GPU (io.write_text_matrix)."""
         colnames = adata.var_names.values if colnames is None else colnames
         rownames = adata.obs_names.values
         print('dca: Saving output(s)...')
         os.makedirs(file_path, exist_ok=True)
         if mode in ('denoise', 'full'):
             print('dca: Saving denoised expression...')
-            write_text_matrix(adata.X, os.path.join(file_path, 'mean.tsv'),
-                              rownames=rownames, colnames=colnames, transpose=True)
+            write_text_matrix(adata.X, os.path.join(file_path, _out_name('mean', gzip)),
+                              rownames=rownames, colnames=colnames, transpose=True, gzip=gzip, device=self._device())
         if mode in ('latent', 'full'):
             print('dca: Saving latent representations...')
-            write_text_matrix(adata.obsm['X_dca'], os.path.join(file_path, 'latent.tsv'),
-                              rownames=rownames, transpose=False)
+            write_text_matrix(adata.obsm['X_dca'], os.path.join(file_path, _out_name('latent', gzip)),
+                              rownames=rownames, transpose=False, gzip=gzip, device=self._device())
 
     def write_predictions(self, file_path, rownames, colnames, mode='full', return_info=True, device_data=None,
-                          stream_data=None, packed_data=None, adata=None, max_block_bytes=None, chunk_bytes=0):
+                          stream_data=None, packed_data=None, adata=None, max_block_bytes=None, chunk_bytes=0,
+                          gzip=False):
         """The files predict(adata, mode, return_info, ...) followed by write(adata, file_path, mode, colnames) write,
         byte for byte and with the same messages, without the cells x genes outputs ever on the host.  rownames: the
         cell labels (adata.obs_names), colnames: the output gene labels.  The input comes from device_data,
@@ -314,7 +325,10 @@ class Autoencoder:
         latent.tsv comes from the first pass; the per-gene dispersion of 'nb' / 'zinb' from the same call as in
         predict, written by write_text_matrix.  The per-cell dispersion and dropout of 'nb-shared' / 'zinb-shared'
         are not cells x genes: with return_info those models go through predict(adata, ...) and write(...) unchanged,
-        which needs adata.  chunk_bytes: the pinned text pieces of the writer (0: 16 MB)."""
+        which needs adata.  chunk_bytes: the pinned text pieces of the writer (0: 16 MB).
+
+        gzip=True writes <name>.tsv.gz in place of each <name>.tsv: the text is compressed on the GPU before it leaves
+        it (one gzip member per gene block), and decompresses to the bytes gzip=False writes."""
         assert mode in ('denoise', 'latent', 'full'), 'Unknown mode'
         info = return_info and isinstance(self, _InfoMixin)
         if info and self.ae_type in ("nb-shared", "zinb-shared"):
@@ -323,7 +337,7 @@ class Autoencoder:
                                  % self.ae_type)
             self.predict(adata, mode=mode, return_info=return_info, device_data=device_data, stream_data=stream_data,
                          packed_data=packed_data)
-            self.write(adata, file_path, mode=mode, colnames=colnames)
+            self.write(adata, file_path, mode=mode, colnames=colnames, gzip=gzip)
             return
         eng, N, bs, run, theta, session = self._source(adata, _one_dataset(device_data, stream_data, packed_data))
         rownames, colnames = list(rownames), list(colnames)
@@ -341,7 +355,7 @@ class Autoencoder:
         if info and cond: widths["disp"] = G
         if want_pi: widths["pi"] = G
         if want_latent: widths["latent"] = eng.latent_dim
-        files = [(k, f) for k, f in (("mean", "mean.tsv"), ("disp", "dispersion.tsv"), ("pi", "dropout.tsv"))
+        files = [(k, _out_name(f, gzip)) for k, f in (("mean", "mean"), ("disp", "dispersion"), ("pi", "dropout"))
                  if k in widths]
         bufs = {k: torch.empty((bs, w), dtype=torch.float32, device=dev) for k, w in widths.items()}
         free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
@@ -372,18 +386,18 @@ class Autoencoder:
                 write_text_matrix_device(blk[k][:, :g1 - g0], os.path.join(file_path, f),
                                          rownames=rownames if (k == "mean" and b == 0) else None,
                                          colnames=colnames[g0:g1], transpose=True, append=b > 0,
-                                         chunk_bytes=chunk_bytes)
+                                         chunk_bytes=chunk_bytes, gzip=gzip)
         del blk, bufs
         if want_latent:
             print('dca: Saving latent representations...')
-            write_text_matrix_device(latent, os.path.join(file_path, 'latent.tsv'), rownames=rownames,
-                                     chunk_bytes=chunk_bytes)
+            write_text_matrix_device(latent, os.path.join(file_path, _out_name('latent', gzip)), rownames=rownames,
+                                     chunk_bytes=chunk_bytes, gzip=gzip)
         if info and not cond:
             th = torch.empty(G, dtype=torch.float32, device=dev)
             with session():
                 theta(th)
-            write_text_matrix(th.cpu().numpy().reshape(1, -1), os.path.join(file_path, 'dispersion.tsv'),
-                              colnames=colnames, transpose=True)
+            write_text_matrix(th.cpu().numpy().reshape(1, -1), os.path.join(file_path, _out_name('dispersion', gzip)),
+                              colnames=colnames, transpose=True, gzip=gzip, device=dev)
 
 
 class _InfoMixin:
@@ -415,19 +429,21 @@ class _InfoMixin:
             adata.X = adata.raw.X.copy()
         return adata if copy else None
 
-    def write(self, adata, file_path, mode='denoise', colnames=None):
+    def write(self, adata, file_path, mode='denoise', colnames=None, gzip=False):
         colnames = adata.var_names.values if colnames is None else colnames
-        Autoencoder.write(self, adata, file_path, mode, colnames=colnames)
+        Autoencoder.write(self, adata, file_path, mode, colnames=colnames, gzip=gzip)
+        z = dict(gzip=gzip, device=self._device())
         if self.const_disp:
             if 'X_dca_dispersion' in adata.var_keys():
                 write_text_matrix(np.asarray(adata.var['X_dca_dispersion']).reshape(1, -1),
-                                  os.path.join(file_path, 'dispersion.tsv'), colnames=colnames, transpose=True)
+                                  os.path.join(file_path, _out_name('dispersion', gzip)), colnames=colnames,
+                                  transpose=True, **z)
         elif 'X_dca_dispersion' in adata.obsm_keys():
-            write_text_matrix(adata.obsm['X_dca_dispersion'], os.path.join(file_path, 'dispersion.tsv'),
-                              colnames=colnames, transpose=True)
+            write_text_matrix(adata.obsm['X_dca_dispersion'], os.path.join(file_path, _out_name('dispersion', gzip)),
+                              colnames=colnames, transpose=True, **z)
         if 'X_dca_dropout' in adata.obsm_keys():
-            write_text_matrix(adata.obsm['X_dca_dropout'], os.path.join(file_path, 'dropout.tsv'),
-                              colnames=colnames, transpose=True)
+            write_text_matrix(adata.obsm['X_dca_dropout'], os.path.join(file_path, _out_name('dropout', gzip)),
+                              colnames=colnames, transpose=True, **z)
 
 
 class NBConstantDispAutoencoder(_InfoMixin, Autoencoder):     # 'nb'

@@ -434,5 +434,6 @@ def train_with_args(args):
     # the files of net.predict(adata, mode='full', return_info=True, ...) + net.write(...), written in gene blocks
     # from the device: host memory holds the labels and the text buffers, never a cells x genes output
     net.write_predictions(args.outputdir, adata.obs_names.values, predict_columns, mode='full', return_info=True,
-                          adata=adata, **({ds.kind: ds} if ds is not None else {}))
+                          adata=adata, gzip=bool(getattr(args, 'gzip', False)),
+                          **({ds.kind: ds} if ds is not None else {}))
     return losses

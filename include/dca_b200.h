@@ -595,6 +595,16 @@ int dca_write_text_device(const char* path, int32_t append, const float* matrix,
                           int32_t transpose, const char* header, int64_t header_len, const char* labels,
                           const int64_t* label_offsets, int64_t chunk_bytes, int32_t device, void* stream,
                           int64_t* info);
+/* dca_write_text_device writing one gzip member (RFC 1952) of the same text instead: the same parameters, and the
+ * file holds one more member per call with append != 0, so a matrix written in blocks of lines is a multi-member
+ * gzip file whose decompressed bytes are those dca_write_text_device writes.  The header and every formatted group
+ * of lines are compressed on `device` (dca_gzip_device's encoder; a group's matches do not reach into the group
+ * before) before the pinned copy, so only compressed bytes cross to the host.  info[0] is the compressed bytes
+ * written; the formatting microseconds in info[2] include the compression's. */
+int dca_write_text_device_gz(const char* path, int32_t append, const float* matrix, int64_t rows, int64_t cols,
+                             int64_t ld, int32_t transpose, const char* header, int64_t header_len, const char* labels,
+                             const int64_t* label_offsets, int64_t chunk_bytes, int32_t device, void* stream,
+                             int64_t* info);
 /* The number formatter of dca_write_text_device run on the CPU, for tests: the '%.6f' text of the float32 bit patterns
  * bits[0..n) back to back in out (at least 47 * n bytes), that of bits[i] at out[offsets[i] .. offsets[i + 1]). */
 int dca_format_fixed6_host(const uint32_t* bits, int64_t n, char* out, int64_t* offsets);
@@ -681,6 +691,20 @@ int dca_inflate_span_host(const uint8_t* in, int64_t n, int32_t eof, int64_t sta
 /* The block-start test of dca_gunzip on the CPU: *found = the first bit in [first_bit, end_bit) of in[0, n) where a
  * dynamic block with a fully valid header or a stored block with LEN = ~NLEN and zero padding could start, or -1. */
 int dca_inflate_find_host(const uint8_t* in, int64_t n, int64_t first_bit, int64_t end_bit, int64_t* found);
+
+/* GPU gzip compressor: one gzip member (RFC 1952; header 1f 8b 08 00, MTIME 0, XFL 0, OS 255) of the n DEVICE bytes
+ * at `in`, written to DEVICE memory `out` (out_cap bytes), with no zlib.  The input is cut into blocks of 32 KB, each
+ * compressed by one CTA: greedy LZ77 whose matches reach up to 32 KB back (into the blocks before), then the smallest
+ * of a dynamic Huffman block (codes limited to 15 bits), a fixed Huffman block and a stored block; a non-final block
+ * ends with an empty stored block so that the blocks concatenate at byte offsets.  The bytes depend on the input
+ * alone, never on scheduling, and equal dca_gzip_host's.  Sizes and offsets are 64-bit (ISIZE is n mod 2^32).
+ *   out == NULL: info[0] = the most bytes the member can take (18 + n + 5 per block; 20 for n = 0).
+ *   out: out_cap must be at least that bound; info[0..2] = the member's bytes, blocks, stored blocks.
+ * Work runs on `stream` (of `device`); it returns when it is done.  Without a CUDA device: DCA_ERR_NO_DEVICE. */
+int dca_gzip_device(const void* in, int64_t n, void* out, int64_t out_cap, int32_t device, void* stream, int64_t* info);
+/* The same encoder on the CPU, for tests: the same bytes from HOST in[0, n) into HOST out; out == NULL: *out_len = the
+ * bound, else out_cap must be at least the bound and *out_len = the member's bytes. */
+int dca_gzip_host(const void* in, int64_t n, void* out, int64_t out_cap, int64_t* out_len);
 
 /* Host-side packer for dca_stream_begin_packed (multi-threaded counterpart of dca_b200/io.py:pack_counts; no
  * reference counterpart).  counts: HOST matrix rows x cols (ld elements per row) of dtype 0 float32, 1 float64,
