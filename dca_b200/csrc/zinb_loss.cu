@@ -6,7 +6,8 @@
 // bytes per tensor per row and the per-gene reduction needed by the constant-dispersion
 // variants stays in registers.  HBM traffic per element: y 4 B + nh*4 B in, nh*(4|2) B out.
 // The loss scalar is reduced thread -> warp shuffle -> shared memory -> one double per block,
-// and a second tiny kernel folds the block partials (deterministic, no float atomics).
+// and a second tiny kernel folds the block partials (deterministic, no float atomics).  The constant-dispersion
+// models' per-gene dL/dtheta likewise: every block stores its column sums, theta_fold_kernel adds them in row order.
 #include "dca_internal.cuh"
 #include <string>
 #include "zinb_math.cuh"
@@ -22,6 +23,9 @@ constexpr int kThreads = 256;
 constexpr int kVec = 4;
 constexpr int kColsPerBlock = kThreads * kVec;   // 1024 genes per block
 constexpr int kMaxBlocks = 65536;                // bound of the per-block loss-partial buffer
+// workspace: kMaxBlocks loss partials (double), the last-block arrival counter, then the dL/dtheta partials of the
+// constant-dispersion backward, one float per (row chunk, gene)
+constexpr size_t kThetaOff = sizeof(double) * (size_t)kMaxBlocks + 256;
 
 // Launch-plan override (dca_set_tunable "loss_target_blocks"): blocks per launch, 0 = auto (make_plan)
 int g_target_blocks = 0;
@@ -121,7 +125,7 @@ __global__ void __launch_bounds__(kThreads)
 zinb_loss_kernel(const float* __restrict__ Y, int64_t ldy, const int32_t* __restrict__ rows,
                  const float* __restrict__ sf, const float* m, const float* d, const float* pi,
                  int64_t ld, int B, int G, float ridge, float inv_n, int rows_per_block,
-                 GT* dzm, GT* dzd, GT* dzp, float* __restrict__ dth_partial,
+                 GT* dzm, GT* dzd, GT* dzp, float* __restrict__ dth_part,
                  double* __restrict__ loss_partial, const float* __restrict__ lf_global) {
   __shared__ double red[8];
   __shared__ float lf[zmath::kLogFactN];
@@ -174,10 +178,10 @@ zinb_loss_kernel(const float* __restrict__ Y, int64_t ldy, const int32_t* __rest
       }
       cur = nxt;
     }
-    if (BWD && !COND_DISP) {
+    if (BWD && !COND_DISP) {                       // this row chunk's dL/dtheta, folded in row order by theta_fold_kernel
 #pragma unroll
       for (int j = 0; j < VEC; ++j)
-        if (col0 + j < G) atomicAdd(dth_partial + col0 + j, tacc[j]);
+        if (col0 + j < G) dth_part[(size_t)blockIdx.y * G + col0 + j] = tacc[j];
     }
   }
   const double tot = block_reduce_sum(lsum, red);
@@ -346,7 +350,7 @@ __global__ void __launch_bounds__(kThreads, 3)
 zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_t* __restrict__ rows,
                           const float* __restrict__ sf, const float* m, const float* d, const float* pi,
                           int64_t ld, int B, int G, float ridge, float inv_n, int rows_per_block,
-                          GT* dzm, GT* dzd, GT* dzp, float* __restrict__ dth_acc,
+                          GT* dzm, GT* dzd, GT* dzp, float* __restrict__ dth_part,
                           double* __restrict__ loss_partial, const float* __restrict__ lf_global, const FoldArgs fa) {
   extern __shared__ __align__(128) unsigned char smem_ring[];
   constexpr int kWarps = kThreads / 32;
@@ -443,10 +447,8 @@ zinb_loss_bwd_ring_kernel(const float* __restrict__ Y, int64_t ldy, const int32_
       om += ld; op += ld;
       if (COND_DISP) od += ld;
     }
-    if (!COND_DISP && active) {
-#pragma unroll
-      for (int j = 0; j < kVec; ++j) atomicAdd(dth_acc + c0 + col + j, tacc[j]);
-    }
+    if (!COND_DISP && active)                      // this row chunk's dL/dtheta, folded in row order by theta_fold_kernel
+      *reinterpret_cast<float4*>(dth_part + (size_t)blockIdx.y * G + c0 + col) = make_float4(tacc[0], tacc[1], tacc[2], tacc[3]);
   }
   // ---- block reduction, then the last block to finish folds the per-block partials in a FIXED order
   block_loss_fold<kThreads>((double)lsum_nb + (double)lsum_r - (double)kLn2 * (double)lsum_lg,   // -log D = -ln2 * lg2 D
@@ -687,6 +689,37 @@ __global__ void fold_partials_kernel(const double* __restrict__ part, int n, dou
   }
 }
 
+// dL/dtheta per gene: the row chunks' partials (dth_part[chunk][gene]) added in row-chunk order, so that the same
+// inputs and plan give the same bits on every run.  One thread per gene reads 16 chunks before it adds them: at 103
+// chunks x 20000 genes the fold takes 7-8 us, against about 10 us with 8 loads in flight (H100 80GB HBM3, 700 W).
+__global__ void theta_fold_kernel(const float* __restrict__ part, int chunks, int G, float* __restrict__ dtheta) {
+  constexpr int kBatch = 16;
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= G) return;
+  const float* p = part + g;
+  float t = 0.f;
+  int c = 0;
+  for (; c + kBatch <= chunks; c += kBatch) {
+    float v[kBatch];
+#pragma unroll
+    for (int k = 0; k < kBatch; ++k) v[k] = p[(size_t)(c + k) * G];
+#pragma unroll
+    for (int k = 0; k < kBatch; ++k) t += v[k];
+  }
+  for (; c < chunks; ++c) t += p[(size_t)c * G];
+  dtheta[g] = t;
+}
+
+// Row chunks of the largest plan launch() can choose for a batch of at most B rows: make_plan's target-driven chunk
+// count at the widest columns (the vector plans), or the ring plan's cdiv(B, kMaxRowsPerBlock) where its row cap binds.
+// Non-decreasing in B, so a workspace sized for max_batch holds the plan of every smaller batch.
+int max_row_chunks(int B, int G) {
+  const int target = g_target_blocks > 0 ? g_target_blocks
+                     : ((long long)B * G <= (32ll << 20) ? 3 * sm_count_cached() : 16 * sm_count_cached());
+  const int chunks = std::max(1, target / cdiv(G, kColsPerBlock));
+  return std::min(B, std::max(chunks, cdiv(B, kMaxRowsPerBlock)));
+}
+
 __device__ float g_log_fact[zmath::kLogFactN];
 
 // log(k!) table in device global memory, filled once per device on first use
@@ -719,8 +752,6 @@ int launch(const LossArgs& a, cudaStream_t s) {
   }
   const float* lf_dev = log_fact_table_device();
   if (!lf_dev) return DCA_ERR_CUDA;
-  const size_t need = loss_workspace_bytes(a.B, a.G);
-  if (!a.ws || a.ws_bytes < need) { set_error("zinb_loss: workspace too small (%zu < %zu)", a.ws_bytes, need); return DCA_ERR_BAD_ARG; }
   double* lpart = reinterpret_cast<double*>(a.ws);
   auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   bool vec = (a.G % 4 == 0) && (a.ld % 4 == 0) && (a.ldy % 4 == 0) && al16(a.Y) && al16(a.m) && (!cond || al16(a.d)) &&
@@ -728,13 +759,26 @@ int launch(const LossArgs& a, cudaStream_t s) {
   if (BWD) vec = vec && al16(a.dzm) && (!cond || al16(a.dzd)) && (!has_pi || al16(a.dzp));
   const Plan p = make_plan(a.B, a.G, vec ? kColsPerBlock : kThreads);
   dim3 grid(p.col_blocks, p.row_chunks), block(kThreads);
-  float* tpart = a.dtheta;                                            // const-disp: accumulated with atomics
-  if (BWD && !cond) DCA_CUDA_OK(cudaMemsetAsync(a.dtheta, 0, sizeof(float) * (size_t)a.G, s));
-
   // ZINB backward on aligned shapes: the ring kernel, unless its plan (at most kMaxRowsPerBlock rows per block) needs
   // more blocks than the partial buffer holds or more row chunks than a grid's y dimension
   const Plan ps = make_plan(a.B, a.G, kColsPerBlock, kMaxRowsPerBlock);
-  if (BWD && vec && has_pi && (long long)ps.row_chunks * ps.col_blocks <= kMaxBlocks && ps.row_chunks <= 65535) {
+  const bool ring = BWD && vec && has_pi && (long long)ps.row_chunks * ps.col_blocks <= kMaxBlocks && ps.row_chunks <= 65535;
+  const int row_chunks = ring ? ps.row_chunks : p.row_chunks;
+  const bool theta = BWD && !cond;                                    // const-disp: dL/dtheta partials per row chunk
+  const size_t need = kThetaOff + (theta ? sizeof(float) * (size_t)row_chunks * (size_t)a.G : 0);
+  if (!a.ws || a.ws_bytes < need) {
+    set_error("zinb_loss: workspace too small for a plan of %d row chunks (%zu < %zu bytes)", row_chunks, a.ws_bytes, need);
+    return DCA_ERR_BAD_ARG;
+  }
+  float* tpart = theta ? reinterpret_cast<float*>(static_cast<char*>(a.ws) + kThetaOff) : nullptr;
+  auto fold_theta = [&]() -> int {
+    if (!theta) return DCA_OK;
+    theta_fold_kernel<<<cdiv(a.G, 128), 128, 0, s>>>(tpart, row_chunks, a.G, a.dtheta);
+    DCA_LAUNCH_CHECK();
+    return DCA_OK;
+  };
+
+  if (ring) {
     grid = dim3(ps.col_blocks, ps.row_chunks);
     FoldArgs fa{reinterpret_cast<unsigned*>(reinterpret_cast<char*>(a.ws) + sizeof(double) * (size_t)kMaxBlocks), a.loss_sum,
                 a.fin_penalty, a.fin_loss_slot, a.fin_epoch_acc, a.fin_batch};
@@ -751,7 +795,7 @@ int launch(const LossArgs& a, cudaStream_t s) {
     else             { if (cond) DCA_RING(true, float); else DCA_RING(false, float); }
 #undef DCA_RING
     DCA_LAUNCH_CHECK();
-    return DCA_OK;                                                      // the fold is done by the last block
+    return fold_theta();                                                // the loss fold is done by the last block
   }
 #define DCA_LOSS_LAUNCH(HP, CD, GT, V)                                                                 \
   zinb_loss_kernel<HP, CD, GT, V, BWD><<<grid, block, 0, s>>>(                                          \
@@ -775,7 +819,7 @@ int launch(const LossArgs& a, cudaStream_t s) {
   fold_partials_kernel<<<1, 256, 0, s>>>(lpart, (int)(grid.x * grid.y), a.loss_sum, BWD ? 0 : 1, a.fin_penalty, a.inv_n,
                                          a.fin_batch, BWD ? a.fin_loss_slot : nullptr, a.fin_epoch_acc);
   DCA_LAUNCH_CHECK();
-  return DCA_OK;
+  return fold_theta();
 }
 
 }  // namespace
@@ -784,8 +828,7 @@ const float* loss_log_fact_table() { return log_fact_table_device(); }
 int g_fused_heads_default = 0;            // 1: engines created from now on use the fused head/loss/backward kernel
 
 size_t loss_workspace_bytes(int B, int G) {
-  (void)B; (void)G;
-  return sizeof(double) * (size_t)kMaxBlocks + 256;
+  return kThetaOff + sizeof(float) * (size_t)max_row_chunks(B, G) * (size_t)G;
 }
 
 int zinb_loss_fwd_bwd(const LossArgs& a, cudaStream_t s) { return launch<true>(a, s); }
@@ -802,7 +845,7 @@ int heads_loss_tc(const HeadsLossArgs& a, cudaStream_t s) {
   }
   const float* lf_dev = log_fact_table_device();
   if (!lf_dev) return DCA_ERR_CUDA;
-  if (!a.ws || a.ws_bytes < loss_workspace_bytes(B, G)) { set_error("heads_loss_tc: workspace too small"); return DCA_ERR_BAD_ARG; }
+  if (!a.ws || a.ws_bytes < kThetaOff) { set_error("heads_loss_tc: workspace too small"); return DCA_ERR_BAD_ARG; }   // loss partials + counter
   CUtensorMap mh, mw[3];
   DCA_TRY(tc::make_tensor_map_2d(&mh, a.H3, 2, 1, (uint64_t)B, 64, 64, 64, 64, 1));
   for (int i = 0; i < 3; ++i) DCA_TRY(tc::make_tensor_map_2d(&mw[i], a.W[i], 2, 1, 64, (uint64_t)G, (uint64_t)G, 64, 64, 1));

@@ -380,7 +380,11 @@ int dca_packed_predict(dca_handle* h, const dca_packed_counts* src, const int32_
  * sf), d = DispAct(zd) (B x G) or, for const-disp types, theta (G values, ld ignored), pi.
  * Outputs (may alias the inputs): gradients of the mean loss w.r.t. the PRE-activations
  * dzm, dzd, dzp scaled by inv_n; for const-disp types dzd receives nothing and
- * dtheta (G floats) receives d(loss)/d(theta) (before the exp/clip chain) summed over rows.
+ * dtheta (G floats) receives d(loss)/d(theta) (before the exp/clip chain) summed over rows: per row chunk of the
+ * launch plan into the workspace, then the chunks in row order, so the result is the same bits on every run.
+ * workspace_bytes: at least dca_zinb_loss_workspace_bytes(batch, genes), which does not shrink as batch grows, so the
+ * size for a larger batch serves too; a plan that does not fit (e.g. after raising the "loss_target_blocks" tunable)
+ * is refused with DCA_ERR_BAD_ARG.
  * loss_sum: device double, receives the SUM of element losses (not the mean).
  * grad_dtype selects float32 or bfloat16 storage for dz*. */
 int dca_zinb_loss_fwd_bwd(const float* Y, int64_t ldy, const int32_t* rows, const float* sf,

@@ -5,7 +5,8 @@ The ring kernel walks at most 256 rows per block and puts the row chunks on the 
 runs on the generic vectorised kernel (zinb_loss_kernel + fold_partials_kernel) instead.  Checked for zinb-conddisp
 and zinb (constant dispersion, dL/dtheta summed per gene), with fp32 and bf16 gradients: the gradients of sampled rows
 against the float64 oracle, dL/dtheta and the loss sum against float64 sums over every row (oracle/torch_ref.py in
-float64 on the device, in row chunks; dL/dtheta by autograd)."""
+float64 on the device, in row chunks; dL/dtheta by autograd).  The workspace dca_zinb_loss_workspace_bytes asks for
+holds zinb's dL/dtheta partials of every row chunk of the plan; one without room for them is refused."""
 import ctypes as C
 
 import numpy as np
@@ -79,7 +80,22 @@ def test_loss_past_the_ring_plan_vs_oracle(ae_type):
     ref = _oracle_rows(ae_type, Y[ts].cpu().numpy(), m[ts].cpu().numpy(), sf[ts].cpu().numpy(),
                        (d[ts] if cond else d).cpu().numpy(), p[ts].cpu().numpy(), inv_n)
     nb = C.c_size_t(); assert lib.dca_zinb_loss_workspace_bytes(B, G, C.byref(nb)) == 0
+    # loss partials of 65536 blocks (double) + 256 bytes, then one float per (row chunk, gene): at most the ring plan's
+    # cdiv(B, 256) = 65536 row chunks
+    base = 8 * 65536 + 256
+    assert nb.value >= base + 4 * 65536 * G, nb.value
     ws = torch.zeros(nb.value, dtype=torch.uint8, device=DEV)
+    if not cond:
+        # declared a workspace of the loss partials alone (the buffer behind it is the full one)
+        gm = torch.empty((B, G), device=DEV); gp = torch.empty_like(gm)
+        dth = torch.empty(G, device=DEV)
+        loss = torch.zeros(1, dtype=torch.float64, device=DEV)
+        st = lib.dca_zinb_loss_fwd_bwd(Y.data_ptr(), G, None, sf.data_ptr(), m.data_ptr(), d.data_ptr(), p.data_ptr(), G,
+                                       B, G, L.AE_TYPE_IDS[ae_type], 0.0, inv_n, gm.data_ptr(), None, gp.data_ptr(), L.F32,
+                                       dth.data_ptr(), loss.data_ptr(), ws.data_ptr(), base, None)
+        torch.cuda.synchronize()
+        assert st == -1 and b"workspace too small" in lib.dca_last_error(), (st, lib.dca_last_error())
+        del gm, gp
     for gdt, tol in ((L.F32, 3e-4), (L.BF16, 6e-3)):
         tdt = torch.bfloat16 if gdt == L.BF16 else torch.float32
         gm = torch.empty((B, G), dtype=tdt, device=DEV); gp = torch.empty_like(gm)

@@ -143,11 +143,9 @@ def _fit(net, **kw):
                                                        ("nb", "float32", "auto"),
                                                        ("zinb-conddisp", "float32", "generic")])
 def test_train_matches_resident(ae_type, x_dtype, gemm_path):
-    """zinb-conddisp on the tensor-core path: history, weights and BatchNorm state bit-identical.  'nb' sums its theta
-    gradient with atomics and the generic path splits K with atomics: there two runs of the SAME arm already differ.
-    Three resident 'nb' runs of this test on an H100 spread by 2.8e-5 of a loss and 5.9e-3 in a weight (RMSprop turns
-    last-bit gradient noise into learning-rate-sized steps), as far as the streamed arm is from them; 'nb' is held to
-    about 3.5 times that (1e-4, 2e-2), the generic path to 1e-3 of the losses."""
+    """zinb-conddisp and nb on the tensor-core path: history, weights and BatchNorm state bit-identical.  The generic
+    path splits K with atomics: there two runs of the SAME arm already differ, and RMSprop turns last-bit gradient noise
+    into learning-rate-sized steps, so it is held to 1e-3 of the losses and 2e-2 of each weight tensor's scale."""
     G = 2000
     Y = synth_counts(1500, G, 12)
     dd, sd = _dd(Y, x_dtype=x_dtype), _sd(Y, x_dtype=x_dtype, batch=256)
@@ -157,14 +155,12 @@ def test_train_matches_resident(ae_type, x_dtype, gemm_path):
     h_d = _fit(n_d, device_data=dd, shuffle=False)
     h_s = _fit(n_s, stream_data=sd, shuffle=False)
     w_d, w_s = n_d.engine.get_weights(), n_s.engine.get_weights()
-    exact = ae_type == "zinb-conddisp" and gemm_path == "auto"
-    if exact:
+    if gemm_path == "auto":
         assert h_d == h_s
         assert all(np.array_equal(w_d[k], w_s[k]) for k in w_d)
     else:
-        tol = 1e-4 if gemm_path == "auto" else 1e-3
         for k in ("loss", "val_loss"):
-            np.testing.assert_allclose(h_s[k], h_d[k], rtol=tol)
+            np.testing.assert_allclose(h_s[k], h_d[k], rtol=1e-3)
         for k in w_d:
             assert np.max(np.abs(w_d[k] - w_s[k]), initial=0.0) <= 2e-2 * max(np.max(np.abs(w_d[k]), initial=0.0), 1.0), k
 

@@ -385,7 +385,8 @@ def test_train_streaming_from_host_equals_resident_training():
 @pytest.mark.parametrize("ae_type", ["zinb", "zinb-conddisp"])
 def test_loss_kernel_variants_vs_oracle(ae_type):
     """The ZINB backward kernel (per-thread cp.async rings) on an aligned shape with row gather, ridge and a partial last
-    column block, against the float64 oracle -- including the per-gene theta gradient of the constant-dispersion model."""
+    column block, against the float64 oracle -- including the per-gene theta gradient of the constant-dispersion model,
+    summed over the row chunks in a fixed order: a second call gives the same bits."""
     from tests.test_gpu_parity import _oracle_loss, _post_act
     L = _L(); lib = L.load()
     B, G = 200, 1028 + 1024                       # three column blocks, the last one 4 genes wide
@@ -398,8 +399,11 @@ def test_loss_kernel_variants_vs_oracle(ae_type):
     ref = _oracle_loss(ae_type, Y, sf, m, d, pi, 0.01, rows)
     dd = _t(d) if cond else _t(d[0])
     for gdt, tol in ((L.F32, 3e-4), (L.BF16, 6e-3)):
-        total, gm, gd, gp, dth = _loss_call(lib, L, _t(Y), G, torch.as_tensor(rows).to(DEV), _t(sf), _t(m), dd, _t(pi), B, G,
-                                            L.AE_TYPE_IDS[ae_type], 0.01, 1.0 / (B * G), gdt, cond=cond)
+        args = (lib, L, _t(Y), G, torch.as_tensor(rows).to(DEV), _t(sf), _t(m), dd, _t(pi), B, G, L.AE_TYPE_IDS[ae_type], 0.01,
+                1.0 / (B * G), gdt)
+        total, gm, gd, gp, dth = _loss_call(*args, cond=cond)
+        again = _loss_call(*args, cond=cond)
+        assert again[0] == total and all(torch.equal(a, b) for a, b in zip(again[1:], (gm, gd, gp, dth))), (ae_type, gdt)
         assert abs(total - ref["sum"]) <= 2e-5 * abs(ref["sum"]), (ae_type, total, ref["sum"])
         assert rel_err(gm.float().cpu().numpy(), ref["dzm"]) < tol
         assert rel_err(gp.float().cpu().numpy(), ref["dzp"]) < tol
