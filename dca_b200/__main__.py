@@ -43,7 +43,11 @@ _OPTIONS = [
     (('--hyper',), dict(dest='hyper', action='store_true', help='Hyperparameter search (not on the accelerated path)')),
     (('--hypern',), dict(dest='hypern', type=int, default=1000, help='(hyper) number of samples')),
     (('--hyperepoch',), dict(dest='hyperepoch', type=int, default=100, help='(hyper) epochs per sample')),
-    (('--debug',), dict(dest='debug', action='store_true', help='Enable debugging (default: False)')),
+    (('--debug',), dict(dest='debug', action='store_true',
+                        help='Check the NB/ZINB loss terms y_pred, t1 and t2 of every element for inf/NaN on the GPU in '
+                             'every training and validation step and stop with FloatingPointError at the first batch '
+                             'that has one, naming its cell and gene; no-op for the nb, poisson and normal types, as in '
+                             'DCA (default: False)')),
     (('--tensorboard',), dict(dest='tensorboard', action='store_true', help='Not on the accelerated path')),
     (('--checkcounts',), dict(dest='checkcounts', action='store_true', help='Check that the matrix has raw counts (default: True)')),
     (('--nocheckcounts',), dict(dest='checkcounts', action='store_false', help='Do not check for raw counts')),

@@ -63,6 +63,12 @@ class PackedCountsDesc(C.Structure):
     ]
 
 
+class DebugReport(C.Structure):
+    """dca_debug_report: the debug checks' report of the last step (include/dca_b200.h)."""
+    _fields_ = [("struct_bytes", C.c_int32), ("reserved", C.c_int32), ("count", C.c_int64 * 3),
+                ("first_row", C.c_int32 * 3), ("first_gene", C.c_int32 * 3)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/dca_b200.h
 _vp, _i32, _i64, _f, _sz = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t
 PROTOTYPES = {
@@ -94,6 +100,9 @@ PROTOTYPES = {
     "dca_predict": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp]),
     "dca_read_loss": (C.c_int, [_vp, C.POINTER(_f), C.POINTER(_i32), _vp]),
     "dca_read_epoch_acc": (C.c_int, [_vp, C.POINTER(C.c_double * 4), _i32, _vp]),
+    "dca_set_debug_checks": (C.c_int, [_vp, _i32]),
+    "dca_read_debug_report": (C.c_int, [_vp, C.POINTER(DebugReport), _vp]),
+    "dca_debug_check": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _i64, _vp, _i64, _i32, _i32, _vp, C.POINTER(DebugReport), _vp]),
     "dca_train_step_host": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _f, _f, C.POINTER(_f), _vp]),
     "dca_set_input_transform": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _vp]),
     "dca_set_loss_ring": (C.c_int, [_vp, _vp, _i32]),

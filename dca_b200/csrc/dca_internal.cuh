@@ -180,6 +180,21 @@ struct HeadsLossArgs {
   float* fin_loss_slot = nullptr; double* fin_epoch_acc = nullptr; const double* fin_penalty = nullptr; int fin_batch = 0;
 };
 int heads_loss_tc(const HeadsLossArgs& a, cudaStream_t s);
+
+// debug checks of dca/loss.py:87-100 (zinb_loss.cu): the reference's NB terms y_pred, t1, t2 of every element of a batch,
+// counted into a 48-byte device report (dca_debug_report's device form).  A kernel of its own that only reads the
+// operands the loss kernels read, so that the loss kernels and their bits are the same with the checks on.
+struct DebugCheckArgs {
+  const float* Y; int64_t ldy; const int32_t* rows; const float* sf;   // counts, batch row -> count row, size factors
+  const float* m; int64_t ldm;                                          // mean (before the size factor)
+  const float* theta; int64_t ld_theta;                                 // dispersion; ld_theta 0: one theta per gene
+  int B, G;
+  void* report;                                                         // accumulated into (cleared by the caller)
+};
+constexpr size_t kDebugReportBytes = 48;
+int debug_check(const DebugCheckArgs& a, cudaStream_t s);
+// device report -> the fields of the C ABI's dca_debug_report
+void debug_report_decode(const unsigned long long raw[6], int64_t count[3], int32_t first_row[3], int32_t first_gene[3]);
 // writes grads[P] = loss_sum*inv_n + penalty, grads[P+1] = nonfinite flag, epoch acc update
 
 }  // namespace dca

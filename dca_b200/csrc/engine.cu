@@ -222,6 +222,7 @@ int Engine::plan(const dca_config& c) {
   }
   o_stage_x = o_sx[0]; o_stage_y = o_sy[0]; o_stage_sf = o_ssf[0];
   if (x_kind) x_plan_arena(B, take);
+  o_dbg = take(kDebugReportBytes);
   arena_bytes = o;
   return DCA_OK;
 }
@@ -479,6 +480,7 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
     X = base + o_xdrop; ldx = cfg.n_in; xrows = nullptr;
   } else if (phase != 2 && !plain_hidden()) DCA_TRY(bump_step(s));
   if (phase != 2) {
+  DCA_TRY(debug_reset(s));
   DCA_CUDA_OK(cudaMemsetAsync(gp(0), 0, sizeof(float) * (size_t)(P + 2), s));
   bool any_pen = false;
   mark(0, s);
@@ -487,7 +489,7 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
   mark(1, s);
   float* Mb = f(o_head[0]); float* Db = f(o_head[1]); float* Pb = f(o_head[2]);
   const float inv_n = 1.0f / ((float)Bn * (float)G);
-  const bool fuse = fused_heads && (ldy % 4 == 0) && ((reinterpret_cast<uintptr_t>(Y) & 15) == 0);
+  const bool fuse = fused_heads && !debug_checks && (ldy % 4 == 0) && ((reinterpret_cast<uintptr_t>(Y) & 15) == 0);
   if (fuse) {
     // heads forward + loss + head backward in ONE kernel (flash_zinb.cu): no B x G tensor reaches HBM
     mark(2, s);
@@ -515,6 +517,14 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
     ha.loss_sum = d(o_acc) + 4; ha.ws = base + o_lossws; ha.ws_bytes = loss_ws_bytes;
     ha.counter_ready = 1;
     ha.fin_loss_slot = gp(P); ha.fin_epoch_acc = d(o_acc); ha.fin_penalty = any_pen ? d(o_acc) + 5 : nullptr; ha.fin_batch = Bn;
+    if (debug_report()) {
+      // the heads + loss kernel keeps m and theta in registers: the checks read the head-forward kernel's outputs
+      DCA_TRY(heads_forward(Bn, Mb, Db, Pb, G, nullptr, s));
+      LossArgs lc{};
+      lc.Y = Y; lc.ldy = ldy; lc.rows = rows; lc.sf = sf; lc.m = Mb; lc.d = Db; lc.ld = G; lc.B = Bn; lc.G = G;
+      lc.ae_type = DCA_AE_ZINB_CONDDISP;
+      DCA_TRY(debug_check_loss(lc, s));
+    }
     DCA_TRY(heads_loss_tc(ha, s));
   } else {
   LossArgs la{};
@@ -531,6 +541,7 @@ int Engine::train_step_body(const void* X, int64_t ldx, const float* Y, int64_t 
   la.loss_sum = d(o_acc) + 4; la.ws = base + o_lossws; la.ws_bytes = loss_ws_bytes;
   la.counter_ready = 1;
   la.fin_loss_slot = gp(P); la.fin_epoch_acc = d(o_acc); la.fin_penalty = any_pen ? d(o_acc) + 5 : nullptr; la.fin_batch = Bn;
+  DCA_TRY(debug_check_loss(la, s));
   DCA_TRY(zinb_loss_fwd_bwd(la, s));
   if (!cond) {
     // dtheta currently holds sum over rows of dL/dtheta (not / N)
@@ -687,6 +698,7 @@ int Engine::eval_step(const void* X, int64_t ldx, const float* Y, int64_t ldy, c
                       int Bn, cudaStream_t s) {
   if (!X || !Y) { set_error("dca_eval_step: X and Y must not be NULL"); return DCA_ERR_BAD_ARG; }
   if (Bn <= 0 || Bn > cfg.max_batch) { set_error("dca_eval_step: batch %d outside (0, max_batch=%d]", Bn, cfg.max_batch); return DCA_ERR_BAD_ARG; }
+  DCA_TRY(debug_reset(s));
   if (x_kind) return x_eval_step(X, ldx, Y, ldy, sf, rows, Bn, s);
   const int G = cfg.n_out;
   DCA_TRY(forward(X, ldx, rows, Bn, false, s));
@@ -698,6 +710,7 @@ int Engine::eval_step(const void* X, int64_t ldx, const float* Y, int64_t ldy, c
   la.m = Mb; la.d = cond ? Db : f(o_theta); la.pi = has_pi ? Pb : nullptr; la.ld = G;
   la.B = Bn; la.G = G; la.ae_type = cfg.ae_type; la.ridge = cfg.ridge; la.inv_n = 1.f;
   la.loss_sum = d(o_acc) + 2; la.ws = base + o_lossws; la.ws_bytes = loss_ws_bytes;
+  DCA_TRY(debug_check_loss(la, s));
   DCA_TRY(zinb_loss_fwd(la, s));
   add_double_kernel<<<1, 1, 0, s>>>(d(o_acc) + 3, (double)Bn * (double)G);
   DCA_LAUNCH_CHECK();
@@ -978,6 +991,30 @@ extern "C" int dca_read_epoch_acc(dca_handle* h, double acc_host[4], int32_t res
   DCA_CUDA_OK(cudaMemcpyAsync(acc_host, h->e.d(h->e.o_acc), 4 * sizeof(double), cudaMemcpyDeviceToHost, s));
   if (reset) DCA_CUDA_OK(cudaMemsetAsync(h->e.d(h->e.o_acc), 0, 4 * sizeof(double), s));
   DCA_CUDA_OK(cudaStreamSynchronize(s));
+  return DCA_OK;
+}
+
+extern "C" int dca_set_debug_checks(dca_handle* h, int32_t on) {
+  DCA_NEED_HANDLE(h);
+  Engine& e = h->e;
+  if (e.debug_checks == (on != 0)) return DCA_OK;
+  e.debug_checks = on != 0;
+  for (auto& g : e.graphs) if (g.exec) cudaGraphExecDestroy(g.exec);     // captured with the other kernel instantiations
+  e.graphs.clear();
+  return DCA_OK;
+}
+
+extern "C" int dca_read_debug_report(dca_handle* h, dca_debug_report* out, void* stream) {
+  if (!out || out->struct_bytes != (int32_t)sizeof(dca_debug_report)) {
+    set_error("dca_read_debug_report: NULL or unversioned dca_debug_report (struct_bytes must be %d)", (int)sizeof(dca_debug_report));
+    return DCA_ERR_BAD_ARG;
+  }
+  DCA_NEED_HANDLE(h);
+  unsigned long long v[6];
+  cudaStream_t s = (cudaStream_t)stream;
+  DCA_CUDA_OK(cudaMemcpyAsync(v, h->e.base + h->e.o_dbg, sizeof(v), cudaMemcpyDeviceToHost, s));
+  DCA_CUDA_OK(cudaStreamSynchronize(s));
+  debug_report_decode(v, out->count, out->first_row, out->first_gene);
   return DCA_OK;
 }
 

@@ -184,6 +184,28 @@ struct Engine {
               float* pi_out, int64_t ld_out, float* latent_out, cudaStream_t s);
   int init_params(uint64_t seed, cudaStream_t s);
 
+  // --debug (dca_set_debug_checks): debug_check_kernel (zinb_loss.cu) checks the reference's NB terms of every element
+  // into a 48-byte report at o_dbg, cleared at the start of every training / validation step, from the operands of the
+  // loss kernel, just before it.  The types whose reference loss has no such check (nb, poisson, normal) get no report
+  // pointer: their report stays zero.
+  bool debug_checks = false;
+  size_t o_dbg = 0;
+  void* debug_report() const {
+    const int t = cfg.ae_type;
+    return debug_checks && t != DCA_AE_NB && t != DCA_AE_POISSON && t != DCA_AE_NORMAL ? base + o_dbg : nullptr;
+  }
+  int debug_reset(cudaStream_t s) {
+    if (void* r = debug_report()) DCA_CUDA_OK(cudaMemsetAsync(r, 0, kDebugReportBytes, s));
+    return DCA_OK;
+  }
+  // the checks of the loss operands a loss kernel is about to read (no-op with the checks off)
+  int debug_check_loss(const LossArgs& la, cudaStream_t s) {
+    void* r = debug_report();
+    if (!r) return DCA_OK;
+    return debug_check(DebugCheckArgs{la.Y, la.ldy, la.rows, la.sf, la.m, la.ld, la.d,
+                                      (la.ae_type == DCA_AE_ZINB || la.ae_type == DCA_AE_NB) ? 0 : la.ld, la.B, la.G, r}, s);
+  }
+
   // tensor-core path hooks (dense_tc.cu)
   bool tc_supported() const;
   const char* tc_reason() const;

@@ -363,6 +363,7 @@ int Engine::x_train_step_body(const void* X, int64_t ldx, const float* Y, int64_
                               int Bn, cudaStream_t s) {
   const int G = cfg.n_out;
   const int64_t n = (int64_t)Bn * G;
+  DCA_TRY(debug_reset(s));
   DCA_CUDA_OK(cudaMemsetAsync(gp(0), 0, sizeof(float) * (size_t)(P + 2), s));
   bool any_pen = false;
   mark(0, s);
@@ -398,6 +399,7 @@ int Engine::x_train_step_body(const void* X, int64_t ldx, const float* Y, int64_
     la.dzm = Mb; la.dzd = Db; la.dzp = has_pi ? Pb : nullptr; la.grad_bf16 = 0;       // gradients in place
     la.loss_sum = d(o_acc) + 4; la.ws = base + o_lossws; la.ws_bytes = loss_ws_bytes; la.counter_ready = 1;
     la.fin_loss_slot = gp(P); la.fin_epoch_acc = d(o_acc); la.fin_penalty = any_pen ? d(o_acc) + 5 : nullptr; la.fin_batch = Bn;
+    DCA_TRY(debug_check_loss(la, s));
     DCA_TRY(zinb_loss_fwd_bwd(la, s));
   }
   mark(3, s);
@@ -489,6 +491,7 @@ int Engine::x_eval_step(const void* X, int64_t ldx, const float* Y, int64_t ldy,
   la.m = Mb; la.d = Db; la.pi = has_pi ? Pb : nullptr; la.ld = G;
   la.B = Bn; la.G = G; la.ae_type = has_pi ? DCA_AE_ZINB_CONDDISP : DCA_AE_NB_CONDDISP; la.ridge = cfg.ridge; la.inv_n = 1.f;
   la.loss_sum = d(o_acc) + 2; la.ws = base + o_lossws; la.ws_bytes = loss_ws_bytes;
+  DCA_TRY(debug_check_loss(la, s));
   DCA_TRY(zinb_loss_fwd(la, s));
   x_add_double_kernel<<<1, 1, 0, s>>>(d(o_acc) + 3, (double)Bn * (double)G);
   DCA_LAUNCH_CHECK();

@@ -661,6 +661,59 @@ heads_loss_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_consta
                             p.loss_partial, fa, p.inv_n);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Debug checks (dca/loss.py:87-100, NB.loss with debug=True), per element in the reference's float32 form:
+//   theta' = min(theta, 1e6) (a NaN theta stays NaN, as with tf.minimum), y_pred = m * sf,
+//   t1 = lgamma(theta' + eps) + lgamma(y + 1) - lgamma(y + theta' + eps),
+//   t2 = (theta' + y) log(1 + y_pred / (theta' + eps)) + y (log(theta' + eps) - log(y_pred + eps)).
+// A launch of its own ahead of the loss kernel, reading the same operands: the loss kernels are not touched, so the
+// loss, the gradients and every accumulator keep their bits with the checks on.  The report holds, per term, the count
+// of non-finite elements and the complement of the smallest key (batch row << 32 | gene), so that an all-zero report
+// means "nothing flagged": integer atomics only, one per warp and term that saw something, the same bits on every run.
+struct DbgReport { unsigned long long count[3], inv_key[3]; };   // y_pred, t1, t2
+static_assert(sizeof(DbgReport) == kDebugReportBytes, "dca_debug_report's device form");
+
+__global__ void __launch_bounds__(256)
+debug_check_kernel(const float* __restrict__ Y, int64_t ldy, const int32_t* __restrict__ rows, const float* __restrict__ sf,
+                   const float* __restrict__ m, int64_t ldm, const float* __restrict__ theta, int64_t ld_theta, int B, int G,
+                   DbgReport* __restrict__ rep) {
+  constexpr float eps = 1e-10f;
+  unsigned cnt[3] = {0u, 0u, 0u};
+  unsigned long long inv_key[3] = {0ull, 0ull, 0ull};
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < G) {
+    for (int r = blockIdx.y; r < B; r += gridDim.y) {
+      const int64_t yr = rows ? (int64_t)rows[r] : (int64_t)r;
+      const float y = Y[yr * ldy + g];
+      const float s = sf ? sf[yr] : 1.0f;
+      const float mv = m[(int64_t)r * ldm + g];
+      const float tv = theta[(int64_t)r * ld_theta + g];
+      const float th = tv > 1e6f ? 1e6f : tv;
+      const float yp = mv * s;
+      const float te = th + eps;
+      const float t1 = lgammaf(te) + lgammaf(y + 1.0f) - lgammaf(y + th + eps);
+      const float t2 = (th + y) * logf(1.0f + yp / te) + y * (logf(te) - logf(yp + eps));
+      const bool bad[3] = {!isfinite(yp), !isfinite(t1), !isfinite(t2)};
+      const unsigned long long inv = ~(((unsigned long long)(unsigned)r << 32) | (unsigned)g);
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        if (bad[k]) { ++cnt[k]; inv_key[k] = inv > inv_key[k] ? inv : inv_key[k]; }
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {                       // warp sum / max, one set of atomics per warp that saw something
+    unsigned c = cnt[k];
+    unsigned long long v = inv_key[k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      c += __shfl_xor_sync(0xffffffffu, c, o);
+      const unsigned long long w = __shfl_xor_sync(0xffffffffu, v, o);
+      v = w > v ? w : v;
+    }
+    if ((threadIdx.x & 31) == 0 && c) { atomicAdd(&rep->count[k], (unsigned long long)c); atomicMax(&rep->inv_key[k], v); }
+  }
+}
+
 __global__ void fold_partials_kernel(const double* __restrict__ part, int n, double* out, int accumulate,
                                      const double* penalty, float inv_n, int batch, float* loss_slot, double* epoch_acc) {
   __shared__ double sm[32];
@@ -834,6 +887,28 @@ size_t loss_workspace_bytes(int B, int G) {
 int zinb_loss_fwd_bwd(const LossArgs& a, cudaStream_t s) { return launch<true>(a, s); }
 int zinb_loss_fwd(const LossArgs& a, cudaStream_t s) { return launch<false>(a, s); }
 
+int debug_check(const DebugCheckArgs& a, cudaStream_t s) {
+  if (a.B <= 0 || a.G <= 0 || !a.Y || !a.m || !a.theta || !a.report || a.ld_theta < 0) {
+    set_error("debug_check: bad argument"); return DCA_ERR_BAD_ARG;
+  }
+  // 256 genes per block; the rows strided over enough blocks to give every SM about eight
+  const int gx = cdiv(a.G, 256);
+  const int gy = std::max(1, std::min(a.B, std::min(65535, 8 * sm_count_cached() / gx + 1)));
+  debug_check_kernel<<<dim3(gx, gy), 256, 0, s>>>(a.Y, a.ldy, a.rows, a.sf, a.m, a.ldm, a.theta, a.ld_theta, a.B, a.G,
+                                                  reinterpret_cast<DbgReport*>(a.report));
+  DCA_LAUNCH_CHECK();
+  return DCA_OK;
+}
+
+void debug_report_decode(const unsigned long long raw[6], int64_t count[3], int32_t first_row[3], int32_t first_gene[3]) {
+  for (int k = 0; k < 3; ++k) {
+    count[k] = (int64_t)raw[k];
+    const unsigned long long key = ~raw[3 + k];                      // raw 0: nothing flagged
+    first_row[k] = raw[3 + k] ? (int32_t)(key >> 32) : -1;
+    first_gene[k] = raw[3 + k] ? (int32_t)(key & 0xffffffffu) : -1;
+  }
+}
+
 int heads_loss_tc(const HeadsLossArgs& a, cudaStream_t s) {
   using namespace hl;
   const int B = a.B, G = a.G;
@@ -929,6 +1004,24 @@ extern "C" int dca_zinb_loss_fwd(const float* Y, int64_t ldy, const int32_t* row
   LossArgs a{Y, ldy, rows, sf, m, d, pi, ld, batch, genes, ae_type, ridge, 1.0f, nullptr, nullptr, nullptr,
              0, nullptr, loss_sum, workspace, workspace_bytes};
   return zinb_loss_fwd(a, (cudaStream_t)stream);
+}
+
+extern "C" int dca_debug_check(const float* Y, int64_t ldy, const int32_t* rows, const float* sf, const float* m, int64_t ldm,
+                               const float* theta, int64_t ld_theta, int32_t batch, int32_t genes, void* workspace,
+                               dca_debug_report* out, void* stream) {
+  if (!out || out->struct_bytes != (int32_t)sizeof(dca_debug_report)) {
+    set_error("dca_debug_check: NULL or unversioned dca_debug_report (struct_bytes must be %d)", (int)sizeof(dca_debug_report));
+    return DCA_ERR_BAD_ARG;
+  }
+  if (!workspace) { set_error("dca_debug_check: NULL workspace"); return DCA_ERR_BAD_ARG; }
+  cudaStream_t s = (cudaStream_t)stream;
+  DCA_CUDA_OK(cudaMemsetAsync(workspace, 0, kDebugReportBytes, s));
+  DCA_TRY(debug_check(DebugCheckArgs{Y, ldy, rows, sf, m, ldm, theta, ld_theta, batch, genes, workspace}, s));
+  unsigned long long raw[6];
+  DCA_CUDA_OK(cudaMemcpyAsync(raw, workspace, sizeof(raw), cudaMemcpyDeviceToHost, s));
+  DCA_CUDA_OK(cudaStreamSynchronize(s));
+  debug_report_decode(raw, out->count, out->first_row, out->first_gene);
+  return DCA_OK;
 }
 
 // Host mirror of the per-element device math (same source, compiled for the CPU) so the

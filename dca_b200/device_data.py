@@ -122,9 +122,10 @@ def _one_dataset(device_data=None, stream_data=None, packed_data=None, stream=Fa
 def _resident_fit(eng, n_tr, n, batch, shuffle, step, evaluate, rows_map=None):
     """(epoch, validate) over n cells of which the first n_tr train: every epoch reshuffles the training rows with the
     global NumPy RNG as Keras does (np.random.shuffle of the index array) and runs step(rows) on each batch, rows an
-    int32 device tensor of storage rows (positions mapped through rows_map when given); validate runs evaluate(s, e)
-    over the held-out positions [n_tr, n) in batches."""
-    def epoch(update):
+    int32 device tensor of storage rows (positions mapped through rows_map when given), then update(); validate runs
+    evaluate(s, e) over the held-out positions [n_tr, n) in batches.  check(positions of the batch's cells), when given,
+    runs after every step, before its update."""
+    def epoch(update, check=None):
         order = np.arange(n_tr)
         if shuffle:
             np.random.shuffle(order)
@@ -133,11 +134,16 @@ def _resident_fit(eng, n_tr, n, batch, shuffle, step, evaluate, rows_map=None):
             order_d = rows_map[order_d.long()]
         for s in range(0, n_tr, batch):
             step(order_d[s:s + batch])
+            if check:
+                check(order[s:s + batch])
             update()
 
-    def validate():
+    def validate(check=None):
         for s in range(n_tr, n, batch):             # inference-mode BN over the held-out tail
-            evaluate(s, min(s + batch, n))
+            e = min(s + batch, n)
+            evaluate(s, e)
+            if check:
+                check(np.arange(s, e))
     return epoch, validate
 
 
@@ -147,7 +153,8 @@ class _Dataset:
       ``kind``: the keyword of train / predict / write_predictions that takes it and the suffix of its adata.uns key;
       ``_bind(eng)``: its checks against the engine and, where the kind needs it, the exact input transform;
       ``_fit(eng, n_tr, batch, shuffle)`` -> (epoch, validate): epoch(update) runs one epoch's training steps over the
-      first n_tr cells, calling update() after each, and validate() the validation pass over the others;
+      first n_tr cells, calling update() after each, and validate() the validation pass over the others; with a
+      second argument check, both call check(positions of the batch's cells) after every step, before its update;
       ``_predictor(eng, bs)`` -> (run, theta, session): run(i, s, e, buffers) is the inference of batch i, cells
       [s, e), into the device buffers {"mean", "disp", "pi", "latent"} (any subset); theta(th) writes the per-gene
       dispersion of the const-disp types; a pass of run over the batches, and theta, go inside ``with session():``."""

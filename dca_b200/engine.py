@@ -77,6 +77,7 @@ class DeviceEngine:
         cfg.bn_momentum, cfg.bn_eps = KERAS_DEFAULTS["bn_momentum"], KERAS_DEFAULTS["bn_eps"]
         cfg.rms_rho, cfg.rms_eps = KERAS_DEFAULTS["rms_rho"], KERAS_DEFAULTS["rms_eps"]
         self.cfg = cfg
+        self.debug_checks = False
         nbytes = C.c_size_t()
         check(self.lib.dca_arena_bytes(C.byref(cfg), C.byref(nbytes)), "dca_arena_bytes")
         with torch.cuda.device(self.device):
@@ -306,6 +307,21 @@ class DeviceEngine:
         acc = (C.c_double * 4)()
         check(self.lib.dca_read_epoch_acc(self.handle, C.byref(acc), int(reset), self._stream()), "dca_read_epoch_acc")
         return list(acc)
+
+    def set_debug_checks(self, on: bool):
+        """The reference's debug checks (dca/loss.py:87-100) inside the loss kernels of every later training and
+        validation step (dca_set_debug_checks); read each step's report with read_debug_report."""
+        check(self.lib.dca_set_debug_checks(self.handle, int(bool(on))), "dca_set_debug_checks")
+        self.debug_checks = bool(on)
+
+    def read_debug_report(self):
+        """The debug report of the last step (waits for it): {"count": [y_pred, t1, t2] non-finite elements,
+        "first": per term (batch row, gene) of its first non-finite element in row-major order, or None}."""
+        r = _lib.DebugReport()
+        r.struct_bytes = C.sizeof(_lib.DebugReport)
+        check(self.lib.dca_read_debug_report(self.handle, C.byref(r), self._stream()), "dca_read_debug_report")
+        return {"count": [int(c) for c in r.count],
+                "first": [None if r.first_row[k] < 0 else (int(r.first_row[k]), int(r.first_gene[k])) for k in range(3)]}
 
     def train_step_host(self, x_host: torch.Tensor, y_host: torch.Tensor, sf_host: Optional[torch.Tensor],
                         lr: float, clip: float = 5.0) -> float:

@@ -76,7 +76,7 @@ class Autoencoder:
         self.activation = activation
         self.init = init
         self.file_path = file_path
-        self.debug = debug
+        self.debug = debug                 # train(): the loss kernels' inf/NaN checks of dca/loss.py:87-100 (train._DebugChecks)
         self.x_dtype = x_dtype
         self.gemm_path = gemm_path
         self.sharedpi = sharedpi           # ZINBAutoencoderElemPi only (dca/network.py:425-427)

@@ -184,18 +184,24 @@ def _pad_stats(v, width, fill):
     return out
 
 
-def stream_epoch(eng, n, batch, shuffle, begin):
+def stream_epoch(eng, n, batch, shuffle, begin, positions):
     """epoch(update) over the n rows of a host stream that begin() starts, in batches of ``batch`` rows: the batches
-    in a new random order every epoch (global NumPy RNG; in order with shuffle=False), update() after each step."""
+    in a new random order every epoch (global NumPy RNG; in order with shuffle=False), update() after each step and
+    before it check(positions of the batch's cells) when given -- ``positions``: each streamed row's, in stream order."""
     nb = (n + batch - 1) // batch
 
-    def epoch(update):
+    def epoch(update, check=None):
         border = np.random.permutation(nb) if shuffle else np.arange(nb)
         begin()
-        for k in range(nb):
-            eng.stream_step(int(border[k]), int(border[k + 1]) if k + 1 < nb else -1)
-            update()
-        eng.stream_end()
+        try:                                       # a failing check leaves no stream open
+            for k in range(nb):
+                b = int(border[k])
+                eng.stream_step(b, int(border[k + 1]) if k + 1 < nb else -1)
+                if check:
+                    check(positions[b * batch: (b + 1) * batch])
+                update()
+        finally:
+            eng.stream_end()
     return epoch
 
 
@@ -331,14 +337,18 @@ class StreamedDataset(_Dataset):
         va = self.rows(n_tr, self.n) if n_tr < self.n else None
         nb_va = (self.n - n_tr + batch - 1) // batch
 
-        def validate():
+        def validate(check=None):
             if va is None:
                 return
             va.stream_batches(eng, batch)
-            for k in range(nb_va):
-                eng.stream_eval(k, k + 1 if k + 1 < nb_va else -1)
-            eng.stream_end()
-        return stream_epoch(eng, n_tr, batch, shuffle, lambda: tr.stream_batches(eng, batch)), validate
+            try:
+                for k in range(nb_va):
+                    eng.stream_eval(k, k + 1 if k + 1 < nb_va else -1)
+                    if check:
+                        check(np.arange(n_tr + k * batch, min(n_tr + (k + 1) * batch, self.n)))
+            finally:
+                eng.stream_end()
+        return stream_epoch(eng, n_tr, batch, shuffle, lambda: tr.stream_batches(eng, batch), order0), validate
 
     def _predictor(self, eng, bs):
         nb = (self.n + bs - 1) // bs

@@ -111,6 +111,7 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
     fit = dict(optimizer=optimizer, learning_rate=learning_rate, epochs=epochs, reduce_lr=reduce_lr,
                early_stop=early_stop, clip_grad=clip_grad, verbose=verbose, save_weights=save_weights,
                output_dir=output_dir)
+    fit["names"] = _cell_gene_names(adata, output_subset)
     data = _one_dataset(device_data, stream_data, packed_data, stream)
     if data is not None:
         _check_target(data, adata, output_subset, use_raw_as_output)
@@ -156,6 +157,14 @@ def train(adata, network, output_dir=None, optimizer='RMSprop', learning_rate=No
     return _fit(eng, network, epoch, validate, va[1] - va[0], gscale=1.0 / world, world=world, rank=rank, **fit)
 
 
+def _cell_gene_names(adata, output_subset):
+    """(cell names, output gene names) of an AnnData for the debug checks' messages; None where unknown."""
+    if adata is None:
+        return None, None
+    genes = list(output_subset) if output_subset else getattr(adata, "var_names", None)
+    return getattr(adata, "obs_names", None), genes
+
+
 def _split(n, validation_split):
     """Training rows of n: the tail ``validation_split`` validates (taken before shuffling, as Keras does)."""
     return int(n * (1. - validation_split)) if validation_split and 0. < validation_split < 1. else n
@@ -197,9 +206,13 @@ def _host_resident(eng, X, Yh, sf, tr, va, batch_size, shuffle, world):
     sfd = _to_device(np.concatenate([sf[tr_lo:tr_hi], sf[va_lo:va_hi]]), torch.float32, dev)
     n_tr = tr_hi - tr_lo
     step = eng.train_step_allreduce if world > 1 else eng.train_step     # NCCL all-reduce overlapped with the backward
-    return _resident_fit(eng, n_tr, n_tr + va_hi - va_lo, batch_size, shuffle,
-                         lambda rows: step(Xd, Yd, sfd, rows=rows),
-                         lambda s, e: eng.eval_step(Xd[s:e], Yd[s:e], sfd[s:e]))
+    epoch, validate = _resident_fit(eng, n_tr, n_tr + va_hi - va_lo, batch_size, shuffle,
+                                    lambda rows: step(Xd, Yd, sfd, rows=rows),
+                                    lambda s, e: eng.eval_step(Xd[s:e], Yd[s:e], sfd[s:e]))
+
+    def cells(check):                             # positions in the copied rows -> rows of adata
+        return check and (lambda p: check(np.where(p < n_tr, tr_lo + p, va_lo + p - n_tr)))
+    return (lambda update, check=None: epoch(update, cells(check))), (lambda check=None: validate(cells(check)))
 
 
 def _host_stream(eng, X, Yh, sf, tr, va, batch_size, shuffle, world):
@@ -240,29 +253,34 @@ def _host_stream(eng, X, Yh, sf, tr, va, batch_size, shuffle, world):
     Xv = _to_device(X[va_lo:va_hi], eng.x_dtype, dev) if n_va else None
     Yv = _to_device(Yh[va_lo:va_hi], torch.float32, dev) if n_va else None
     sfv = _to_device(sf[va_lo:va_hi], torch.float32, dev) if n_va else None
-    steps = stream_epoch(eng, n_tr, batch_size, shuffle, lambda: eng.stream_begin(packed, sf_h, batch_size))
+    steps = stream_epoch(eng, n_tr, batch_size, shuffle, lambda: eng.stream_begin(packed, sf_h, batch_size), order0)
 
-    def epoch(update):
+    def epoch(update, check=None):
         if world == 1:
-            return steps(update)
+            return steps(update, check)
 
         def reduced():                            # the gradients summed over the ranks before every update
             eng.allreduce_grads() if getattr(eng, "_comm", False) else D.all_reduce_sum_(eng.grads)
             update()
-        steps(reduced)
+        steps(reduced, check)
 
-    def validate():
+    def validate(check=None):
         for s0 in range(0, n_va, batch_size):
             e = min(s0 + batch_size, n_va)
             eng.eval_step(Xv[s0:e], Yv[s0:e], sfv[s0:e])
+            if check:
+                check(np.arange(va_lo + s0, va_lo + e))
     return epoch, validate
 
 
 def _fit(eng, network, epoch, validate, n_va, optimizer, learning_rate, epochs, reduce_lr, early_stop, clip_grad, verbose,
-         save_weights, output_dir, gscale=1.0, world=1, rank=0):
+         save_weights, output_dir, names=(None, None), gscale=1.0, world=1, rank=0):
     """The fit loop of every input: optimizer, ReduceLROnPlateau / EarlyStopping, history and ModelCheckpoint around
     epoch(update) -- one epoch's training steps, update() after each -- and validate(), the pass over the n_va
-    validation rows."""
+    validation rows.  With network.debug, both also get a check of every step's debug report (_DebugChecks)."""
+    debug = bool(getattr(network, "debug", False))
+    if debug or getattr(eng, "debug_checks", False) is True:       # a run without --debug touches no engine state
+        eng.set_debug_checks(debug)
     # opt.__dict__[optimizer](clipvalue=clip_grad[, lr=learning_rate])                   (dca/train.py:54-57)
     default_lr = eng.set_optimizer(optimizer)
     eng.reset_optimizer()
@@ -279,8 +297,15 @@ def _fit(eng, network, epoch, validate, n_va, optimizer, learning_rate, epochs, 
     try:
         for e in range(epochs):
             eng.read_epoch_acc(reset=True)
-            epoch(lambda: eng.apply_update(ctl.lr, clip_grad, gscale))
-            validate()
+            update = lambda: eng.apply_update(ctl.lr, clip_grad, gscale)     # noqa: E731
+            if debug:
+                dbg = _DebugChecks(eng, e + 1, names, world, dev)
+                epoch(update, dbg.training)
+                validate(dbg.validation)
+                dbg.end_validation()
+            else:
+                epoch(update)
+                validate()
             stop, best_val = _epoch_end(eng, network, hist, ctl, e, epochs, n_va, world, rank, dev, verbose, save_weights,
                                         output_dir, best_val)
             if stop:
@@ -291,6 +316,79 @@ def _fit(eng, network, epoch, validate, n_va, optimizer, learning_rate, epochs, 
     if not hist.history["val_loss"]:
         del hist.history["val_loss"]
     return hist
+
+
+DEBUG_TERMS = ("y_pred", "t1", "t2")
+
+
+def debug_message(report, epoch, phase, batch, positions, obs_names=None, gene_names=None):
+    """The FloatingPointError message of a failing debug report: the reference's message for the first failing term,
+    in the order y_pred, t1, t2 (dca/loss.py:87-100), then where -- epoch (from 1), 'training' or 'validation', the
+    batch index (from 0), the cell (its position in the dataset, positions[batch row], and its name) and the gene of
+    that term's first non-finite element -- and the three counts.  report: engine.read_debug_report()'s dict, with
+    counts summed over the ranks; its "first" entry is None when the element lies in another rank's share."""
+    counts = [int(c) for c in report["count"]]
+    k = next(i for i in range(3) if counts[i] > 0)
+
+    def named(names, i):
+        return "" if names is None or i >= len(names) else " (%s)" % names[i]
+    msg = "%s has inf/nans: epoch %d, %s batch %d" % (DEBUG_TERMS[k], epoch, phase, batch)
+    first = report["first"][k]
+    if first is None:
+        msg += ", in another rank's share of the batch"
+    else:
+        row, gene = first
+        cell = int(positions[row])
+        msg += ", cell %d%s, gene %d%s" % (cell, named(obs_names, cell), gene, named(gene_names, gene))
+    return msg + "; non-finite elements: y_pred %d, t1 %d, t2 %d" % tuple(counts)
+
+
+class _DebugChecks:
+    """--debug in the fit loop of one epoch: the report of every training step is read before its update, so a
+    failing batch's update is never applied (the network keeps the weights from before it, as the reference's abort
+    leaves them, and the BatchNorm moving statistics that batch's forward pass moved are put back); the report of every
+    validation batch after it.  With world > 1 the training counts are summed over
+    the ranks every step, so every rank raises at the same step; the validation counts once after the pass (the ranks'
+    validation shares need not have the same number of batches)."""
+
+    def __init__(self, eng, epoch, names, world, dev):
+        self.eng, self.epoch, self.world, self.dev = eng, epoch, world, dev
+        self.obs_names, self.gene_names = names
+        self.n_train = self.n_val = 0
+        self.val_failure = None
+        self.bn = eng.bn_state.clone() if eng.bn_state.numel() else None      # as after the last clean step
+
+    def _summed(self, counts):
+        return [int(c) for c in D.all_reduce_sum_host(np.asarray(counts, dtype=np.float64), self.dev)]
+
+    def training(self, positions):
+        r = self.eng.read_debug_report()
+        if self.world > 1:
+            r["count"] = self._summed(r["count"])
+        batch, self.n_train = self.n_train, self.n_train + 1
+        if any(r["count"]):
+            if self.bn is not None:
+                self.eng.bn_state.copy_(self.bn)
+            raise FloatingPointError(debug_message(r, self.epoch, "training", batch, positions, self.obs_names,
+                                                   self.gene_names))
+        if self.bn is not None:
+            self.bn.copy_(self.eng.bn_state)
+
+    def validation(self, positions):
+        r = self.eng.read_debug_report()
+        batch, self.n_val = self.n_val, self.n_val + 1
+        if any(r["count"]) and self.val_failure is None:
+            self.val_failure = debug_message(r, self.epoch, "validation", batch, positions, self.obs_names,
+                                             self.gene_names)
+            if self.world == 1:
+                raise FloatingPointError(self.val_failure)
+
+    def end_validation(self):
+        failed = self.val_failure is not None
+        if self.world > 1:
+            failed = self._summed([int(failed)])[0] > 0
+        if failed:
+            raise FloatingPointError(self.val_failure or "validation has inf/nans on another rank: epoch %d" % self.epoch)
 
 
 def _epoch_end(eng, network, hist, ctl, epoch, epochs, n_va, world, rank, dev, verbose, save_weights, output_dir, best_val):

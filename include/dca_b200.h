@@ -223,6 +223,35 @@ int dca_predict(dca_handle* h, const void* X, int64_t ldx, const float* sf, cons
 int dca_read_loss(dca_handle* h, float* loss_host, int32_t* nonfinite_host, void* stream);
 int dca_read_epoch_acc(dca_handle* h, double acc_host[4], int32_t reset, void* stream);
 
+/* Debug checks (--debug, dca/loss.py:87-100): with `on`, every training step (dca_train_step*, the streamed and packed
+ * steps) and every dca_eval_step* evaluates the reference's NB terms of every element of the batch, in float32 and in
+ * the reference's form -- theta' = min(theta, 1e6), eps = 1e-10, y_pred = mean * sf,
+ * t1 = lgamma(theta' + eps) + lgamma(y + 1) - lgamma(y + theta' + eps),
+ * t2 = (theta' + y) log(1 + y_pred / (theta' + eps)) + y (log(theta' + eps) - log(y_pred + eps)) -- and records which
+ * are not finite in a report the step clears first.  Types whose reference loss has no such check (nb, poisson,
+ * normal) always report nothing.  The checks are a kernel of their own, launched ahead of the loss kernel on the
+ * operands it reads (on the tensor-core heads + loss path, the head-forward kernel first writes the head outputs for
+ * them), so the loss, the gradients and every accumulator have the same bits with the checks on.  Toggling drops the
+ * captured step graphs; the fused flash_zinb path is not taken while the checks are on.  Off (the default), every
+ * kernel, launch and graph is the one without checks. */
+int dca_set_debug_checks(dca_handle* h, int32_t on);
+typedef struct dca_debug_report {
+  int32_t struct_bytes;      /* sizeof(dca_debug_report), set by the caller: ABI guard */
+  int32_t reserved;
+  int64_t count[3];          /* non-finite y_pred, t1, t2 elements of the last step */
+  int32_t first_row[3];      /* per term: batch row of its first non-finite element in row-major order, -1 if none */
+  int32_t first_gene[3];     /* ... and its gene (output column), -1 if none */
+} dca_debug_report;
+/* Blocking: copies the report of the last step on `stream` to *out.  The same report on every run of the same step. */
+int dca_read_debug_report(dca_handle* h, dca_debug_report* out, void* stream);
+/* The checks of one batch on their own (the kernel the steps run ahead of their loss kernel): counts Y (device, row
+ * rows[r] for batch row r, rows NULL: r; leading dim ldy), size factors sf (indexed like Y's rows; NULL: 1), mean m
+ * (before the size factor, [batch x genes], leading dim ldm), dispersion theta (leading dim ld_theta; 0: one theta per
+ * gene).  workspace: 48 bytes of device memory.  Blocking; writes *out (struct_bytes set by the caller). */
+int dca_debug_check(const float* Y, int64_t ldy, const int32_t* rows, const float* sf, const float* m, int64_t ldm,
+                    const float* theta, int64_t ld_theta, int32_t batch, int32_t genes, void* workspace,
+                    dca_debug_report* out, void* stream);
+
 /* Mirror every step's loss into pinned (mapped) HOST memory without a copy in the stream: the k-th
  * dca_apply_update after this call stores grads[P] * grad_scale (the batch loss, averaged over ranks once the
  * gradient buffer was all-reduced) into host_ring[k % n_slots] from inside the update kernel.  The host reads a
