@@ -29,6 +29,40 @@ GEMM_AUTO, GEMM_GENERIC, GEMM_TCGEN05 = 0, 1, 2
 REGION_PARAMS, REGION_GRADS, REGION_RMS, REGION_BN_STATE, REGION_EPOCH_ACC = 0, 1, 2, 3, 4
 
 
+INIT_VARIANCE_SCALING, INIT_RANDOM_NORMAL, INIT_RANDOM_UNIFORM, INIT_TRUNCATED_NORMAL = 0, 1, 2, 3
+INIT_CONSTANT, INIT_ORTHOGONAL, INIT_IDENTITY = 4, 5, 6
+FAN_MODES = {"fan_in": 0, "fan_out": 1, "fan_avg": 2}
+DISTRIBUTIONS = {"truncated_normal": 0, "untruncated_normal": 1, "uniform": 2}
+
+
+def _vs(scale, mode, distribution):
+    return dict(kind=INIT_VARIANCE_SCALING, scale=scale, mode=FAN_MODES[mode], distribution=DISTRIBUTIONS[distribution])
+
+
+# Keras 2 / tf.keras 2.x `kernel_initializer` names (the CLI's --init, dca/network.py:124-126) with their default
+# arguments: the snake_case names and the class names
+_INITS = {
+    "glorot_uniform": _vs(1.0, "fan_avg", "uniform"), "glorot_normal": _vs(1.0, "fan_avg", "truncated_normal"),
+    "he_uniform": _vs(2.0, "fan_in", "uniform"), "he_normal": _vs(2.0, "fan_in", "truncated_normal"),
+    "lecun_uniform": _vs(1.0, "fan_in", "uniform"), "lecun_normal": _vs(1.0, "fan_in", "truncated_normal"),
+    "variance_scaling": _vs(1.0, "fan_in", "truncated_normal"),
+    "random_normal": dict(kind=INIT_RANDOM_NORMAL, stddev=0.05),
+    "random_uniform": dict(kind=INIT_RANDOM_UNIFORM, minval=-0.05, maxval=0.05),
+    "truncated_normal": dict(kind=INIT_TRUNCATED_NORMAL, stddev=0.05),
+    "zeros": dict(kind=INIT_CONSTANT, value=0.0), "ones": dict(kind=INIT_CONSTANT, value=1.0),
+    "constant": dict(kind=INIT_CONSTANT, value=0.0),
+    "orthogonal": dict(kind=INIT_ORTHOGONAL, gain=1.0), "identity": dict(kind=INIT_IDENTITY, gain=1.0),
+}
+_INIT_ALIASES = {
+    "GlorotUniform": "glorot_uniform", "GlorotNormal": "glorot_normal", "HeUniform": "he_uniform", "HeNormal": "he_normal",
+    "LecunUniform": "lecun_uniform", "LecunNormal": "lecun_normal", "VarianceScaling": "variance_scaling",
+    "normal": "random_normal", "RandomNormal": "random_normal", "uniform": "random_uniform",
+    "RandomUniform": "random_uniform", "TruncatedNormal": "truncated_normal", "zero": "zeros", "Zeros": "zeros",
+    "one": "ones", "Ones": "ones", "Constant": "constant", "Orthogonal": "orthogonal", "Identity": "identity",
+}
+INITIALIZERS = dict(_INITS, **{k: _INITS[v] for k, v in _INIT_ALIASES.items()})
+
+
 class DcaError(RuntimeError):
     pass
 
@@ -63,6 +97,20 @@ class PackedCountsDesc(C.Structure):
     ]
 
 
+class Initializer(C.Structure):
+    """dca_initializer: a kernel initializer (include/dca_b200.h)."""
+    _fields_ = [("struct_bytes", C.c_int32), ("kind", C.c_int32), ("scale", C.c_float), ("mode", C.c_int32),
+                ("distribution", C.c_int32), ("stddev", C.c_float), ("minval", C.c_float), ("maxval", C.c_float),
+                ("value", C.c_float), ("gain", C.c_float)]
+
+
+def initializer(name: str) -> Initializer:
+    """The dca_initializer of a Keras initializer name; ValueError for a name Keras would not resolve here."""
+    if not isinstance(name, str) or name not in INITIALIZERS:
+        raise ValueError("unknown initializer %r (accepted: %s)" % (name, ", ".join(sorted(INITIALIZERS))))
+    return Initializer(struct_bytes=C.sizeof(Initializer), **INITIALIZERS[name])
+
+
 class DebugReport(C.Structure):
     """dca_debug_report: the debug checks' report of the last step (include/dca_b200.h)."""
     _fields_ = [("struct_bytes", C.c_int32), ("reserved", C.c_int32), ("count", C.c_int64 * 3),
@@ -84,6 +132,8 @@ PROTOTYPES = {
     "dca_state_info": (C.c_int, [_vp, _i32, C.POINTER(TensorInfo)]),
     "dca_region": (C.c_int, [_vp, _i32, C.POINTER(_vp), C.POINTER(_i64)]),
     "dca_init_params": (C.c_int, [_vp, C.c_uint64, _vp]),
+    "dca_init_params_ex": (C.c_int, [_vp, C.c_uint64, C.POINTER(Initializer), _vp]),
+    "dca_init_fill_host": (C.c_int, [C.POINTER(Initializer), C.c_uint64, C.c_uint64, _i32, _i32, _i32, _vp]),
     "dca_params_changed": (C.c_int, [_vp, _vp]),
     "dca_train_step": (C.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _i32, _vp]),
     "dca_train_step_phase": (C.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _vp, _i32, _i32, _vp]),

@@ -95,7 +95,14 @@ int rmsprop_update(float* params, const float* grads, float* rms, int64_t n, flo
 struct OptScalars { int kind; float lr, clip, gs, c0, c1, c2, c3, c4; };
 int optimizer_update(float* params, const float* grads, float* s1, float* s2, int64_t n, OptScalars o, __nv_bfloat16* shadow,
                      float* loss_out, cudaStream_t s);
-int glorot_fill(float* w, int64_t n, int fan_in, int fan_out, uint64_t seed, uint64_t stream_id, cudaStream_t s);
+// weight initialisers (dca_initializer): one kernel tensor of a model; sid keys its draws (seed, sid, element);
+// fan_out = cols, fan_in as the model defines it (Keras: ndim 1 -> cols, ndim 2 -> rows)
+struct InitTensor { float* w; int ndim, rows, cols, fan_in; uint64_t sid; const char* name; };
+int check_initializer(const dca_initializer* ini);   // non-NULL, struct_bytes
+// DCA_OK, or DCA_ERR_BAD_ARG with the message set when the spec is invalid or one of the tensors does not allow it
+int check_init_tensors(const dca_initializer& ini, const InitTensor* t, int n);
+// fills the n tensors (checked first, so a spec a tensor does not allow writes nothing)
+int init_kernels(const dca_initializer& ini, const InitTensor* t, int n, uint64_t seed, cudaStream_t s);
 int fill_value(float* p, int64_t n, float v, cudaStream_t s);
 int cast_to_bf16(const float* in, __nv_bfloat16* out, int64_t n, cudaStream_t s);
 

@@ -767,20 +767,36 @@ int Engine::refresh_shadows(cudaStream_t s) {
   return cast_to_bf16(pp(0), bf(o_pbf), P, s);
 }
 
-int Engine::init_params(uint64_t seed, cudaStream_t s) {
-  DCA_CUDA_OK(cudaMemsetAsync(pp(0), 0, sizeof(float) * (size_t)P, s));
-  DCA_TRY(reset_optimizer(s));
-  DCA_CUDA_OK(cudaMemsetAsync(gp(0), 0, sizeof(float) * (size_t)(P + 2), s));
-  DCA_CUDA_OK(cudaMemsetAsync(d(o_acc), 0, sizeof(double) * 8, s));
-  uint64_t sid = 0;
+int Engine::init_params(uint64_t seed, const dca_initializer& ini, cudaStream_t s) {
+  // the kernels and their stream ids (include/dca_b200.h): the tensor table in order for the other types (zinb-elempi's
+  // element-wise "pi/kernel" is 1-D), hidden layers 0.. and heads 100 + k for the flagship types
+  std::vector<InitTensor> ks;
+  auto name_at = [&](int64_t off) {
+    for (auto& t : params)
+      if (t.offset == off) return (const char*)t.name;
+    return "";
+  };
   if (x_kind) {
-    // Glorot-uniform for every kernel of the tensor table (1-D element-wise kernels: fan_in = fan_out = length, like Keras)
+    uint64_t sid = 0;
     for (auto& t : params) {
       const std::string nm(t.name);
       if (nm.size() < 7 || nm.compare(nm.size() - 7, 7, "/kernel") != 0) continue;
-      const int fi = t.rows == 1 ? t.cols : t.rows, fo = t.cols;
-      DCA_TRY(glorot_fill(pp(t.offset), (int64_t)t.rows * t.cols, fi, fo, seed, sid++, s));
+      // fan_in = cols for every one-row kernel, as glorot_uniform has always drawn these types (Keras: the length
+      // for zinb-elempi's 1-D pi/kernel, but 1 for a 2-D kernel of one input row, e.g. a hidden width of 1)
+      ks.push_back(InitTensor{pp(t.offset), t.offset == epi_k ? 1 : 2, t.rows, t.cols, t.rows == 1 ? t.cols : t.rows, sid++, t.name});
     }
+  } else {
+    for (int i = 0; i < L; ++i) ks.push_back(InitTensor{pp(lay[i].W), 2, lay[i].in, lay[i].out, lay[i].in, (uint64_t)i, name_at(lay[i].W)});
+    for (int k = 0; k < 3; ++k)
+      if (head_W[k] >= 0) ks.push_back(InitTensor{pp(head_W[k]), 2, K_head, cfg.n_out, K_head, (uint64_t)(100 + k), name_at(head_W[k])});
+  }
+  DCA_TRY(check_init_tensors(ini, ks.data(), (int)ks.size()));     // a spec a kernel does not allow changes nothing
+  DCA_CUDA_OK(cudaMemsetAsync(pp(0), 0, sizeof(float) * (size_t)P, s));
+  DCA_TRY(init_kernels(ini, ks.data(), (int)ks.size(), seed, s));
+  DCA_TRY(reset_optimizer(s));
+  DCA_CUDA_OK(cudaMemsetAsync(gp(0), 0, sizeof(float) * (size_t)(P + 2), s));
+  DCA_CUDA_OK(cudaMemsetAsync(d(o_acc), 0, sizeof(double) * 8, s));
+  if (x_kind) {
     if (cfg.batchnorm)
       for (auto& t : states) {
         const std::string nm(t.name);
@@ -788,10 +804,6 @@ int Engine::init_params(uint64_t seed, cudaStream_t s) {
       }
     return DCA_OK;
   }
-  for (int i = 0; i < L; ++i)
-    DCA_TRY(glorot_fill(pp(lay[i].W), (int64_t)lay[i].in * lay[i].out, lay[i].in, lay[i].out, seed, sid++, s));
-  for (int k = 0; k < 3; ++k)
-    if (head_W[k] >= 0) DCA_TRY(glorot_fill(pp(head_W[k]), (int64_t)K_head * cfg.n_out, K_head, cfg.n_out, seed, 100 + k, s));
   if (cfg.batchnorm)
     for (int i = 0; i < L; ++i) {
       DCA_TRY(fill_value(st(lay[i].mm), lay[i].out, 0.f, s));
@@ -921,8 +933,17 @@ extern "C" int dca_region(dca_handle* h, int32_t id, void** ptr, int64_t* count)
 }
 
 extern "C" int dca_init_params(dca_handle* h, uint64_t seed, void* stream) {
+  dca_initializer glorot_uniform;
+  memset(&glorot_uniform, 0, sizeof(glorot_uniform));
+  glorot_uniform.struct_bytes = (int32_t)sizeof(dca_initializer);
+  glorot_uniform.kind = DCA_INIT_VARIANCE_SCALING;
+  glorot_uniform.scale = 1.f; glorot_uniform.mode = DCA_FAN_AVG; glorot_uniform.distribution = DCA_DIST_UNIFORM;
+  return dca_init_params_ex(h, seed, &glorot_uniform, stream);
+}
+extern "C" int dca_init_params_ex(dca_handle* h, uint64_t seed, const dca_initializer* init, void* stream) {
   DCA_NEED_HANDLE(h);
-  DCA_TRY(h->e.init_params(seed, (cudaStream_t)stream));
+  DCA_TRY(check_initializer(init));
+  DCA_TRY(h->e.init_params(seed, *init, (cudaStream_t)stream));
   return h->e.refresh_shadows((cudaStream_t)stream);
 }
 extern "C" int dca_params_changed(dca_handle* h, void* stream) {

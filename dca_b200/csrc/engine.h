@@ -182,7 +182,7 @@ struct Engine {
                 cudaStream_t s);
   int predict(const void* X, int64_t ldx, const float* sf, const int32_t* rows, int Bn, float* mean_out, float* disp_out,
               float* pi_out, int64_t ld_out, float* latent_out, cudaStream_t s);
-  int init_params(uint64_t seed, cudaStream_t s);
+  int init_params(uint64_t seed, const dca_initializer& init, cudaStream_t s);
 
   // --debug (dca_set_debug_checks): debug_check_kernel (zinb_loss.cu) checks the reference's NB terms of every element
   // into a 48-byte report at o_dbg, cleared at the start of every training / validation step, from the operands of the

@@ -4,7 +4,8 @@
 //   ConstantDispersionLayer theta = clip(exp(theta_raw), 1e-3, 1e4)             (dca/layers.py:17-21)
 //   l1_l2 kernel regulariser gradient + penalty                                (dca/network.py:125)
 //   clipvalue + RMSprop                                                        (dca/train.py:54-57)
-//   Glorot-uniform initialiser                                                 (dca/network.py:124-126)
+//   kernel initialisers: Keras' VarianceScaling family, normal, uniform, constant,
+//   identity and orthogonal (fp64 Householder QR)                              (dca/network.py:124-126)
 #include "dca_internal.cuh"
 
 namespace dca {
@@ -282,19 +283,164 @@ __global__ void optimizer_kernel(float* __restrict__ p, const float* __restrict_
   if (shadow) shadow[i] = __float2bfloat16_rn(pn);
 }
 
-__device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
+// ---- weight initialisers (include/dca_b200.h, "initializers").  Every element is a function of (seed, sid, i): sid
+// numbers the kernel tensor, i is the element's flat index.  The same source runs on the host (dca_init_fill_host).
+__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
   x += 0x9E3779B97F4A7C15ull;
   x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
   x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
   return x ^ (x >> 31);
 }
+__host__ __device__ __forceinline__ uint64_t init_hash(uint64_t seed, uint64_t sid, int64_t i) {
+  return splitmix64(splitmix64(seed ^ (sid * 0xD1B54A32D192ED03ull)) + (uint64_t)i);
+}
 
-__global__ void glorot_kernel(float* __restrict__ w, int64_t n, float limit, uint64_t seed, uint64_t sid) {
+enum InitFill : int { FILL_UNIFORM = 0, FILL_NORMAL = 1, FILL_TRUNC_NORMAL = 2, FILL_CONST = 3, FILL_IDENTITY = 4 };
+// One kernel tensor's element rule, derived on the host from a dca_initializer and the tensor's fans
+struct InitDraw {
+  int kind;             // InitFill
+  float center, half;   // uniform: center + (2u - 1) * half, one fused multiply-add in float
+  double sigma;         // normal kinds: float(z * sigma), z a standard normal in fp64
+  float value;          // constant; identity: the diagonal
+  int cols;             // identity
+};
+// Re-draws of a truncated normal before the element is set to 0: all 16 fail with probability 0.0455^16 < 4e-22
+constexpr int kTruncAttempts = 16;
+
+// Box-Muller in fp64 on two 53-bit uniforms of draw `attempt` of the element with hash h
+__host__ __device__ __forceinline__ double init_std_normal(uint64_t h, uint32_t attempt) {
+  const uint64_t h1 = splitmix64(h ^ (0x632BE59BD9B4E019ull * (2ull * attempt + 1)));
+  const uint64_t h2 = splitmix64(h ^ (0x632BE59BD9B4E019ull * (2ull * attempt + 2)));
+  const double u1 = (double)((h1 >> 11) + 1) * 0x1p-53;     // (0, 1]
+  const double u2 = (double)(h2 >> 11) * 0x1p-53;           // [0, 1)
+  return sqrt(-2.0 * log(u1)) * cos(6.283185307179586476925 * u2);
+}
+
+__host__ __device__ __forceinline__ float init_draw(const InitDraw& d, uint64_t seed, uint64_t sid, int64_t i) {
+  if (d.kind == FILL_CONST) return d.value;
+  if (d.kind == FILL_IDENTITY) return i / d.cols == i % d.cols ? d.value : 0.f;
+  const uint64_t h = init_hash(seed, sid, i);
+  if (d.kind == FILL_UNIFORM) {
+    const float u = (float)(h >> 40) * (1.0f / 16777216.0f);   // [0,1)
+    return fmaf(2.0f * u - 1.0f, d.half, d.center);
+  }
+  double z = 0.0;
+  if (d.kind == FILL_NORMAL) {
+    z = init_std_normal(h, 0);
+  } else {
+    for (int a = 0; a < kTruncAttempts; ++a) {
+      const double t = init_std_normal(h, (uint32_t)a);
+      if (fabs(t) < 2.0) { z = t; break; }
+    }
+  }
+  return (float)(z * d.sigma);
+}
+
+__global__ void init_fill_kernel(float* __restrict__ w, int64_t n, InitDraw d, uint64_t seed, uint64_t sid) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint64_t h = splitmix64(splitmix64(seed ^ (sid * 0xD1B54A32D192ED03ull)) + (uint64_t)i);
-  const float u = (float)(h >> 40) * (1.0f / 16777216.0f);   // [0,1)
-  w[i] = (2.0f * u - 1.0f) * limit;
+  if (i < n) w[i] = init_draw(d, seed, sid, i);
+}
+
+// Orthogonal: A (m x n, m = max(rows, cols), n = min) of standard normals rounded to float, Householder QR of A in
+// fp64, Q <- Q sign(diag R), W = gain Q (rows >= cols) or gain Q^T.  One CTA per tensor; A, tau and the signs live in a
+// fp64 workspace.  Every reduction runs in a fixed order, so the result is the same bits on every run.
+constexpr int kMaxOrthoJobs = 2 * DCA_MAX_HIDDEN + 4;
+struct OrthoJob { float* w; double* a; int rows, cols; uint64_t sid; };
+struct OrthoJobs { OrthoJob job[kMaxOrthoJobs]; uint64_t seed; float gain; };
+constexpr int kQrWarps = 16;
+
+// sum over the CTA of v, in a fixed order; every thread gets the result
+__device__ double qr_block_sum(double v, double* red) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  double t = 0.0;
+  for (int k = 0; k < kQrWarps; ++k) t += red[k];
+  return t;
+}
+
+// A(i:m, i+1:n) <- (I - tau v v^T) A(i:m, i+1:n), v = A(i:m, i) with v_i = 1.  Lanes own columns, warps stride rows:
+// each pass reads a row's 64 trailing columns as one coalesced piece.
+__device__ void qr_reflect(double* A, int m, int n, int i, double tau, double* red, double* wsum) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int c0 = i + 1; c0 < n; c0 += 64) {
+    const int ca = c0 + lane, cb = c0 + 32 + lane;
+    double sa = 0.0, sb = 0.0;
+    for (int r = i + warp; r < m; r += kQrWarps) {
+      const double* row = A + (int64_t)r * n;
+      const double v = r == i ? 1.0 : row[i];
+      if (ca < n) sa += v * row[ca];
+      if (cb < n) sb += v * row[cb];
+    }
+    red[warp * 64 + lane] = sa;
+    red[warp * 64 + 32 + lane] = sb;
+    __syncthreads();
+    if (threadIdx.x < 64) {
+      double t = 0.0;
+      for (int k = 0; k < kQrWarps; ++k) t += red[k * 64 + threadIdx.x];
+      wsum[threadIdx.x] = tau * t;
+    }
+    __syncthreads();
+    const double wa = wsum[lane], wb = wsum[32 + lane];
+    for (int r = i + warp; r < m; r += kQrWarps) {
+      double* row = A + (int64_t)r * n;
+      const double v = r == i ? 1.0 : row[i];
+      if (ca < n) row[ca] -= v * wa;
+      if (cb < n) row[cb] -= v * wb;
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(kQrWarps * 32) orthogonal_kernel(OrthoJobs jobs) {
+  __shared__ double red[kQrWarps * 64], wsum[64];
+  const OrthoJob jb = jobs.job[blockIdx.x];
+  const bool tall = jb.rows >= jb.cols;
+  const int m = tall ? jb.rows : jb.cols, n = tall ? jb.cols : jb.rows;
+  double* A = jb.a;
+  double* tau = A + (int64_t)m * n;
+  double* sgn = tau + n;
+  const InitDraw nd{FILL_NORMAL, 0.f, 0.f, 1.0, 0.f, 0};
+  for (int64_t e = threadIdx.x; e < (int64_t)m * n; e += blockDim.x) A[e] = (double)init_draw(nd, jobs.seed, jb.sid, e);
+  __syncthreads();
+  // A = QR: reflectors below the diagonal (LAPACK dgeqr2 / dlarfg)
+  for (int i = 0; i < n; ++i) {
+    double t = 0.0;
+    for (int r = i + 1 + threadIdx.x; r < m; r += blockDim.x) { const double x = A[(int64_t)r * n + i]; t += x * x; }
+    const double xnorm2 = qr_block_sum(t, red);
+    const double alpha = A[(int64_t)i * n + i];
+    double beta = alpha, ti = 0.0;
+    if (xnorm2 > 0.0) {
+      beta = -copysign(sqrt(alpha * alpha + xnorm2), alpha);
+      ti = (beta - alpha) / beta;
+      const double sc = 1.0 / (alpha - beta);
+      for (int r = i + 1 + threadIdx.x; r < m; r += blockDim.x) A[(int64_t)r * n + i] *= sc;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) { A[(int64_t)i * n + i] = beta; tau[i] = ti; sgn[i] = beta < 0.0 ? -1.0 : 1.0; }
+    // qr_reflect has no barrier when no column is left (i = n - 1): without this one, the first step of the Q
+    // formation below could read tau[n - 1] and write A(n-1, n-1) before thread 0's stores
+    __syncthreads();
+    qr_reflect(A, m, n, i, ti, red, wsum);
+  }
+  // Q (m x n) in place of the reflectors (LAPACK dorg2r)
+  for (int i = n - 1; i >= 0; --i) {
+    const double ti = tau[i];
+    if (i < n - 1) qr_reflect(A, m, n, i, ti, red, wsum);
+    for (int r = threadIdx.x; r < m; r += blockDim.x) {
+      double* p = A + (int64_t)r * n + i;
+      *p = r > i ? -ti * *p : (r == i ? 1.0 - ti : 0.0);
+    }
+    __syncthreads();
+  }
+  const double g = (double)jobs.gain;
+  for (int64_t e = threadIdx.x; e < (int64_t)jb.rows * jb.cols; e += blockDim.x) {
+    const int r = (int)(e / jb.cols), c = (int)(e % jb.cols);
+    const int qrow = tall ? r : c, qcol = tall ? c : r;
+    jb.w[e] = (float)(g * sgn[qcol] * A[(int64_t)qrow * n + qcol]);
+  }
 }
 
 __global__ void fill_kernel(float* __restrict__ p, int64_t n, float v) {
@@ -675,10 +821,114 @@ int optimizer_update(float* params, const float* grads, float* s1, float* s2, in
   return DCA_OK;
 }
 
-int glorot_fill(float* w, int64_t n, int fan_in, int fan_out, uint64_t seed, uint64_t sid, cudaStream_t s) {
-  const float limit = sqrtf(6.0f / (float)(fan_in + fan_out));
-  glorot_kernel<<<blocks_for(n), 256, 0, s>>>(w, n, limit, seed, sid);
-  DCA_LAUNCH_CHECK();
+// The element rule of `ini` on one kernel tensor (fans: t.fan_in and fan_out = cols).  Orthogonal gives no rule (its elements come from the QR); DCA_ERR_BAD_ARG with the
+// message set for an invalid spec or a kind the tensor's rank does not allow.
+static int init_rule(const dca_initializer& ini, const InitTensor& t, InitDraw& d) {
+  d = InitDraw{FILL_CONST, 0.f, 0.f, 0.0, 0.f, t.cols};
+  if (t.ndim != 1 && t.ndim != 2) { set_error("initializer: %s has rank %d (1 or 2 expected)", t.name, t.ndim); return DCA_ERR_BAD_ARG; }
+  if (t.rows < 1 || t.cols < 1 || (t.ndim == 1 && t.rows != 1)) {
+    set_error("initializer: %s has shape (%d, %d) at rank %d", t.name, t.rows, t.cols, t.ndim); return DCA_ERR_BAD_ARG;
+  }
+  const int fan_in = t.fan_in, fan_out = t.cols;
+  switch (ini.kind) {
+    case DCA_INIT_VARIANCE_SCALING: {
+      if (!(ini.scale > 0.f)) { set_error("initializer: variance_scaling needs scale > 0 (got %g)", ini.scale); return DCA_ERR_BAD_ARG; }
+      if (ini.mode < DCA_FAN_IN || ini.mode > DCA_FAN_AVG) { set_error("initializer: unknown fan mode %d", ini.mode); return DCA_ERR_BAD_ARG; }
+      if (ini.distribution == DCA_DIST_UNIFORM) {
+        // in float, as glorot_uniform has always been drawn: limit = sqrt(3 scale / n) (= sqrt(6 / (in + out)) for it)
+        const float n = ini.mode == DCA_FAN_IN ? (float)fan_in : ini.mode == DCA_FAN_OUT ? (float)fan_out
+                                                                                      : 0.5f * (float)(fan_in + fan_out);
+        d.kind = FILL_UNIFORM; d.center = 0.f; d.half = sqrtf(3.0f * ini.scale / fmaxf(1.0f, n));
+        return DCA_OK;
+      }
+      if (ini.distribution != DCA_DIST_TRUNCATED_NORMAL && ini.distribution != DCA_DIST_UNTRUNCATED_NORMAL) {
+        set_error("initializer: unknown distribution %d", ini.distribution); return DCA_ERR_BAD_ARG;
+      }
+      const double n = ini.mode == DCA_FAN_IN ? (double)fan_in : ini.mode == DCA_FAN_OUT ? (double)fan_out
+                                                                                       : 0.5 * ((double)fan_in + fan_out);
+      const double sd = sqrt((double)ini.scale / (n > 1.0 ? n : 1.0));
+      // 0.8796...: the standard deviation of a standard normal truncated to [-2, 2]
+      if (ini.distribution == DCA_DIST_TRUNCATED_NORMAL) { d.kind = FILL_TRUNC_NORMAL; d.sigma = sd / 0.87962566103423978; }
+      else { d.kind = FILL_NORMAL; d.sigma = sd; }
+      return DCA_OK;
+    }
+    case DCA_INIT_RANDOM_NORMAL:
+    case DCA_INIT_TRUNCATED_NORMAL:
+      if (!(ini.stddev >= 0.f)) { set_error("initializer: stddev must be >= 0 (got %g)", ini.stddev); return DCA_ERR_BAD_ARG; }
+      d.kind = ini.kind == DCA_INIT_RANDOM_NORMAL ? FILL_NORMAL : FILL_TRUNC_NORMAL;
+      d.sigma = (double)ini.stddev;
+      return DCA_OK;
+    case DCA_INIT_RANDOM_UNIFORM:
+      if (!(ini.maxval >= ini.minval)) { set_error("initializer: needs minval <= maxval (got %g, %g)", ini.minval, ini.maxval); return DCA_ERR_BAD_ARG; }
+      d.kind = FILL_UNIFORM; d.center = 0.5f * (ini.minval + ini.maxval); d.half = 0.5f * (ini.maxval - ini.minval);
+      return DCA_OK;
+    case DCA_INIT_CONSTANT:
+      d.value = ini.value;
+      return DCA_OK;
+    case DCA_INIT_ORTHOGONAL:
+    case DCA_INIT_IDENTITY:
+      if (t.ndim != 2) {
+        set_error("initializer: %s needs a 2-D kernel; %s is 1-D", ini.kind == DCA_INIT_ORTHOGONAL ? "orthogonal" : "identity", t.name);
+        return DCA_ERR_BAD_ARG;
+      }
+      d.kind = FILL_IDENTITY; d.value = ini.gain;
+      return DCA_OK;
+    default:
+      set_error("initializer: unknown kind %d", ini.kind);
+      return DCA_ERR_BAD_ARG;
+  }
+}
+
+int check_initializer(const dca_initializer* ini) {
+  if (!ini) { set_error("initializer is NULL"); return DCA_ERR_BAD_ARG; }
+  if (ini->struct_bytes != (int32_t)sizeof(dca_initializer)) {
+    set_error("initializer: struct_bytes %d != sizeof(dca_initializer) %d", ini->struct_bytes, (int)sizeof(dca_initializer));
+    return DCA_ERR_BAD_ARG;
+  }
+  return DCA_OK;
+}
+
+int check_init_tensors(const dca_initializer& ini, const InitTensor* t, int n) {
+  InitDraw d;
+  for (int k = 0; k < n; ++k) DCA_TRY(init_rule(ini, t[k], d));
+  if (ini.kind == DCA_INIT_ORTHOGONAL && n > kMaxOrthoJobs) {
+    set_error("initializer: orthogonal supports at most %d kernels (got %d)", kMaxOrthoJobs, n); return DCA_ERR_BAD_ARG;
+  }
+  return DCA_OK;
+}
+
+int init_kernels(const dca_initializer& ini, const InitTensor* t, int n, uint64_t seed, cudaStream_t s) {
+  DCA_TRY(check_init_tensors(ini, t, n));
+  InitDraw d;
+  if (ini.kind != DCA_INIT_ORTHOGONAL) {
+    for (int k = 0; k < n; ++k) {
+      init_rule(ini, t[k], d);
+      init_fill_kernel<<<blocks_for((int64_t)t[k].rows * t[k].cols), 256, 0, s>>>(t[k].w, (int64_t)t[k].rows * t[k].cols, d, seed, t[k].sid);
+      DCA_LAUNCH_CHECK();
+    }
+    return DCA_OK;
+  }
+  if (n == 0) return DCA_OK;
+  OrthoJobs jobs{};
+  jobs.seed = seed; jobs.gain = ini.gain;
+  size_t bytes = 0;
+  for (int k = 0; k < n; ++k) {
+    const int mn = t[k].rows < t[k].cols ? t[k].rows : t[k].cols;
+    bytes += sizeof(double) * ((size_t)t[k].rows * t[k].cols + 2 * (size_t)mn);
+  }
+  void* ws = nullptr;
+  DCA_CUDA_OK(cudaMallocAsync(&ws, bytes, s));
+  size_t at = 0;
+  for (int k = 0; k < n; ++k) {
+    const int mn = t[k].rows < t[k].cols ? t[k].rows : t[k].cols;
+    jobs.job[k] = OrthoJob{t[k].w, reinterpret_cast<double*>(static_cast<char*>(ws) + at), t[k].rows, t[k].cols, t[k].sid};
+    at += sizeof(double) * ((size_t)t[k].rows * t[k].cols + 2 * (size_t)mn);
+  }
+  orthogonal_kernel<<<n, kQrWarps * 32, 0, s>>>(jobs);
+  const cudaError_t le = cudaGetLastError();
+  count_launch();
+  DCA_CUDA_OK(cudaFreeAsync(ws, s));
+  if (le != cudaSuccess) { set_error("orthogonal_kernel launch failed: %s", cudaGetErrorString(le)); return DCA_ERR_CUDA; }
   return DCA_OK;
 }
 
@@ -732,3 +982,18 @@ int cast_to_bf16(const float* in, __nv_bfloat16* out, int64_t n, cudaStream_t s)
 }
 
 }  // namespace dca
+
+// ---- host mirror (include/dca_b200.h)
+extern "C" int dca_init_fill_host(const dca_initializer* init, uint64_t seed, uint64_t sid, int32_t ndim, int32_t rows,
+                                  int32_t cols, float* out) {
+  DCA_TRY(dca::check_initializer(init));
+  if (!out) { dca::set_error("dca_init_fill_host: out is NULL"); return DCA_ERR_BAD_ARG; }
+  // Keras _compute_fans: 2-D (in, out) -> fan_in = in; 1-D of length n -> n
+  const dca::InitTensor t{out, ndim, rows, cols, ndim == 1 ? cols : rows, sid, "the kernel"};
+  dca::InitDraw d;
+  DCA_TRY(dca::init_rule(*init, t, d));
+  const int64_t n = (int64_t)rows * cols;
+  if (init->kind == DCA_INIT_ORTHOGONAL) d = dca::InitDraw{dca::FILL_NORMAL, 0.f, 0.f, 1.0, 0.f, 0};   // the draws of A
+  for (int64_t i = 0; i < n; ++i) out[i] = dca::init_draw(d, seed, sid, i);
+  return DCA_OK;
+}

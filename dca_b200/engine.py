@@ -31,11 +31,13 @@ class DeviceEngine:
                  l1_enc: float = 0.0, l2_enc: float = 0.0, gemm_path: str = "auto",
                  device: Optional[torch.device] = None, seed: Optional[int] = 0, sharedpi: bool = False,
                  sync_bn: bool = False, activation: str = "relu", hidden_dropout=0.0, input_dropout: float = 0.0,
-                 dropout_seed: Optional[int] = None):
+                 dropout_seed: Optional[int] = None, init: str = "glorot_uniform"):
         if ae_type not in _lib.AE_TYPE_IDS:
             raise NotImplementedError("ae_type %r is not on the accelerated path (supported: %s)"
                                       % (ae_type, sorted(_lib.AE_TYPE_IDS)))
         self.lib = _lib.load()
+        self.init = init
+        self._init_spec = _lib.initializer(init)         # kernel_initializer of every kernel (dca/network.py:124-126)
         if not torch.cuda.is_available():
             raise _lib.DcaError("dca_b200 needs a CUDA device (H100); there is no CPU fallback")
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
@@ -99,7 +101,11 @@ class DeviceEngine:
         self.param_info = self._infos(self.lib.dca_param_count, self.lib.dca_param_info)
         self.state_info = self._infos(self.lib.dca_state_count, self.lib.dca_state_info)
         if seed is not None:
-            self.init_params(seed)
+            try:
+                self.init_params(seed)
+            except ValueError:
+                self.close()
+                raise
 
     # ------------------------------------------------------------------ plumbing
     def _stream(self):
@@ -139,7 +145,11 @@ class DeviceEngine:
 
     # ------------------------------------------------------------------ parameters
     def init_params(self, seed: int):
-        check(self.lib.dca_init_params(self.handle, C.c_uint64(seed & (2 ** 64 - 1)), self._stream()), "dca_init_params")
+        """Kernels drawn by the engine's initializer (``init``), biases, BatchNorm and theta at their Keras defaults.
+        ValueError when the initializer does not apply to a kernel of the model (orthogonal / identity on the 1-D
+        'pi/kernel' of zinb-elempi)."""
+        check(self.lib.dca_init_params_ex(self.handle, C.c_uint64(seed & (2 ** 64 - 1)), C.byref(self._init_spec),
+                                          self._stream()), "dca_init_params_ex")
 
     def params_changed(self):
         check(self.lib.dca_params_changed(self.handle, self._stream()), "dca_params_changed")

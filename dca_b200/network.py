@@ -98,8 +98,6 @@ class Autoencoder:
         if self.ae_type is None:
             raise NotImplementedError("autoencoder type %s is not on the GPU-accelerated path"
                                       % type(self).__name__)
-        if self.init != 'glorot_uniform':
-            raise NotImplementedError("only init='glorot_uniform' is on the accelerated path")
         if seed is not None:
             self._seed = seed
         self._max_batch = max_batch
@@ -109,7 +107,8 @@ class Autoencoder:
                                    l1_enc=self.l1_enc_coef, l2_enc=self.l2_enc_coef,
                                    gemm_path=self.gemm_path, seed=self._seed, sharedpi=self.sharedpi,
                                    sync_bn=self.sync_bn, activation=self.activation,
-                                   hidden_dropout=self.hidden_dropout, input_dropout=self.input_dropout)
+                                   hidden_dropout=self.hidden_dropout, input_dropout=self.input_dropout,
+                                   init=self.init)
         self.model = self.engine
         self.encoder = self.engine
         self.loss = self.ae_type

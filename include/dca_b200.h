@@ -150,6 +150,55 @@ int dca_region(dca_handle* h, int32_t region_id, void** dev_ptr, int64_t* count)
 /* Glorot-uniform kernels, zero biases/beta/theta, moving_mean 0, moving_var 1, rms 0
  * (Keras initialisers named at dca/network.py:124-126, dca/layers.py:17-20). */
 int dca_init_params(dca_handle* h, uint64_t seed, void* stream);
+
+/* ---- initializers: the `kernel_initializer` of every Dense / ElementwiseDense kernel (dca/network.py:124-126,
+ * CLI --init), Keras 2 / tf.keras 2.x semantics.  Fans (Keras _compute_fans): a 2-D kernel (in, out) has fan_in = in,
+ * fan_out = out; a 1-D kernel of length n (zinb-elempi's "pi/kernel") has fan_in = fan_out = n.  In the types other
+ * than the four flagship ones, a 2-D kernel with one input row (n_in or a hidden width of 1) also takes fan_in = out,
+ * as glorot_uniform has always drawn it there (Keras: 1); it is still 2-D for ORTHOGONAL and IDENTITY.
+ *   VARIANCE_SCALING(scale > 0, mode, distribution): n = fan_in, fan_out or (fan_in + fan_out) / 2 by mode,
+ *     s = scale / max(1, n); uniform: U(-sqrt(3 s), sqrt(3 s)) (limit computed in float); untruncated normal:
+ *     N(0, sqrt(s)); truncated normal: N(0, sqrt(s) / 0.87962566103423978) re-drawn beyond 2 sigma.
+ *   RANDOM_NORMAL(stddev): N(0, stddev).  TRUNCATED_NORMAL(stddev): the same re-drawn beyond 2 stddev.
+ *   RANDOM_UNIFORM(minval, maxval): U(minval, maxval).  CONSTANT(value).
+ *   ORTHOGONAL(gain): A = (max(rows, cols) x min(rows, cols)) standard normals, Q R = A (reduced), Q <- Q sign(diag R),
+ *     W = gain Q, transposed when rows < cols; an fp64 Householder QR on the device, one CTA per kernel.
+ *   IDENTITY(gain): gain * eye(rows, cols).  ORTHOGONAL and IDENTITY need 2-D kernels.
+ * Draws are counter-based: element i of the kernel with stream id sid is a function of (seed, sid, i) alone.
+ *   uniform: u = (h >> 40) 2^-24 from a 64-bit hash h of (seed, sid, i); w = fmaf(2u - 1, half, center).
+ *   normal: Box-Muller in fp64 from two 53-bit uniforms of draw a (0, 1, ...) of the element, rounded once to float;
+ *     a truncated normal takes the first draw with |z| < 2, and 0 if 16 draws all fail (probability < 4e-22).
+ * Kernel stream ids: the four flagship types (zinb-conddisp, zinb, nb-conddisp, nb) number their hidden layers 0, 1,
+ * ... and the head kernels 100 (mean), 101 (dispersion), 102 (pi); the other types number every kernel in the order
+ * of dca_param_info. */
+typedef enum dca_init_kind {
+  DCA_INIT_VARIANCE_SCALING = 0, DCA_INIT_RANDOM_NORMAL = 1, DCA_INIT_RANDOM_UNIFORM = 2, DCA_INIT_TRUNCATED_NORMAL = 3,
+  DCA_INIT_CONSTANT = 4, DCA_INIT_ORTHOGONAL = 5, DCA_INIT_IDENTITY = 6
+} dca_init_kind;
+typedef enum dca_fan_mode { DCA_FAN_IN = 0, DCA_FAN_OUT = 1, DCA_FAN_AVG = 2 } dca_fan_mode;
+typedef enum dca_distribution {
+  DCA_DIST_TRUNCATED_NORMAL = 0, DCA_DIST_UNTRUNCATED_NORMAL = 1, DCA_DIST_UNIFORM = 2
+} dca_distribution;
+typedef struct dca_initializer {
+  int32_t struct_bytes;       /* sizeof(dca_initializer), ABI guard */
+  int32_t kind;               /* dca_init_kind */
+  float scale;                /* VARIANCE_SCALING */
+  int32_t mode;               /* VARIANCE_SCALING: dca_fan_mode */
+  int32_t distribution;       /* VARIANCE_SCALING: dca_distribution */
+  float stddev;               /* RANDOM_NORMAL, TRUNCATED_NORMAL */
+  float minval, maxval;       /* RANDOM_UNIFORM */
+  float value;                /* CONSTANT */
+  float gain;                 /* ORTHOGONAL, IDENTITY */
+} dca_initializer;
+/* dca_init_params with `init` for every kernel (biases, BatchNorm, PReLU slopes, theta and the optimizer state as
+ * there).  glorot_uniform is VARIANCE_SCALING(1, FAN_AVG, UNIFORM): the same bits as dca_init_params.  An invalid
+ * spec, or ORTHOGONAL / IDENTITY on a model with a 1-D kernel, returns DCA_ERR_BAD_ARG and changes nothing. */
+int dca_init_params_ex(dca_handle* h, uint64_t seed, const dca_initializer* init, void* stream);
+/* HOST restatement of the draws (same source as the device code): the rows x cols elements (ndim 1: rows = 1) of the
+ * kernel with stream id sid into out, row-major.  ORTHOGONAL writes its matrix A instead (max(rows, cols) x
+ * min(rows, cols), row-major), whose QR the device takes. */
+int dca_init_fill_host(const dca_initializer* init, uint64_t seed, uint64_t sid, int32_t ndim, int32_t rows, int32_t cols,
+                       float* out);
 /* Call after writing DCA_REGION_PARAMS directly (refreshes operand-layout shadow copies). */
 int dca_params_changed(dca_handle* h, void* stream);
 
