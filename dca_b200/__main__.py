@@ -3,9 +3,13 @@ import argparse
 
 # (flags, kwargs) in the reference's order; paired --x/--nox booleans share a dest
 _OPTIONS = [
-    (('input',), dict(type=str, help='Input is raw count data in TSV/CSV or H5AD (anndata) format. Row/col names '
-                                     'are mandatory. TSV/CSV files must be gene x cell (use -t for cell x gene); '
-                                     'H5AD files must be cell x gene.')),
+    (('input',), dict(type=str, help='Input is raw count data in TSV/CSV, Matrix Market (.mtx), their .gz, or H5AD '
+                                     '(anndata) format, or a Cell Ranger matrix directory (matrix.mtx[.gz], '
+                                     'features.tsv[.gz] or genes.tsv[.gz], barcodes.tsv[.gz], with or without a GEO '
+                                     'sample prefix: cells named by barcode, genes by unique gene symbol, Gene '
+                                     'Expression rows only). Row/col names are mandatory. TSV/CSV and Matrix Market '
+                                     'files and directories must be gene x cell (use -t for cell x gene); H5AD files '
+                                     'must be cell x gene.')),
     (('outputdir',), dict(type=str, help='The path of the output directory')),
     (('--normtype',), dict(type=str, default='zheng', help='Type of size factor estimation (parsed, unused; default: zheng)')),
     (('-t', '--transpose'), dict(dest='transpose', action='store_true', help='Transpose input matrix (default: False)')),

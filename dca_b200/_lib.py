@@ -202,6 +202,8 @@ PROTOTYPES = {
     "dca_read_mtx_counts": (C.c_int, [C.c_char_p, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
     "dca_read_text_counts_gz": (C.c_int, [C.c_char_p, _i32, _i32, _i64, _i32, _vp, _vp, _i64, _vp, _vp, _i64, _vp]),
     "dca_read_mtx_counts_gz": (C.c_int, [C.c_char_p, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "dca_read_mtx_counts_map": (C.c_int, [C.c_char_p, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64]),
+    "dca_read_mtx_counts_gz_map": (C.c_int, [C.c_char_p, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64]),
     "dca_gunzip": (C.c_int, [C.c_char_p, _i32, _vp, _vp, _i64, _vp]),
     "dca_inflate_span_host": (C.c_int, [_vp, _i64, _i32, _i64, _i64, _vp, _i64, _vp]),
     "dca_inflate_find_host": (C.c_int, [_vp, _i64, _i64, _i64, _vp]),

@@ -22,7 +22,8 @@ def _dense(X):
 def read_text_or_h5ad(path: str):
     """sc.read(path, first_column_names=True) -- dca/io.py:59.  Text tables go through the GPU reader when it can take
     them (read_counts_text), otherwise through pandas; Matrix Market files through read_counts_mtx, otherwise through
-    scipy; gzip files of either through read_counts_gzip first; all give the same AnnData."""
+    scipy; gzip files of either through read_counts_gzip first; all give the same AnnData.  A Cell Ranger matrix
+    directory goes through read_counts_10x, otherwise through _read_10x_scipy."""
     return _read_path(path, False)[0]
 
 
@@ -32,7 +33,13 @@ _COMPRESSED_MAGIC = (b"\x1f\x8b", b"BZh", b"\xfd7zXZ\x00", b"\x28\xb5\x2f\xfd", 
 
 
 def _read_path(path, transpose):
-    """(AnnData, transposed): transposed is True when the GPU reader already returned the cells x genes orientation."""
+    """(AnnData, transposed): transposed is True when the reader already returned the cells x genes orientation."""
+    if os.path.isdir(path):
+        if _cuda_available():
+            ad = read_counts_10x(path, transpose)
+            if ad is not None:
+                return ad, transpose
+        return _read_10x_scipy(path, transpose), transpose
     ext = os.path.splitext(path)[1].lower()
     if ext == ".h5ad":
         try:
@@ -168,8 +175,9 @@ def read_counts_mtx(path, transpose=False, chunk_bytes=0, device=None):
     return _read_mtx_gpu(path, transpose, chunk_bytes, device, "dca_read_mtx_counts")
 
 
-def _read_mtx_gpu(path, transpose, chunk_bytes, device, entry):
-    """read_counts_mtx through the native reader `entry` (the file's bytes, or those of its inflated stream)."""
+def _read_mtx_gpu(path, transpose, chunk_bytes, device, entry, feature_map=None):
+    """read_counts_mtx through the native reader `entry` (the file's bytes, or those of its inflated stream).  The
+    '_map' entries take feature_map (int32 per file row: its output index, or -1 to drop it; None keeps every row)."""
     import ctypes as C
     import torch
     import scipy.sparse as sp
@@ -184,7 +192,11 @@ def _read_mtx_gpu(path, transpose, chunk_bytes, device, entry):
     stream = torch.cuda.current_stream(dev)
     with torch.cuda.device(dev):
         args = (os.fsencode(path), int(bool(transpose)), int(chunk_bytes), dev.index, C.c_void_p(stream.cuda_stream))
-        st = read(*args, None, None, None, info.ctypes.data)
+        tail = ()
+        if entry.endswith("_map"):
+            fmap = None if feature_map is None else np.ascontiguousarray(feature_map, dtype=np.int32)
+            tail = (None, 0) if fmap is None else (fmap.ctypes.data, fmap.size)
+        st = read(*args, None, None, None, info.ctypes.data, *tail)
         if st == -3:
             return None
         _lib.check(st, entry)
@@ -195,10 +207,11 @@ def _read_mtx_gpu(path, transpose, chunk_bytes, device, entry):
         indices = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
         data = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
         st = read(*args, C.c_void_p(indptr.data_ptr()), C.c_void_p(indices.data_ptr()), C.c_void_p(data.data_ptr()),
-                  info.ctypes.data)
+                  info.ctypes.data, *tail)
         if st == -3:
             return None
         _lib.check(st, entry)
+        nnz = int(info[2])                           # the entries kept (all of them without a feature map)
         indptr, indices, data = indptr.cpu().numpy(), indices[:nnz].cpu().numpy(), data[:nnz].cpu().numpy()
     if max(rows, cols, nnz) < 2 ** 31:
         indptr = indptr.astype(np.int32)
@@ -219,6 +232,158 @@ def read_counts_gzip(path, transpose=False, chunk_bytes=0, device=None):
     if path.lower().endswith(".mtx.gz"):
         return _read_mtx_gpu(path, transpose, chunk_bytes, device, "dca_read_mtx_counts_gz")
     return _read_text_gpu(path, "\t", transpose, chunk_bytes, device, "dca_read_text_counts_gz")
+
+
+# Cell Ranger's matrix directory: the files of each role, by suffix after the shared prefix (GEO's sample prefix, or '')
+_10X_ROLES = (("matrix", ("matrix.mtx.gz", "matrix.mtx")),
+              ("features", ("features.tsv.gz", "features.tsv", "genes.tsv.gz", "genes.tsv")),
+              ("barcodes", ("barcodes.tsv.gz", "barcodes.tsv")))
+_10X_WANT = {"matrix": "matrix.mtx[.gz]", "features": "features.tsv[.gz] (or genes.tsv[.gz])",
+             "barcodes": "barcodes.tsv[.gz]"}
+
+
+def _find_10x(path):
+    """(matrix, features, barcodes): the paths of the one Cell Ranger triple in directory `path` that share a prefix;
+    ValueError naming the files when a file is missing or there is more than one triple."""
+    found = {}                                   # prefix -> role -> [file names]
+    for name in sorted(os.listdir(path)):
+        if not os.path.isfile(os.path.join(path, name)):
+            continue
+        for role, suffixes in _10X_ROLES:
+            suf = next((x for x in suffixes if name.endswith(x)), None)
+            if suf is not None:
+                found.setdefault(name[:-len(suf)], {}).setdefault(role, []).append(name)
+                break
+    triples = []
+    for prefix, roles in found.items():
+        if len(roles) == 3:
+            triples += [(m, f, b) for m in roles["matrix"] for f in roles["features"] for b in roles["barcodes"]]
+    if len(triples) > 1:
+        raise ValueError("%s holds %d candidate Cell Ranger matrix triples (matrix, features, barcodes): %s" % (
+            path, len(triples), "; ".join(", ".join(t) for t in triples)))
+    if not triples:
+        if not found:
+            raise ValueError("%s is not a Cell Ranger matrix directory: it has no %s, %s or %s" % (
+                path, _10X_WANT["matrix"], _10X_WANT["features"], _10X_WANT["barcodes"]))
+        missing = ["%s (beside %s)" % (prefix + _10X_WANT[role], ", ".join(sum(roles.values(), [])))
+                   for prefix, roles in sorted(found.items()) for role, _ in _10X_ROLES if role not in roles]
+        raise ValueError("%s is not a Cell Ranger matrix directory: missing %s" % (path, "; ".join(missing)))
+    return tuple(os.path.join(path, n) for n in triples[0])
+
+
+def _read_tsv_columns(path, most):
+    """The first `most` tab-separated columns of a headerless label file (gzip or plain, by magic bytes) as strings,
+    taken literally (no NA values, no quoting)."""
+    import csv
+    try:
+        tab = pd.read_csv(path, sep="\t", header=None, dtype=str, na_filter=False, quoting=csv.QUOTE_NONE,
+                          compression="gzip" if _is_gzip(path) else None)
+    except pd.errors.EmptyDataError:
+        return [np.empty(0, dtype=object)]
+    return [tab[c].to_numpy(dtype=object) for c in tab.columns[:most]]
+
+
+def make_index_unique(names, join="-"):
+    """anndata.utils.make_index_unique: the first occurrence of a name stays; each later duplicate v takes v-1, v-2, ...
+    (one counter per name), skipping any candidate already among the names or already given."""
+    idx = pd.Index(names)
+    if idx.is_unique:
+        return idx
+    values = idx.to_numpy(dtype=object).copy()
+    taken = set(values)
+    counter = {}
+    for i in np.flatnonzero(idx.duplicated(keep="first")):
+        v = values[i]
+        while True:
+            counter[v] = counter.get(v, 0) + 1
+            cand = "%s%s%d" % (v, join, counter[v])
+            if cand not in taken:
+                taken.add(cand)
+                values[i] = cand
+                break
+    return pd.Index(values, name=idx.name)
+
+
+def _mtx_size(path):
+    """(M, N) of a Matrix Market file's size line (gzip or plain, by magic bytes); None when there is none."""
+    import gzip
+    with (gzip.open if _is_gzip(path) else open)(path, "rb") as f:
+        for line in f:
+            if not line.startswith(b"%"):
+                parts = line.split()
+                return (int(parts[0]), int(parts[1])) if len(parts) >= 2 and parts[0].isdigit() and \
+                    parts[1].isdigit() else None
+    return None
+
+
+def _10x_labels(path, shape=None):
+    """(matrix path, barcodes, var, keep) of the Cell Ranger directory `path`: var (one row per feature of the file,
+    indexed by the unique gene symbols) holds gene_ids and, for the v3 layout, feature_types; keep marks the rows
+    read_10x_mtx(gex_only=True) keeps.  shape: (M, N) of the matrix, checked against the label counts (ValueError)."""
+    matrix, features, barcodes = _find_10x(path)
+    cols = _read_tsv_columns(features, 3)
+    v3 = os.path.basename(features)[:-len(".tsv.gz" if features.endswith(".gz") else ".tsv")].endswith("features")
+    bc = _read_tsv_columns(barcodes, 1)[0]
+    if len(cols) < 2:
+        raise ValueError("%s: a features file needs gene ids and symbols (2 tab-separated columns)" % features)
+    if shape is None:
+        shape = _mtx_size(matrix)
+    if shape is not None and (len(cols[0]), len(bc)) != tuple(shape):
+        raise ValueError("%s is %d x %d (features x barcodes), but %s lists %d features and %s %d barcodes" % (
+            matrix, shape[0], shape[1], features, len(cols[0]), barcodes, len(bc)))
+    var = pd.DataFrame({"gene_ids": cols[0]}, index=make_index_unique(cols[1]))
+    keep = np.ones(len(var), dtype=bool)
+    if v3 and len(cols) > 2:
+        var["feature_types"] = cols[2]
+        keep = cols[2] == "Gene Expression"
+    return matrix, pd.Index(bc), var, keep
+
+
+def _10x_anndata(X, barcodes, var, keep, transpose):
+    """The AnnData of a Cell Ranger read: X cells x genes (transpose) or genes x cells, with the kept features."""
+    var = var[keep]
+    obs = pd.DataFrame(index=barcodes)
+    return AnnData(X, obs=obs, var=var, keep_sparse=True) if transpose else \
+        AnnData(X, obs=var, var=obs, keep_sparse=True)
+
+
+def _read_10x_scipy(path, transpose):
+    """scanpy's read_10x_mtx(path, var_names='gene_symbols', make_unique=True, gex_only=True), transposed to genes x
+    cells unless `transpose`: X = csr_matrix(mmread(matrix).astype(float32)), .T.tocsr() with transpose, then the
+    Gene Expression features (columns with transpose, rows without); labels as _10x_labels reads them."""
+    import gzip
+    import warnings
+    import scipy.io
+    import scipy.sparse as sp
+    matrix, barcodes, var, keep = _10x_labels(path)
+    with warnings.catch_warnings(), (gzip.open if _is_gzip(matrix) else open)(matrix, "rb") as f:
+        warnings.simplefilter("ignore", DeprecationWarning)
+        X = sp.csr_matrix(scipy.io.mmread(f).astype(np.float32))
+    if X.shape != (len(var), len(barcodes)):
+        raise ValueError("%s is %d x %d, but its directory lists %d features and %d barcodes" % (
+            matrix, X.shape[0], X.shape[1], len(var), len(barcodes)))
+    if transpose:
+        X = X.T.tocsr()
+    if not keep.all():
+        kept = np.flatnonzero(keep)
+        X = X[:, kept] if transpose else X[kept]
+    return _10x_anndata(X, barcodes, var, keep, transpose)
+
+
+def read_counts_10x(path, transpose=False, chunk_bytes=0, device=None):
+    """The AnnData _read_10x_scipy(path, transpose) gives, with the matrix parsed on a CUDA device by
+    dca_read_mtx_counts_map / dca_read_mtx_counts_gz_map (csrc/read_mtx.cu, gzip detected by magic bytes): the
+    features other than Gene Expression are dropped inside the parse, so they never reach the CSR arrays, whose
+    indptr, indices and data equal scipy's in dtype and bytes.  The labels are read on the host (_10x_labels).  None
+    when the GPU reader does not take the matrix (as read_counts_mtx), or the arrays do not fit in free device memory.
+    ValueError when the directory is not one Cell Ranger triple or its label counts do not match the matrix."""
+    matrix, barcodes, var, keep = _10x_labels(path)
+    fmap = None if keep.all() else np.where(keep, np.cumsum(keep) - 1, -1).astype(np.int32)
+    entry = "dca_read_mtx_counts_gz_map" if _is_gzip(matrix) else "dca_read_mtx_counts_map"
+    ad = _read_mtx_gpu(matrix, transpose, chunk_bytes, device, entry, fmap)
+    if ad is None:
+        return None
+    return _10x_anndata(ad.X, barcodes, var, keep, transpose)
 
 
 def _pandas_chunk_rows(width):

@@ -747,6 +747,26 @@ int dca_read_text_counts_gz(const char* path, int32_t sep, int32_t transpose, in
 int dca_read_mtx_counts_gz(const char* path, int32_t transpose, int64_t chunk_bytes, int32_t device, void* stream,
                            int64_t* indptr, int32_t* indices, float* data, int64_t* info);
 
+/* dca_read_mtx_counts and dca_read_mtx_counts_gz keeping only some features, the file's rows (dca_b200/io.py:
+ * read_counts_10x drops the rows of a Cell Ranger matrix whose feature type is not "Gene Expression").  The same
+ * parameters, accepted files and two calls, plus host int32 feature_map[map_len] with map_len = M (the file's rows):
+ * feature_map[i - 1] is -1 to drop the entries of file row i, or the output index of its feature, which must be the
+ * number of features kept before it (0, 1, 2, ... over the kept rows, so the kept entries stay in CSR order; any other
+ * map returns DCA_ERR_BAD_ARG).  The output is the input's output with the dropped features taken out: with transpose
+ * the map renumbers the output's columns, without it its rows.  feature_map NULL keeps every feature, with the bytes
+ * of dca_read_mtx_counts / dca_read_mtx_counts_gz.
+ *   1. indptr == NULL: info[0..3] = output rows, output columns (after the map), NNZ of the file (an upper bound of
+ *      the kept entries, which the outputs must hold), device bytes besides the outputs.
+ *   2. as before, and info[2] = the kept NNZ on return.  Kept entry k goes to slot k (a scan over the entries, carried
+ *      across chunks; no atomics), and the order check applies to the kept entries only.
+ * Entries of dropped rows are parsed and checked like the others. */
+int dca_read_mtx_counts_map(const char* path, int32_t transpose, int64_t chunk_bytes, int32_t device, void* stream,
+                            int64_t* indptr, int32_t* indices, float* data, int64_t* info, const int32_t* feature_map,
+                            int64_t map_len);
+int dca_read_mtx_counts_gz_map(const char* path, int32_t transpose, int64_t chunk_bytes, int32_t device, void* stream,
+                               int64_t* indptr, int32_t* indices, float* data, int64_t* info,
+                               const int32_t* feature_map, int64_t map_len);
+
 /* GPU inflate of a gzip file (RFC 1952: one or more members of DEFLATE data, RFC 1951) into DEVICE memory, with no
  * zlib: the host reads the compressed file in 64 MB segments and the device decodes each segment in spans of about
  * 32 KB in parallel, speculatively from block starts it finds, then checks the chain of spans, the CRC-32 and the
